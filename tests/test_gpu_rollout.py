@@ -293,6 +293,17 @@ def test_engine_obs_tiles_matches_fp32_forward():
             tb = wb.cuda_data_manager.data_on_device_via_torch(name)
             assert torch.equal(ta, tb), name
     assert int(ea.num_completed_episodes) == int(eb.num_completed_episodes) > 0
+    # the tiles the env step wrote (store_obs_chunk, incl. the rows of envs that reset) are
+    # byte for byte what pack_obs makes of the same observations, K padding and the zero rows
+    # of the last tile included: that padding must be finite, since 0 * NaN in the MMA would
+    # poison every row
+    for p in pm:
+        fwd = ea.fused_forward[p]
+        rows = ea.cur_obs[p].numel() // fwd.F
+        ref = torch.full((fwd.tiles_bytes(rows),), 0xFF, dtype=torch.uint8, device="cuda")
+        fwd.pack_obs(ea.cur_obs[p], ref)
+        torch.cuda.synchronize()
+        assert torch.equal(ea.obs_tiles[p], ref), p
 
 
 
