@@ -274,35 +274,44 @@ int wdb_acrobot_step(void *stream, int n_envs, float *state, const int *action, 
                      float *reward, float *obs, int *env_timestep, int episode_length);
 
 /* ------------------------------------------ whole rollout, single-agent envs ---- */
-/* ONE launch = n_steps rollout timesteps of a discrete-action single-agent env, one thread
- * per env replica: FullyConnected forward (fp32, weights in shared memory) -> categorical
- * sample -> step -> bookkeeping -> done-masked reset -> push to the batch slots.  Replaces
- * the body of TrainerBase._generate_rollout_batch (trainer_base.py:383-428) for
- * ClassicControl{CartPole,MountainCar,Acrobot}Env: per timestep the reference issues the
- * model forward, sample_actions, Numba...EnvStep, ~20 bookkeeping torch ops and one reset
- * kernel per registered array.  The step physics are the same compiled functions the
- * stand-alone step kernels call. */
-enum { WDB_SA_CARTPOLE = 0, WDB_SA_MOUNTAIN_CAR = 1, WDB_SA_ACROBOT = 2 };
+/* ONE launch = n_steps rollout timesteps of a single-agent classic-control env, one thread
+ * per env replica: FullyConnected forward (fp32, weights in shared memory) -> action sample
+ * -> step -> bookkeeping -> done-masked reset -> push to the batch slots.  Replaces the body
+ * of TrainerBase._generate_rollout_batch (trainer_base.py:383-428) for
+ * ClassicControl{CartPole,MountainCar,Acrobot}Env, and the DDPG rollout of
+ * ClassicControl{ContinuousMountainCar,Pendulum}Env (trainer_ddpg.py): per timestep the
+ * reference issues the model forward, sample_actions / sample_ou_process, Numba...EnvStep,
+ * ~20 bookkeeping torch ops and one reset kernel per registered array.
+ * Discrete kinds: softmax head, categorical sample, int32 actions.  Continuous kinds: a head
+ * of width 1, mean = action_scale * tanh(z) + action_bias, OU noise exactly as
+ * wdb_sample_ou_process (stream = env), float32 actions.  The step physics and the OU update
+ * are the same compiled functions the stand-alone kernels call. */
+enum {
+  WDB_SA_CARTPOLE = 0, WDB_SA_MOUNTAIN_CAR = 1, WDB_SA_ACROBOT = 2,
+  WDB_SA_CONTINUOUS_MOUNTAIN_CAR = 3,  /* state 2, obs 2, done at episode end or goal */
+  WDB_SA_PENDULUM = 4                  /* state 2, obs 3, done at episode end */
+};
 
 typedef struct wdb_sa_rollout {
   int env_kind, n_envs, n_steps, episode_length, state_dim, use_argmax;
   float env_params[12];              /* the scalar arguments of the env's step function, in
-                                      * the order of wdb_cartpole_step / wdb_mountain_car_step */
+                                      * the order of wdb_cartpole_step / wdb_mountain_car_step /
+                                      * wdb_continuous_mountain_car_step (Pendulum: none) */
   float *state;                      /* [E, state_dim] */
   float *observations;               /* [E, F] current observation (read and updated) */
   int *done, *env_timestep;          /* [E] */
   float *rewards;                    /* [E] */
-  int *sampled_actions;              /* [E] */
-  int n_hidden;                      /* hidden Linear + ReLU layers (0..3), then the softmax head */
-  int dims[5];                       /* F, H1, ..., A */
+  void *sampled_actions;             /* [E]: int32 (discrete kinds) or float32 (continuous) */
+  int n_hidden;                      /* hidden Linear + ReLU layers (0..3), then the head */
+  int dims[5];                       /* F, H1, ..., A (continuous kinds: A = 1) */
   const float *w[4], *b[4];          /* nn.Linear weights [out, in] and biases, fp32 */
   void *rng_state;
   const float *uniforms;             /* test hook [n_steps, E]; NULL = device RNG */
   float *obs_batch;                  /* [n_steps, E, F] or NULL */
-  int *actions_batch;                /* [n_steps, E] or NULL */
+  void *actions_batch;               /* [n_steps, E] or NULL; element type of sampled_actions */
   float *rewards_batch;              /* [n_steps, E] or NULL */
   int *done_batch;                   /* [n_steps, E] or NULL */
-  float *probs_batch;                /* [n_steps, E, A] or NULL (tests) */
+  float *probs_batch;                /* [n_steps, E, A] or NULL (tests); continuous: the mean */
   float *reward_running_sum;         /* [E] or NULL */
   int *step_running_sum;             /* [E] or NULL */
   float *episodic_reward_sum;        /* scalar or NULL */
@@ -311,6 +320,11 @@ typedef struct wdb_sa_rollout {
   int n_reset_arrays;
   void *pool_rng;                    /* RNG state of the reset pools, or NULL */
   int reset_done_envs;
+  /* continuous kinds only (ignored otherwise) */
+  float ou_damping, ou_stddev, ou_scale;  /* as wdb_sample_ou_process; scale < 1e-8: no noise */
+  float *ou_state;                   /* [E] OU state; required unless scale < 1e-8 */
+  float action_scale, action_bias;   /* the actor's output_w / output_b */
+  const float *normals;              /* test hook [n_steps, E]; NULL = device RNG */
 } wdb_sa_rollout;
 
 int wdb_single_agent_rollout_supported(int n_hidden, const int *dims);

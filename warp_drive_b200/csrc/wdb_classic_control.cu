@@ -53,10 +53,7 @@ mountain_car_step_kernel(int n_envs, float2 *__restrict__ state, const int *__re
 }
 
 // ============================================================ ContinuousMountainCar
-// NumbaClassicControlContinuousMountainCarEnvStep, continuous_mountain_car_step_numba.py:
-// 14-71.  force = clip(action) and force * power stay float32; the rest is float64
-// (reference SASS: FMUL force*power; DFMA cos * -0.0025 + that; DADD velocity).
-// reward = (terminated ? 100 : 0) - pow(action, 2) * 0.1 in float64 (:64-69).
+// continuous_mountain_car_physics (wdb_sa_physics.cuh); done = 1 at the episode end or the goal.
 __global__ void __launch_bounds__(kCcThreads)
 continuous_mountain_car_step_kernel(int n_envs, float2 *__restrict__ state,
                                     const float *__restrict__ action, int *__restrict__ done,
@@ -69,46 +66,17 @@ continuous_mountain_car_step_kernel(int n_envs, float2 *__restrict__ state,
   if (env >= n_envs) return;
   const int t = env_timestep[env] + 1;
   env_timestep[env] = t;
-  const float a = action[env];
-  const float2 s = state[env];
-  float f = a;
-  if (a < min_action) f = min_action;
-  else if (a > max_action) f = max_action;
-  const float fp = __fmul_rn(f, power);
-  const double pos0 = (double)s.x;
-  const double c = cos(__dmul_rn(pos0, 3.0));
-  double vel = __dadd_rn(__fma_rn(c, -0.0025, (double)fp), (double)s.y);
-  vel = sa_clip_f64(vel, (double)(-max_speed), (double)max_speed);
-  double pos = __dadd_rn(pos0, vel);
-  pos = sa_clip_f64(pos, (double)min_position, (double)max_position);
-  if (pos == (double)min_position && vel < 0.0) vel = 0.0;
-  const float2 n = make_float2((float)pos, (float)vel);
-  state[env] = n;
-  obs[env] = n;
-  const bool terminated = pos >= (double)goal_position && vel >= (double)goal_velocity;
-  const double rew = terminated ? 100.0 : 0.0;
-  reward[env] = (float)__dsub_rn(rew, __dmul_rn(pow((double)a, 2.0), 0.1));
-  if (t == episode_length || terminated) done[env] = 1;
+  const ContinuousStep r = continuous_mountain_car_physics(
+      state[env], action[env], min_action, max_action, min_position, max_position, max_speed,
+      goal_position, goal_velocity, power);
+  state[env] = r.s;
+  obs[env] = r.s;
+  reward[env] = r.reward;
+  if (t == episode_length || r.terminated) done[env] = 1;
 }
 
 // ========================================================================= Pendulum
-// NumbaClassicControlPendulumEnvStep, pendulum_step_numba.py:30-72 (g = 9.81, m = l = 1,
-// dt = 0.05, max_speed = 8, max_torque = 2 are module constants there, :9-14).
-//   u = clip(action, -2, 2) in float64; angle_normalize(th) = ((th + pi) % 2pi) - pi in
-//   float64, where NVVM lowers `%` to  a - floor(|a| / b) * b  with the sign of a restored
-//   and Python's "result takes the divisor's sign" fix-up; sin(th) is the FLOAT32 routine
-//   (th is float32), cos/sin(newth) the float64 ones.  FMA placement from the reference SASS:
-//   costs = fma(u*u, 0.001, fma(an, an, 0.1 * (double)(thdot*thdot)))
-//   newthdot = fma(fma(u, 3, 14.715 * sin(th)), dt, thdot);  newth = fma(newthdot, dt, th).
-__device__ __forceinline__ double python_mod_2pi(double a) {
-  const double b = 2.0 * 3.141592653589793;
-  const double q = floor(__ddiv_rn(fabs(a), b));
-  double r = __fma_rn(-q, b, fabs(a));
-  if (!(a >= 0.0)) r = -r;
-  if (r < 0.0) r = __dadd_rn(r, b);
-  return r;
-}
-
+// pendulum_physics (wdb_sa_physics.cuh); done = 1 at the episode end only.
 __global__ void __launch_bounds__(kCcThreads)
 pendulum_step_kernel(int n_envs, float2 *__restrict__ state, const float *__restrict__ action,
                      int *__restrict__ done, float *__restrict__ reward,
@@ -118,24 +86,9 @@ pendulum_step_kernel(int n_envs, float2 *__restrict__ state, const float *__rest
   if (env >= n_envs) return;
   const int t = env_timestep[env] + 1;
   env_timestep[env] = t;
-  constexpr double kPi = 3.141592653589793;
-  constexpr double kDt = 0.05;
-  constexpr double kGain = 3 * 9.81 / (2 * 1.0);  // 3 * g / (2 * l)
-  const double u = sa_clip_f64((double)action[env], -2.0, 2.0);
-  const float2 s = state[env];
-  const double th = (double)s.x, thdot = (double)s.y;
-  const double an = __dsub_rn(python_mod_2pi(__dadd_rn(th, kPi)), kPi);
-  const double td2 = (double)__fmul_rn(s.y, s.y);
-  const double costs = __fma_rn(__dmul_rn(u, u), 0.001, __fma_rn(an, an, __dmul_rn(td2, 0.1)));
-  double newthdot = __fma_rn(__fma_rn(u, 3.0, __dmul_rn((double)sinf(s.x), kGain)), kDt, thdot);
-  newthdot = sa_clip_f64(newthdot, -8.0, 8.0);
-  const double newth = __fma_rn(newthdot, kDt, th);
-  state[env] = make_float2((float)newth, (float)newthdot);
-  float *o = obs + (size_t)env * 3;
-  o[0] = (float)cos(newth);
-  o[1] = (float)sin(newth);
-  o[2] = (float)newthdot;
-  reward[env] = (float)(-costs);
+  const ContinuousStep r = pendulum_physics(state[env], action[env], obs + (size_t)env * 3);
+  state[env] = r.s;
+  reward[env] = r.reward;
   if (t == episode_length) done[env] = 1;
 }
 

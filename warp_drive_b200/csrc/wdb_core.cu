@@ -1,6 +1,7 @@
 // wdb_core.cu -- RNG, samplers, fused done-masked reset, episode log, testkernel.
 // Each kernel cites the reference kernel it replaces (paths under /root/reference).
 #include "wdb_common.cuh"
+#include "wdb_sa_physics.cuh"
 
 namespace wdb {
 long long g_launch_count = 0;
@@ -139,32 +140,25 @@ WDB_API int wdb_sample_actions(void *stream, void *rng_state, const float *probs
   return finish_launch();
 }
 
-// replaces sample_ou_process (numba_includes/core/random.py:74-105)
+// replaces sample_ou_process (numba_includes/core/random.py:74-105); the update itself is
+// ou_step (wdb_sa_physics.cuh), which the whole-rollout kernel calls as well
 __global__ void sample_ou_kernel(void *rng_state, const float *__restrict__ mean,
                                  float *__restrict__ actions, float *__restrict__ ou,
                                  long long n, float damping, float stddev, float scale,
                                  const float *__restrict__ normals) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  if (scale < 1.0e-8f) {  // random.py:90-93 deterministic bypass
-    actions[i] = mean[i];
-    return;
+  RngHeader h = {0ull, 0ull};
+  unsigned long long o = 0;
+  if (rng_state && !normals) {
+    h = *reinterpret_cast<const RngHeader *>(rng_state);
+    o = rng_offsets(rng_state)[i];
   }
-  float nv;
-  if (normals) {
-    nv = normals[i];
-  } else {
-    const RngHeader h = *reinterpret_cast<const RngHeader *>(rng_state);
-    unsigned long long *off = rng_offsets(rng_state);
-    const unsigned long long o = off[i];
-    const uint4 d = rng_draw4(h, (unsigned long long)i, o);
-    nv = u32x2_to_normal(d.x, d.y);
-    off[i] = o + 1;
-  }
-  nv = stddev * nv;
-  const float s = (1.0f - damping) * ou[i] + nv;
-  ou[i] = s;
-  actions[i] = mean[i] + scale * s;
+  const OuStep r = ou_step(mean[i], ou[i], normals ? normals + i : nullptr, h,
+                           (unsigned long long)i, o, damping, stddev, scale);
+  actions[i] = r.action;
+  ou[i] = r.ou;
+  if (r.draws) rng_offsets(rng_state)[i] = o + r.draws;
 }
 
 WDB_API int wdb_sample_ou_process(void *stream, void *rng_state, const float *mean,

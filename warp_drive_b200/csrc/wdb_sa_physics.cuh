@@ -1,8 +1,9 @@
-// wdb_sa_physics.cuh -- one-step physics of the discrete-action single-agent envs as
-// out-of-line device functions, shared by the stand-alone step kernels (wdb_small_envs.cu,
-// wdb_classic_control.cu) and the whole-rollout kernel (wdb_sa_rollout.cu): ONE compiled body
-// per env, so the fused path produces the same bits as the step kernels that are pinned to
-// the reference's numba binaries (tests/test_gpu_classic_control.py).
+// wdb_sa_physics.cuh -- one-step physics of the single-agent classic-control envs, and the
+// Ornstein-Uhlenbeck exploration step of their continuous actions, as out-of-line device
+// functions shared by the stand-alone kernels (wdb_small_envs.cu, wdb_classic_control.cu,
+// wdb_core.cu) and the whole-rollout kernel (wdb_sa_rollout.cu): ONE compiled body each, so
+// the fused path produces the same bits as the stand-alone kernels that are pinned to the
+// reference's numba binaries (tests/test_gpu_classic_control.py).
 #pragma once
 #include <math.h>
 
@@ -74,6 +75,120 @@ static __device__ __noinline__ float2 mountain_car_physics(float2 s, int action,
   if (pos == (double)min_position && vel < 0.0) vel = 0.0;
   *terminated = (pos >= (double)goal_position && vel >= (double)goal_velocity) ? 1 : 0;
   return make_float2((float)pos, (float)vel);
+}
+
+// new state, reward and terminal flag of one continuous-action step
+struct ContinuousStep {
+  float2 s;
+  float reward;
+  int terminated;
+};
+
+// ============================================================ ContinuousMountainCar
+// NumbaClassicControlContinuousMountainCarEnvStep, continuous_mountain_car_step_numba.py:
+// 14-71.  force = clip(action) and force * power stay float32; the rest is float64
+// (reference SASS: FMUL force*power; DFMA cos * -0.0025 + that; DADD velocity).
+// reward = (terminated ? 100 : 0) - pow(action, 2) * 0.1 in float64 (:64-69).
+static __device__ __noinline__ ContinuousStep continuous_mountain_car_physics(
+    float2 s, float a, float min_action, float max_action, float min_position,
+    float max_position, float max_speed, float goal_position, float goal_velocity,
+    float power) {
+  float f = a;
+  if (a < min_action) f = min_action;
+  else if (a > max_action) f = max_action;
+  const float fp = __fmul_rn(f, power);
+  const double pos0 = (double)s.x;
+  const double c = cos(__dmul_rn(pos0, 3.0));
+  double vel = __dadd_rn(__fma_rn(c, -0.0025, (double)fp), (double)s.y);
+  vel = sa_clip_f64(vel, (double)(-max_speed), (double)max_speed);
+  double pos = __dadd_rn(pos0, vel);
+  pos = sa_clip_f64(pos, (double)min_position, (double)max_position);
+  if (pos == (double)min_position && vel < 0.0) vel = 0.0;
+  ContinuousStep r;
+  r.s = make_float2((float)pos, (float)vel);
+  const bool terminated = pos >= (double)goal_position && vel >= (double)goal_velocity;
+  const double rew = terminated ? 100.0 : 0.0;
+  r.reward = (float)__dsub_rn(rew, __dmul_rn(pow((double)a, 2.0), 0.1));
+  r.terminated = terminated ? 1 : 0;
+  return r;
+}
+
+// ========================================================================= Pendulum
+// NumbaClassicControlPendulumEnvStep, pendulum_step_numba.py:30-72 (g = 9.81, m = l = 1,
+// dt = 0.05, max_speed = 8, max_torque = 2 are module constants there, :9-14).
+//   u = clip(action, -2, 2) in float64; angle_normalize(th) = ((th + pi) % 2pi) - pi in
+//   float64, where NVVM lowers `%` to  a - floor(|a| / b) * b  with the sign of a restored
+//   and Python's "result takes the divisor's sign" fix-up; sin(th) is the FLOAT32 routine
+//   (th is float32), cos/sin(newth) the float64 ones.  FMA placement from the reference SASS:
+//   costs = fma(u*u, 0.001, fma(an, an, 0.1 * (double)(thdot*thdot)))
+//   newthdot = fma(fma(u, 3, 14.715 * sin(th)), dt, thdot);  newth = fma(newthdot, dt, th).
+static __device__ __forceinline__ double python_mod_2pi(double a) {
+  const double b = 2.0 * 3.141592653589793;
+  const double q = floor(__ddiv_rn(fabs(a), b));
+  double r = __fma_rn(-q, b, fabs(a));
+  if (!(a >= 0.0)) r = -r;
+  if (r < 0.0) r = __dadd_rn(r, b);
+  return r;
+}
+
+// writes the 3-wide observation row `o` (global memory); never terminates
+static __device__ __noinline__ ContinuousStep pendulum_physics(float2 s, float action,
+                                                               float *o) {
+  constexpr double kPi = 3.141592653589793;
+  constexpr double kDt = 0.05;
+  constexpr double kGain = 3 * 9.81 / (2 * 1.0);  // 3 * g / (2 * l)
+  const double u = sa_clip_f64((double)action, -2.0, 2.0);
+  const double th = (double)s.x, thdot = (double)s.y;
+  const double an = __dsub_rn(python_mod_2pi(__dadd_rn(th, kPi)), kPi);
+  const double td2 = (double)__fmul_rn(s.y, s.y);
+  const double costs = __fma_rn(__dmul_rn(u, u), 0.001, __fma_rn(an, an, __dmul_rn(td2, 0.1)));
+  double newthdot = __fma_rn(__fma_rn(u, 3.0, __dmul_rn((double)sinf(s.x), kGain)), kDt, thdot);
+  newthdot = sa_clip_f64(newthdot, -8.0, 8.0);
+  const double newth = __fma_rn(newthdot, kDt, th);
+  ContinuousStep r;
+  r.s = make_float2((float)newth, (float)newthdot);
+  o[0] = (float)cos(newth);
+  o[1] = (float)sin(newth);
+  o[2] = (float)newthdot;
+  r.reward = (float)(-costs);
+  r.terminated = 0;
+  return r;
+}
+
+// ================================================================ OU exploration
+// sample_ou_process (numba_includes/core/random.py:74-105) for one action:
+//   n ~ N(0, 1): `*normal` if given (test hook), else ONE Philox draw at (stream, off);
+//   ou' = (1 - damping) * ou + stddev * n;  action = mean + scale * ou'.
+// scale < 1e-8 is the deterministic bypass: action = mean, nothing drawn, ou' = ou.
+struct OuStep {
+  float action, ou;
+  int draws;          // Philox draws consumed (0 or 1)
+};
+
+static __device__ __noinline__ OuStep ou_step(float mean, float ou, const float *normal,
+                                              RngHeader h, unsigned long long stream,
+                                              unsigned long long off, float damping,
+                                              float stddev, float scale) {
+  OuStep r;
+  r.draws = 0;
+  if (scale < 1.0e-8f) {
+    r.action = mean;
+    r.ou = ou;
+    return r;
+  }
+  float nv;
+  if (normal) {
+    nv = *normal;
+  } else {
+    const uint4 d = rng_draw4(h, stream, off);
+    nv = u32x2_to_normal(d.x, d.y);
+    r.draws = 1;
+  }
+  nv = stddev * nv;
+  const float s = (1.0f - damping) * ou + nv;
+  r.ou = s;
+  r.action = mean + scale * s;
+  return r;
 }
 
 // ========================================================================== Acrobot

@@ -1,8 +1,10 @@
-// wdb_sa_rollout.cu -- the WHOLE T-step rollout of a discrete-action single-agent env
-// (CartPole, MountainCar, Acrobot; BASELINE config 3: CartPole x 10 000 replicas) in ONE
-// launch: policy forward -> categorical sample -> env.step -> reward / done bookkeeping ->
+// wdb_sa_rollout.cu -- the WHOLE T-step rollout of a single-agent classic-control env in ONE
+// launch: policy forward -> action sample -> env.step -> reward / done bookkeeping ->
 // done-masked reset -> push to the training batch, T times; eight lanes share one env replica
 // (the forward pass is split over them, lane 0 does the serial part of the timestep).
+// Discrete kinds (CartPole, MountainCar, Acrobot; BASELINE config 3: CartPole x 10 000
+// replicas) sample a softmax head; continuous kinds (ContinuousMountainCar, Pendulum: the
+// DDPG configs) evaluate the actor's tanh head and add Ornstein-Uhlenbeck exploration noise.
 //
 // Replaces, per timestep, the reference's TrainerBase._generate_rollout_batch body
 // (warp_drive/training/trainers/trainer_base.py:383-428): FullyConnected.forward
@@ -23,10 +25,14 @@
 //
 // Per timestep and env (order = the reference's): obs -> batch[t]; probs = softmax(MLP(obs));
 // u ~ Philox stream `env`, one draw per call (identical to wdb_sample_actions); action via the
-// reference's float32 CDF + binary search; step physics = the SAME compiled device function the
+// reference's float32 CDF + binary search (continuous kinds: mean = scale * tanh(MLP(obs)) +
+// bias, then ou_step -- the stand-alone OU sampler's own update, normal from Philox stream
+// `env`); step physics = the SAME compiled device function the
 // stand-alone step kernel calls (wdb_sa_physics.cuh); rewards / done -> batch[t], episodic
 // sums; if done: every registered array <- its `_at_reset` row or a pool row, done = 0,
 // timestep = 0 (core/reset.cu:9-75, pool_reset.py:15-52).
+#include <type_traits>
+
 #include "wdb_sa_physics.cuh"
 
 using namespace wdb;
@@ -68,6 +74,10 @@ __device__ __forceinline__ int sa_search(const float *cdf, float p, int r) {
 // (16-byte weight / activation loads in the forward, 5 loads per 16 FMAs instead of 20, do
 // not help: the step is bound by lane 0's serial softmax / sample / physics chain, not by
 // the forward's load count.)
+// kContinuous: Pendulum / ContinuousMountainCar (deterministic tanh head + OU exploration,
+// float32 actions) instead of the softmax head + categorical sample; a compile-time switch,
+// so the discrete instantiation is the code it was before the continuous kinds existed.
+template <bool kContinuous>
 __global__ void __launch_bounds__(kSaThreads, 9)
 sa_rollout_kernel(const __grid_constant__ wdb_sa_rollout R) {
   extern __shared__ float s_w[];               // per layer: [Wt (in x out) | b (out)]
@@ -99,7 +109,7 @@ sa_rollout_kernel(const __grid_constant__ wdb_sa_rollout R) {
 
   RngHeader rh = {0ull, 0ull}, ph = {0ull, 0ull};
   unsigned long long rng_off = 0, pool_off = 0;
-  float run = 0.0f;
+  float run = 0.0f, ou = 0.0f;
   int steps_run = 0, tstep = 0, done_flag = 0;
   if (lead) {
     if (R.rng_state) {
@@ -114,6 +124,9 @@ sa_rollout_kernel(const __grid_constant__ wdb_sa_rollout R) {
     steps_run = R.step_running_sum ? R.step_running_sum[env] : 0;
     tstep = R.env_timestep[env];
     done_flag = R.done[env];
+    if constexpr (kContinuous) {
+      if (R.ou_state) ou = R.ou_state[env];
+    }
   }
 
   for (int t = 0; t < R.n_steps; t++) {
@@ -161,36 +174,52 @@ sa_rollout_kernel(const __grid_constant__ wdb_sa_rollout R) {
       float *tmp = cur; cur = nxt; nxt = tmp;
     }
     if (lead) {
-      // softmax over the A logits in cur[] (torch.softmax: subtract the max, exp, normalise)
-      float mx = cur[0];
-      for (int i = 1; i < A; i++) mx = fmaxf(mx, cur[i]);
-      float z = 0.0f;
-      for (int i = 0; i < A; i++) { cur[i] = expf(cur[i] - mx); z += cur[i]; }
-      for (int i = 0; i < A; i++) cur[i] = cur[i] / z;
-      if (R.probs_batch) {
-        float *pb = R.probs_batch + ((size_t)t * E + env) * A;
-        for (int i = 0; i < A; i++) pb[i] = cur[i];
-      }
-      // ---- categorical sample (core/random.cu:51-85): u in (0, 1], float32 CDF, binary search
-      float u;
-      if (R.uniforms) {
-        u = R.uniforms[(size_t)t * E + env];
+      std::conditional_t<kContinuous, float, int> action;
+      if constexpr (kContinuous) {
+        // deterministic head (FullyConnectedActor._policy_outputs): scale * tanh(z) + bias,
+        // a separate multiply and add as torch evaluates it
+        const float mean = __fadd_rn(__fmul_rn(R.action_scale, tanhf(cur[0])), R.action_bias);
+        if (R.probs_batch) R.probs_batch[(size_t)t * E + env] = mean;
+        // ---- OU exploration (sample_ou_process): the stand-alone sampler's own update
+        const OuStep o = ou_step(mean, ou, R.normals ? R.normals + (size_t)t * E + env : nullptr,
+                                 rh, (unsigned long long)env, rng_off, R.ou_damping,
+                                 R.ou_stddev, R.ou_scale);
+        ou = o.ou;
+        rng_off += o.draws;
+        action = o.action;
+        static_cast<float *>(R.sampled_actions)[env] = action;
+        if (R.actions_batch) static_cast<float *>(R.actions_batch)[(size_t)t * E + env] = action;
       } else {
-        u = u32_to_uniform(rng_draw4(rh, (unsigned long long)env, rng_off).x);
-        rng_off++;
+        // softmax over the A logits in cur[] (torch.softmax: subtract the max, exp, normalise)
+        float mx = cur[0];
+        for (int i = 1; i < A; i++) mx = fmaxf(mx, cur[i]);
+        float z = 0.0f;
+        for (int i = 0; i < A; i++) { cur[i] = expf(cur[i] - mx); z += cur[i]; }
+        for (int i = 0; i < A; i++) cur[i] = cur[i] / z;
+        if (R.probs_batch) {
+          float *pb = R.probs_batch + ((size_t)t * E + env) * A;
+          for (int i = 0; i < A; i++) pb[i] = cur[i];
+        }
+        // ---- categorical sample (core/random.cu:51-85): u in (0, 1], float32 CDF, binary search
+        float u;
+        if (R.uniforms) {
+          u = R.uniforms[(size_t)t * E + env];
+        } else {
+          u = u32_to_uniform(rng_draw4(rh, (unsigned long long)env, rng_off).x);
+          rng_off++;
+        }
+        if (R.use_argmax) {
+          action = 0;
+          float best = cur[0];
+          for (int i = 1; i < A; i++) if (best < cur[i]) { best = cur[i]; action = i; }
+        } else {
+          float c = cur[0];
+          for (int i = 1; i < A; i++) { c = cur[i] + c; cur[i] = c; }
+          action = sa_search(cur, u, A - 1);
+        }
+        static_cast<int *>(R.sampled_actions)[env] = action;
+        if (R.actions_batch) static_cast<int *>(R.actions_batch)[(size_t)t * E + env] = action;
       }
-      int action;
-      if (R.use_argmax) {
-        action = 0;
-        float best = cur[0];
-        for (int i = 1; i < A; i++) if (best < cur[i]) { best = cur[i]; action = i; }
-      } else {
-        float c = cur[0];
-        for (int i = 1; i < A; i++) { c = cur[i] + c; cur[i] = c; }
-        action = sa_search(cur, u, A - 1);
-      }
-      R.sampled_actions[env] = action;
-      if (R.actions_batch) R.actions_batch[(size_t)t * E + env] = action;
 
       // ---- env step: the stand-alone step kernels' own physics functions
       tstep += 1;
@@ -198,30 +227,46 @@ sa_rollout_kernel(const __grid_constant__ wdb_sa_rollout R) {
       int terminated = 0, done_code = 0;
       float *st = R.state + (size_t)env * S;
       float *ow = R.observations + (size_t)env * F;
-      if (R.env_kind == WDB_SA_CARTPOLE) {
-        const float *p = R.env_params;      // gravity, masspole, total_mass, length,
-        const float4 n = cartpole_physics(*reinterpret_cast<const float4 *>(st), action, p[0],
-                                          p[1], p[2], p[3], p[4], p[5], p[6]);
-        *reinterpret_cast<float4 *>(st) = n;     // polemass_length, force_mag, tau,
-        *reinterpret_cast<float4 *>(ow) = n;     // theta_threshold_radians, x_threshold
-        terminated = cartpole_terminated(n, p[7], p[8]) ? 1 : 0;
-        reward = 1.0f;
-        done_code = (tstep == R.episode_length || terminated) ? 1 : 0;
-      } else if (R.env_kind == WDB_SA_MOUNTAIN_CAR) {
-        const float *p = R.env_params;      // min_position, max_position, max_speed,
-        const float2 n = mountain_car_physics(*reinterpret_cast<const float2 *>(st), action, p[0],
-                                              p[1], p[2], p[3], p[4], p[5], p[6], &terminated);
-        *reinterpret_cast<float2 *>(st) = n;     // goal_position, goal_velocity, force, gravity
-        *reinterpret_cast<float2 *>(ow) = n;
-        reward = -1.0f;
-        done_code = (tstep == R.episode_length) ? 1 : (terminated ? 2 : 0);   // :66-70
-      } else {                              // WDB_SA_ACROBOT
-        float o6[6];
-        *reinterpret_cast<float4 *>(st) = acrobot_physics(*reinterpret_cast<const float4 *>(st),
-                                                          action, o6, &reward, &terminated);
+      if constexpr (kContinuous) {
+        ContinuousStep c;
+        if (R.env_kind == WDB_SA_CONTINUOUS_MOUNTAIN_CAR) {
+          const float *p = R.env_params;    // min_action, max_action, min_position, max_position,
+          c = continuous_mountain_car_physics(  // max_speed, goal_position, goal_velocity, power
+              *reinterpret_cast<const float2 *>(st), action, p[0], p[1], p[2], p[3], p[4], p[5],
+              p[6], p[7]);
+          *reinterpret_cast<float2 *>(ow) = c.s;
+        } else {                            // WDB_SA_PENDULUM
+          c = pendulum_physics(*reinterpret_cast<const float2 *>(st), action, ow);
+        }
+        *reinterpret_cast<float2 *>(st) = c.s;
+        reward = c.reward;
+        done_code = (tstep == R.episode_length || c.terminated) ? 1 : 0;
+      } else {
+        if (R.env_kind == WDB_SA_CARTPOLE) {
+          const float *p = R.env_params;      // gravity, masspole, total_mass, length,
+          const float4 n = cartpole_physics(*reinterpret_cast<const float4 *>(st), action, p[0],
+                                            p[1], p[2], p[3], p[4], p[5], p[6]);
+          *reinterpret_cast<float4 *>(st) = n;     // polemass_length, force_mag, tau,
+          *reinterpret_cast<float4 *>(ow) = n;     // theta_threshold_radians, x_threshold
+          terminated = cartpole_terminated(n, p[7], p[8]) ? 1 : 0;
+          reward = 1.0f;
+          done_code = (tstep == R.episode_length || terminated) ? 1 : 0;
+        } else if (R.env_kind == WDB_SA_MOUNTAIN_CAR) {
+          const float *p = R.env_params;      // min_position, max_position, max_speed,
+          const float2 n = mountain_car_physics(*reinterpret_cast<const float2 *>(st), action, p[0],
+                                                p[1], p[2], p[3], p[4], p[5], p[6], &terminated);
+          *reinterpret_cast<float2 *>(st) = n;     // goal_position, goal_velocity, force, gravity
+          *reinterpret_cast<float2 *>(ow) = n;
+          reward = -1.0f;
+          done_code = (tstep == R.episode_length) ? 1 : (terminated ? 2 : 0);   // :66-70
+        } else {                              // WDB_SA_ACROBOT
+          float o6[6];
+          *reinterpret_cast<float4 *>(st) = acrobot_physics(*reinterpret_cast<const float4 *>(st),
+                                                            action, o6, &reward, &terminated);
 #pragma unroll
-        for (int i = 0; i < 6; i++) ow[i] = o6[i];
-        done_code = (tstep == R.episode_length || terminated) ? 1 : 0;
+          for (int i = 0; i < 6; i++) ow[i] = o6[i];
+          done_code = (tstep == R.episode_length || terminated) ? 1 : 0;
+        }
       }
       R.rewards[env] = reward;
       // the reference's done flag is sticky until a reset clears it
@@ -273,7 +318,12 @@ sa_rollout_kernel(const __grid_constant__ wdb_sa_rollout R) {
   if (lead) {
     R.env_timestep[env] = tstep;
     R.done[env] = done_flag;
-    if (R.rng_state && !R.uniforms) rng_offsets(R.rng_state)[env] = rng_off;
+    if constexpr (kContinuous) {
+      if (R.rng_state && !R.normals) rng_offsets(R.rng_state)[env] = rng_off;
+      if (R.ou_state) R.ou_state[env] = ou;
+    } else {
+      if (R.rng_state && !R.uniforms) rng_offsets(R.rng_state)[env] = rng_off;
+    }
     if (R.pool_rng) rng_offsets(R.pool_rng)[env] = pool_off;
     if (R.reward_running_sum) R.reward_running_sum[env] = run;
     if (R.step_running_sum) R.step_running_sum[env] = steps_run;
@@ -291,22 +341,52 @@ WDB_API int wdb_single_agent_rollout_supported(int n_hidden, const int *dims) {
   return total <= kSaMaxWeights ? 1 : 0;
 }
 
+namespace {
+// state / observation widths per kind: CartPole, MountainCar, Acrobot, ContinuousMountainCar,
+// Pendulum
+constexpr int kSaStateDim[] = {4, 2, 4, 2, 2};
+constexpr int kSaObsDim[] = {4, 2, 6, 2, 3};
+
+template <bool kContinuous>
+int sa_launch(void *stream, const wdb_sa_rollout *r, size_t smem) {
+  static size_t configured = 0;
+  if (smem > 48 * 1024 && smem > configured) {
+    cudaError_t e = cudaFuncSetAttribute(sa_rollout_kernel<kContinuous>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return (int)e;
+    configured = smem;
+  }
+  const int grid = (r->n_envs + kSaEnvsPerCta - 1) / kSaEnvsPerCta;
+  sa_rollout_kernel<kContinuous><<<grid, kSaThreads, smem, as_stream(stream)>>>(*r);
+  return finish_launch();
+}
+}  // namespace
+
 WDB_API int wdb_single_agent_rollout(void *stream, const wdb_sa_rollout *r) {
   if (!r) return (int)cudaErrorInvalidValue;
-  if (r->env_kind < WDB_SA_CARTPOLE || r->env_kind > WDB_SA_ACROBOT) return (int)cudaErrorInvalidValue;
+  if (r->env_kind < WDB_SA_CARTPOLE || r->env_kind > WDB_SA_PENDULUM) return (int)cudaErrorInvalidValue;
+  const bool continuous = r->env_kind >= WDB_SA_CONTINUOUS_MOUNTAIN_CAR;
   if (r->n_envs <= 0 || r->n_steps <= 0 || !r->state || !r->observations || !r->done ||
       !r->env_timestep || !r->rewards || !r->sampled_actions)
     return (int)cudaErrorInvalidValue;
   if (!wdb_single_agent_rollout_supported(r->n_hidden, r->dims)) return (int)cudaErrorInvalidValue;
   for (int l = 0; l <= r->n_hidden; l++)
     if (!r->w[l] || !r->b[l]) return (int)cudaErrorInvalidValue;
-  if (!r->use_argmax && !r->uniforms && !r->rng_state) return (int)cudaErrorInvalidValue;
-  const int want_state = r->env_kind == WDB_SA_MOUNTAIN_CAR ? 2 : 4;
-  const int want_obs = r->env_kind == WDB_SA_ACROBOT ? 6 : want_state;
+  if (continuous) {
+    // one tanh action; the OU state and a normal source unless the bypass (scale < 1e-8)
+    // draws nothing
+    if (r->dims[r->n_hidden + 1] != 1) return (int)cudaErrorInvalidValue;
+    if (!(r->ou_scale < 1.0e-8f) && (!r->ou_state || (!r->normals && !r->rng_state)))
+      return (int)cudaErrorInvalidValue;
+  } else if (!r->use_argmax && !r->uniforms && !r->rng_state) {
+    return (int)cudaErrorInvalidValue;
+  }
+  const int want_state = kSaStateDim[r->env_kind], want_obs = kSaObsDim[r->env_kind];
   if (r->state_dim != want_state || r->dims[0] != want_obs) return (int)cudaErrorInvalidValue;
   const uintptr_t mask = want_state == 2 ? 7 : 15;
   if ((uintptr_t)r->state & mask) return (int)cudaErrorMisalignedAddress;
-  if (r->env_kind != WDB_SA_ACROBOT && ((uintptr_t)r->observations & mask))
+  // Acrobot (6) and Pendulum (3) write their observation rows element by element
+  if (want_obs == want_state && ((uintptr_t)r->observations & mask))
     return (int)cudaErrorMisalignedAddress;
   if (r->reset_done_envs && r->n_reset_arrays > 0 && !r->reset_table)
     return (int)cudaErrorInvalidValue;
@@ -314,14 +394,5 @@ WDB_API int wdb_single_agent_rollout(void *stream, const wdb_sa_rollout *r) {
   for (int l = 0; l <= r->n_hidden; l++)
     total += (long long)r->dims[l] * r->dims[l + 1] + r->dims[l + 1];
   const size_t smem = ((size_t)total + (size_t)kSaEnvsPerCta * 2 * kSaPitch) * sizeof(float);
-  static size_t configured = 0;
-  if (smem > 48 * 1024 && smem > configured) {
-    cudaError_t e = cudaFuncSetAttribute(sa_rollout_kernel,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return (int)e;
-    configured = smem;
-  }
-  const int grid = (r->n_envs + kSaEnvsPerCta - 1) / kSaEnvsPerCta;
-  sa_rollout_kernel<<<grid, kSaThreads, smem, as_stream(stream)>>>(*r);
-  return finish_launch();
+  return continuous ? sa_launch<true>(stream, r, smem) : sa_launch<false>(stream, r, smem);
 }

@@ -135,6 +135,8 @@ class SaRollout(ctypes.Structure):
         ("episodic_step_sum", _fp), ("num_completed", _fp),
         ("reset_table", _fp), ("n_reset_arrays", _i), ("pool_rng", _fp),
         ("reset_done_envs", _i),
+        ("ou_damping", _f), ("ou_stddev", _f), ("ou_scale", _f), ("ou_state", _fp),
+        ("action_scale", _f), ("action_bias", _f), ("normals", _fp),
     ]
 
 

@@ -1,10 +1,12 @@
-"""The whole T-step rollout of a discrete-action single-agent env in ONE launch
+"""The whole T-step rollout of a single-agent classic-control env in ONE launch
 (`wdb_single_agent_rollout`, csrc/wdb_sa_rollout.cu): forward -> sample -> step ->
 bookkeeping -> done-masked reset -> push to batch, one thread per env replica.
 
 H100 re-design of TrainerBase._generate_rollout_batch (warp_drive/training/trainers/
 trainer_base.py:383-428) for ClassicControl{CartPole,MountainCar,Acrobot}Env with a small
-FullyConnected policy (BASELINE config 3): the reference issues ~50 launches and >= 5 host
+FullyConnected policy (BASELINE config 3), and of the DDPG rollout of
+ClassicControl{ContinuousMountainCar,Pendulum}Env with a small FullyConnectedActor (tanh head
++ Ornstein-Uhlenbeck exploration noise): the reference issues ~50 launches and >= 5 host
 synchronisations per timestep, this path one launch per T timesteps and no synchronisation.
 """
 import ctypes
@@ -28,17 +30,29 @@ _ENVS = {
     "ClassicControlMountainCarEnv": (1, ("min_position", "max_position", "max_speed",
                                          "goal_position", "goal_velocity", "force", "gravity"), 2),
     "ClassicControlAcrobotEnv": (2, (), 4),
+    "ClassicControlContinuousMountainCarEnv": (3, ("min_action", "max_action", "min_position",
+                                                   "max_position", "max_speed", "goal_position",
+                                                   "goal_velocity", "power"), 2),
+    "ClassicControlPendulumEnv": (4, (), 2),
 }
+_CONTINUOUS_KINDS = (3, 4)
 
 
 def _p(t):
     return _lib.ptr(t)
 
 
+def _unwrap(model):
+    """The FullyConnected / FullyConnectedActor behind the rollout engine's ActorAsPolicy."""
+    return getattr(model, "actor", model)
+
+
 def _layers(model):
     """[(weight, bias)] of the hidden layers followed by the (single) action head."""
+    model = _unwrap(model)
     out = [(model.fc[str(i)][0].weight, model.fc[str(i)][0].bias) for i in range(len(model.fc))]
-    head = model.policy_head[0]
+    # the discrete heads are an nn.ModuleList, the deterministic (tanh) head one nn.Linear
+    head = model.policy_head if model.is_deterministic else model.policy_head[0]
     out.append((head.weight, head.bias))
     return out
 
@@ -51,9 +65,13 @@ class FusedSingleAgentRollout:
             return False
         if len(policy_map) != 1 or len(models) != 1:
             return False
-        model = next(iter(models.values()))
+        model = _unwrap(next(iter(models.values())))
+        continuous = _ENVS[env.name][0] in _CONTINUOUS_KINDS
         try:
-            if getattr(model, "is_deterministic", True) or len(model.output_dims) != 1:
+            # discrete kinds: one softmax head; continuous kinds: one tanh head of width 1
+            if getattr(model, "is_deterministic", not continuous) != continuous:
+                return False
+            if len(model.output_dims) != 1 or (continuous and model.output_dims[0] != 1):
                 return False
             if getattr(model, "action_mask", None) is not None:
                 return False
@@ -88,7 +106,7 @@ class FusedSingleAgentRollout:
         r.sampled_actions = _p(dm.device_data(_ACTIONS))
         layers = _layers(model)
         r.n_hidden = len(layers) - 1
-        dims = [int(model.flattened_obs_size)] + [int(w.shape[0]) for w, _ in layers]
+        dims = [int(_unwrap(model).flattened_obs_size)] + [int(w.shape[0]) for w, _ in layers]
         for i, d in enumerate(dims):
             r.dims[i] = d
         self.F, self.A = dims[0], dims[-1]
@@ -98,6 +116,12 @@ class FusedSingleAgentRollout:
             r.w[i], r.b[i] = _p(w.data), _p(b.data)
         r.rng_state = _p(sampler.rng_state)
         r.reset_done_envs = 1
+        self.continuous = kind in _CONTINUOUS_KINDS
+        if self.continuous:
+            actor = _unwrap(model)
+            r.action_scale = float(actor.action_scale)
+            r.action_bias = float(actor.action_bias)
+            r.ou_state = _p(dm.device_data(f"{_ACTIONS}_ou_state"))
         self._table = None
 
     def set_bookkeeping(self, reward_running_sum, episodic_reward_sum, step_running_sum,
@@ -120,9 +144,14 @@ class FusedSingleAgentRollout:
         return table, n, resetter._pool_rng
 
     def launch(self, n_steps, t0=0, record=True, uniforms=None, probs_out=None,
-               use_argmax=False, reset_done_envs=True):
+               use_argmax=False, reset_done_envs=True, damping=None, stddev=None, scale=None,
+               normals=None):
         """Run `n_steps` timesteps.  record=True pushes them into batch slots t0 .. t0+n_steps-1
-        of the policy's training batch."""
+        of the policy's training batch.  Discrete kinds sample the softmax head (`uniforms`
+        [n_steps, E] replaces the RNG draw, `probs_out` [n_steps, E, A] records the
+        probabilities); continuous kinds add OU noise to the actor's mean with the parameters
+        of CUDASampler.sample (`normals` [n_steps, E] replaces the RNG draw, `probs_out`
+        [n_steps, E] records the mean)."""
         dm, r, p = self.dm, self.r, self.policy
         # parameters may have been re-allocated (load_state_dict keeps storage; .to() does not)
         for i, (w, b) in enumerate(self._params):
@@ -131,6 +160,10 @@ class FusedSingleAgentRollout:
         r.use_argmax = int(bool(use_argmax))
         r.uniforms = _p(uniforms)
         r.probs_batch = _p(probs_out)
+        r.ou_damping = float(0.15 if damping is None else damping)
+        r.ou_stddev = float(0.2 if stddev is None else stddev)
+        r.ou_scale = float(1.0 if scale is None else scale)
+        r.normals = _p(normals)
         if record:
             obs_b = dm.data_on_device_via_torch(f"{_PROCESSED_OBSERVATIONS}_batch_{p}")
             assert t0 + n_steps <= obs_b.shape[0]

@@ -80,12 +80,13 @@ class RolloutEngine:
             self.cur_obs = {p: obs.index_select(1, self.ids[p]).contiguous()
                             for p in self.policies}
 
-        # ---- whole-rollout single launch (discrete single-agent envs, small FullyConnected)
+        # ---- whole-rollout single launch (single-agent classic control, small FullyConnected
+        #      policy or actor)
         self.sa = None
         if use_fused_step and self.fused is None:
             from warp_drive_b200.training.fused_single_agent import FusedSingleAgentRollout
 
-            if (self.T >= 1 and not self.continuous
+            if (self.T >= 1
                     and FusedSingleAgentRollout.eligible(env_wrapper, models, self.policy_map)):
                 p0 = self.policies[0]
                 self.sa = FusedSingleAgentRollout(env_wrapper, models[p0], p0, sampler)
@@ -451,9 +452,11 @@ class RolloutEngine:
         for t in range(self.T):
             self.step(t, **sample_params)
 
-    @staticmethod
-    def _sa_params_ok(sample_params):
-        return all(k == "use_argmax" for k in sample_params)
+    def _sa_params_ok(self, sample_params):
+        """The whole-rollout kernel takes the categorical sampler's argmax switch, or the OU
+        parameters of a continuous action (the other sampler arguments are test hooks)."""
+        allowed = ("damping", "stddev", "scale") if self.continuous else ("use_argmax",)
+        return all(k in allowed for k in sample_params)
 
     def rollout(self, **sample_params):
         """Generate one training batch (T timesteps for every env replica)."""

@@ -8,9 +8,11 @@ for the OU noise), same `{policy}_actor_{t}.state_dict` / `{policy}_critic_{t}.s
 checkpoints, same losses (algorithms/ddpg.py).
 
 Underneath:
-  * the rollout is the device-resident generic step of RolloutEngine: actor forward ->
-    wdb_sample_ou_process (Ornstein-Uhlenbeck exploration noise, state on the device) ->
-    env step kernel -> bookkeeping -> done-masked reset (incl. reset pools), no host sync;
+  * the rollout is ONE launch of the whole-rollout kernel (wdb_single_agent_rollout: actor
+    forward -> Ornstein-Uhlenbeck exploration noise -> env step -> bookkeeping -> done-masked
+    reset, incl. reset pools) for actors it supports (<= 3 hidden layers of width <= 64), else
+    the device-resident generic step of RolloutEngine: actor forward ->
+    wdb_sample_ou_process -> env step kernel -> bookkeeping -> reset; no host sync either way;
   * the replay window is the batch arrays themselves used as ONE ring (capacity
     `train_batch_size_per_env + n_step - 1`, trainer_base.py:246) with a single shared
     cursor -- every array is written in lock step, so the per-array queue objects of the
@@ -65,15 +67,26 @@ class RingRolloutEngine(RolloutEngine):
     (cursor + t) mod capacity of every `*_batch*` array."""
 
     def __init__(self, *args, ring_capacity=None, **kwargs):
-        kwargs.update(use_cuda_graph=False, use_fused_step=False)
+        kwargs.update(use_cuda_graph=False)
         super().__init__(*args, **kwargs)
         assert ring_capacity is not None and ring_capacity >= self.T
         self.ring_capacity = int(ring_capacity)
         self.ring_cursor = 0          # slot of the next timestep
         self.ring_filled = 0          # valid slots (<= capacity)
 
+    def _fused_eligible(self):
+        # the tag_continuous per-step kernel writes batch slot t itself (no ring mapping)
+        return False
+
     def _slot(self, t):
         return t if t < 0 else (self.ring_cursor + t) % self.ring_capacity
+
+    def step(self, t, **sample_params):
+        if self.sa is not None and t >= 0 and self._sa_params_ok(sample_params):
+            with torch.no_grad():
+                self.sa.launch(1, t0=self._slot(t), **sample_params)
+            return None
+        return super().step(t, **sample_params)
 
     def evaluate_policies(self, t):
         return super().evaluate_policies(self._slot(t))
@@ -85,7 +98,16 @@ class RingRolloutEngine(RolloutEngine):
         return super().bookkeep(self._slot(t))
 
     def rollout(self, **sample_params):
-        self._rollout_eager(**sample_params)
+        if self.sa is not None and self._sa_params_ok(sample_params):
+            # slots cursor .. cursor + T - 1 (mod capacity): at most two launches, split at
+            # the wrap point
+            with torch.no_grad():
+                first = min(self.T, self.ring_capacity - self.ring_cursor)
+                self.sa.launch(first, t0=self.ring_cursor, **sample_params)
+                if first < self.T:
+                    self.sa.launch(self.T - first, t0=0, **sample_params)
+        else:
+            self._rollout_eager(**sample_params)
         self.ring_cursor = (self.ring_cursor + self.T) % self.ring_capacity
         self.ring_filled = min(self.ring_capacity, self.ring_filled + self.T)
 
