@@ -228,6 +228,15 @@ typedef struct wdb_tc_rollout {
 int wdb_tag_continuous_rollout_step(void *stream, const wdb_tc_env *env,
                                     const wdb_tc_rollout *rollout);
 
+/* Whether wdb_tag_continuous_rollout_step can run this env and rollout shape: 0, or the code
+ * it would return once every pointer of `rollout` is valid, with obs_next written for every
+ * policy and obs_next_tiles for every policy iff with_obs_tiles.  Only the shape fields of
+ * `rollout` are read (n_policies, n_actions0/1, policy[].n_agents, the reset fields); `env`
+ * is read as the step reads it.  No pointer is dereferenced and no CUDA call is made.  The
+ * verdict depends on the wdb_set_option switches at the time of the call. */
+int wdb_tag_continuous_rollout_supported(const wdb_tc_env *env, const wdb_tc_rollout *rollout,
+                                         int with_obs_tiles);
+
 /* Replaces NumbaClassicControlCartPoleEnvStep (example_envs/single_agent/
  * classic_control/cartpole/cartpole_step_numba.py:6-83; argument order of
  * cartpole.py:105-122). */

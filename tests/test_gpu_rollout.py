@@ -19,13 +19,13 @@ ENV_KW = dict(num_taggers=3, num_runners=20, grid_length=10.0, episode_length=40
 _BPE = 1     # blocks_per_env of the wrappers built here (tests/test_gpu_wide.py re-runs with 2)
 
 
-def _setup(E, T, full_obs=False, seed=11):
+def _setup(E, T, full_obs=False, seed=11, **env_kw):
     from warp_drive_b200.env_wrapper import EnvWrapper
     from warp_drive_b200.envs.tag_continuous import TagContinuous
     from warp_drive_b200.managers.function_manager import CUDASampler
     from warp_drive_b200.training.utils.data_loader import create_and_push_data_placeholders
 
-    kw = dict(ENV_KW, use_full_observation=full_obs)
+    kw = dict(ENV_KW, use_full_observation=full_obs, **env_kw)
     env = TagContinuous(**kw)
     wrapper = EnvWrapper(env, num_envs=E, env_backend="b200", blocks_per_env=_BPE)
     wrapper.reset_all_envs()
@@ -143,11 +143,11 @@ def test_fused_step_without_reset_keeps_done_set():
                        dm.data_on_device_via_torch("loc_x_at_reset"))
 
 
-def _engine(E, T, use_graph, fused, seed=3, **engine_kw):
+def _engine(E, T, use_graph, fused, seed=3, env_kw=None, **engine_kw):
     from warp_drive_b200.training.models.fully_connected import FullyConnected
     from warp_drive_b200.training.rollout import RolloutEngine
 
-    w, s, pm = _setup(E, T, seed=seed)
+    w, s, pm = _setup(E, T, seed=seed, **(env_kw or {}))
     torch.manual_seed(0)
     cfg = {"type": "fully_connected", "fc_dims": [32, 32], "model_ckpt_filepath": ""}
     models = {p: FullyConnected(w, cfg, p, pm).cuda().eval() for p in pm}
@@ -249,6 +249,26 @@ def test_engine_fused_matches_unfused_batches():
     assert float(e.episodic_step_sum) / float(e.num_completed_episodes) <= 40
 
 
+def test_engine_takes_the_generic_path_where_the_fused_step_has_no_plan():
+    """23 agents observing K = 11 neighbours, 16 envs: the packed kernel cannot stage the
+    observation tile the fused step pushes from, and the library refuses the fused step for
+    that shape.  The engine asks the library, so it builds the generic multi-launch timestep
+    instead, and its rollouts fill the batch from the env arrays."""
+    E, T = 16, 8
+    w, e, pm = _engine(E, T, True, True, env_kw=dict(num_other_agents_observed=11))
+    assert e.fused is None
+    dm = w.cuda_data_manager
+    for _ in range(3):
+        e.rollout()
+    torch.cuda.synchronize()
+    for p, ids in pm.items():
+        i = torch.as_tensor(ids, device="cuda")
+        assert torch.equal(dm.data_on_device_via_torch(f"sampled_actions_batch_{p}")[T - 1],
+                           dm.data_on_device_via_torch("sampled_actions")[:, i])
+        assert torch.equal(dm.data_on_device_via_torch(f"rewards_batch_{p}")[T - 1],
+                           dm.data_on_device_via_torch("rewards")[:, i])
+
+
 def test_step_with_host_buffers_matches_pull():
     """EnvWrapper.step_with_host_buffers (pinned host actions in; observations / rewards /
     done out over several copy streams) returns exactly what step_all_envs followed by
@@ -338,7 +358,7 @@ def test_config4_agent_count_through_wrapper_and_engine():
     torch.manual_seed(0)
     cfg = {"type": "fully_connected", "fc_dims": [32, 32], "model_ckpt_filepath": ""}
     models = {p: FullyConnected(w, cfg, p, pm).cuda().eval() for p in pm}
-    eng = RolloutEngine(w, models, pm, s, T, use_cuda_graph=False, use_fused_step=False)
+    eng = RolloutEngine(w, models, pm, s, T, use_cuda_graph=False)
     assert eng.fused is None
     try:
         for _ in range(3):

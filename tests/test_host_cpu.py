@@ -9,6 +9,7 @@ import subprocess
 
 import numpy as np
 import pytest
+import torch
 
 from conftest import ROOT, load_golden
 from helpers import close
@@ -113,6 +114,106 @@ def test_single_agent_steps_refuse_bad_arrays_before_a_launch(wdb_lib, fn, n_sca
         assert call(state=base + off) == 716, off
         if obs_dim == state_dim:
             assert call(obs=base + 0x4000 + off) == 716, off
+
+
+def _tc_request(lib_mod, N, K, full=0, bpe=1, scratch=False, E=2000, sizes=None, heads=21,
+                tiles=False):
+    """A TagContinuous rollout request with distinct, aligned dummy pointers (never
+    dereferenced), obs_next written for every policy, and its shape-only twin."""
+    base, count = 1 << 24, iter(range(1, 1000))
+
+    def p():
+        return base + 0x100000 * next(count)
+
+    env = lib_mod.TcEnv()
+    env.n_envs, env.n_agents, env.num_other_agents_observed = E, N, K
+    for name in ("loc_x", "loc_y", "speed", "direction", "acceleration", "agent_types",
+                 "edge_hit_reward_penalty", "acceleration_actions", "turn_actions",
+                 "skill_levels", "still_in_the_game", "nearest_neighbor_ids", "step_rewards",
+                 "num_runners", "obs", "rewards", "done", "env_timestep", "stats"):
+        setattr(env, name, p())
+    if scratch:
+        env.neighbor_distances, env.neighbor_ids_sorted_by_distance = p(), p()
+    env.use_full_observation, env.blocks_per_env, env.episode_length = full, bpe, 100
+    sizes = sizes or [N]
+    ro, shape = lib_mod.TcRollout(), lib_mod.TcRollout()
+    for r in (ro, shape):
+        r.n_policies, r.n_actions0, r.n_actions1 = len(sizes), heads, heads
+        for k, n in enumerate(sizes):
+            r.policy[k].n_agents = n
+    ro.rng_state, ro.agent_policy, ro.agent_slot, ro.sampled_actions = p(), p(), p(), p()
+    for k in range(len(sizes)):
+        io = ro.policy[k]
+        io.probs0, io.probs1, io.actions_batch, io.rewards_batch = p(), p(), p(), p()
+        io.obs_next = p()
+        io.obs_next_tiles = p() if tiles else None
+    return env, ro, shape
+
+
+def _tc_supported(lib, env, shape, tiles):
+    return lib.wdb_tag_continuous_rollout_supported(ctypes.byref(env), ctypes.byref(shape),
+                                                    int(tiles))
+
+
+@pytest.mark.skipif(
+    torch.cuda.is_available(),
+    reason="calls the rollout step with dummy pointers: only where no CUDA device can run it")
+def test_tag_continuous_support_query_agrees_with_the_rollout_step(wdb_lib):
+    """wdb_tag_continuous_rollout_supported runs the rollout step's checks and launch plan:
+    wherever it refuses, the step refuses with the same code; wherever it accepts, the step
+    gets past every check and reaches the CUDA runtime, which without a GPU returns 35
+    (cudaErrorInsufficientDriver).  Every agent count up to 320 and around the large-env
+    paths, every K <= min(N - 1, 16), both observation modes, one or several CTAs per env and
+    obs tiles on / off are covered; the scratch, env count, policy split and head width
+    rotate through their combinations.  Repeated under the options that change the route."""
+    from warp_drive_b200 import lib as wlib
+
+    Ns = list(range(2, 321)) + [321, 400, 1024, 1025, 2000]
+    variants = [(None, None, None), (b"tc_variant", 2, 1), (b"tc_wide_single", 0, 1),
+                (b"tc_cta_threads", 128, 320)]
+    checked = accepted = 0
+    for opt, value, default in variants:
+        if opt:
+            assert wdb_lib.wdb_set_option(opt, value) == 0
+        try:
+            for N in Ns:
+                for K in range(min(N - 1, 16) + 1):
+                    for full in (0, 1):
+                        for bpe in (1, 2, 4, 9):
+                            for tiles in (False, True):
+                                c = checked
+                                env, ro, shape = _tc_request(
+                                    wlib, N, K, full, bpe, scratch=bool(c & 1),
+                                    E=(1, 2000)[(c >> 1) & 1],
+                                    sizes=[N] if (c >> 2) & 1 else [max(1, N // 4), N - max(1, N // 4)],
+                                    heads=(21, 33)[(c >> 3) & 1], tiles=tiles)
+                                q = _tc_supported(wdb_lib, env, shape, tiles)
+                                rc = wdb_lib.wdb_tag_continuous_rollout_step(
+                                    None, ctypes.byref(env), ctypes.byref(ro))
+                                assert rc == (q if q else 35), (opt, N, K, full, bpe, c, q, rc)
+                                checked += 1
+                                accepted += q == 0
+        finally:
+            if opt:
+                wdb_lib.wdb_set_option(opt, default)
+    assert 0 < accepted < checked
+
+
+def test_tag_continuous_support_query_anchors(wdb_lib):
+    """Shapes the fused rollout step takes or refuses, answered without a CUDA call."""
+    from warp_drive_b200 import lib as wlib
+
+    def supported(N, K, tiles=False, **kw):
+        env, _, shape = _tc_request(wlib, N, K, tiles=tiles, **kw)
+        return _tc_supported(wdb_lib, env, shape, tiles)
+
+    assert supported(105, 10, sizes=[100, 5]) == 0            # config 2: 100 runners, 5 taggers
+    assert supported(23, 11) == 1        # the packed kernel's staged tile does not fit
+    assert supported(23, 10) == 0
+    assert supported(1024, 10, bpe=4, E=3, sizes=[24, 1000]) == 0     # config 4 on clusters
+    assert supported(400, 10) == 0                            # one large env per CTA ...
+    assert supported(400, 10, tiles=True) == 1                # ... writes no obs tiles
+    assert supported(105, 10, sizes=[100, 5], tiles=True) == 0
 
 
 def test_product_never_imports_the_oracle():

@@ -91,7 +91,7 @@ tag_continuous_kernel(const __grid_constant__ TcParams P, const __grid_constant_
   const int lane = tid & 31, warp = tid >> 5;
   const int le = tid / N;
   const int a = tid - le * N;
-  // CTAs past full_ctas carry ONE env each (see plan_launch: the last, partly filled wave)
+  // CTAs past full_ctas carry ONE env each (see plan_packed: the last, partly filled wave)
   const bool tail_cta = (int)blockIdx.x >= P.full_ctas;
   const int env0 = tail_cta ? P.full_ctas * epb + ((int)blockIdx.x - P.full_ctas)
                             : (int)blockIdx.x * epb;
@@ -1004,14 +1004,10 @@ int g_tc_threads = 320; // wdb_set_option("tc_cta_threads", n): thread budget of
 
 int g_tc_tail_split = 0;   // wdb_set_option("tc_tail_split", 0/1/2), off by default
 
-struct LaunchPlan {
-  int epb, block, grid;
-  size_t smem;
-};
-
-// shared-memory carve-up; must mirror the kernel prologue
-int plan_launch(TcParams &P, const FusedParams *Q, bool have_gscratch, LaunchPlan &plan) {
+// The packed kernel's geometry; shared-memory carve-up, must mirror the kernel prologue
+int plan_packed(TcParams &P, const FusedParams *Q, TcPlan &plan) {
   const int N = P.N, K = P.K;
+  const bool have_gscratch = P.g_nd && P.g_nid;
   int epb = N >= g_tc_threads ? 1 : g_tc_threads / N;
   if (epb > P.n_envs) epb = P.n_envs;
   const int block = round_up(epb * N, 32);
@@ -1063,7 +1059,7 @@ int plan_launch(TcParams &P, const FusedParams *Q, bool have_gscratch, LaunchPla
     P.scr_warp_bytes = 0;
     smem = base + tile;
   }
-  plan.epb = epb;
+  plan.kernel = TcPlan::kPacked;
   plan.block = block;
   plan.grid = (P.n_envs + epb - 1) / epb;
   P.full_ctas = plan.grid;
@@ -1092,7 +1088,7 @@ int plan_launch(TcParams &P, const FusedParams *Q, bool have_gscratch, LaunchPla
 }
 
 template <bool FUSED, int MAXT>
-int launch_t(const TcParams &P, const FusedParams &Q, const LaunchPlan &plan, cudaStream_t st) {
+int launch_t(const TcParams &P, const FusedParams &Q, const TcPlan &plan, cudaStream_t st) {
   static size_t configured = 0;
   if (plan.smem > 48 * 1024 && plan.smem > configured) {
     cudaError_t e = cudaFuncSetAttribute(tag_continuous_kernel<FUSED, MAXT>,
@@ -1119,48 +1115,132 @@ int launch_t(const TcParams &P, const FusedParams &Q, const LaunchPlan &plan, cu
   return finish_launch();
 }
 
-template <bool FUSED>
-int launch(const TcParams &P, const FusedParams &Q, const LaunchPlan &plan, cudaStream_t st) {
-  return plan.block <= 320 ? launch_t<FUSED, 320>(P, Q, plan, st)
-                           : launch_t<FUSED, 1024>(P, Q, plan, st);
+// TcParams of one step of `e`, after the checks both entry points apply to it
+int fill_params(TcParams &P, const wdb_tc_env &e) {
+  if (!e.loc_x || !e.loc_y || !e.speed || !e.direction || !e.acceleration || !e.agent_types ||
+      !e.edge_hit_reward_penalty || !e.acceleration_actions || !e.turn_actions ||
+      !e.skill_levels || !e.still_in_the_game || !e.nearest_neighbor_ids || !e.rewards ||
+      !e.step_rewards || !e.num_runners || !e.done || !e.env_timestep)
+    return (int)cudaErrorInvalidValue;
+  if (e.n_envs <= 0 || e.n_agents < 2 || e.n_agents > 4096 || e.num_other_agents_observed < 0)
+    return (int)cudaErrorInvalidValue;
+  P = {};
+  P.n_envs = e.n_envs; P.N = e.n_agents; P.K = e.num_other_agents_observed;
+  P.episode_length = e.episode_length;
+  P.use_full_obs = e.use_full_observation; P.runner_exits = e.runner_exits_game_after_tagged;
+  P.loc_x = e.loc_x; P.loc_y = e.loc_y; P.speed = e.speed; P.direction = e.direction;
+  P.acceleration = e.acceleration; P.agent_types = e.agent_types;
+  P.edge_pen = e.edge_hit_reward_penalty; P.edge_hit_penalty = e.edge_hit_penalty;
+  P.grid_length = e.grid_length; P.acc_actions = e.acceleration_actions;
+  P.turn_actions = e.turn_actions; P.max_speed = e.max_speed; P.skill = e.skill_levels;
+  P.alive = e.still_in_the_game; P.obs = e.obs;
+  P.g_nd = e.neighbor_distances; P.g_nid = e.neighbor_ids_sorted_by_distance;
+  P.nearest = e.nearest_neighbor_ids; P.rewards = e.rewards; P.step_rewards = e.step_rewards;
+  P.num_runners = e.num_runners; P.margin = e.distance_margin_for_reward;
+  P.tag_reward = e.tag_reward_for_tagger; P.tag_penalty = e.tag_penalty_for_runner;
+  P.end_reward = e.end_of_game_reward_for_runner; P.done = e.done;
+  P.timestep = e.env_timestep; P.stats = e.stats;
+  return 0;
 }
 
-int fill_params(TcParams &P, int n_envs, int n_agents, float *loc_x, float *loc_y,
-                float *speed, float *direction, float *acceleration, const int *agent_types,
-                float *edge_hit_reward_penalty, float edge_hit_penalty, float grid_length,
-                const float *acceleration_actions, const float *turn_actions, float max_speed,
-                int num_other_agents_observed, const float *skill_levels,
-                int runner_exits_game_after_tagged, int *still_in_the_game,
-                int use_full_observation, float *obs, const int *action_indices,
-                float *neighbor_distances, int *neighbor_ids_sorted_by_distance,
-                int *nearest_neighbor_ids, float *rewards, const float *step_rewards,
-                int *num_runners, float distance_margin_for_reward,
-                float tag_reward_for_tagger, float tag_penalty_for_runner,
-                float end_of_game_reward_for_runner, int *done, int *env_timestep,
-                int episode_length, int *stats) {
-  if (!loc_x || !loc_y || !speed || !direction || !acceleration || !agent_types ||
-      !edge_hit_reward_penalty || !acceleration_actions || !turn_actions || !skill_levels ||
-      !still_in_the_game || !nearest_neighbor_ids || !rewards || !step_rewards ||
-      !num_runners || !done || !env_timestep)
+// Which kernel runs one TagContinuous step, with what geometry, or cudaErrorInvalidValue when
+// none can.  Q is NULL for the env step alone; obs_next / obs_tiles: the fused step writes the
+// next observations / their bf16 tiles for some policy.  Fills P's derived fields and `plan`;
+// makes no CUDA call.
+int tc_plan(TcParams &P, const FusedParams *Q, bool obs_next, bool obs_tiles, int blocks_per_env,
+            TcPlan &plan) {
+  plan = {};
+  // blocks_per_env > 1: the env is spread over that many CTAs, launched as one thread-block
+  // cluster (wdb_tc_wide.cu) -- the reference's multi-block mode, env_dim_mapper.h:22-31.
+  // Observation tiles come from the packed kernel's staged tile only.
+  if (blocks_per_env > 1) {
+    if (obs_tiles) return (int)cudaErrorInvalidValue;
+    return tc_wide_plan(P, Q, blocks_per_env, plan);
+  }
+  if (P.N > 1024) return (int)cudaErrorInvalidValue;   // one CTA per env: <= 1024 threads
+  // envs too large for the packed kernel's shared-memory tile: the x-binned kernel with the
+  // whole env in ONE CTA (a cluster of 1); wdb_set_option("tc_wide_single", 0) keeps the
+  // first-generation single-CTA path for A/B runs
+  if (g_tc_wide_single && P.N > 320 && !P.use_full_obs && P.K + 2 <= kListLen) {
+    if (obs_tiles) return (int)cudaErrorInvalidValue;
+    return tc_wide_plan(P, Q, 1, plan);
+  }
+  if (tc_v2_eligible(P, Q, obs_tiles)) return tc_v2_plan(P, plan);
+  const int err = plan_packed(P, Q, plan);
+  if (err) return err;
+  // the per-policy observation push needs the shared-memory tile
+  if (!P.stage_obs && !P.use_full_obs && (obs_next || obs_tiles))
     return (int)cudaErrorInvalidValue;
-  if (n_envs <= 0 || n_agents < 2 || n_agents > 4096 || num_other_agents_observed < 0)
-    return (int)cudaErrorInvalidValue;
-  P.n_envs = n_envs; P.N = n_agents; P.K = num_other_agents_observed;
-  P.episode_length = episode_length;
-  P.use_full_obs = use_full_observation; P.runner_exits = runner_exits_game_after_tagged;
-  P.loc_x = loc_x; P.loc_y = loc_y; P.speed = speed; P.direction = direction;
-  P.acceleration = acceleration; P.agent_types = agent_types;
-  P.edge_pen = edge_hit_reward_penalty; P.edge_hit_penalty = edge_hit_penalty;
-  P.grid_length = grid_length; P.acc_actions = acceleration_actions;
-  P.turn_actions = turn_actions; P.max_speed = max_speed; P.skill = skill_levels;
-  P.alive = still_in_the_game; P.obs = obs; P.actions = action_indices;
-  P.g_nd = neighbor_distances; P.g_nid = neighbor_ids_sorted_by_distance;
-  P.nearest = nearest_neighbor_ids; P.rewards = rewards; P.step_rewards = step_rewards;
-  P.num_runners = num_runners; P.margin = distance_margin_for_reward;
-  P.tag_reward = tag_reward_for_tagger; P.tag_penalty = tag_penalty_for_runner;
-  P.end_reward = end_of_game_reward_for_runner; P.done = done; P.timestep = env_timestep;
-  P.stats = stats;
+  if (P.use_full_obs && obs_tiles) return (int)cudaErrorInvalidValue;
   return 0;
+}
+
+int tc_launch(const TcParams &P, const FusedParams *Q, const TcPlan &plan, cudaStream_t st) {
+  if (plan.kernel == TcPlan::kWide) return tc_wide_launch(P, Q, plan, st);
+  if (plan.kernel == TcPlan::kV2) return tc_v2_launch(P, Q, plan, st);
+  const FusedParams none = {};
+  if (!Q)
+    return plan.block <= 320 ? launch_t<false, 320>(P, none, plan, st)
+                             : launch_t<false, 1024>(P, none, plan, st);
+  return plan.block <= 320 ? launch_t<true, 320>(P, *Q, plan, st)
+                           : launch_t<true, 1024>(P, *Q, plan, st);
+}
+
+// The rollout step's checks, in the order it applies them, then its plan.  shapes_only: no
+// pointer of `ro` is checked, obs_next counts as written for every policy and the obs tiles
+// as `with_tiles` says (wdb_tag_continuous_rollout_supported).
+int plan_rollout(const wdb_tc_env *env, const wdb_tc_rollout *ro, bool shapes_only,
+                 bool with_tiles, TcParams &P, FusedParams &Q, TcPlan &plan) {
+  if (!env || !ro) return (int)cudaErrorInvalidValue;
+  int err = fill_params(P, *env);
+  if (err) return err;
+  if (ro->n_policies < 1 || ro->n_policies > kMaxPolicies || ro->n_actions0 < 1 ||
+      ro->n_actions1 < 1)
+    return (int)cudaErrorInvalidValue;
+  if (!shapes_only) {
+    if (!ro->agent_policy || !ro->agent_slot) return (int)cudaErrorInvalidValue;
+    if (!ro->uniforms && !ro->rng_state) return (int)cudaErrorInvalidValue;
+    if (ro->sampled_actions && ((uintptr_t)ro->sampled_actions & 7))
+      return (int)cudaErrorMisalignedAddress;
+  }
+  Q = {};
+  Q.rng = ro->rng_state; Q.uniforms = ro->uniforms;
+  Q.n_policies = ro->n_policies; Q.A0 = ro->n_actions0; Q.A1 = ro->n_actions1;
+  Q.agent_policy = ro->agent_policy; Q.agent_slot = ro->agent_slot;
+  bool obs_next = shapes_only, obs_tiles = shapes_only && with_tiles;
+  int total = 0;
+  for (int p = 0; p < ro->n_policies; p++) {
+    const wdb_tc_policy_io &io = ro->policy[p];
+    if (io.n_agents < 1) return (int)cudaErrorInvalidValue;
+    if (!shapes_only) {
+      if (!io.probs0 || !io.probs1) return (int)cudaErrorInvalidValue;
+      if (io.actions_batch && ((uintptr_t)io.actions_batch & 7))
+        return (int)cudaErrorMisalignedAddress;
+      if (io.obs_next_tiles && ((uintptr_t)io.obs_next_tiles & 15))
+        return (int)cudaErrorMisalignedAddress;
+      obs_next = obs_next || io.obs_next;
+      obs_tiles = obs_tiles || io.obs_next_tiles;
+    }
+    Q.policy_size[p] = io.n_agents;
+    Q.probs0[p] = io.probs0; Q.probs1[p] = io.probs1;
+    Q.actions_batch[p] = io.actions_batch; Q.rewards_batch[p] = io.rewards_batch;
+    Q.obs_next[p] = io.obs_next; Q.reward_running_sum[p] = io.reward_running_sum;
+    Q.obs_tiles[p] = reinterpret_cast<unsigned char *>(io.obs_next_tiles);
+    Q.episodic_reward_sum[p] = io.episodic_reward_sum;
+    total += io.n_agents;
+  }
+  if (total != env->n_agents) return (int)cudaErrorInvalidValue;
+  // a NULL actions_batch[0] disables the action push for every policy (kernel fast test)
+  Q.actions_out = ro->sampled_actions;
+  Q.actions_head0 = ro->sampled_actions_0; Q.actions_head1 = ro->sampled_actions_1;
+  Q.done_batch = ro->done_batch; Q.step_running_sum = ro->step_running_sum;
+  Q.episodic_step_sum = ro->episodic_step_sum; Q.num_completed = ro->num_completed_episodes;
+  Q.reset_table = ro->reset_table; Q.n_reset = ro->n_reset_arrays;
+  Q.obs_at_reset = ro->obs_at_reset; Q.do_reset = ro->reset_done_envs;
+  Q.pdl = ro->launch_after_forward;
+  if (!shapes_only && Q.do_reset && Q.n_reset > 0 && !Q.reset_table)
+    return (int)cudaErrorInvalidValue;
+  return tc_plan(P, &Q, obs_next, obs_tiles, env->blocks_per_env, plan);
 }
 
 }  // namespace
@@ -1222,118 +1302,42 @@ WDB_API int wdb_tag_continuous_step(
     int *num_runners, float distance_margin_for_reward, float tag_reward_for_tagger,
     float tag_penalty_for_runner, float end_of_game_reward_for_runner, int *done,
     int *env_timestep, int episode_length, int *stats) {
-  // blocks_per_env == 1: whole env replicas packed into one CTA (geometry chosen here);
-  // blocks_per_env > 1: the env is spread over that many CTAs, launched as one thread-block
-  // cluster (wdb_tc_wide.cu) -- the reference's multi-block mode, env_dim_mapper.h:22-31
   if (blocks_per_env < 1) return (int)cudaErrorInvalidValue;
+  const wdb_tc_env env = {   // in the field order of wdb_tc_env
+      n_envs, n_agents, loc_x, loc_y, speed, direction, acceleration, agent_types,
+      edge_hit_reward_penalty, edge_hit_penalty, grid_length, acceleration_actions,
+      turn_actions, max_speed, num_other_agents_observed, skill_levels,
+      runner_exits_game_after_tagged, still_in_the_game, use_full_observation, obs,
+      neighbor_distances, neighbor_ids_sorted_by_distance, nearest_neighbor_ids, rewards,
+      step_rewards, num_runners, distance_margin_for_reward, tag_reward_for_tagger,
+      tag_penalty_for_runner, end_of_game_reward_for_runner, done, env_timestep,
+      episode_length, stats, blocks_per_env};
   TcParams P;
-  int err = fill_params(P, n_envs, n_agents, loc_x, loc_y, speed, direction, acceleration,
-                        agent_types, edge_hit_reward_penalty, edge_hit_penalty, grid_length,
-                        acceleration_actions, turn_actions, max_speed,
-                        num_other_agents_observed, skill_levels,
-                        runner_exits_game_after_tagged, still_in_the_game,
-                        use_full_observation, obs, action_indices, neighbor_distances,
-                        neighbor_ids_sorted_by_distance, nearest_neighbor_ids, rewards,
-                        step_rewards, num_runners, distance_margin_for_reward,
-                        tag_reward_for_tagger, tag_penalty_for_runner,
-                        end_of_game_reward_for_runner, done, env_timestep, episode_length,
-                        stats);
+  int err = fill_params(P, env);
   if (err) return err;
   if (!obs || !action_indices) return (int)cudaErrorInvalidValue;
   if ((uintptr_t)action_indices & 7) return (int)cudaErrorMisalignedAddress;
-  if (blocks_per_env > 1) return tc_wide_launch(P, nullptr, blocks_per_env, as_stream(stream));
-  if (n_agents > 1024) return (int)cudaErrorInvalidValue;   // one CTA per env: <= 1024 threads
-  // envs too large for the packed kernel's shared-memory tile: the x-binned kernel with the
-  // whole env in ONE CTA (a cluster of 1); wdb_set_option("tc_wide_single", 0) keeps the
-  // first-generation single-CTA path for A/B runs
-  if (g_tc_wide_single && n_agents > 320 && !use_full_observation &&
-      num_other_agents_observed + 2 <= kListLen)
-    return tc_wide_launch(P, nullptr, 1, as_stream(stream));
-  if (tc_v2_eligible(P, nullptr)) return tc_v2_launch(P, nullptr, as_stream(stream));
-  LaunchPlan plan;
-  err = plan_launch(P, nullptr, neighbor_distances && neighbor_ids_sorted_by_distance, plan);
+  P.actions = action_indices;
+  TcPlan plan;
+  err = tc_plan(P, nullptr, false, false, blocks_per_env, plan);
   if (err) return err;
-  FusedParams Q = {};
-  return launch<false>(P, Q, plan, as_stream(stream));
+  return tc_launch(P, nullptr, plan, as_stream(stream));
 }
 
 WDB_API int wdb_tag_continuous_rollout_step(void *stream, const wdb_tc_env *env,
                                             const wdb_tc_rollout *ro) {
-  if (!env || !ro) return (int)cudaErrorInvalidValue;
   TcParams P;
-  int err = fill_params(
-      P, env->n_envs, env->n_agents, env->loc_x, env->loc_y, env->speed, env->direction,
-      env->acceleration, env->agent_types, env->edge_hit_reward_penalty,
-      env->edge_hit_penalty, env->grid_length, env->acceleration_actions, env->turn_actions,
-      env->max_speed, env->num_other_agents_observed, env->skill_levels,
-      env->runner_exits_game_after_tagged, env->still_in_the_game,
-      env->use_full_observation, env->obs, nullptr, env->neighbor_distances,
-      env->neighbor_ids_sorted_by_distance, env->nearest_neighbor_ids, env->rewards,
-      env->step_rewards, env->num_runners, env->distance_margin_for_reward,
-      env->tag_reward_for_tagger, env->tag_penalty_for_runner,
-      env->end_of_game_reward_for_runner, env->done, env->env_timestep, env->episode_length,
-      env->stats);
+  FusedParams Q;
+  TcPlan plan;
+  const int err = plan_rollout(env, ro, false, false, P, Q, plan);
   if (err) return err;
-  if (ro->n_policies < 1 || ro->n_policies > kMaxPolicies || !ro->agent_policy ||
-      !ro->agent_slot || ro->n_actions0 < 1 || ro->n_actions1 < 1)
-    return (int)cudaErrorInvalidValue;
-  if (!ro->uniforms && !ro->rng_state) return (int)cudaErrorInvalidValue;
-  if (ro->sampled_actions && ((uintptr_t)ro->sampled_actions & 7))
-    return (int)cudaErrorMisalignedAddress;
-  FusedParams Q = {};
-  Q.rng = ro->rng_state; Q.uniforms = ro->uniforms;
-  Q.n_policies = ro->n_policies; Q.A0 = ro->n_actions0; Q.A1 = ro->n_actions1;
-  Q.agent_policy = ro->agent_policy; Q.agent_slot = ro->agent_slot;
-  int total = 0;
-  for (int p = 0; p < ro->n_policies; p++) {
-    const wdb_tc_policy_io &io = ro->policy[p];
-    if (!io.probs0 || !io.probs1 || io.n_agents < 1) return (int)cudaErrorInvalidValue;
-    if (io.actions_batch && ((uintptr_t)io.actions_batch & 7))
-      return (int)cudaErrorMisalignedAddress;
-    Q.policy_size[p] = io.n_agents;
-    Q.probs0[p] = io.probs0; Q.probs1[p] = io.probs1;
-    Q.actions_batch[p] = io.actions_batch; Q.rewards_batch[p] = io.rewards_batch;
-    Q.obs_next[p] = io.obs_next; Q.reward_running_sum[p] = io.reward_running_sum;
-    Q.obs_tiles[p] = reinterpret_cast<unsigned char *>(io.obs_next_tiles);
-    if (io.obs_next_tiles && ((uintptr_t)io.obs_next_tiles & 15))
-      return (int)cudaErrorMisalignedAddress;
-    Q.episodic_reward_sum[p] = io.episodic_reward_sum;
-    total += io.n_agents;
-  }
-  if (total != env->n_agents) return (int)cudaErrorInvalidValue;
-  // a NULL actions_batch[0] disables the action push for every policy (kernel fast test)
-  Q.actions_out = ro->sampled_actions;
-  Q.actions_head0 = ro->sampled_actions_0; Q.actions_head1 = ro->sampled_actions_1;
-  Q.done_batch = ro->done_batch; Q.step_running_sum = ro->step_running_sum;
-  Q.episodic_step_sum = ro->episodic_step_sum; Q.num_completed = ro->num_completed_episodes;
-  Q.reset_table = ro->reset_table; Q.n_reset = ro->n_reset_arrays;
-  Q.obs_at_reset = ro->obs_at_reset; Q.do_reset = ro->reset_done_envs;
-  Q.pdl = ro->launch_after_forward;
-  if (Q.do_reset && Q.n_reset > 0 && !Q.reset_table) return (int)cudaErrorInvalidValue;
-  if (env->blocks_per_env > 1) {
-    for (int p = 0; p < Q.n_policies; p++)
-      if (Q.obs_tiles[p]) return (int)cudaErrorInvalidValue;   // tiles come from the CTA tile
-    return tc_wide_launch(P, &Q, env->blocks_per_env, as_stream(stream));
-  }
-  if (env->n_agents > 1024) return (int)cudaErrorInvalidValue;
-  if (g_tc_wide_single && env->n_agents > 320 && !env->use_full_observation &&
-      env->num_other_agents_observed + 2 <= kListLen) {
-    for (int p = 0; p < Q.n_policies; p++)
-      if (Q.obs_tiles[p]) return (int)cudaErrorInvalidValue;
-    return tc_wide_launch(P, &Q, 1, as_stream(stream));
-  }
-  if (tc_v2_eligible(P, &Q)) return tc_v2_launch(P, &Q, as_stream(stream));
-  LaunchPlan plan;
-  err = plan_launch(P, &Q, env->neighbor_distances && env->neighbor_ids_sorted_by_distance,
-                    plan);
-  if (err) return err;
-  if (!P.stage_obs && !P.use_full_obs) {
-    // the per-policy observation push needs the shared-memory tile
-    for (int p = 0; p < Q.n_policies; p++)
-      if (Q.obs_next[p] || Q.obs_tiles[p]) return (int)cudaErrorInvalidValue;
-  }
-  if (P.use_full_obs)
-    for (int p = 0; p < Q.n_policies; p++)
-      if (Q.obs_tiles[p]) return (int)cudaErrorInvalidValue;   // tiles come from the staged tile
-  return launch<true>(P, Q, plan, as_stream(stream));
+  return tc_launch(P, &Q, plan, as_stream(stream));
+}
+
+WDB_API int wdb_tag_continuous_rollout_supported(const wdb_tc_env *env,
+                                                 const wdb_tc_rollout *ro, int with_obs_tiles) {
+  TcParams P;
+  FusedParams Q;
+  TcPlan plan;
+  return plan_rollout(env, ro, true, with_obs_tiles != 0, P, Q, plan);
 }

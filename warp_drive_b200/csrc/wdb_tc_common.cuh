@@ -90,13 +90,52 @@ struct FusedParams {
   int pdl;                          // host only: launch programmatically dependent on the forward
 };
 
-// launch of the cluster kernel (wdb_tc_wide.cu); `fused` may be NULL (step-only)
+struct V2Params {
+  int chunk_rows;        // rows of the observation tile (multiple of 4)
+  int tile_bytes;
+};
+
+struct WideParams {
+  int C;            // CTAs per env (cluster size)
+  int S;            // agents per CTA slice (id order): ceil(N / C)
+  int nbins;        // x-bins (power of two <= 64); bin `nbins` holds the dead agents
+  int npad;         // sorted planes length: round_up(N, 16), all +inf behind the alive agents
+  int sw;           // staging row pitch in floats (odd)
+  int fpp;          // feature planes per staging pass (7: one pass ... 1: seven passes)
+  int o_idcol;      // byte offset of the id columns inside a warp's scratch
+  int o_rowptr;     // ... of the 32 x 2 destination row pointers (the staging rows follow)
+  int use_window;   // 0: scan every alive agent (A/B switch)
+  // byte offsets into dynamic shared memory (identical in every CTA: DSMEM addressing)
+  int o_pos, o_sp, o_acc, o_dir, o_alive, o_cross, o_type, o_kx, o_ky, o_sid, o_tag,
+      o_tagcnt, o_wcount, o_binbase, o_leftmax, o_rightmin, o_misc, o_tab, o_scr, o_stage,
+      o_exact;
+  int scr_warp_bytes, stage_warp_bytes;
+};
+
+// One TagContinuous launch as tc_plan decided it: which kernel, and its geometry.
+struct TcPlan {
+  enum Kernel { kPacked, kV2, kWide } kernel;
+  int grid, block;
+  int cluster;      // kWide: CTAs per env, launched as one thread-block cluster
+  int minb;         // kV2: CTAs per SM the kernel instance is built for (3, 4 or 7)
+  size_t smem;      // dynamic shared memory per CTA
+  V2Params v2;      // kV2 only
+  WideParams wide;  // kWide only
+};
+
+// The plan and launch halves of the cluster kernel (wdb_tc_wide.cu) and of the
+// second-generation small-env kernel (wdb_tc_small_v2.cu, wdb_set_option("tc_variant", 2)).
+// `fused` is NULL for the env step alone.  A plan function fills P's derived fields and
+// `plan`, or returns cudaErrorInvalidValue; it makes no CUDA call.
 extern int g_pdl;                   // wdb_set_option("pdl", 0/1), wdb_mlp.cu
-int tc_wide_launch(TcParams &P, const FusedParams *fused, int blocks_per_env, cudaStream_t st);
+int tc_wide_plan(TcParams &P, const FusedParams *fused, int blocks_per_env, TcPlan &plan);
+int tc_wide_launch(const TcParams &P, const FusedParams *fused, const TcPlan &plan,
+                   cudaStream_t st);
 int tc_wide_set_option(const char *name, int value, bool *handled);
-// second-generation small-env kernel (wdb_tc_small_v2.cu), wdb_set_option("tc_variant", 2)
-bool tc_v2_eligible(const TcParams &P, const FusedParams *fused);
-int tc_v2_launch(TcParams &P, const FusedParams *fused, cudaStream_t st);
+bool tc_v2_eligible(const TcParams &P, const FusedParams *fused, bool obs_tiles);
+int tc_v2_plan(TcParams &P, TcPlan &plan);
+int tc_v2_launch(const TcParams &P, const FusedParams *fused, const TcPlan &plan,
+                 cudaStream_t st);
 int tc_v2_set_option(const char *name, int value, bool *handled);
 extern int g_tc_history, g_tc_force_exact, g_tc_wide_single;
 
@@ -117,7 +156,7 @@ __constant__ float kTwoPi = 6.283185308;
 __constant__ float kEpsilon = 1.0e-10;
 
 // Byte offsets of the small shared-memory arrays (must agree between the kernel and
-// plan_launch): everything before the per-warp scratch, rounded up to 16 bytes so that the
+// plan_packed): everything before the per-warp scratch, rounded up to 16 bytes so that the
 // scratch and the big tile behind it are valid TMA (cp.async.bulk) destinations.
 __host__ __device__ inline int tc_key_stride(int N) { return (N + 15) & ~15; }
 __host__ __device__ inline size_t tc_small_bytes(int epb, int N) {

@@ -32,11 +32,6 @@ namespace {
 
 constexpr int kHistIds = kListLen - 2;   // neighbour ids kept per agent for the threshold
 
-struct V2Params {
-  int chunk_rows;        // rows of the observation tile (multiple of 4)
-  int tile_bytes;
-};
-
 // Register CDF + the reference's binary search on bit masks (A <= W, W = 24 or 32).
 template <int W>
 __device__ __forceinline__ int sample_row_regs_w(const float *__restrict__ src, int A, float u) {
@@ -805,18 +800,18 @@ tc_small_v2_kernel(const __grid_constant__ TcParams P, const __grid_constant__ F
 int g_tc_v2_threads = 320;   // wdb_set_option("tc_v2_threads", 320 | 224 | 128)
 
 template <bool FUSED, int MAXT, int MINB>
-int v2_launch_t(const TcParams &P, const FusedParams &Q, const V2Params &V, int grid, int block,
-                size_t smem, cudaStream_t st) {
+int v2_launch_t(const TcParams &P, const FusedParams &Q, const TcPlan &plan, cudaStream_t st) {
   static size_t configured = 0;
-  if (smem > configured) {
+  if (plan.smem > configured) {
     cudaError_t e = cudaFuncSetAttribute(tc_small_v2_kernel<FUSED, MAXT, MINB>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)plan.smem);
     if (e != cudaSuccess) return (int)e;
     cudaFuncSetAttribute(tc_small_v2_kernel<FUSED, MAXT, MINB>,
                          cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-    configured = smem;
+    configured = plan.smem;
   }
-  tc_small_v2_kernel<FUSED, MAXT, MINB><<<grid, block, smem, st>>>(P, Q, V);
+  tc_small_v2_kernel<FUSED, MAXT, MINB><<<plan.grid, plan.block, plan.smem, st>>>(P, Q, plan.v2);
   return finish_launch();
 }
 
@@ -847,18 +842,14 @@ int tc_v2_set_option(const char *name, int value, bool *handled) {
   return 0;
 }
 
-bool tc_v2_eligible(const TcParams &P, const FusedParams *Q) {
+bool tc_v2_eligible(const TcParams &P, const FusedParams *Q, bool obs_tiles) {
   if (g_tc_variant != 2) return false;
   if (P.use_full_obs || P.K < 1 || P.K + 2 > kListLen || P.N > 128 || P.N < 2) return false;
-  if (Q) {
-    if (Q->A0 > 32 || Q->A1 > 32) return false;
-    for (int p = 0; p < Q->n_policies; p++)
-      if (Q->obs_tiles[p]) return false;
-  }
-  return true;
+  if (Q && (Q->A0 > 32 || Q->A1 > 32)) return false;
+  return !obs_tiles;
 }
 
-int tc_v2_launch(TcParams &P, const FusedParams *Qp, cudaStream_t st) {
+int tc_v2_plan(TcParams &P, TcPlan &plan) {
   const int N = P.N, K = P.K, F = 7 * K + 1;
   const int budget_threads = g_tc_v2_threads;
   const int minb = budget_threads == 320 ? 3 : (budget_threads == 224 ? 4 : 7);
@@ -894,20 +885,26 @@ int tc_v2_launch(TcParams &P, const FusedParams *Qp, cudaStream_t st) {
   // balance the chunks (same number of chunks, equal sizes)
   const int n_chunks = (EN + chunk - 1) / chunk;
   chunk = (((EN + n_chunks - 1) / n_chunks) + 3) & ~3;
-  V2Params V;
-  V.chunk_rows = chunk;
-  V.tile_bytes = chunk * F * 4;
-  const size_t smem = fixed + (size_t)V.tile_bytes;
-  const int grid = (P.n_envs + epb - 1) / epb;
-  FusedParams Q = {};
-  if (Qp) Q = *Qp;
+  plan.kernel = TcPlan::kV2;
+  plan.v2.chunk_rows = chunk;
+  plan.v2.tile_bytes = chunk * F * 4;
+  plan.smem = fixed + (size_t)plan.v2.tile_bytes;
+  plan.grid = (P.n_envs + epb - 1) / epb;
+  plan.block = block;
+  plan.minb = minb;
+  return 0;
+}
+
+int tc_v2_launch(const TcParams &P, const FusedParams *Qp, const TcPlan &plan,
+                 cudaStream_t st) {
+  const FusedParams none = {};
   if (Qp)
-    return minb == 3   ? v2_launch_t<true, 320, 3>(P, Q, V, grid, block, smem, st)
-           : minb == 4 ? v2_launch_t<true, 224, 4>(P, Q, V, grid, block, smem, st)
-                       : v2_launch_t<true, 128, 7>(P, Q, V, grid, block, smem, st);
-  return minb == 3   ? v2_launch_t<false, 320, 3>(P, Q, V, grid, block, smem, st)
-         : minb == 4 ? v2_launch_t<false, 224, 4>(P, Q, V, grid, block, smem, st)
-                     : v2_launch_t<false, 128, 7>(P, Q, V, grid, block, smem, st);
+    return plan.minb == 3   ? v2_launch_t<true, 320, 3>(P, *Qp, plan, st)
+           : plan.minb == 4 ? v2_launch_t<true, 224, 4>(P, *Qp, plan, st)
+                            : v2_launch_t<true, 128, 7>(P, *Qp, plan, st);
+  return plan.minb == 3   ? v2_launch_t<false, 320, 3>(P, none, plan, st)
+         : plan.minb == 4 ? v2_launch_t<false, 224, 4>(P, none, plan, st)
+                          : v2_launch_t<false, 128, 7>(P, none, plan, st);
 }
 
 }  // namespace wdb

@@ -52,23 +52,6 @@ constexpr int kWideMaxThreads = 1024;   // one CTA may carry a whole 1024-agent 
 constexpr int kWideMaxBins = 64;
 constexpr int kWideCap = 32;     // candidates one lane may collect (kHistCap)
 
-struct WideParams {
-  int C;            // CTAs per env (cluster size)
-  int S;            // agents per CTA slice (id order): ceil(N / C)
-  int nbins;        // x-bins (power of two <= 64); bin `nbins` holds the dead agents
-  int npad;         // sorted planes length: round_up(N, 16), all +inf behind the alive agents
-  int sw;           // staging row pitch in floats (odd)
-  int fpp;          // feature planes per staging pass (7: one pass ... 1: seven passes)
-  int o_idcol;      // byte offset of the id columns inside a warp's scratch
-  int o_rowptr;     // ... of the 32 x 2 destination row pointers (the staging rows follow)
-  int use_window;   // 0: scan every alive agent (A/B switch)
-  // byte offsets into dynamic shared memory (identical in every CTA: DSMEM addressing)
-  int o_pos, o_sp, o_acc, o_dir, o_alive, o_cross, o_type, o_kx, o_ky, o_sid, o_tag,
-      o_tagcnt, o_wcount, o_binbase, o_leftmax, o_rightmin, o_misc, o_tab, o_scr, o_stage,
-      o_exact;
-  int scr_warp_bytes, stage_warp_bytes;
-};
-
 // misc words
 enum { M_T = 0, M_NRUN, M_DONEPREV, M_NALIVE, M_NTAG, M_EXITS, M_LOCK, M_STEPS, M_COUNT };
 
@@ -941,6 +924,34 @@ int g_tc_wide_fpp = 0;      // wdb_set_option("tc_wide_fpp", n): feature planes 
 
 inline int align_up(int v, int a) { return (v + a - 1) / a * a; }
 
+template <bool FUSED>
+int wide_launch_t(const TcParams &P, const FusedParams &Q, const TcPlan &plan, cudaStream_t st) {
+  static size_t configured = 0;
+  if (plan.smem > configured) {
+    const cudaError_t e = cudaFuncSetAttribute(
+        tc_wide_kernel<FUSED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem);
+    if (e != cudaSuccess) return (int)e;
+    configured = plan.smem;
+  }
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)plan.grid, 1, 1);
+  cfg.blockDim = dim3((unsigned)plan.block, 1, 1);
+  cfg.dynamicSmemBytes = plan.smem;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[2];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = (unsigned)plan.cluster;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[1].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = (FUSED && Q.pdl && g_pdl) ? 2 : 1;
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, tc_wide_kernel<FUSED>, P, Q, plan.wide);
+  if (e != cudaSuccess) return (int)e;
+  return finish_launch();
+}
+
 }  // namespace
 
 namespace wdb {
@@ -967,8 +978,8 @@ int tc_wide_set_option(const char *name, int value, bool *handled) {
   return 0;
 }
 
-// Launch geometry of the cluster kernel; shared-memory carve-up.  Returns a cudaError.
-int tc_wide_launch(TcParams &P, const FusedParams *Qp, int blocks_per_env, cudaStream_t st) {
+// Launch geometry of the cluster kernel; shared-memory carve-up.
+int tc_wide_plan(TcParams &P, const FusedParams *Qp, int blocks_per_env, TcPlan &plan) {
   const int N = P.N, K = P.K, C = blocks_per_env;
   if (C < 1 || C > 8) return (int)cudaErrorInvalidValue;        // portable cluster size
   const int S = (N + C - 1) / C;
@@ -1043,45 +1054,20 @@ int tc_wide_launch(TcParams &P, const FusedParams *Qp, int blocks_per_env, cudaS
   }
   if (!fits) return (int)cudaErrorInvalidValue;
   if (!P.use_full_obs && !P.obs && !Qp) return (int)cudaErrorInvalidValue;
+  plan.kernel = TcPlan::kWide;
+  plan.grid = P.n_envs * C;
+  plan.block = block;
+  plan.cluster = C;
+  plan.smem = smem;
+  plan.wide = W;
+  return 0;
+}
 
-  FusedParams Q = {};
-  if (Qp) Q = *Qp;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(P.n_envs * C), 1, 1);
-  cfg.blockDim = dim3((unsigned)block, 1, 1);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = (unsigned)C;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = (Qp && Qp->pdl && g_pdl) ? 2 : 1;
-  cudaError_t e;
-  if (Qp) {
-    static size_t configured = 0;
-    if (smem > configured) {
-      e = cudaFuncSetAttribute(tc_wide_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               (int)smem);
-      if (e != cudaSuccess) return (int)e;
-      configured = smem;
-    }
-    e = cudaLaunchKernelEx(&cfg, tc_wide_kernel<true>, P, Q, W);
-  } else {
-    static size_t configured = 0;
-    if (smem > configured) {
-      e = cudaFuncSetAttribute(tc_wide_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               (int)smem);
-      if (e != cudaSuccess) return (int)e;
-      configured = smem;
-    }
-    e = cudaLaunchKernelEx(&cfg, tc_wide_kernel<false>, P, Q, W);
-  }
-  if (e != cudaSuccess) return (int)e;
-  return finish_launch();
+int tc_wide_launch(const TcParams &P, const FusedParams *Qp, const TcPlan &plan,
+                   cudaStream_t st) {
+  if (Qp) return wide_launch_t<true>(P, *Qp, plan, st);
+  const FusedParams none = {};
+  return wide_launch_t<false>(P, none, plan, st);
 }
 
 }  // namespace wdb

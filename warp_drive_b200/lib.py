@@ -178,6 +178,8 @@ _SIGNATURES = {
     ),
     "wdb_tag_continuous_rollout_step": (
         _i, [_vp, ctypes.POINTER(TcEnv), ctypes.POINTER(TcRollout)]),
+    "wdb_tag_continuous_rollout_supported": (
+        _i, [ctypes.POINTER(TcEnv), ctypes.POINTER(TcRollout), _i]),
     "wdb_mlp_blob_bytes": (_ll, [_i, _i, _i, _i]),
     "wdb_mlp_pack_weights": (_i, [_vp] * 12 + [_i, _i, _i, _i]),
     "wdb_mlp_policy_forward": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _ll, _vp, _vp, _vp]),

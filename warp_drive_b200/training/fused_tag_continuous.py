@@ -56,6 +56,20 @@ def fill_tc_env(dm, stats=None, with_scratch=False, write_observations=True):
 
 
 class FusedTagContinuousStep:
+    @staticmethod
+    def eligible(env_wrapper, policy_map, obs_tiles=False):
+        """Whether the library runs the fused step for this env, these policies and (with
+        obs_tiles) the bf16 observation tiles; it applies the same launch plan as the step."""
+        ro = _lib.TcRollout()
+        ro.n_policies = len(policy_map)
+        heads = env_wrapper.env.action_space[0].nvec
+        ro.n_actions0, ro.n_actions1 = int(heads[0]), int(heads[1])
+        for pi, ids in enumerate(policy_map.values()):
+            ro.policy[pi].n_agents = len(ids)
+        env = fill_tc_env(env_wrapper.cuda_data_manager)
+        return _lib.load().wdb_tag_continuous_rollout_supported(
+            ctypes.byref(env), ctypes.byref(ro), int(bool(obs_tiles))) == 0
+
     def __init__(self, env_wrapper, policy_map, sampler, resetter=None, stats=None,
                  write_observations=True, write_head_actions=True):
         self.dm = dm = env_wrapper.cuda_data_manager

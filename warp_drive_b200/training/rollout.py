@@ -111,8 +111,7 @@ class RolloutEngine:
                 # (off by default: at config 2 the env step's extra pass costs about what the
                 #  forward saves)
                 if (use_obs_tiles and self.fused is not None
-                        and int(getattr(env_wrapper, "blocks_per_env", 1) or 1) == 1
-                        and not getattr(env_wrapper.env, "use_full_observation", False)):
+                        and self.fused.eligible(env_wrapper, self.policy_map, obs_tiles=True)):
                     self.obs_tiles = {
                         p: torch.zeros(self.fused_forward[p].tiles_bytes(
                             self.E * len(self.policy_map[p])), dtype=torch.uint8, device=dev)
@@ -138,25 +137,13 @@ class RolloutEngine:
             return False
         if self.T < 1 or self.dm.reset_target_to_pool:
             return False
-        bpe = int(getattr(self.env_wrapper, "blocks_per_env", 1) or 1)
-        k_obs = int(getattr(env, "num_other_agents_observed", 0))
-        full = bool(getattr(env, "use_full_observation", False))
-        if bpe > 1 or (self.N > 320 and not full and k_obs + 2 <= 16):
-            # one env per thread-block cluster, or one large env per CTA (wdb_tc_wide.cu):
-            # <= 1024 agents per CTA
-            if -(-self.N // bpe) > 1024:
-                return False
-        elif not full:
-            # the fused step pushes the per-policy observations from its shared-memory tile
-            # (same sizing rule as plan_launch in wdb_tag_continuous.cu); envs too large for
-            # that (e.g. 1024 agents) take the generic multi-launch path
-            n, f = self.N, 7 * int(env.num_other_agents_observed) + 1
-            epb = max(1, 320 // n)
-            n_warps = (epb * n + 31) // 32
-            small = 36 * epb * n + 16 * n + max(8 * n, 1056) * n_warps
-            if small + 4 * epb * n * f > 113 * 1024:
-                return False
-        return all(getattr(m, "action_mask", None) is None for m in self.models.values())
+        if any(getattr(m, "action_mask", None) is not None for m in self.models.values()):
+            return False
+        # the library's launch plan decides the rest (shapes no kernel takes, e.g. envs too
+        # large for the shared-memory observation tile, run the generic multi-launch path)
+        from warp_drive_b200.training.fused_tag_continuous import FusedTagContinuousStep
+
+        return FusedTagContinuousStep.eligible(self.env_wrapper, self.policy_map)
 
     def resync_observations(self):
         """Re-gather the per-policy observation buffers from `observations` (call after
