@@ -570,7 +570,7 @@ def test_tail_split_ctas_bit_exact_vs_reference_cuda(wdb_lib, shape, tc_history)
     assert wdb_lib.wdb_set_option(b"tc_tail_split", 2) == 0
     try:
         test_tag_continuous_bit_exact_vs_reference_cuda(wdb_lib, shape, False, tc_history)
-        roll.test_fused_step_equals_separate_calls(False)
+        roll.test_fused_step_equals_separate_calls(False, 1)
         roll.test_engine_cuda_graph_matches_eager(True)
     finally:
         assert wdb_lib.wdb_set_option(b"tc_tail_split", 0) == 0

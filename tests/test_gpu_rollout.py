@@ -2,6 +2,8 @@
 RolloutEngine: the single-launch path must produce exactly what the separate
 sample / step / bookkeeping / reset calls produce (which are themselves pinned to the
 oracle and to the reference kernels in test_gpu_envs.py / test_gpu_core.py)."""
+import os
+
 import numpy as np
 import pytest
 import torch
@@ -43,8 +45,30 @@ STATE = ("loc_x", "loc_y", "speed", "direction", "acceleration", "edge_hit_rewar
          "observations", "rewards", "sampled_actions")
 
 
-@pytest.mark.parametrize("full_obs", [False, True])
-def test_fused_step_equals_separate_calls(full_obs):
+def _process_tc_variant():
+    """tc_variant as the library set it when it loaded: from WDB_OPTIONS, else 1."""
+    for item in os.environ.get("WDB_OPTIONS", "").split(","):
+        key, _, val = item.partition("=")
+        if key.strip() == "tc_variant":
+            return int(val)
+    return 1
+
+
+@pytest.fixture
+def tc_variant(request, wdb_lib):
+    """The kernel of a small-env step: 1 = packed, 2 = second-generation (tc_v2_eligible
+    accepts this file's 23-agent, K = 5, partial-observation shape)."""
+    assert wdb_lib.wdb_set_option(b"tc_variant", request.param) == 0
+    try:
+        yield request.param
+    finally:
+        wdb_lib.wdb_set_option(b"tc_variant", _process_tc_variant())
+
+
+@pytest.mark.parametrize("full_obs, tc_variant", [
+    pytest.param(False, 1, id="False"), pytest.param(True, 1, id="True"),
+    pytest.param(False, 2, id="False-v2")], indirect=["tc_variant"])
+def test_fused_step_equals_separate_calls(full_obs, tc_variant):
     from warp_drive_b200.training.fused_tag_continuous import FusedTagContinuousStep
 
     E, T = 10, 4
@@ -141,6 +165,11 @@ def test_fused_step_without_reset_keeps_done_set():
     assert int(dm.data_on_device_via_torch("_done_").sum()) == 0
     assert torch.equal(dm.data_on_device_via_torch("loc_x"),
                        dm.data_on_device_via_torch("loc_x_at_reset"))
+
+
+@pytest.mark.parametrize("tc_variant", [2], ids=["v2"], indirect=True)
+def test_fused_step_without_reset_keeps_done_set_second_generation(tc_variant):
+    test_fused_step_without_reset_keeps_done_set()
 
 
 def _engine(E, T, use_graph, fused, seed=3, env_kw=None, **engine_kw):

@@ -177,7 +177,7 @@ def test_wide_reference_multiblock_shape(wdb_lib, tc_history):  # noqa: F811
 # ---------------------------------------------------------------- fused rollout step, clusters
 @pytest.mark.parametrize("full_obs", [False, True])
 def test_wide_fused_step_equals_separate_calls(full_obs, bpe):
-    roll.test_fused_step_equals_separate_calls(full_obs)
+    roll.test_fused_step_equals_separate_calls(full_obs, 1)
 
 
 def test_wide_fused_step_without_reset_keeps_done_set(bpe):

@@ -73,6 +73,20 @@ __device__ __forceinline__ float u32x2_to_normal(uint32_t a, uint32_t b) {
   return sqrtf(-2.0f * logf(u1)) * cosf(6.2831853071795864f * u2);
 }
 
+// Source row of reset descriptor `d` for `env`: the env's own row, or from a reset pool
+// (pool_rows > 0) a draw p of the env's pool stream at pool_off + n_pool and row =
+// int(p * pool_rows) (pool_reset.py:24-27), clamped for the p == 1.0 edge of (0, 1].
+// n_pool counts the pool draws of this reset; it advances for pool descriptors only.
+__device__ __forceinline__ long long reset_src_row(const wdb_reset_desc &d, const RngHeader &h,
+                                                   int env, unsigned long long pool_off,
+                                                   int &n_pool) {
+  if (d.pool_rows <= 0) return env;
+  const float p = u32_to_uniform(rng_draw4(h, (unsigned long long)env, pool_off + n_pool).x);
+  const long long row = (long long)(p * (float)d.pool_rows);
+  n_pool++;
+  return row < d.pool_rows ? row : d.pool_rows - 1;
+}
+
 __device__ __forceinline__ unsigned long long *rng_offsets(void *rng_state) {
   return reinterpret_cast<unsigned long long *>(
       reinterpret_cast<char *>(rng_state) + sizeof(RngHeader));

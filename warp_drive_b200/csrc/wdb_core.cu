@@ -200,16 +200,8 @@ reset_when_done_kernel(const wdb_reset_desc *__restrict__ table, int n_arrays,
     const long long words = d.bytes_per_env >> 2;
     uint32_t *dst = reinterpret_cast<uint32_t *>(
         reinterpret_cast<char *>(d.dst) + (long long)env * d.bytes_per_env);
-    long long src_row = env;
-    if (d.pool_rows > 0) {
-      // pool_reset.py:24-27 : p ~ U, ref_id = int(p * pool_size); every thread of the
-      // env derives the same draw from the counter-based stream
-      float p = u32_to_uniform(rng_draw4(h, (unsigned long long)env, pool_off + n_pool).x);
-      long long row = (long long)(p * (float)d.pool_rows);
-      if (row >= d.pool_rows) row = d.pool_rows - 1;  // p == 1.0 edge of (0,1]
-      src_row = row;
-      n_pool++;
-    }
+    // every thread of the env derives the same pool draw from the counter-based stream
+    const long long src_row = reset_src_row(d, h, env, pool_off, n_pool);
     const uint32_t *src = reinterpret_cast<const uint32_t *>(
         reinterpret_cast<const char *>(d.ref) + src_row * d.bytes_per_env);
     const long long begin = (long long)blockIdx.y * blockDim.x + threadIdx.x;

@@ -264,15 +264,7 @@ sa_rollout_kernel(const __grid_constant__ wdb_sa_rollout R) {
         for (int arr = 0; arr < R.n_reset_arrays; arr++) {
           const wdb_reset_desc d = R.reset_table[arr];
           const long long words = d.bytes_per_env >> 2;
-          long long src_row = env;
-          if (d.pool_rows > 0) {
-            const float pr = u32_to_uniform(
-                rng_draw4(ph, (unsigned long long)env, pool_off + n_pool).x);
-            long long row = (long long)(pr * (float)d.pool_rows);
-            if (row >= d.pool_rows) row = d.pool_rows - 1;
-            src_row = row;
-            n_pool++;
-          }
+          const long long src_row = reset_src_row(d, ph, env, pool_off, n_pool);
           uint32_t *dst = reinterpret_cast<uint32_t *>(
               reinterpret_cast<char *>(d.dst) + (long long)env * d.bytes_per_env);
           const uint32_t *src = reinterpret_cast<const uint32_t *>(

@@ -868,54 +868,14 @@ tag_continuous_kernel(const __grid_constant__ TcParams P, const __grid_constant_
     done_now = (t_env == P.episode_length || nr == 0) ? 1 : 0;   // :341-348
     if (a == 0) {
       P.num_runners[env] = nr;
-      if (FUSED) {
-        // done is sticky in the reference (only the reset kernel clears it)
-        const int d = done_now | (done_prev > 0 ? 1 : 0);
-        s_done[le] = d;
-        if (Q.done_batch) Q.done_batch[env] = d;
-        const bool will_reset = d && Q.do_reset;
-        if (!will_reset) { if (d) P.done[env] = 1; }
-        else { P.done[env] = 0; P.timestep[env] = 0; }
-        if (Q.step_running_sum) {
-          const int steps = steps_prev + 1;
-          if (d) {
-            if (Q.episodic_step_sum) atomicAdd(Q.episodic_step_sum, (unsigned long long)steps);
-            if (Q.num_completed) atomicAdd(Q.num_completed, 1ull);
-            Q.step_running_sum[env] = 0;
-          } else {
-            Q.step_running_sum[env] = steps;
-          }
-        }
-      } else if (done_now) {
-        P.done[env] = 1;
-      }
+      if (FUSED) s_done[le] = tc_book_env(P, Q, env, done_now, done_prev, steps_prev);
+      else if (done_now) P.done[env] = 1;
     }
   }
-  if (FUSED) {
-    if (active) {
-      const int pol = my_pol;
-      // done is sticky in the reference; every thread derives it (no barrier: s_done is only
-      // for the reset phase, which synchronises first)
-      const int d = done_now | (done_prev > 0 ? 1 : 0);
-#pragma unroll
-      for (int p = 0; p < kMaxPolicies; p++) {
-        if (p == pol) {
-          const long long pi = pi_slot;
-          if (Q.rewards_batch[p]) Q.rewards_batch[p][pi] = r;
-          if (Q.reward_running_sum[p]) {
-            const float run = run_prev + r;
-            if (d) {
-              // one atomic per agent of a finished env (rare: once per episode)
-              if (Q.episodic_reward_sum[p]) atomicAdd(Q.episodic_reward_sum[p], run);
-              Q.reward_running_sum[p][pi] = 0.0f;
-            } else {
-              Q.reward_running_sum[p][pi] = run;
-            }
-          }
-        }
-      }
-    }
-  }
+  // every thread derives its env's done flag (no barrier: s_done is only for the reset phase,
+  // which synchronises first)
+  if (FUSED && active)
+    tc_book_agent(Q, my_pol, pi_slot, r, run_prev, tc_sticky_done(done_now, done_prev));
 
   if (!P.use_full_obs && P.stage_obs) {
     // coalesced copy-out of the observation tile
@@ -957,45 +917,10 @@ tag_continuous_kernel(const __grid_constant__ TcParams P, const __grid_constant_
   WDB_MARK(16)  // TMA stores complete
 
   if (FUSED && Q.do_reset) {
-    // done-masked reset of this CTA's envs (core/reset.cu:9-75 for every registered array
-    // + undo of done/timestep, already applied above)
+    // done-masked reset of this CTA's envs (done / timestep already cleared above)
     __syncthreads();   // all global writes of this step by this CTA are issued
-    for (int e = 0; e < envs_here; e++) {
-      if (!s_done[e]) continue;
-      const int renv = env0 + e;
-      for (int arr = 0; arr < Q.n_reset; arr++) {
-        const wdb_reset_desc d = Q.reset_table[arr];
-        const long long words = d.bytes_per_env >> 2;
-        uint32_t *dst = reinterpret_cast<uint32_t *>(
-            reinterpret_cast<char *>(d.dst) + (long long)renv * d.bytes_per_env);
-        const uint32_t *src = reinterpret_cast<const uint32_t *>(
-            reinterpret_cast<const char *>(d.ref) + (long long)renv * d.bytes_per_env);
-        for (long long i = tid; i < words; i += blockDim.x) dst[i] = src[i];
-      }
-      if (Q.obs_at_reset) {
-        const float *src = Q.obs_at_reset + (long long)renv * N * F;
-        for (int row = warp; row < N; row += nwarps) {
-          const int pol = Q.agent_policy[row];
-          float *dst = nullptr;
-#pragma unroll
-          for (int p = 0; p < kMaxPolicies; p++)
-            if (p == pol && Q.obs_next[p])
-              dst = Q.obs_next[p] + ((long long)renv * Q.policy_size[p] + Q.agent_slot[row]) * F;
-          if (dst)
-            for (int f = lane; f < F; f += kWarp) dst[f] = src[(long long)row * F + f];
-#pragma unroll
-          for (int p = 0; p < kMaxPolicies; p++) {
-            if (p == pol && Q.obs_tiles[p]) {
-              const int K1 = (F + 15) & ~15;
-              if (lane < K1 / 8)
-                store_obs_chunk(Q.obs_tiles[p],
-                                (long long)renv * Q.policy_size[p] + Q.agent_slot[row], lane, K1,
-                                src + (long long)row * F, F);
-            }
-          }
-        }
-      }
-    }
+    for (int e = 0; e < envs_here; e++)
+      if (s_done[e]) tc_reset_env<true>(Q, env0 + e, N, F, tid, blockDim.x, warp, nwarps, lane);
   }
   WDB_MARK(17)  // reset done
 }

@@ -333,6 +333,100 @@ __device__ __noinline__ void store_obs_chunk(unsigned char *tiles, long long gro
                              (r & 7) * 16) = o;
 }
 
+// ---- end of a fused step, shared by the packed, second-generation and cluster kernels:
+// episodic bookkeeping (trainer_base.py:514-601) and the done-masked reset.  No
+// synchronisation in here: the kernels order these against the rest of the step.
+
+// done is sticky in the reference (only the reset kernel clears it)
+__device__ __forceinline__ int tc_sticky_done(int done_now, int done_prev) {
+  return done_now | (done_prev > 0 ? 1 : 0);
+}
+
+// Per env, by the one thread that owns it; `done_prev` / `steps_prev` are done[env] and
+// step_running_sum[env] as loaded before the step.  An env that resets in this launch gets
+// done / timestep cleared here (core/reset.cu:65-75).  Returns the env's done flag.
+__device__ __forceinline__ int tc_book_env(const TcParams &P, const FusedParams &Q, int env,
+                                           int done_now, int done_prev, int steps_prev) {
+  const int d = tc_sticky_done(done_now, done_prev);
+  if (Q.done_batch) Q.done_batch[env] = d;
+  const bool will_reset = d && Q.do_reset;
+  if (!will_reset) { if (d) P.done[env] = 1; }
+  else { P.done[env] = 0; P.timestep[env] = 0; }
+  if (Q.step_running_sum) {
+    const int steps = steps_prev + 1;
+    if (d) {
+      if (Q.episodic_step_sum) atomicAdd(Q.episodic_step_sum, (unsigned long long)steps);
+      if (Q.num_completed) atomicAdd(Q.num_completed, 1ull);
+      Q.step_running_sum[env] = 0;
+    } else {
+      Q.step_running_sum[env] = steps;
+    }
+  }
+  return d;
+}
+
+// Per agent of policy `pol` at row `pi` of its [E, Np] batch arrays, with reward `r` and its
+// env's done flag `d`; `run_prev` is reward_running_sum[pol][pi] as loaded before the step.
+__device__ __forceinline__ void tc_book_agent(const FusedParams &Q, int pol, long long pi,
+                                              float r, float run_prev, int d) {
+#pragma unroll
+  for (int p = 0; p < kMaxPolicies; p++) {
+    if (p == pol) {
+      if (Q.rewards_batch[p]) Q.rewards_batch[p][pi] = r;
+      if (Q.reward_running_sum[p]) {
+        const float run = run_prev + r;
+        if (d) {
+          // one atomic per agent of a finished env (rare: once per episode)
+          if (Q.episodic_reward_sum[p]) atomicAdd(Q.episodic_reward_sum[p], run);
+          Q.reward_running_sum[p][pi] = 0.0f;
+        } else {
+          Q.reward_running_sum[p][pi] = run;
+        }
+      }
+    }
+  }
+}
+
+// Done-masked reset of one finished env: every registered array from its reference
+// (core/reset.cu:9-75), words w0, w0 + dw, ...; then the env's obs_at_reset rows into
+// obs_next (and, with TILES, into the bf16 obs tiles), rows r0, r0 + dr, ... one warp each.
+template <bool TILES>
+__device__ __forceinline__ void tc_reset_env(const FusedParams &Q, int env, int N, int F,
+                                             int w0, int dw, int r0, int dr, int lane) {
+  for (int arr = 0; arr < Q.n_reset; arr++) {
+    const wdb_reset_desc d = Q.reset_table[arr];
+    const long long words = d.bytes_per_env >> 2;
+    uint32_t *dst = reinterpret_cast<uint32_t *>(
+        reinterpret_cast<char *>(d.dst) + (long long)env * d.bytes_per_env);
+    const uint32_t *src = reinterpret_cast<const uint32_t *>(
+        reinterpret_cast<const char *>(d.ref) + (long long)env * d.bytes_per_env);
+    for (long long i = w0; i < words; i += dw) dst[i] = src[i];
+  }
+  if (!Q.obs_at_reset) return;
+  const float *src = Q.obs_at_reset + (long long)env * N * F;
+  for (int row = r0; row < N; row += dr) {
+    const int pol = Q.agent_policy[row];
+    float *dst = nullptr;
+#pragma unroll
+    for (int p = 0; p < kMaxPolicies; p++)
+      if (p == pol && Q.obs_next[p])
+        dst = Q.obs_next[p] + ((long long)env * Q.policy_size[p] + Q.agent_slot[row]) * F;
+    if (dst)
+      for (int f = lane; f < F; f += kWarp) dst[f] = src[(long long)row * F + f];
+    if (TILES) {
+#pragma unroll
+      for (int p = 0; p < kMaxPolicies; p++) {
+        if (p == pol && Q.obs_tiles[p]) {
+          const int K1 = (F + 15) & ~15;
+          if (lane < K1 / 8)
+            store_obs_chunk(Q.obs_tiles[p], (long long)env * Q.policy_size[p] + Q.agent_slot[row],
+                            lane, K1, src + (long long)row * F, F);
+        }
+      }
+    }
+  }
+}
+
 // Squared distance with a FIXED operation order (dx * dx rounded, then fused dy * dy + .):
 // the history scan, its threshold tau, the sort keys and the exact
 // check must all see the same float for the same pair of agents.

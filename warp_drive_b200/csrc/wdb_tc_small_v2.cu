@@ -617,45 +617,11 @@ tc_small_v2_kernel(const __grid_constant__ TcParams P, const __grid_constant__ F
     done_now = (t_env == P.episode_length || nr == 0) ? 1 : 0;   // :341-348
     if (a == 0) {
       P.num_runners[env] = nr;
-      if (FUSED) {
-        const int d = done_now | (done_prev > 0 ? 1 : 0);     // done is sticky in the reference
-        s_done[le] = d;
-        if (Q.done_batch) Q.done_batch[env] = d;
-        const bool will_reset = d && Q.do_reset;
-        if (!will_reset) { if (d) P.done[env] = 1; }
-        else { P.done[env] = 0; P.timestep[env] = 0; }
-        if (Q.step_running_sum) {
-          const int steps = steps_prev + 1;
-          if (d) {
-            if (Q.episodic_step_sum) atomicAdd(Q.episodic_step_sum, (unsigned long long)steps);
-            if (Q.num_completed) atomicAdd(Q.num_completed, 1ull);
-            Q.step_running_sum[env] = 0;
-          } else {
-            Q.step_running_sum[env] = steps;
-          }
-        }
-      } else if (done_now) {
-        P.done[env] = 1;
-      }
+      if (FUSED) s_done[le] = tc_book_env(P, Q, env, done_now, done_prev, steps_prev);
+      else if (done_now) P.done[env] = 1;
     }
-    if (FUSED) {
-      const int d = done_now | (done_prev > 0 ? 1 : 0);
-#pragma unroll
-      for (int p = 0; p < kMaxPolicies; p++) {
-        if (p == pol_w) {
-          if (Q.rewards_batch[p]) Q.rewards_batch[p][pi_slot] = r;
-          if (Q.reward_running_sum[p]) {
-            const float run = run_prev + r;
-            if (d) {
-              if (Q.episodic_reward_sum[p]) atomicAdd(Q.episodic_reward_sum[p], run);
-              Q.reward_running_sum[p][pi_slot] = 0.0f;
-            } else {
-              Q.reward_running_sum[p][pi_slot] = run;
-            }
-          }
-        }
-      }
-    }
+    if (FUSED)
+      tc_book_agent(Q, pol_w, pi_slot, r, run_prev, tc_sticky_done(done_now, done_prev));
   }
 
   // ------------------------------------------------------------------ observations (:29-256)
@@ -766,34 +732,10 @@ tc_small_v2_kernel(const __grid_constant__ TcParams P, const __grid_constant__ F
   }
 
   if (FUSED && Q.do_reset) {
-    // done-masked reset of this CTA's envs (core/reset.cu:9-75 for every registered array)
+    // done-masked reset of this CTA's envs (done / timestep already cleared above)
     __syncthreads();   // all global writes of this step by this CTA are issued
-    for (int e = 0; e < envs_here; e++) {
-      if (!s_done[e]) continue;
-      const int renv = env0 + e;
-      for (int arr = 0; arr < Q.n_reset; arr++) {
-        const wdb_reset_desc d = Q.reset_table[arr];
-        const long long words = d.bytes_per_env >> 2;
-        uint32_t *dst = reinterpret_cast<uint32_t *>(
-            reinterpret_cast<char *>(d.dst) + (long long)renv * d.bytes_per_env);
-        const uint32_t *src = reinterpret_cast<const uint32_t *>(
-            reinterpret_cast<const char *>(d.ref) + (long long)renv * d.bytes_per_env);
-        for (long long i = tid; i < words; i += blockDim.x) dst[i] = src[i];
-      }
-      if (Q.obs_at_reset) {
-        const float *src = Q.obs_at_reset + (long long)renv * N * F;
-        for (int row = warp; row < N; row += nwarps) {
-          const int pol = Q.agent_policy[row];
-          float *dst = nullptr;
-#pragma unroll
-          for (int p = 0; p < kMaxPolicies; p++)
-            if (p == pol && Q.obs_next[p])
-              dst = Q.obs_next[p] + ((long long)renv * Q.policy_size[p] + Q.agent_slot[row]) * F;
-          if (dst)
-            for (int f = lane; f < F; f += kWarp) dst[f] = src[(long long)row * F + f];
-        }
-      }
-    }
+    for (int e = 0; e < envs_here; e++)
+      if (s_done[e]) tc_reset_env<false>(Q, env0 + e, N, F, tid, blockDim.x, warp, nwarps, lane);
   }
 }
 

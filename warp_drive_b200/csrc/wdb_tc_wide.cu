@@ -842,80 +842,36 @@ tc_wide_kernel(const __grid_constant__ TcParams P, const __grid_constant__ Fused
   for (int i = 0; i < credits; i++) r += P.tag_reward;      // same float adds as the atomics
   const int nr = g_nrun - exits;
   const int done_now = (t_env == P.episode_length || nr == 0) ? 1 : 0;   // :341-348
-  const int d_env = FUSED ? (done_now | (done_prev > 0 ? 1 : 0)) : done_now;
+  const int d_env = FUSED ? tc_sticky_done(done_now, done_prev) : done_now;
   const bool will_reset = FUSED && d_env && Q.do_reset;
   if (have) P.rewards[gi2] = r;
   if (rank == 0 && tid == 0) {
     P.num_runners[env] = nr;
-    if (!FUSED) {
-      P.timestep[env] = t_env;
-      if (done_now) P.done[env] = 1;
-    } else {
-      if (Q.done_batch) Q.done_batch[env] = d_env;
-      if (!will_reset) { P.timestep[env] = t_env; if (d_env) P.done[env] = 1; }
-      else { P.done[env] = 0; P.timestep[env] = 0; }
-      if (Q.step_running_sum) {
-        const int steps = misc[M_STEPS] + 1;
-        if (d_env) {
-          if (Q.episodic_step_sum) atomicAdd(Q.episodic_step_sum, (unsigned long long)steps);
-          if (Q.num_completed) atomicAdd(Q.num_completed, 1ull);
-          Q.step_running_sum[env] = 0;
-        } else {
-          Q.step_running_sum[env] = steps;
-        }
-      }
-    }
+    if (!will_reset) P.timestep[env] = t_env;
+    if (FUSED) tc_book_env(P, Q, env, done_now, done_prev, misc[M_STEPS]);
+    else if (done_now) P.done[env] = 1;
   }
   if (FUSED && have) {
     const int pol = Q.agent_policy[a2], slot = Q.agent_slot[a2];
+    long long pi = 0;
+    float run_prev = 0.0f;
 #pragma unroll
     for (int p = 0; p < kMaxPolicies; p++) {
       if (p == pol) {
-        const long long pi = (long long)env * Q.policy_size[p] + slot;
-        if (Q.rewards_batch[p]) Q.rewards_batch[p][pi] = r;
-        if (Q.reward_running_sum[p]) {
-          const float run = Q.reward_running_sum[p][pi] + r;
-          if (d_env) {
-            if (Q.episodic_reward_sum[p]) atomicAdd(Q.episodic_reward_sum[p], run);
-            Q.reward_running_sum[p][pi] = 0.0f;
-          } else {
-            Q.reward_running_sum[p][pi] = run;
-          }
-        }
+        pi = (long long)env * Q.policy_size[p] + slot;
+        if (Q.reward_running_sum[p]) run_prev = Q.reward_running_sum[p][pi];
       }
     }
+    tc_book_agent(Q, pol, pi, r, run_prev, d_env);
   }
   // #3: (a) no CTA may exit while a peer still reads its shared memory; (b) the reset below
   // overwrites rows that other CTAs of the env wrote in this step
   cluster_sync_all();
 
-  if (will_reset) {
-    // done-masked reset of this env (core/reset.cu:9-75 for every registered array), the
-    // words dealt over all threads of the cluster
-    const int nthr = C * blockDim.x, me = rank * blockDim.x + tid;
-    for (int arr = 0; arr < Q.n_reset; arr++) {
-      const wdb_reset_desc d = Q.reset_table[arr];
-      const long long words = d.bytes_per_env >> 2;
-      uint32_t *dst = reinterpret_cast<uint32_t *>(
-          reinterpret_cast<char *>(d.dst) + (long long)env * d.bytes_per_env);
-      const uint32_t *src = reinterpret_cast<const uint32_t *>(
-          reinterpret_cast<const char *>(d.ref) + (long long)env * d.bytes_per_env);
-      for (long long i = me; i < words; i += nthr) dst[i] = src[i];
-    }
-    if (Q.obs_at_reset) {
-      const float *src = Q.obs_at_reset + (long long)env * N * F;
-      for (int row = warp * C + rank; row < N; row += nw * C) {
-        const int pol = Q.agent_policy[row];
-        float *dst = nullptr;
-#pragma unroll
-        for (int p = 0; p < kMaxPolicies; p++)
-          if (p == pol && Q.obs_next[p])
-            dst = Q.obs_next[p] + ((long long)env * Q.policy_size[p] + Q.agent_slot[row]) * F;
-        if (dst)
-          for (int f = lane; f < F; f += kWarp) dst[f] = src[(long long)row * F + f];
-      }
-    }
-  }
+  // done-masked reset of this env, the words dealt over all threads of the cluster
+  if (will_reset)
+    tc_reset_env<false>(Q, env, N, F, rank * blockDim.x + tid, C * blockDim.x, warp * C + rank,
+                        nw * C, lane);
 }
 
 int g_tc_wide_window = 1;   // wdb_set_option("tc_wide_window", 0/1)
