@@ -458,6 +458,10 @@ int wdb_heads_softmax_backward(void *stream, const float *probs0, const float *p
                                const float *grad_probs0, const float *grad_probs1,
                                const float *grad_values, long long rows, int A0, int A1,
                                int pitch, float *grad_logits);
+/* 1 if BOTH wdb_heads_softmax and wdb_heads_softmax_backward take heads of A0 / A1 actions at
+ * this logits pitch (the backward stages two row tiles: it takes pitches below 200, the
+ * forward below 400), else 0.  The launches refuse exactly the shapes this refuses. */
+int wdb_heads_softmax_supported(int A0, int A1, int pitch);
 int wdb_pad_rows(void *stream, const float *src, long long rows, int width, int pitch,
                  float *dst /* [rows, pitch], columns >= width zero-filled */);
 int wdb_relu_backward_bias_rows(long long rows);
@@ -486,6 +490,9 @@ typedef struct wdb_pg_loss {
   double *sums;                      /* out [4], accumulated atomically */
 } wdb_pg_loss;
 int wdb_pg_loss_and_grads(void *stream, const wdb_pg_loss *loss);
+/* 1 if wdb_pg_loss_and_grads takes n_heads heads of n_actions[k] actions (1..4 heads, each of
+ * 1..399 actions: one 32-row tile of the widest head per warp), else 0.  No CUDA call. */
+int wdb_pg_loss_supported(int n_heads, const int *n_actions);
 
 /* Gradient-norm clipping + Adam over one flat float32 arena (torch.optim.Adam semantics, no
  * weight decay; torch.nn.utils.clip_grad_norm_ semantics for the clip factor, which the Adam

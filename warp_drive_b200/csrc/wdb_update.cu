@@ -115,7 +115,9 @@ pg_loss_kernel(const __grid_constant__ wdb_pg_loss L, int tile_pitch) {
           float *p = tile + lane * tile_pitch;                 // this lane's row, overwritten by
           const int a = L.actions[idx * L.n_heads + k];        // its gradient in pass 2
           // torch.distributions.Categorical(probs=p): probs / sum, logits = log(clamp(probs,
-          // eps, 1 - eps)); log_prob = logits[a]; entropy = -sum(logits * probs)
+          // eps, 1 - eps)); log_prob = logits[a]; entropy = -sum(logits * probs).  torch.clamp's
+          // backward passes the gradient for eps <= q <= 1 - eps, both ends inclusive: a
+          // near-deterministic float32 row holds q == 1 - eps exactly
           float z = 0.0f;
           for (int j = 0; j < A; j++) z += p[j];
           const float inv_z = 1.0f / z;
@@ -123,7 +125,7 @@ pg_loss_kernel(const __grid_constant__ wdb_pg_loss L, int tile_pitch) {
           float ent = 0.0f, S = 0.0f;
           for (int j = 0; j < A; j++) {
             const float q = p[j] * inv_z;
-            const bool inside = q > kProbEps && q < 1.0f - kProbEps;
+            const bool inside = q >= kProbEps && q <= 1.0f - kProbEps;
             const float lq = logf(fminf(fmaxf(q, kProbEps), 1.0f - kProbEps));
             ent -= lq * q;
             float gq = L.entropy_coeff * (lq + (inside ? 1.0f : 0.0f));   // -c_ent * dH/dq_j
@@ -137,7 +139,7 @@ pg_loss_kernel(const __grid_constant__ wdb_pg_loss L, int tile_pitch) {
           if (L.grad_probs[k]) {
             for (int j = 0; j < A; j++) {
               const float q = p[j] * inv_z;
-              const bool inside = q > kProbEps && q < 1.0f - kProbEps;
+              const bool inside = q >= kProbEps && q <= 1.0f - kProbEps;
               const float lq = logf(fminf(fmaxf(q, kProbEps), 1.0f - kProbEps));
               float gq = L.entropy_coeff * (lq + (inside ? 1.0f : 0.0f));
               if (j == a && inside) gq -= adv / q;
@@ -390,20 +392,55 @@ pad_rows_kernel(const float *__restrict__ src, long long rows, int width, int pi
 
 }  // namespace
 
+namespace {
+
+constexpr size_t kRowSmemLimit = 200 * 1024;   // dynamic shared memory the row-tile kernels opt into
+
+// shared memory of pg_loss_kernel: one 32-row tile per warp of the widest head (odd pitch);
+// 0 for a head set the kernel does not take
+size_t pg_loss_smem(int n_heads, const int *n_actions, int *tile_pitch) {
+  if (n_heads < 1 || n_heads > 4 || !n_actions) return 0;
+  int amax = 1;
+  for (int k = 0; k < n_heads; k++) {
+    if (n_actions[k] < 1) return 0;
+    amax = n_actions[k] > amax ? n_actions[k] : amax;
+  }
+  const int pitch = amax | 1;                                   // odd: no bank conflicts
+  const size_t smem = (size_t)(kPgThreads / 32) * 32 * pitch * sizeof(float);
+  if (smem > kRowSmemLimit) return 0;
+  if (tile_pitch) *tile_pitch = pitch;
+  return smem;
+}
+
+// shared memory of the heads softmax forward (tiles == 1) / backward (tiles == 2) at a logits
+// pitch; 0 for a shape the kernel does not take
+size_t heads_softmax_smem(int A0, int A1, int pitch, int tiles) {
+  if (A0 < 1 || A1 < 0 || pitch < A0 + A1 + 1) return 0;
+  const size_t smem = (size_t)(kRowThreads / 32) * 32 * tiles * (pitch | 1) * sizeof(float);
+  return smem > kRowSmemLimit ? 0 : smem;
+}
+
+}  // namespace
+
+WDB_API int wdb_pg_loss_supported(int n_heads, const int *n_actions) {
+  return pg_loss_smem(n_heads, n_actions, nullptr) > 0;
+}
+
+WDB_API int wdb_heads_softmax_supported(int A0, int A1, int pitch) {
+  return heads_softmax_smem(A0, A1, pitch, 1) > 0 && heads_softmax_smem(A0, A1, pitch, 2) > 0;
+}
+
 WDB_API int wdb_pg_loss_and_grads(void *stream, const wdb_pg_loss *l) {
-  if (!l || l->T < 1 || l->n_envs < 1 || l->n_agents < 1 || l->n_heads < 1 || l->n_heads > 4)
-    return (int)cudaErrorInvalidValue;
+  if (!l || l->T < 1 || l->n_envs < 1 || l->n_agents < 1) return (int)cudaErrorInvalidValue;
+  int pitch = 0;
+  const size_t smem = pg_loss_smem(l->n_heads, l->n_actions, &pitch);
+  if (!smem) return (int)cudaErrorInvalidValue;
   if (!l->values || !l->actions || !l->rewards || !l->done || !l->sums)
     return (int)cudaErrorInvalidValue;
   for (int k = 0; k < l->n_heads; k++)
-    if (!l->probs[k] || l->n_actions[k] < 1) return (int)cudaErrorInvalidValue;
+    if (!l->probs[k]) return (int)cudaErrorInvalidValue;
   const long long n = (long long)l->n_envs * l->n_agents;
   const int grid = (int)((n + kPgThreads - 1) / kPgThreads);
-  int amax = 1;
-  for (int k = 0; k < l->n_heads; k++) amax = l->n_actions[k] > amax ? l->n_actions[k] : amax;
-  const int pitch = amax | 1;                                   // odd: no bank conflicts
-  const size_t smem = (size_t)(kPgThreads / 32) * 32 * pitch * sizeof(float);
-  if (smem > 200 * 1024) return (int)cudaErrorInvalidValue;
   static size_t configured = 48 * 1024;
   if (smem > configured) {
     cudaError_t e = cudaFuncSetAttribute(pg_loss_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -440,12 +477,10 @@ WDB_API int wdb_adam_step(void *stream, float *params, float *grads, float *exp_
 
 WDB_API int wdb_heads_softmax(void *stream, const float *logits, long long rows, int A0, int A1,
                               int pitch, float *probs0, float *probs1, float *values) {
-  if (!logits || !probs0 || !values || rows < 1 || A0 < 1 || A1 < 0 || (A1 > 0 && !probs1) ||
-      pitch < A0 + A1 + 1)
+  const size_t smem = heads_softmax_smem(A0, A1, pitch, 1);
+  if (!logits || !probs0 || !values || rows < 1 || !smem || (A1 > 0 && !probs1))
     return (int)cudaErrorInvalidValue;
   const int tp = pitch | 1;
-  const size_t smem = (size_t)(kRowThreads / 32) * 32 * tp * sizeof(float);
-  if (smem > 200 * 1024) return (int)cudaErrorInvalidValue;
   {
     static size_t configured = 48 * 1024;
     if (smem > configured) {
@@ -465,12 +500,10 @@ WDB_API int wdb_heads_softmax_backward(void *stream, const float *probs0, const 
                                        const float *grad_probs0, const float *grad_probs1,
                                        const float *grad_values, long long rows, int A0, int A1,
                                        int pitch, float *grad_logits) {
-  if (!probs0 || !grad_logits || rows < 1 || A0 < 1 || A1 < 0 || (A1 > 0 && !probs1) ||
-      pitch < A0 + A1 + 1)
+  const size_t smem = heads_softmax_smem(A0, A1, pitch, 2);
+  if (!probs0 || !grad_logits || rows < 1 || !smem || (A1 > 0 && !probs1))
     return (int)cudaErrorInvalidValue;
   const int tp = pitch | 1;
-  const size_t smem = (size_t)(kRowThreads / 32) * 64 * tp * sizeof(float);
-  if (smem > 200 * 1024) return (int)cudaErrorInvalidValue;
   {
     static size_t configured = 48 * 1024;
     if (smem > configured) {

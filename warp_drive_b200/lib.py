@@ -191,8 +191,10 @@ _SIGNATURES = {
     "wdb_mlp_policy_forward_tiles": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _ll, _vp, _vp, _vp]),
     "wdb_discounted_returns": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f]),
     "wdb_pg_loss_and_grads": (_i, [_vp, ctypes.POINTER(PgLoss)]),
+    "wdb_pg_loss_supported": (_i, [_i, ctypes.POINTER(_i)]),
     "wdb_heads_softmax": (_i, [_vp, _vp, _ll, _i, _i, _i, _vp, _vp, _vp]),
     "wdb_heads_softmax_backward": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _ll, _i, _i, _i, _vp]),
+    "wdb_heads_softmax_supported": (_i, [_i, _i, _i]),
     "wdb_pad_rows": (_i, [_vp, _vp, _ll, _i, _i, _vp]),
     "wdb_relu_backward_bias_rows": (_i, [_ll]),
     "wdb_relu_backward_bias": (_i, [_vp, _vp, _vp, _ll, _i, _vp]),

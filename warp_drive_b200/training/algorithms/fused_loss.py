@@ -59,6 +59,13 @@ class _FusedPGLoss(torch.autograd.Function):
                 *[g * grad_loss for g in g_probs])
 
 
+def fused_pg_loss_supported(probs):
+    """True if `wdb_pg_loss_and_grads` takes these heads (the library's own launch check)."""
+    widths = [int(p.shape[-1]) for p in probs]
+    arr = (ctypes.c_int * max(1, len(widths)))(*widths)
+    return bool(_lib.load().wdb_pg_loss_supported(len(widths), arr))
+
+
 def fused_pg_loss(values, probs, actions, rewards, done, gamma, vf_coeff, entropy_coeff,
                   ppo=False, want_returns=False):
     """values [T,E,Np] (requires grad), probs: list of [T,E,Np,A_k] (require grad), actions

@@ -11,6 +11,7 @@ import torch
 from torch import nn
 from torch.distributions import Categorical
 
+from warp_drive_b200.training.algorithms.fused_loss import fused_pg_loss, fused_pg_loss_supported
 from warp_drive_b200.training.utils.param_scheduler import ParamScheduler
 
 _EPSILON = 1e-10
@@ -83,7 +84,8 @@ class _PolicyGradient:
                 action_probabilities_batch = [p[:, keep] for p in action_probabilities_batch]
                 value_functions_batch = value_functions_batch[:, keep]
         if (self.use_fused_loss and value_functions_batch.is_cuda and n_pos is None
-                and not self.normalize_return and not self.normalize_advantage):
+                and not self.normalize_return and not self.normalize_advantage
+                and fused_pg_loss_supported(action_probabilities_batch)):
             return self._fused_loss_and_metrics(
                 timestep, actions_batch, rewards_batch, done_flags_batch,
                 action_probabilities_batch, value_functions_batch, perform_logging)
@@ -135,8 +137,6 @@ class _PolicyGradient:
     def _fused_loss_and_metrics(self, timestep, actions_batch, rewards_batch, done_flags_batch,
                                 action_probabilities_batch, value_functions_batch,
                                 perform_logging):
-        from warp_drive_b200.training.algorithms.fused_loss import fused_pg_loss
-
         vf_c = self.vf_loss_coeff_schedule.get_param_value(timestep)
         ent_c = self.entropy_coeff_schedule.get_param_value(timestep)
         loss, parts, returns = fused_pg_loss(

@@ -65,7 +65,7 @@ class _FusedMLPTrain(torch.autograd.Function):
         h1 = torch._addmm_activation(b1, obs, w1.t(), use_gelu=False)
         h2 = torch._addmm_activation(b2, h1, w2.t(), use_gelu=False)
         a = a0 + a1 + 1
-        ap = -(-a // 4) * 4
+        ap = _head_pitch(a0, a1)
         heads = [wh0] + ([wh1] if a1 else []) + [wv]
         biases = [bh0] + ([bh1] if a1 else []) + [bv]
         if ap != a:
@@ -116,13 +116,23 @@ class _FusedMLPTrain(torch.autograd.Function):
         return None, dw1, db1, dw2, db2, dwh0, dbh0, dwh1, dbh1, dwv, dbv
 
 
+def _head_pitch(a0, a1):
+    """Row pitch of the head GEMM's logits: both heads and the value column, padded to 4."""
+    return -(-(a0 + a1 + 1) // 4) * 4
+
+
 def supported(model, obs):
-    """Two hidden layers, one or two softmax heads, no action mask, float32 CUDA tensors."""
+    """Two hidden layers, one or two softmax heads that both softmax kernels take (the
+    library's own launch check), no action mask, float32 CUDA tensors."""
     if getattr(model, "is_deterministic", True) or len(model.fc) != 2:
         return False
     if len(model.output_dims) not in (1, 2) or getattr(model, "action_mask", None) is not None:
         return False
     if not obs.is_cuda or obs.dtype != torch.float32 or obs.requires_grad:
+        return False
+    a0 = int(model.output_dims[0])
+    a1 = int(model.output_dims[1]) if len(model.output_dims) == 2 else 0
+    if not _lib.load().wdb_heads_softmax_supported(a0, a1, _head_pitch(a0, a1)):
         return False
     return all(p.is_cuda and p.dtype == torch.float32 for p in model.parameters())
 
