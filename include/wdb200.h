@@ -503,6 +503,49 @@ int wdb_adam_step(void *stream, float *params, float *grads, float *exp_avg, flo
                   long long n, float lr, float beta1, float beta2, float eps, int step,
                   float max_grad_norm /* <= 0: no clipping */, const double *grad_sumsq);
 
+/* Every gradient of one DDPG update of one policy (trainer_ddpg.py:380-420,
+ * algorithms/ddpg.py:62-120 of the reference) read in place from the replay ring: logical slot
+ * k is physical slot (cursor + k) mod capacity, k = 0 the oldest.  With valid = capacity -
+ * n_step + 1 and M = valid * E * Np loss rows:
+ *   critic_loss = mean over the loss rows of (Q(obs, actions) - R)^2,
+ *   actor_loss  = -mean of J = Q(obs, actor(obs)),
+ *   R = the n-step return bootstrapped with target_critic(obs', target_actor(obs')) at slot
+ *       i + n_step (the last window: slot capacity - 1, undiscounted, ddpg.py:68-73),
+ * the actor gradient = d actor_loss, the critic gradient = d critic_loss + d actor_loss (the
+ * reference's actor_loss.backward() also reaches the critic).  Networks: hidden Linear + ReLU
+ * layers, then the head (the critic's input is obs ++ action; the actor's output is
+ * action_scale * tanh(z) + action_bias).  Float32 FMA; the per-CTA partial gradients are
+ * summed in a fixed order by a second kernel that writes them to gw / gb: no float atomics,
+ * bit-reproducible.  Two launches. */
+typedef struct wdb_ddpg_net {
+  int n_hidden;                      /* 0..3 */
+  int widths[3];                     /* hidden widths (1..64) */
+  const float *w[4], *b[4];          /* nn.Linear weights [out, in] and biases, hidden then head */
+  float *gw[4], *gb[4];              /* gradients, same shapes (actor / critic; NULL for targets) */
+} wdb_ddpg_net;
+typedef struct wdb_ddpg_update_args {
+  int n_envs, n_agents, obs_dim, action_dim;   /* E, Np, F, A */
+  int capacity, cursor, n_step;      /* ring slots C, oldest slot, n-step horizon (1..C) */
+  float gamma, action_scale, action_bias;
+  const float *obs;                  /* [C, E, Np, F] */
+  const float *actions;              /* [C, E, Np, A] */
+  const float *rewards;              /* [C, E, Np] */
+  const int *done;                   /* [C, E] */
+  wdb_ddpg_net actor, critic, target_actor, target_critic;   /* targets: the online shapes */
+  float *values, *j_values, *returns;  /* out [valid, E * Np] in logical slot order, or NULL */
+  double *sums;                      /* out [2]: sum (Q - R)^2, sum J over the loss rows */
+  void *workspace;                   /* wdb_ddpg_update_workspace_bytes() bytes */
+} wdb_ddpg_update_args;
+/* 1 if the shapes are supported: 0..3 hidden layers of width 1..64 per network, F + A <= 64,
+ * targets shaped as the online networks, E, Np >= 1, 1 <= n_step <= capacity, capacity >= 2
+ * (the last window's bootstrap value is the target critic at slot capacity - 1), cursor in
+ * [0, capacity), and all four networks' weights, the gradient accumulators and a row tile fit
+ * one CTA's shared memory (227 KB).  No CUDA call. */
+int wdb_ddpg_update_supported(const wdb_ddpg_update_args *update);
+long long wdb_ddpg_update_workspace_bytes(const wdb_ddpg_update_args *update);  /* -1: unsupported */
+/* cudaErrorInvalidValue without launching if unsupported or a required pointer is NULL. */
+int wdb_ddpg_update(void *stream, const wdb_ddpg_update_args *update);
+
 #ifdef __cplusplus
 }
 #endif

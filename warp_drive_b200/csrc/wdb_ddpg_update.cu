@@ -1,0 +1,498 @@
+// wdb_ddpg_update.cu -- every gradient of one DDPG update of one policy in one launch, read in
+// place from the replay ring, plus a fixed-order reduction of the per-CTA partials into the
+// gradient arena (include/wdb200.h, wdb_ddpg_update).
+//
+// Replaces TrainerDDPG._update_model_params' torch autograd body (trainer_ddpg.py:380-420 of
+// the reference): five MLP forwards over the whole unrolled ring, the n-step returns
+// (ddpg.py:62-79), both losses and two backward passes -- over a hundred small launches.
+//
+// Per tile of kRows loss rows (row g = logical slot i * E * Np + agent row n), in shared
+// memory and in this order:
+//   target actor, target critic on obs at slot i + n_step (the last window: capacity - 1)
+//   -> the bootstrap value; critic on (obs, actions) -> Q; actor on obs -> pi; critic on
+//   (obs, pi) -> J; n-step return R; dL/dQ = 2 (Q - R) / M, dL/dJ = -1 / M; back through the
+//   critic on both paths (the reference's actor_loss.backward() also reaches the critic), the
+//   J path on to the action inputs, the tanh head and the actor.
+// The weight gradients of a tile are added to per-CTA accumulators in shared memory; each CTA
+// writes them once as its partial, and the second kernel sums the partials in CTA order.  No
+// float atomics: an update is bit-reproducible.
+//
+// Why no tensor cores: the reasons of wdb_sa_rollout.cu -- the networks are tiny (3 or 4 ->
+// 64 -> 64 -> 1), all four fit shared memory, and the torch reference is float32 (TF32 off).
+//
+// Thread layout (256 threads, 16-row tiles): forward and input-gradient steps give each
+// thread one output column and four rows (one float4 weight load feeds sixteen FMAs);
+// weight-gradient steps give each thread one input column and sixteen output rows.
+#include "wdb_common.cuh"
+
+using namespace wdb;
+
+namespace {
+
+constexpr int kThreads = 256;
+constexpr int kRows = 16;                     // loss rows per tile
+constexpr int kPitch = 68;                    // activation row pitch: float4 rows
+constexpr int kTile = kRows * kPitch;         // floats of one activation buffer
+constexpr int kMaxWidth = 64;
+constexpr long long kMaxDynSmem = 227 * 1024 - 1024;   // the rest: the static Plan copy
+
+struct Plan {
+  int L[2];                // Linear layers (hidden + head): actor (0), critic (1)
+  int in[2][4], out[2][4];
+  int pw[2][4];            // smem pitch of a weight row: multiple of 4, = 4 mod 8
+  int woff[2][4];          // W of layer l in the net's smem block; the bias follows W
+  int wfloats[2];
+  int goff[2][4];          // W gradient of layer l in the packed gradients; the bias follows
+  int gfloats[2];          // actor's, critic's (the critic's start at gfloats[0])
+  int n_buf;               // activation buffers
+  int valid, grid;
+  long long EN, M;
+  long long smem_floats;
+};
+
+bool make_plan(const wdb_ddpg_update_args *u, Plan *p) {
+  if (!u) return false;
+  const int F = u->obs_dim, A = u->action_dim;
+  if (u->n_envs < 1 || u->n_agents < 1 || F < 1 || A < 1 || F + A > kMaxWidth) return false;
+  if (u->n_step < 1 || u->capacity < 2 || u->capacity < u->n_step || u->cursor < 0 || u->cursor >= u->capacity)
+    return false;
+  const wdb_ddpg_net *nets[2] = {&u->actor, &u->critic};
+  const wdb_ddpg_net *targets[2] = {&u->target_actor, &u->target_critic};
+  for (int k = 0; k < 2; k++) {
+    const wdb_ddpg_net &n = *nets[k], &t = *targets[k];
+    if (n.n_hidden < 0 || n.n_hidden > 3 || t.n_hidden != n.n_hidden) return false;
+    int prev = k == 0 ? F : F + A, woff = 0, goff = 0;
+    p->L[k] = n.n_hidden + 1;
+    for (int l = 0; l <= n.n_hidden; l++) {
+      const int out = l < n.n_hidden ? n.widths[l] : (k == 0 ? A : 1);
+      if (l < n.n_hidden && (out < 1 || out > kMaxWidth || t.widths[l] != out)) return false;
+      int pw = round_up(prev, 4);
+      if (pw % 8 == 0) pw += 4;               // float4 rows of 8 lanes hit distinct banks
+      p->in[k][l] = prev;
+      p->out[k][l] = out;
+      p->pw[k][l] = pw;
+      p->woff[k][l] = woff;
+      woff += round_up(out * pw + out, 4);
+      p->goff[k][l] = goff;
+      goff += out * prev + out;
+      prev = out;
+    }
+    p->wfloats[k] = woff;
+    p->gfloats[k] = goff;
+  }
+  p->valid = u->capacity - u->n_step + 1;
+  p->EN = (long long)u->n_envs * u->n_agents;
+  p->M = p->valid * p->EN;
+  if (p->M > (1ll << 31)) return false;
+  p->n_buf = 6 + 2 * (p->L[1] - 1) + (p->L[0] - 1);
+  p->smem_floats = 2ll * (p->wfloats[0] + p->wfloats[1]) +
+                   round_up(p->gfloats[0] + p->gfloats[1], 4) + (long long)p->n_buf * kTile;
+  if (p->smem_floats * 4 > kMaxDynSmem) return false;
+  const long long tiles = (p->M + kRows - 1) / kRows;
+  p->grid = (int)(tiles < kNumSMs ? tiles : kNumSMs);
+  return true;
+}
+
+__device__ __forceinline__ float4 ld4(const float *p) {
+  return *reinterpret_cast<const float4 *>(p);
+}
+
+// Y[r][j] = act(b[j] + sum_i W[j][i] X[r][i]) for the tile's rows; thread: column j, rows
+// r0, r0 + 4, r0 + 8, r0 + 12.  Every sum runs i = 0, 1, 2, ... in order.
+__device__ __forceinline__ void layer_forward(const float *W, int pw, int in, int out,
+                                              const float *X, float *Y, bool relu) {
+  const int j = threadIdx.x & 63, r0 = threadIdx.x >> 6;
+  if (j >= out) return;
+  const float *w = W + j * pw;
+  float a[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+  int i = 0;
+  for (; i + 4 <= in; i += 4) {
+    const float4 wv = ld4(w + i);
+#pragma unroll
+    for (int m = 0; m < 4; m++) {
+      const float4 x = ld4(X + (r0 + 4 * m) * kPitch + i);
+      a[m] = fmaf(wv.x, x.x, a[m]);
+      a[m] = fmaf(wv.y, x.y, a[m]);
+      a[m] = fmaf(wv.z, x.z, a[m]);
+      a[m] = fmaf(wv.w, x.w, a[m]);
+    }
+  }
+  for (; i < in; i++) {
+    const float wv = w[i];
+#pragma unroll
+    for (int m = 0; m < 4; m++) a[m] = fmaf(wv, X[(r0 + 4 * m) * kPitch + i], a[m]);
+  }
+  const float bj = W[out * pw + j];
+#pragma unroll
+  for (int m = 0; m < 4; m++) {
+    const float y = a[m] + bj;
+    Y[(r0 + 4 * m) * kPitch + j] = relu ? fmaxf(y, 0.0f) : y;
+  }
+}
+
+// DX[r][i] = sum_j W[j][i] D[r][j] for columns i in [i_lo, in), zeroed where mask[r][i] <= 0
+// (ReLU backward; mask = the layer's input, a ReLU output) unless mask is NULL.
+__device__ __forceinline__ void layer_backward(const float *W, int pw, int in, int out,
+                                               const float *D, float *DX, const float *mask,
+                                               int i_lo) {
+  const int i = threadIdx.x & 63, r0 = threadIdx.x >> 6;
+  if (i < i_lo || i >= in) return;
+  float a[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+  int j = 0;
+  for (; j + 4 <= out; j += 4) {
+    const float w0 = W[j * pw + i], w1 = W[(j + 1) * pw + i], w2 = W[(j + 2) * pw + i],
+                w3 = W[(j + 3) * pw + i];
+#pragma unroll
+    for (int m = 0; m < 4; m++) {
+      const float4 d = ld4(D + (r0 + 4 * m) * kPitch + j);
+      a[m] = fmaf(w0, d.x, a[m]);
+      a[m] = fmaf(w1, d.y, a[m]);
+      a[m] = fmaf(w2, d.z, a[m]);
+      a[m] = fmaf(w3, d.w, a[m]);
+    }
+  }
+  for (; j < out; j++) {
+    const float wv = W[j * pw + i];
+#pragma unroll
+    for (int m = 0; m < 4; m++) a[m] = fmaf(wv, D[(r0 + 4 * m) * kPitch + j], a[m]);
+  }
+#pragma unroll
+  for (int m = 0; m < 4; m++) {
+    const int at = (r0 + 4 * m) * kPitch + i;
+    DX[at] = (mask && !(mask[at] > 0.0f)) ? 0.0f : a[m];
+  }
+}
+
+// G[j][i] += sum_r D[r][j] X[r][i], G[out * in + j] += sum_r D[r][j] (the tile's rows in
+// order).  Thread: column i, rows j0 .. j0 + 15 of G.  D rows are read 16 columns at a time;
+// columns past `out` are in the row and never stored.
+__device__ __forceinline__ void layer_grad(float *G, int in, int out, const float *D,
+                                           const float *X) {
+  const int i = threadIdx.x & 63, j0 = (threadIdx.x >> 6) * 16;
+  if (i < in && j0 < out) {
+    float acc[16];
+#pragma unroll
+    for (int m = 0; m < 16; m++) acc[m] = 0.0f;
+    for (int r = 0; r < kRows; r++) {
+      const float x = X[r * kPitch + i];
+      const float *d = D + r * kPitch + j0;
+#pragma unroll
+      for (int q = 0; q < 4; q++) {
+        const float4 dv = ld4(d + 4 * q);
+        acc[4 * q + 0] = fmaf(dv.x, x, acc[4 * q + 0]);
+        acc[4 * q + 1] = fmaf(dv.y, x, acc[4 * q + 1]);
+        acc[4 * q + 2] = fmaf(dv.z, x, acc[4 * q + 2]);
+        acc[4 * q + 3] = fmaf(dv.w, x, acc[4 * q + 3]);
+      }
+    }
+#pragma unroll
+    for (int m = 0; m < 16; m++)
+      if (j0 + m < out) G[(j0 + m) * in + i] += acc[m];
+  }
+  if ((int)threadIdx.x < out) {
+    float acc = 0.0f;
+    for (int r = 0; r < kRows; r++) acc += D[r * kPitch + threadIdx.x];
+    G[out * in + threadIdx.x] += acc;
+  }
+}
+
+// All layers of net k on the tile; outbuf(l) is where layer l writes.
+template <class OutBuf>
+__device__ __forceinline__ void net_forward(const float *W, const Plan &P, int k,
+                                            const float *X, OutBuf outbuf) {
+  const float *x = X;
+  for (int l = 0; l < P.L[k]; l++) {
+    float *y = outbuf(l);
+    layer_forward(W + P.woff[k][l], P.pw[k][l], P.in[k][l], P.out[k][l], x, y, l < P.L[k] - 1);
+    __syncthreads();
+    x = y;
+  }
+}
+
+// Back-propagates the head delta Dh through net k, adding every weight gradient to G;
+// inbuf(l) is layer l's input.  i_lo >= 0 also forms the input gradient of columns
+// [i_lo, in) of layer 0; the buffer that holds it (D0 or D1) is returned.
+template <class InBuf>
+__device__ __forceinline__ const float *net_backward(const float *W, const Plan &P, int k,
+                                                     float *G, const float *Dh, InBuf inbuf,
+                                                     float *D0, float *D1, int i_lo) {
+  const float *d = Dh;
+  float *nxt = Dh == D0 ? D1 : D0;
+  for (int l = P.L[k] - 1; l >= 0; l--) {
+    const float *x = inbuf(l);
+    layer_grad(G + P.goff[k][l], P.in[k][l], P.out[k][l], d, x);
+    const float *Wl = W + P.woff[k][l];
+    if (l > 0)
+      layer_backward(Wl, P.pw[k][l], P.in[k][l], P.out[k][l], d, nxt, x, 0);
+    else if (i_lo >= 0)
+      layer_backward(Wl, P.pw[k][l], P.in[k][l], P.out[k][l], d, nxt, nullptr, i_lo);
+    __syncthreads();
+    d = nxt;
+    nxt = nxt == D0 ? D1 : D0;
+  }
+  return d;
+}
+
+__device__ void load_net(float *dst, const wdb_ddpg_net &net, const Plan &P, int k) {
+  for (int l = 0; l < P.L[k]; l++) {
+    const int in = P.in[k][l], out = P.out[k][l], pw = P.pw[k][l];
+    float *W = dst + P.woff[k][l];
+    const float *w = net.w[l], *b = net.b[l];
+    for (int e = threadIdx.x; e < out * pw; e += kThreads) {
+      const int j = e / pw, i = e - j * pw;
+      W[e] = i < in ? w[j * in + i] : 0.0f;
+    }
+    for (int j = threadIdx.x; j < out; j += kThreads) W[out * pw + j] = b[j];
+  }
+}
+
+__global__ void __launch_bounds__(kThreads, 1)
+ddpg_update_kernel(const __grid_constant__ wdb_ddpg_update_args U, const __grid_constant__ Plan Pg,
+                   float *partials, double *psums) {
+  extern __shared__ __align__(16) float smem[];
+  __shared__ Plan P;                           // dynamic indexing of the kernel parameter goes
+  __shared__ double s_err[kRows], s_j[kRows];  // through local memory: copy it once
+  if (threadIdx.x == 0) P = Pg;
+  __syncthreads();
+  const int tid = threadIdx.x;
+  float *Wa = smem, *Wc = Wa + P.wfloats[0], *Wta = Wc + P.wfloats[1], *Wtc = Wta + P.wfloats[0];
+  float *Ga = Wtc + P.wfloats[1], *Gc = Ga + P.gfloats[0];
+  const int g_total = P.gfloats[0] + P.gfloats[1];
+  float *XQ = Ga + ((g_total + 3) / 4) * 4;      // obs ++ actions
+  float *XJ = XQ + kTile;                      // obs ++ pi (target path: scratch)
+  float *V = XJ + kTile;                       // columns: 0 target Q, 1 Q, 2 J, 4 dQ, 8 dJ
+  float *Z = V + kTile;                        // actor head pre-activation
+  float *D0 = Z + kTile, *D1 = D0 + kTile;     // deltas (target path: obs' and scratch)
+  float *HQ = D1 + kTile;                      // critic hidden outputs, (obs, actions) path
+  float *HJ = HQ + (P.L[1] - 1) * kTile;       // critic hidden outputs, (obs, pi) path
+  float *HA = HJ + (P.L[1] - 1) * kTile;       // actor hidden outputs
+
+  load_net(Wa, U.actor, P, 0);
+  load_net(Wc, U.critic, P, 1);
+  load_net(Wta, U.target_actor, P, 0);
+  load_net(Wtc, U.target_critic, P, 1);
+  for (int e = tid; e < g_total; e += kThreads) Ga[e] = 0.0f;
+  for (int e = tid; e < P.n_buf * kTile; e += kThreads) XQ[e] = 0.0f;
+  __syncthreads();
+
+  const int F = U.obs_dim, A = U.action_dim, FA = F + A;
+  const int C = U.capacity, cursor = U.cursor, ns = U.n_step, valid = P.valid;
+  const long long EN = P.EN, M = P.M, E = U.n_envs, Np = U.n_agents;
+  const float gamma = U.gamma, scale = U.action_scale, bias = U.action_bias;
+  const float norm_q = (float)(2.0 / (double)M);         // mse_loss backward: 2 / numel
+  const float d_j = -1.0f / (float)M;                    // -mean backward
+  auto phys = [&](int k) { const int s = cursor + k; return s >= C ? s - C : s; };
+  auto target_slot = [&](int i) { return i < valid - 1 ? i + ns : C - 1; };
+  double err_acc = 0.0, j_acc = 0.0;
+
+  for (long long g0 = (long long)blockIdx.x * kRows; g0 < M; g0 += (long long)gridDim.x * kRows) {
+    // ---- inputs: XQ = obs ++ actions at slot i, D0 = obs at the bootstrap slot
+    for (int e = tid; e < kRows * FA; e += kThreads) {
+      const int r = e / FA, c = e - r * FA;
+      const long long g = g0 + r;
+      float xq = 0.0f, xt = 0.0f;
+      if (g < M) {
+        const int i = (int)(g / EN);
+        const long long n = g - (long long)i * EN;
+        const long long row = (long long)phys(i) * EN + n;
+        if (c < F) {
+          xq = U.obs[row * F + c];
+          xt = U.obs[((long long)phys(target_slot(i)) * EN + n) * F + c];
+        } else {
+          xq = U.actions[row * A + (c - F)];
+        }
+      }
+      XQ[r * kPitch + c] = xq;
+      if (c < F) D0[r * kPitch + c] = xt;
+    }
+    __syncthreads();
+    // ---- target actor -> a' = scale * tanh(z) + bias into D0's action columns
+    net_forward(Wta, P, 0, D0,
+                [&](int l) { return l == P.L[0] - 1 ? Z : (l % 2 == 0 ? D1 : XJ); });
+    for (int e = tid; e < kRows * A; e += kThreads) {
+      const int r = e / A, c = e - r * A;
+      D0[r * kPitch + F + c] = __fadd_rn(__fmul_rn(scale, tanhf(Z[r * kPitch + c])), bias);
+    }
+    __syncthreads();
+    // ---- target critic -> V[., 0]; critic on (obs, actions) -> V[., 1]; actor -> Z
+    net_forward(Wtc, P, 1, D0,
+                [&](int l) { return l == P.L[1] - 1 ? V : (l % 2 == 0 ? D1 : XJ); });
+    net_forward(Wc, P, 1, XQ,
+                [&](int l) { return l == P.L[1] - 1 ? V + 1 : HQ + l * kTile; });
+    net_forward(Wa, P, 0, XQ,
+                [&](int l) { return l == P.L[0] - 1 ? Z : HA + l * kTile; });
+    // ---- critic on (obs, pi) -> V[., 2]
+    for (int e = tid; e < kRows * FA; e += kThreads) {
+      const int r = e / FA, c = e - r * FA;
+      XJ[r * kPitch + c] = c < F ? XQ[r * kPitch + c]
+                                 : __fadd_rn(__fmul_rn(scale, tanhf(Z[r * kPitch + c - F])), bias);
+    }
+    __syncthreads();
+    net_forward(Wc, P, 1, XJ,
+                [&](int l) { return l == P.L[1] - 1 ? V + 2 : HJ + l * kTile; });
+    // ---- n-step return (ddpg.py:62-79, same float32 operations) and the loss gradients
+    if (tid < kRows) {
+      const int r = tid;
+      const long long g = g0 + r;
+      float dq = 0.0f, dj = 0.0f;
+      if (g < M) {
+        const int i = (int)(g / EN);
+        const long long n = g - (long long)i * EN, env = n / Np;
+        const float qt = V[r * kPitch], q = V[r * kPitch + 1], jv = V[r * kPitch + 2];
+        const int pl = phys(i + ns - 1);
+        const float rl = U.rewards[(long long)pl * EN + n];
+        const float dl = (float)U.done[(long long)pl * E + env];
+        const float om = __fsub_rn(1.0f, dl);
+        float ret = i < valid - 1 ? __fadd_rn(rl, __fmul_rn(__fmul_rn(om, gamma), qt))
+                                  : __fadd_rn(__fmul_rn(dl, rl), __fmul_rn(om, qt));
+        for (int j = 1; j < ns; j++) {
+          const int pk = phys(ns - 1 - j + i);
+          const float dk = (float)U.done[(long long)pk * E + env];
+          ret = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(1.0f, dk), gamma), ret),
+                          U.rewards[(long long)pk * EN + n]);
+        }
+        const float diff = __fsub_rn(q, ret);
+        dq = __fmul_rn(diff, norm_q);
+        dj = d_j;
+        err_acc += (double)diff * (double)diff;
+        j_acc += (double)jv;
+        if (U.values) U.values[g] = q;
+        if (U.j_values) U.j_values[g] = jv;
+        if (U.returns) U.returns[g] = ret;
+      }
+      V[r * kPitch + 4] = dq;
+      V[r * kPitch + 8] = dj;
+    }
+    __syncthreads();
+    // ---- backward: critic on both paths, then the tanh head and the actor
+    net_backward(Wc, P, 1, Gc, V + 4,
+                 [&](int l) { return l == 0 ? XQ : HQ + (l - 1) * kTile; }, D0, D1, -1);
+    const float *dpi = net_backward(
+        Wc, P, 1, Gc, V + 8, [&](int l) { return l == 0 ? XJ : HJ + (l - 1) * kTile; }, D0, D1, F);
+    float *dz = dpi == D0 ? D1 : D0;
+    for (int e = tid; e < kRows * A; e += kThreads) {
+      const int r = e / A, c = e - r * A;
+      const float y = tanhf(Z[r * kPitch + c]);
+      dz[r * kPitch + c] = __fmul_rn(__fmul_rn(dpi[r * kPitch + F + c], scale),
+                                     __fsub_rn(1.0f, __fmul_rn(y, y)));
+    }
+    __syncthreads();
+    net_backward(Wa, P, 0, Ga, dz, [&](int l) { return l == 0 ? XQ : HA + (l - 1) * kTile; },
+                 D0, D1, -1);
+  }
+
+  // ---- this CTA's partials
+  float *part = partials + (long long)blockIdx.x * g_total;
+  for (int e = tid; e < g_total; e += kThreads) part[e] = Ga[e];
+  if (tid < kRows) {
+    s_err[tid] = err_acc;
+    s_j[tid] = j_acc;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    double a = 0.0, b = 0.0;
+    for (int r = 0; r < kRows; r++) {
+      a += s_err[r];
+      b += s_j[r];
+    }
+    psums[2 * blockIdx.x] = a;
+    psums[2 * blockIdx.x + 1] = b;
+  }
+}
+
+struct Reduce {
+  int grid, g_total, nseg;
+  int off[16], n[16];      // segment: packed offset and length (a weight or a bias)
+  float *dst[16];
+};
+
+// dst[seg][e] = sum over CTAs c = 0, 1, ... of partials[c][off[seg] + e]; sums = the same
+// over the CTAs' double sums.
+__global__ void ddpg_reduce_kernel(const __grid_constant__ Reduce R, const float *partials,
+                                   const double *psums, double *sums) {
+  const int seg = blockIdx.y;
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e < R.n[seg]) {
+    const float *p = partials + R.off[seg] + e;
+    float s = 0.0f;
+    for (int c = 0; c < R.grid; c++) s += p[(long long)c * R.g_total];
+    R.dst[seg][e] = s;
+  }
+  if (sums && seg == 0 && blockIdx.x == 0 && threadIdx.x == 0) {
+    double a = 0.0, b = 0.0;
+    for (int c = 0; c < R.grid; c++) {
+      a += psums[2 * c];
+      b += psums[2 * c + 1];
+    }
+    sums[0] = a;
+    sums[1] = b;
+  }
+}
+
+long long workspace_bytes(const Plan &P) {
+  return 16ll * P.grid + 4ll * P.grid * (P.gfloats[0] + P.gfloats[1]);
+}
+
+bool nets_ok(const wdb_ddpg_update_args *u, const Plan &P) {
+  const wdb_ddpg_net *nets[4] = {&u->actor, &u->critic, &u->target_actor, &u->target_critic};
+  for (int k = 0; k < 4; k++)
+    for (int l = 0; l < P.L[k % 2]; l++) {
+      if (!nets[k]->w[l] || !nets[k]->b[l]) return false;
+      if (k < 2 && (!nets[k]->gw[l] || !nets[k]->gb[l])) return false;
+    }
+  return true;
+}
+
+}  // namespace
+
+WDB_API int wdb_ddpg_update_supported(const wdb_ddpg_update_args *update) {
+  Plan P;
+  return make_plan(update, &P) ? 1 : 0;
+}
+
+WDB_API long long wdb_ddpg_update_workspace_bytes(const wdb_ddpg_update_args *update) {
+  Plan P;
+  return make_plan(update, &P) ? workspace_bytes(P) : -1;
+}
+
+WDB_API int wdb_ddpg_update(void *stream, const wdb_ddpg_update_args *u) {
+  Plan P;
+  if (!make_plan(u, &P) || !nets_ok(u, P)) return (int)cudaErrorInvalidValue;
+  if (!u->obs || !u->actions || !u->rewards || !u->done || !u->workspace)
+    return (int)cudaErrorInvalidValue;
+  const size_t smem = (size_t)P.smem_floats * sizeof(float);
+  static size_t configured = 0;
+  if (smem > 48 * 1024 && smem > configured) {
+    cudaError_t e = cudaFuncSetAttribute(ddpg_update_kernel,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return (int)e;
+    configured = smem;
+  }
+  double *psums = static_cast<double *>(u->workspace);
+  float *partials = reinterpret_cast<float *>(psums + 2 * P.grid);
+  ddpg_update_kernel<<<P.grid, kThreads, smem, as_stream(stream)>>>(*u, P, partials, psums);
+  int rc = finish_launch();
+  if (rc != cudaSuccess) return rc;
+
+  Reduce R = {};
+  R.grid = P.grid;
+  R.g_total = P.gfloats[0] + P.gfloats[1];
+  int widest = 1;
+  for (int k = 0; k < 2; k++) {
+    const wdb_ddpg_net &net = k == 0 ? u->actor : u->critic;
+    const int base = k == 0 ? 0 : P.gfloats[0];
+    for (int l = 0; l < P.L[k]; l++) {
+      const int nw = P.in[k][l] * P.out[k][l];
+      R.off[R.nseg] = base + P.goff[k][l];
+      R.n[R.nseg] = nw;
+      R.dst[R.nseg++] = net.gw[l];
+      R.off[R.nseg] = base + P.goff[k][l] + nw;
+      R.n[R.nseg] = P.out[k][l];
+      R.dst[R.nseg++] = net.gb[l];
+      widest = nw > widest ? nw : widest;
+    }
+  }
+  const dim3 grid((widest + 255) / 256, R.nseg);
+  ddpg_reduce_kernel<<<grid, 256, 0, as_stream(stream)>>>(R, partials, psums, u->sums);
+  return finish_launch();
+}

@@ -151,6 +151,28 @@ class PgLoss(ctypes.Structure):
     ]
 
 
+class DdpgNet(ctypes.Structure):
+    """struct wdb_ddpg_net (include/wdb200.h)."""
+
+    _fields_ = [("n_hidden", _i), ("widths", _i * 3), ("w", _fp * 4), ("b", _fp * 4),
+                ("gw", _fp * 4), ("gb", _fp * 4)]
+
+
+class DdpgUpdate(ctypes.Structure):
+    """struct wdb_ddpg_update_args (include/wdb200.h)."""
+
+    _fields_ = [
+        ("n_envs", _i), ("n_agents", _i), ("obs_dim", _i), ("action_dim", _i),
+        ("capacity", _i), ("cursor", _i), ("n_step", _i),
+        ("gamma", _f), ("action_scale", _f), ("action_bias", _f),
+        ("obs", _fp), ("actions", _fp), ("rewards", _fp), ("done", _fp),
+        ("actor", DdpgNet), ("critic", DdpgNet), ("target_actor", DdpgNet),
+        ("target_critic", DdpgNet),
+        ("values", _fp), ("j_values", _fp), ("returns", _fp), ("sums", _fp),
+        ("workspace", _fp),
+    ]
+
+
 _SIGNATURES = {
     "wdb_abi_version": (_i, []),
     "wdb_error_string": (ctypes.c_char_p, [_i]),
@@ -200,6 +222,9 @@ _SIGNATURES = {
     "wdb_relu_backward_bias": (_i, [_vp, _vp, _vp, _ll, _i, _vp]),
     "wdb_grad_sumsq": (_i, [_vp, _vp, _ll, _vp]),
     "wdb_adam_step": (_i, [_vp, _vp, _vp, _vp, _vp, _ll, _f, _f, _f, _f, _i, _f, _vp]),
+    "wdb_ddpg_update_supported": (_i, [ctypes.POINTER(DdpgUpdate)]),
+    "wdb_ddpg_update_workspace_bytes": (_ll, [ctypes.POINTER(DdpgUpdate)]),
+    "wdb_ddpg_update": (_i, [_vp, ctypes.POINTER(DdpgUpdate)]),
     "wdb_single_agent_rollout_supported": (_i, [_i, ctypes.POINTER(_i)]),
     "wdb_single_agent_rollout": (_i, [_vp, ctypes.POINTER(SaRollout)]),
     "wdb_mountain_car_step": (

@@ -14,6 +14,10 @@ _EPSILON = 1e-10
 
 
 class DDPG:
+    # TrainerDDPG runs this policy's update as native kernels (fused_ddpg.py) when the shapes
+    # allow it; False keeps the torch autograd update below (a test switch, not a config key)
+    use_fused_update = True
+
     def __init__(self, discount_factor_gamma=1.0, normalize_advantage=False,
                  normalize_return=False, n_step=1):
         assert 0 <= discount_factor_gamma <= 1
@@ -59,36 +63,46 @@ class DDPG:
         norm_returns = self._normalize(returns) if self.normalize_return else returns
         values = value_functions_batch[:valid]
         critic_loss = nn.functional.mse_loss(values, norm_returns)
-        advantages = norm_returns - values
-        norm_adv = self._normalize(advantages) if self.normalize_advantage else advantages
         j_values = j_functions_batch[:valid]
         norm_j = self._normalize(j_values) if self.normalize_return else j_values
         actor_loss = -norm_j.mean()
         metrics = {}
         if perform_logging:
-            var_expl = max(-1.0, float(1 - norm_adv.detach().var()
-                                       / (norm_returns.detach().var() + _EPSILON)))
-            metrics = {
-                "Total loss": actor_loss.item() + critic_loss.item(),
-                "Actor loss": actor_loss.item(), "Critic loss": critic_loss.item(),
-                "Mean rewards": rewards_batch.mean().item(),
-                "Max. rewards": rewards_batch.max().item(),
-                "Min. rewards": rewards_batch.min().item(),
-                "Mean value function": values.mean().item(),
-                "Mean J function": j_values.mean().item(),
-                "Mean advantages": advantages.mean().item(),
-                "Mean (norm.) advantages": norm_adv.mean().item(),
-                "Mean (discounted) returns": returns.mean().item(),
-                "Mean normalized returns": norm_returns.mean().item(),
-                "Variance explained by the value function": var_expl,
-            }
-            a = actions_batch.float()
-            for k in range(a.shape[-1]):
-                metrics.update({
-                    f"Std. of action_{k} over agents": a[..., k].std(dim=2).mean().item(),
-                    f"Std. of action_{k} over envs": a[..., k].std(dim=1).mean().item(),
-                    f"Std. of action_{k} over time": a[..., k].std(dim=0).mean().item(),
-                    f"Max of action_{k}": a[..., k].max().item(),
-                    f"Min of action_{k}": a[..., k].min().item(),
-                })
+            metrics = self.loss_metrics(actor_loss.item(), critic_loss.item(), rewards_batch,
+                                        actions_batch, values.detach(), j_values.detach(),
+                                        returns)
         return actor_loss, critic_loss, metrics
+
+    def loss_metrics(self, actor_loss, critic_loss, rewards_batch, actions_batch, values,
+                     j_values, returns):
+        """The logged metrics of one update: the losses as floats, values / j_values / returns
+        over the loss rows [valid, E, Np]; shared by the torch loss above and the fused update
+        (fused_ddpg.py)."""
+        norm_returns = self._normalize(returns) if self.normalize_return else returns
+        advantages = norm_returns - values
+        norm_adv = self._normalize(advantages) if self.normalize_advantage else advantages
+        var_expl = max(-1.0, float(1 - norm_adv.var() / (norm_returns.var() + _EPSILON)))
+        metrics = {
+            "Total loss": actor_loss + critic_loss,
+            "Actor loss": actor_loss, "Critic loss": critic_loss,
+            "Mean rewards": rewards_batch.mean().item(),
+            "Max. rewards": rewards_batch.max().item(),
+            "Min. rewards": rewards_batch.min().item(),
+            "Mean value function": values.mean().item(),
+            "Mean J function": j_values.mean().item(),
+            "Mean advantages": advantages.mean().item(),
+            "Mean (norm.) advantages": norm_adv.mean().item(),
+            "Mean (discounted) returns": returns.mean().item(),
+            "Mean normalized returns": norm_returns.mean().item(),
+            "Variance explained by the value function": var_expl,
+        }
+        a = actions_batch.float()
+        for k in range(a.shape[-1]):
+            metrics.update({
+                f"Std. of action_{k} over agents": a[..., k].std(dim=2).mean().item(),
+                f"Std. of action_{k} over envs": a[..., k].std(dim=1).mean().item(),
+                f"Std. of action_{k} over time": a[..., k].std(dim=0).mean().item(),
+                f"Max of action_{k}": a[..., k].max().item(),
+                f"Min of action_{k}": a[..., k].min().item(),
+            })
+        return metrics

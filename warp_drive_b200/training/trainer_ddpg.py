@@ -18,7 +18,13 @@ Underneath:
     cursor -- every array is written in lock step, so the per-array queue objects of the
     reference (ring_buffer.py) collapse to two integers; `RingBuffer` is still provided
     for API parity (training/utils/ring_buffer.py);
-  * target networks are tracked with fused `torch._foreach` updates;
+  * the update is two launches per policy (wdb_ddpg_update, algorithms/fused_ddpg.py: every
+    actor and critic gradient read in place from the ring) for the shapes it supports, else
+    torch autograd over the unrolled ring;
+  * one flat parameter / gradient arena over the actor and critic of every policy, with one
+    FlatAdam (clipping + Adam as flat kernels) per network, so each network is clipped by its
+    own norm as clip_grad_norm_ does; target networks are tracked with fused `torch._foreach`
+    updates;
   * multi-GPU: one flat NCCL all-reduce over actor + critic gradients per iteration.
 """
 import json
@@ -33,6 +39,7 @@ from torch import nn
 
 from warp_drive_b200.managers.function_manager import CUDASampler
 from warp_drive_b200.training.algorithms.ddpg import DDPG
+from warp_drive_b200.training.algorithms.fused_ddpg import FusedDDPGUpdate, fused_ddpg_supported
 from warp_drive_b200.training.models.fully_connected import ModelFactory
 from warp_drive_b200.training.models.fully_connected_actor_critic import ActorAsPolicy
 from warp_drive_b200.training.rollout import RolloutEngine
@@ -40,6 +47,7 @@ from warp_drive_b200.training.trainer import (
     _CONFIG_DIR, PerfStats, Trainer, recursive_merge_config_dicts, verbose_print)
 from warp_drive_b200.training.utils.data_loader import (
     create_and_push_data_placeholders, validate_policy_map)
+from warp_drive_b200.training.utils.flat_adam import FlatAdam
 from warp_drive_b200.training.utils.param_scheduler import ParamScheduler
 from warp_drive_b200.utils.constants import Constants
 
@@ -210,7 +218,18 @@ class TrainerDDPG(Trainer):
             for group in (self.actor_models, self.critic_models, self.target_actor_models,
                           self.target_critic_models):
                 group[policy].cuda()
+        # ONE flat float32 arena for the parameters and one for the gradients of every actor
+        # and critic (Trainer's layout): the multi-GPU all-reduce is one in-place NCCL call on
+        # `_arena_grads`
+        nets = [g[p] for p in self.policies for g in (self.actor_models, self.critic_models)]
+        total = sum(FlatAdam.numel(m.parameters()) for m in nets)
+        dev = next(nets[0].parameters()).device
+        self._arena_params = torch.zeros(total, dtype=torch.float32, device=dev)
+        self._arena_grads = torch.zeros(total, dtype=torch.float32, device=dev)
+        self._arena_off = 0
+        for policy in self.policies:
             self._initialize_optimizer(policy)
+        self.fused_updates = {}
         for policy in self.policies_to_train:
             self._initialize_policy_algorithm(policy)
         if self.num_devices > 1:
@@ -259,12 +278,18 @@ class TrainerDDPG(Trainer):
         self.actor_lr_schedules[policy] = ParamScheduler(actor_lr)
         self.critic_lr_schedules[policy] = ParamScheduler(critic_lr)
         ts = self.current_timestep[policy]
-        self.actor_optimizers[policy] = torch.optim.Adam(
-            self.actor_models[policy].parameters(),
-            lr=self.actor_lr_schedules[policy].get_param_value(ts))
-        self.critic_optimizers[policy] = torch.optim.Adam(
-            self.critic_models[policy].parameters(),
-            lr=self.critic_lr_schedules[policy].get_param_value(ts))
+
+        def flat_adam(model, lr):
+            n = FlatAdam.numel(model.parameters())
+            lo = self._arena_off
+            self._arena_off += n
+            return FlatAdam(model.parameters(), lr=lr, arena=(
+                self._arena_params[lo:lo + n], self._arena_grads[lo:lo + n]))
+
+        self.actor_optimizers[policy] = flat_adam(
+            self.actor_models[policy], self.actor_lr_schedules[policy].get_param_value(ts))
+        self.critic_optimizers[policy] = flat_adam(
+            self.critic_models[policy], self.critic_lr_schedules[policy].get_param_value(ts))
 
     def _initialize_policy_algorithm(self, policy):
         c = self._get_config(["policy", policy])
@@ -276,6 +301,13 @@ class TrainerDDPG(Trainer):
         self.trainers[policy] = DDPG(
             discount_factor_gamma=c["gamma"], normalize_advantage=c["normalize_advantage"],
             normalize_return=c["normalize_return"], n_step=self.n_step)
+        n_agents = len(self.policy_tag_to_agent_id_map[policy])
+        args = (self.num_envs, n_agents, self.ring_capacity, self.n_step)
+        actor, critic = self.actor_models[policy], self.critic_models[policy]
+        if fused_ddpg_supported(self.trainers[policy], actor, critic, *args):
+            self.fused_updates[policy] = FusedDDPGUpdate(
+                actor, critic, self.target_actor_models[policy],
+                self.target_critic_models[policy], *args, gamma=c["gamma"])
 
     # ------------------------------------------------------------------ multi-GPU
     def _trained_params(self):
@@ -301,37 +333,19 @@ class TrainerDDPG(Trainer):
         metrics_dict = {}
         stepped = []
         if eng.isfull():
-            done_flags = eng.unroll(f"{_DONE_FLAGS}_batch")
             for policy in self.policies_to_train:
-                actions = eng.unroll(f"{_ACTIONS}_batch_{policy}")
-                rewards = eng.unroll(f"{_REWARDS}_batch_{policy}")
-                obs = eng.unroll(f"{_PROCESSED_OBSERVATIONS}_batch_{policy}")
-                actor, critic = self.actor_models[policy], self.critic_models[policy]
-                probs = actor(obs=obs)
-                with torch.no_grad():
-                    target_probs = self.target_actor_models[policy](obs=obs)
-                    next_values = self.target_critic_models[policy](
-                        obs=obs[1:], action=[p[1:] for p in target_probs])
-                values = critic(obs=obs, action=actions)
-                j_values = critic(obs=obs, action=probs)
                 self.current_timestep[policy] += self.training_batch_size
-                actor_loss, critic_loss, metrics = self.trainers[policy].compute_loss_and_metrics(
-                    self.current_timestep[policy], actions, rewards, done_flags, values,
-                    next_values, j_values, perform_logging=logging_flag)
                 actor_lr = self.actor_lr_schedules[policy].get_param_value(
                     self.current_timestep[policy])
                 critic_lr = self.critic_lr_schedules[policy].get_param_value(
                     self.current_timestep[policy])
-                for group in self.actor_optimizers[policy].param_groups:
-                    group["lr"] = actor_lr
-                for group in self.critic_optimizers[policy].param_groups:
-                    group["lr"] = critic_lr
-                self.actor_optimizers[policy].zero_grad()
-                self.critic_optimizers[policy].zero_grad()
-                # the order and the (shared) critic gradient of the reference
-                # (trainer_ddpg.py:412-415): the actor loss also back-propagates into the critic
-                actor_loss.backward()
-                critic_loss.backward()
+                self.actor_optimizers[policy].param_groups[0]["lr"] = actor_lr
+                self.critic_optimizers[policy].param_groups[0]["lr"] = critic_lr
+                fused = self.fused_updates.get(policy)
+                if fused is not None and self.trainers[policy].use_fused_update:
+                    metrics = self._fused_gradients(policy, fused, logging_flag)
+                else:
+                    metrics = self._torch_gradients(policy, logging_flag)
                 stepped.append((policy, metrics, actor_lr, critic_lr))
             if self.num_devices > 1 and stepped:
                 self._allreduce_gradients()
@@ -342,11 +356,10 @@ class TrainerDDPG(Trainer):
                     p.grad.norm(2) for p in actor.parameters() if p.grad is not None))
                 metrics["Gradient norm (Critic)"] = float(sum(
                     p.grad.norm(2) for p in critic.parameters() if p.grad is not None))
-            if self.clip_grad_norm[policy]:
-                nn.utils.clip_grad_norm_(actor.parameters(), self.max_grad_norm[policy])
-                nn.utils.clip_grad_norm_(critic.parameters(), self.max_grad_norm[policy])
-            self.actor_optimizers[policy].step()
-            self.critic_optimizers[policy].step()
+            # clip_grad_norm_ + Adam per network as two flat kernels each
+            clip = self.max_grad_norm[policy] if self.clip_grad_norm[policy] else None
+            self.actor_optimizers[policy].step(max_grad_norm=clip)
+            self.critic_optimizers[policy].step(max_grad_norm=clip)
             soft_update(self.target_actor_models[policy], actor, self.tau[policy])
             soft_update(self.target_critic_models[policy], critic, self.tau[policy])
             if logging_flag:
@@ -373,6 +386,54 @@ class TrainerDDPG(Trainer):
                         "Mean episodic reward (test)": float(reward_sum[policy].mean()),
                         "Mean episodic steps (test)": float(step_sum[policy].float().mean())})
         return metrics_dict
+
+    def _torch_gradients(self, policy, logging_flag):
+        """Actor / critic gradients by torch autograd over the unrolled ring (accumulated into
+        the arena's .grad views); returns the metrics of a logging iteration."""
+        eng = self.engine
+        done_flags = eng.unroll(f"{_DONE_FLAGS}_batch")
+        actions = eng.unroll(f"{_ACTIONS}_batch_{policy}")
+        rewards = eng.unroll(f"{_REWARDS}_batch_{policy}")
+        obs = eng.unroll(f"{_PROCESSED_OBSERVATIONS}_batch_{policy}")
+        actor, critic = self.actor_models[policy], self.critic_models[policy]
+        probs = actor(obs=obs)
+        with torch.no_grad():
+            target_probs = self.target_actor_models[policy](obs=obs)
+            next_values = self.target_critic_models[policy](
+                obs=obs[1:], action=[p[1:] for p in target_probs])
+        values = critic(obs=obs, action=actions)
+        j_values = critic(obs=obs, action=probs)
+        actor_loss, critic_loss, metrics = self.trainers[policy].compute_loss_and_metrics(
+            self.current_timestep[policy], actions, rewards, done_flags, values,
+            next_values, j_values, perform_logging=logging_flag)
+        self.actor_optimizers[policy].zero_grad()
+        self.critic_optimizers[policy].zero_grad()
+        # the order and the (shared) critic gradient of the reference
+        # (trainer_ddpg.py:412-415): the actor loss also back-propagates into the critic
+        actor_loss.backward()
+        critic_loss.backward()
+        return metrics
+
+    def _fused_gradients(self, policy, fused, logging_flag):
+        """The same gradients as _torch_gradients from wdb_ddpg_update, written straight into
+        the arena's .grad views; the host waits only on logging iterations (metrics)."""
+        eng = self.engine
+        rewards = eng._tensor(f"{_REWARDS}_batch_{policy}")
+        actions = eng._tensor(f"{_ACTIONS}_batch_{policy}")
+        outputs = None
+        if logging_flag:
+            shape = (fused.valid,) + tuple(rewards.shape[1:])
+            outputs = tuple(torch.empty(shape, device=rewards.device) for _ in range(3))
+        sums = fused.launch(eng._tensor(f"{_PROCESSED_OBSERVATIONS}_batch_{policy}"), actions,
+                            rewards, eng._tensor(f"{_DONE_FLAGS}_batch"), eng.ring_cursor,
+                            outputs)
+        if not logging_flag:
+            return {}
+        s = sums.tolist()
+        values, j_values, returns = outputs
+        # the ring in slot order: the metrics are means / extremes / spreads over all of it
+        return self.trainers[policy].loss_metrics(
+            -s[1] / fused.rows, s[0] / fused.rows, rewards, actions, values, j_values, returns)
 
     # ------------------------------------------------------------------ checkpoints
     def save_model_checkpoint(self, iteration=0):
