@@ -16,8 +16,11 @@
 //     a hidden layer, after bias + ReLU + bf16 packing, IS the A fragment of the next layer,
 //     so hidden activations never touch shared or global memory.  B is always read from
 //     the shared-memory weights through a matrix descriptor;
-//   * a layer is computed in 32-column slices (wgmma m64n32k16) so that only one slice of
-//     accumulators is live next to the packed input and output activations;
+//   * a layer is computed in 32-column slices (wgmma m64n32k16).  For the config-2 shape
+//     (FastShape) the slices are pipelined: slice c + 1's MMAs run while slice c's epilogue
+//     packs it, each packed slice of layer 2 feeds its two layer-3 k-steps at once, and the
+//     next tile's observations are loaded during layer 2.  Other shapes run one slice at a
+//     time, holding both hidden layers' packed activations;
 //   * final epilogue = bias + two softmaxes + value: the logits go through the staging
 //     buffer, two threads per row (head 0 | head 1 + value) compute the softmaxes, and the
 //     warpgroup's 64 rows of each output are copied to global memory with coalesced stores.
@@ -74,8 +77,13 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t sbo_bytes
 __device__ __forceinline__ void wgmma_fence() {
   asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void wgmma_commit_wait() {
-  asm volatile("wgmma.commit_group.sync.aligned;\n\twgmma.wait_group.sync.aligned 0;" ::: "memory");
+__device__ __forceinline__ void wgmma_commit() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+}
+// wait until at most N committed groups of this warp are still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
 
 // The descriptor of make_desc, built inside the asm of a register-A wgmma from the 32-bit
@@ -169,16 +177,62 @@ __device__ __forceinline__ void wg_sync(int wg) {
   else asm volatile("bar.sync 1, 128;" ::: "memory");
 }
 
-// One hidden layer of a warpgroup: out (packed bf16 A fragments of the next layer, 4 per
+// A hidden layer of a warpgroup is computed in 32-column slices (wgmma m64n32k16, one
+// commit group per slice) with two accumulator sets: slice c + 1's MMAs are issued before
+// the epilogue of slice c (`epi`) runs, so the tensor cores always have a slice in flight.
+// issue(c, d) issues slice c into d; its first MMA
+// runs with scale-d = 0, so the accumulators need no zeroing (a zeroing store between the
+// fence and the MMAs would serialise the pipeline).  epi(c, d) may itself commit MMA groups:
+// the wait before slice c's epilogue leaves only slice c + 1 in flight.
+// Accumulator fragment of m64nNk16: lane (g = lane / 4, t = lane % 4) of warp w holds rows
+// 16 w + g (+ 8), columns 8 j + 2 t (+ 1); the k-step kk of the next layer's A fragment is
+// columns 16 kk .. 16 kk + 15 of the same rows in the same lanes, so the repacking is
+// register-to-register.
+template <class Issue, class Epi>
+__device__ __forceinline__ void slice_pipeline(int n_slices, Issue issue, Epi epi) {
+  float d[2][16];
+  wgmma_fence();
+  issue(0, d[0]);
+  wgmma_commit();
+#pragma unroll
+  for (int c = 0; c < kMaxK / 32; c++) {
+    if (c < n_slices) {
+      if (c + 1 < n_slices) {
+        wgmma_fence();                 // (slice c - 1's epilogue read this accumulator set)
+        issue(c + 1, d[(c + 1) & 1]);
+        wgmma_commit();
+        wgmma_wait<1>();
+      } else {
+        wgmma_wait<0>();
+      }
+      epi(c, d[c & 1]);
+    }
+  }
+}
+
+// slice c of a hidden layer's accumulators + bias -> ReLU -> packed bf16 A fragments
+// out[8 c .. 8 c + 7] (the next layer's k-steps 2 c and 2 c + 1)
+__device__ __forceinline__ void bias_relu_slice(const float (&d)[16], const float *bias, int c,
+                                                uint32_t *out) {
+  const int t = threadIdx.x & 3;
+#pragma unroll
+  for (int j = 0; j < 4; j++) {
+    const float2 b = *reinterpret_cast<const float2 *>(bias + 32 * c + 8 * j + 2 * t);
+    out[2 * j] = bias_relu_pack(d[4 * j], d[4 * j + 1], b.x, b.y);
+    out[2 * j + 1] = bias_relu_pack(d[4 * j + 2], d[4 * j + 3], b.x, b.y);
+  }
+}
+
+// One hidden layer of a warpgroup, one slice at a time (the schedule of runtime shapes):
+// out (packed bf16 A fragments of the next layer, 4 per
 // 16 columns) = ReLU(A * W^T + bias), W = [N, K] in the canonical K-major layout at shared
 // address w.  A (K / 16 k-steps) is `in` (register fragments) or, with SS, the canonical
 // tile at the shared address a_smem (row-group stride a_sbo).  Accumulator fragment
 // of m64nNk16: lane (g = lane / 4, t = lane % 4) of warp w holds rows 16 w + g (+ 8),
 // columns 8 j + 2 t (+ 1); the k-step kk of the next layer's A fragment is columns
 // 16 kk .. 16 kk + 15 of the same rows in the same lanes, so the repacking is
-// register-to-register.
-// The first MMA of a slice runs with scale-d = 0: the accumulators need no zeroing (a
-// zeroing store between the fence and the MMAs would serialise the wgmma pipeline).
+// register-to-register (see bias_relu_slice).  Scale-d = 0 on the first MMA of a slice,
+// as in slice_pipeline.
 template <bool SS>
 __device__ __forceinline__ void hidden_layer(const uint32_t (&in)[kMaxK / 4], uint32_t a_smem,
                                              uint32_t a_sbo, int K, uint32_t w, uint32_t sbo,
@@ -199,7 +253,8 @@ __device__ __forceinline__ void hidden_layer(const uint32_t (&in)[kMaxK / 4], ui
         for (int kk = 0; kk < kMaxK / 16; kk++)
           if (kk < K / 16) wgmma_n32(d, &in[4 * kk], w + 4 * c * sbo + kk * 256, sbo, kk);
       }
-      wgmma_commit_wait();
+      wgmma_commit();
+      wgmma_wait<0>();
 #pragma unroll
       for (int j = 0; j < 4; j++) {
         const float2 b = *reinterpret_cast<const float2 *>(bias + 32 * c + 8 * j + 2 * t);
@@ -210,6 +265,84 @@ __device__ __forceinline__ void hidden_layer(const uint32_t (&in)[kMaxK / 4], ui
   }
 }
 
+// ---- layer-1 A operand staging.  A warpgroup's operand is 64 rows x K1 bf16 in the
+// canonical K-major layout: (r, k) at (r / 8) * K1 * 16 + (k / 8) * 128 + (r % 8) * 16 +
+// (k % 8) * 2.  Task i (thread lt takes i = lt + 128 j) is one 16-byte chunk (8 consecutive
+// k) of one row; consecutive lanes take the 8 rows of a core matrix, so each shared store of
+// a warp is bank-conflict free.  A thread handles its tasks kObsBatch at a time, the loads of
+// a batch all in flight together; batch 0 of the NEXT tile is loaded during the current
+// tile's layer 2 (for K1 <= 80, e.g. the config-2 F = 71, that is the whole operand).
+constexpr int kObsBatch = 5;
+
+template <bool TILES> struct ObsBatch;
+template <> struct ObsBatch<false> { float v[kObsBatch][8]; };   // fp32 obs [rows, F]
+template <> struct ObsBatch<true> { uint4 v[kObsBatch]; };       // bf16 obs tiles, as stored
+
+struct ObsSource {
+  const void *input;
+  long long rows;
+  int F, K1;
+};
+
+// the row (within the warpgroup) and chunk of task i; false past the operand's end
+__device__ __forceinline__ bool obs_task(int i, int nchunk, int &r, int &c) {
+  const int grp = i / (8 * nchunk), in = i - grp * 8 * nchunk;
+  c = in >> 3;
+  r = 8 * grp + (in & 7);
+  return i < kWgRows * nchunk;
+}
+
+// rows beyond `rows` and k >= F read as 0
+__device__ __forceinline__ void obs_load(ObsBatch<false> &b, const ObsSource &s, long long row0,
+                                         int j0) {
+  const float *obs = reinterpret_cast<const float *>(s.input);
+  const int lt = threadIdx.x & 127, nchunk = s.K1 / 8;
+#pragma unroll
+  for (int j = 0; j < kObsBatch; j++) {
+    int r, c;
+    const bool ok = obs_task(lt + 128 * (j0 + j), nchunk, r, c) && row0 + r < s.rows;
+    const float *src = obs + (row0 + r) * s.F + 8 * c;
+#pragma unroll
+    for (int k = 0; k < 8; k++) b.v[j][k] = (ok && 8 * c + k < s.F) ? __ldg(src + k) : 0.0f;
+  }
+}
+__device__ __forceinline__ void obs_store(const ObsBatch<false> &b, const ObsSource &s,
+                                          unsigned char *s_a, int j0) {
+  const int lt = threadIdx.x & 127, nchunk = s.K1 / 8;
+#pragma unroll
+  for (int j = 0; j < kObsBatch; j++) {
+    int r, c;
+    if (obs_task(lt + 128 * (j0 + j), nchunk, r, c)) {
+      uint4 o4;
+      o4.x = pack_bf16(b.v[j][0], b.v[j][1]); o4.y = pack_bf16(b.v[j][2], b.v[j][3]);
+      o4.z = pack_bf16(b.v[j][4], b.v[j][5]); o4.w = pack_bf16(b.v[j][6], b.v[j][7]);
+      *reinterpret_cast<uint4 *>(s_a + (r >> 3) * (s.K1 * 16) + c * 128 + (r & 7) * 16) = o4;
+    }
+  }
+}
+// the warpgroup's 64 rows are one contiguous block of a tile (rows past the end are the
+// zero padding of the tile buffer), already in the staging layout
+__device__ __forceinline__ void obs_load(ObsBatch<true> &b, const ObsSource &s, long long row0,
+                                         int j0) {
+  const uint4 *src = reinterpret_cast<const uint4 *>(
+      reinterpret_cast<const unsigned char *>(s.input) + row0 * (s.K1 * 2));
+  const int lt = threadIdx.x & 127;
+#pragma unroll
+  for (int j = 0; j < kObsBatch; j++) {
+    const int i = lt + 128 * (j0 + j);
+    if (i < kWgRows * s.K1 / 8) b.v[j] = __ldg(src + i);
+  }
+}
+__device__ __forceinline__ void obs_store(const ObsBatch<true> &b, const ObsSource &s,
+                                          unsigned char *s_a, int j0) {
+  const int lt = threadIdx.x & 127;
+#pragma unroll
+  for (int j = 0; j < kObsBatch; j++) {
+    const int i = lt + 128 * (j0 + j);
+    if (i < kWgRows * s.K1 / 8) reinterpret_cast<uint4 *>(s_a)[i] = b.v[j];
+  }
+}
+
 // TILES = false: `input` is the fp32 obs [rows, F]; TILES = true: `input` is the bf16 copy of
 // the obs already in A-operand layout (128-row tiles of the canonical K-major layout, K
 // padded with zeros -- written by wdb_mlp_pack_obs or by the env-step kernel's epilogue).
@@ -217,17 +350,33 @@ __device__ __forceinline__ void hidden_layer(const uint32_t (&in)[kMaxK / 4], ui
 // policies side by side in one grid).  flags & kMlpWeightsStable: the weight blob was not
 // written by the grid this launch programmatically depends on, so its TMA load may start
 // before griddepcontrol.wait (see the PDL note at launch_forward_pair).
-template <bool TILES>
+// Shape: MlpShape<0, 0, 0> reads K1, H and N3 from the blob's header; a non-zero shape is
+// the header's, fixed at compile time (FastShape).
+template <int K1_, int H_, int N3_> struct MlpShape {
+  static constexpr int K1 = K1_, H = H_, N3 = N3_;
+};
+using AnyShape = MlpShape<0, 0, 0>;
+// The config-2 policies (F = 71 -> K1 = 80, H = 256, 21 + 21 + 1 -> N3 = 48).  With every
+// MMA loop bound a constant, ptxas can follow the wgmma groups of the overlapped schedule
+// (slice_pipeline<true>, the next tile's observations prefetched during layer 2): it keeps
+// slice c + 1's MMAs in flight across slice c's epilogue and injects no warpgroup.arrive.
+// With runtime bounds it would serialise those wgmmas (C7514) and the extra live registers
+// would spill, so every other shape runs one slice at a time and loads its observations
+// at the top of the tile.
+using FastShape = MlpShape<80, 256, 48>;
+
+template <bool TILES, class Shape>
 __device__ __forceinline__ void
 mlp_forward_body(const unsigned char *__restrict__ blob, const void *__restrict__ input,
                  long long rows, float *__restrict__ probs0, float *__restrict__ probs1,
                  float *__restrict__ values, const unsigned bid, const unsigned gdim,
                  const int flags) {
-  const float *obs = reinterpret_cast<const float *>(input);
-  const unsigned char *tiles = reinterpret_cast<const unsigned char *>(input);
   extern __shared__ __align__(128) unsigned char smem[];
   const MlpHeader hd = *reinterpret_cast<const MlpHeader *>(blob);
-  const int F = hd.F, K1 = hd.K1, H = hd.H, A0 = hd.A0, A1 = hd.A1, N3 = hd.N3;
+  const int F = hd.F, A0 = hd.A0, A1 = hd.A1;
+  const int K1 = Shape::K1 ? Shape::K1 : hd.K1, H = Shape::H ? Shape::H : hd.H,
+            N3 = Shape::N3 ? Shape::N3 : hd.N3;
+  constexpr bool kOverlap = Shape::H != 0;
   const int w_bytes = hd.total_bytes - hd.off_w1;        // W1 | W2 | W3 | biases, contiguous
   unsigned char *s_w = smem;                             // packed weights + biases
   const uint32_t s_w1 = smem_addr(s_w);
@@ -267,63 +416,129 @@ mlp_forward_body(const unsigned char *__restrict__ blob, const void *__restrict_
   }
   if (flags & kMlpWeightsStable) griddep_wait();
   griddep_launch_dependents();
+
+  const ObsSource obs_src = {input, rows, F, K1};
+  const int lt = tid & 127;
+  // kOverlap: layer-1 operand tasks per thread, in batches of kObsBatch
+  const int n_batches = ((kWgRows * K1 / 8 + 127) / 128 + kObsBatch - 1) / kObsBatch;
+  const long long n_tiles = (rows + kTileM - 1) / kTileM;
+  ObsBatch<TILES> next;           // kOverlap: batch 0 of the warpgroup's next tile, prefetched
+  if (kOverlap && bid < n_tiles && bid * kTileM + wg * kWgRows < rows)   // (overlaps the weight load)
+    obs_load(next, obs_src, bid * kTileM + wg * kWgRows, 0);
   mbar_wait(bar_w, 0);
 
   const uint32_t sbo_a = (uint32_t)(K1 / 8) * 128u;       // W1: K1/8 core matrices per row group
   const uint32_t sbo_h = (uint32_t)(H / 8) * 128u;        // W2 / W3: H/8 core matrices per row group
-  const long long n_tiles = (rows + kTileM - 1) / kTileM;
   for (long long tile = bid; tile < n_tiles; tile += gdim) {
-    if (tile * kTileM + wg * kWgRows >= rows) continue;   // (warpgroup-uniform)
+    const long long row0 = tile * kTileM + wg * kWgRows;  // first row of the warpgroup
+    if (row0 >= rows) continue;                           // (warpgroup-uniform; so are all later tiles)
 
-    // ---- layer 1 A operand -> this warpgroup's staging buffer (canonical K-major layout:
-    // (r, k) at (r / 8) * K1 * 16 + (k / 8) * 128 + (r % 8) * 16 + (k % 8) * 2).  The
-    // previous tile's layer-1 MMAs have completed (wait_group 0) in every warp.
-    wg_sync(wg);
-    const int lt = tid & 127;
-    if (TILES) {
-      // the warpgroup's 64 rows are one contiguous block of the tile
-      const uint4 *src = reinterpret_cast<const uint4 *>(
-          tiles + tile * ((long long)kTileM * K1 * 2) + wg * a_bytes);
-      for (int i = lt; i < a_bytes / 16; i += 128)
-        reinterpret_cast<uint4 *>(s_a)[i] = __ldg(src + i);
+    float o[kMaxN3 / 16][8];   // layer-3 logits
+    if constexpr (kOverlap) {
+      // ---- layer 1 A operand -> this warpgroup's staging buffer.  The previous tile's
+      // output copy, the last reader of the buffer, is done in every warp.
+      wg_sync(wg);
+      obs_store(next, obs_src, s_a, 0);
+      for (int b = 1; b < n_batches; b++) {                 // (K1 > 80 only)
+        ObsBatch<TILES> rest;
+        obs_load(rest, obs_src, row0, b * kObsBatch);
+        obs_store(rest, obs_src, s_a, b * kObsBatch);
+      }
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // visible to wgmma
+      wg_sync(wg);
+
+      // ---- layer 1 (A from the staging buffer) -> h: packed bf16 A fragments of layer 2
+      uint32_t h[kMaxK / 4];
+      const uint32_t a_smem = smem_addr(s_a);
+      slice_pipeline(
+          H / 32,
+          [&](int c, float(&d)[16]) {
+            for (int kk = 0; kk < K1 / 16; kk++)
+              wgmma_n32_ss(d, make_desc(a_smem + kk * 256, sbo_a),
+                           make_desc(s_w1 + 4 * c * sbo_a + kk * 256, sbo_a), kk);
+          },
+          [&](int c, const float(&d)[16]) { bias_relu_slice(d, s_b1, c, &h[8 * c]); });
+
+      // ---- layer 2 (A = h) streamed into layer 3 ([head0 | head1 | value | pad] in
+      // 16-column slices, accumulated in o): as soon as a 32-column slice of layer 2 is packed,
+      // the two layer-3 k-steps it feeds are issued, so layer 2's output is never held whole.
+      // Every layer-3 output still accumulates its k-steps 0, 1, ..., H / 16 - 1 in order, the
+      // first with scale-d = 0.  The next tile's observations load meanwhile.
+      slice_pipeline(
+          H / 32,
+          [&](int c, float(&d)[16]) {
+#pragma unroll
+            for (int kk = 0; kk < kMaxK / 16; kk++)
+              if (kk < H / 16) wgmma_n32(d, &h[4 * kk], s_w2 + 4 * c * sbo_h + kk * 256, sbo_h, kk);
+          },
+          [&](int c, const float(&d)[16]) {
+            uint32_t a[8];
+            bias_relu_slice(d, s_b2, c, a);
+            wgmma_fence();
+#pragma unroll
+            for (int n = 0; n < kMaxN3 / 16; n++) {
+              if (n < N3 / 16) {
+#pragma unroll
+                for (int k = 0; k < 2; k++)
+                  wgmma_n16(o[n], &a[4 * k], s_w3 + 2 * n * sbo_h + (2 * c + k) * 256, sbo_h,
+                            2 * c + k);
+              }
+            }
+            wgmma_commit();
+            if (c == 0 && row0 + (long long)gdim * kTileM < rows)
+              obs_load(next, obs_src, row0 + (long long)gdim * kTileM, 0);
+          });
+      wgmma_wait<0>();
     } else {
-      // task = one 16-byte chunk (8 consecutive k) of one row; consecutive lanes take the
-      // 8 rows of a core matrix, so each shared store of a warp is bank-conflict free
-      const int nchunk = K1 / 8;
-      for (int i = lt; i < kWgRows * nchunk; i += 128) {
-        const int grp = i / (8 * nchunk), in = i - grp * 8 * nchunk;
-        const int c = in >> 3, r = 8 * grp + (in & 7);
-        const long long row = tile * kTileM + wg * kWgRows + r;
-        const float *src = obs + row * F + 8 * c;
-        float v[8];
+      // ---- layer 1 A operand -> this warpgroup's staging buffer (canonical K-major layout:
+      // (r, k) at (r / 8) * K1 * 16 + (k / 8) * 128 + (r % 8) * 16 + (k % 8) * 2).  The
+      // previous tile's layer-1 MMAs have completed (wait_group 0) in every warp.
+      wg_sync(wg);
+      if (TILES) {
+        // the warpgroup's 64 rows are one contiguous block of the tile
+        const uint4 *src = reinterpret_cast<const uint4 *>(
+            reinterpret_cast<const unsigned char *>(input) + row0 * (K1 * 2));
+        for (int i = lt; i < a_bytes / 16; i += 128)
+          reinterpret_cast<uint4 *>(s_a)[i] = __ldg(src + i);
+      } else {
+        // task = one 16-byte chunk (8 consecutive k) of one row; consecutive lanes take the
+        // 8 rows of a core matrix, so each shared store of a warp is bank-conflict free
+        const int nchunk = K1 / 8;
+        for (int i = lt; i < kWgRows * nchunk; i += 128) {
+          const int grp = i / (8 * nchunk), in = i - grp * 8 * nchunk;
+          const int c = in >> 3, r = 8 * grp + (in & 7);
+          const long long row = row0 + r;
+          const float *src = reinterpret_cast<const float *>(input) + row * F + 8 * c;
+          float v[8];
 #pragma unroll
-        for (int k = 0; k < 8; k++) v[k] = (row < rows && 8 * c + k < F) ? __ldg(src + k) : 0.0f;
-        uint4 o4;
-        o4.x = pack_bf16(v[0], v[1]); o4.y = pack_bf16(v[2], v[3]);
-        o4.z = pack_bf16(v[4], v[5]); o4.w = pack_bf16(v[6], v[7]);
-        *reinterpret_cast<uint4 *>(s_a + grp * (K1 * 16) + c * 128 + (r & 7) * 16) = o4;
+          for (int k = 0; k < 8; k++) v[k] = (row < rows && 8 * c + k < F) ? __ldg(src + k) : 0.0f;
+          uint4 o4;
+          o4.x = pack_bf16(v[0], v[1]); o4.y = pack_bf16(v[2], v[3]);
+          o4.z = pack_bf16(v[4], v[5]); o4.w = pack_bf16(v[6], v[7]);
+          *reinterpret_cast<uint4 *>(s_a + grp * (K1 * 16) + c * 128 + (r & 7) * 16) = o4;
+        }
       }
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // visible to wgmma
-    wg_sync(wg);
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // visible to wgmma
+      wg_sync(wg);
 
-    uint32_t a[kMaxK / 4], h[kMaxK / 4];
-    hidden_layer<true>(a, smem_addr(s_a), sbo_a, K1, s_w1, sbo_a, H, s_b1, h);   // layer 1
-    hidden_layer<false>(h, 0, 0, H, s_w2, sbo_h, H, s_b2, a);                     // layer 2
+      uint32_t a[kMaxK / 4], h[kMaxK / 4];
+      hidden_layer<true>(a, smem_addr(s_a), sbo_a, K1, s_w1, sbo_a, H, s_b1, h);   // layer 1
+      hidden_layer<false>(h, 0, 0, H, s_w2, sbo_h, H, s_b2, a);                     // layer 2
 
-    // ---- layer 3: [head0 | head1 | value | pad] in 16-column slices
-    float o[kMaxN3 / 16][8];   // (scale-d = 0 on the first MMA of a slice: no zeroing)
-    wgmma_fence();
+      // ---- layer 3: [head0 | head1 | value | pad] in 16-column slices
+      wgmma_fence();
 #pragma unroll
-    for (int c = 0; c < kMaxN3 / 16; c++) {
-      if (c < N3 / 16) {
+      for (int c = 0; c < kMaxN3 / 16; c++) {
+        if (c < N3 / 16) {
 #pragma unroll
-        for (int kk = 0; kk < kMaxK / 16; kk++)
-          if (kk < H / 16)
-            wgmma_n16(o[c], &a[4 * kk], s_w3 + 2 * c * sbo_h + kk * 256, sbo_h, kk);
+          for (int kk = 0; kk < kMaxK / 16; kk++)
+            if (kk < H / 16)
+              wgmma_n16(o[c], &a[4 * kk], s_w3 + 2 * c * sbo_h + kk * 256, sbo_h, kk);
+        }
       }
+      wgmma_commit();
+      wgmma_wait<0>();
     }
-    wgmma_commit_wait();
 
     // ---- output epilogue.  Logits (+ bias) -> staging [64 rows x N3]: o[c][4 j + 0/1] is
     // row 16 wr + g, o[c][4 j + 2/3] row + 8, columns 16 c + 8 j + 2 t (+1).  (The layer-1
@@ -386,12 +601,12 @@ mlp_forward_body(const unsigned char *__restrict__ blob, const void *__restrict_
   }
 }
 
-template <bool TILES>
+template <bool TILES, class Shape>
 __global__ void __launch_bounds__(kThreads, 1)
 mlp_forward_kernel(const unsigned char *__restrict__ blob, const void *__restrict__ input,
                    long long rows, float *__restrict__ probs0, float *__restrict__ probs1,
                    float *__restrict__ values, int flags) {
-  mlp_forward_body<TILES>(blob, input, rows, probs0, probs1, values, blockIdx.x, gridDim.x, flags);
+  mlp_forward_body<TILES, Shape>(blob, input, rows, probs0, probs1, values, blockIdx.x, gridDim.x, flags);
 }
 
 // Two policies in ONE grid: CTAs [0, split) run policy A, the rest policy B (each persistent
@@ -407,9 +622,9 @@ struct MlpPairArgs {
 __global__ void __launch_bounds__(kThreads, 1)
 mlp_forward_pair_kernel(const __grid_constant__ MlpPairArgs a) {
   const int w = blockIdx.x >= a.split ? 1 : 0;
-  mlp_forward_body<false>(a.blob[w], a.obs[w], a.rows[w], a.probs0[w], a.probs1[w], a.values[w],
-                          w ? blockIdx.x - a.split : blockIdx.x,
-                          w ? gridDim.x - a.split : a.split, a.flags);
+  mlp_forward_body<false, AnyShape>(a.blob[w], a.obs[w], a.rows[w], a.probs0[w], a.probs1[w],
+                                    a.values[w], w ? blockIdx.x - a.split : blockIdx.x,
+                                    w ? gridDim.x - a.split : a.split, a.flags);
 }
 
 // ---- weight packing: fp32 nn.Linear weights [out, in] -> bf16 canonical K-major tiles ------
@@ -521,6 +736,24 @@ WDB_API int wdb_mlp_pack_weights(void *stream, void *blob, const float *w1, cons
 
 namespace {
 
+template <bool TILES, class Shape>
+int launch_forward_shape(cudaStream_t stream, const void *blob, size_t smem, const void *input,
+                         long long rows, float *probs0, float *probs1, float *values) {
+  static size_t configured = 0;
+  if (smem > configured) {
+    cudaError_t e = cudaFuncSetAttribute(mlp_forward_kernel<TILES, Shape>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return (int)e;
+    configured = smem;
+  }
+  const long long n_tiles = (rows + kTileM - 1) / kTileM;
+  const int sm_budget = (g_mlp_max_ctas > 0 && g_mlp_max_ctas < kNumSMs) ? g_mlp_max_ctas : kNumSMs;
+  const int grid = (int)min((long long)sm_budget, n_tiles);
+  mlp_forward_kernel<TILES, Shape><<<grid, kThreads, smem, stream>>>(
+      reinterpret_cast<const unsigned char *>(blob), input, rows, probs0, probs1, values, 0);
+  return finish_launch();
+}
+
 template <bool TILES>
 int launch_forward(void *stream, const void *blob, int F, int H, int A0, int A1,
                    const void *input, long long rows, float *probs0, float *probs1,
@@ -532,19 +765,9 @@ int launch_forward(void *stream, const void *blob, int F, int H, int A0, int A1,
   const MlpHeader hd = make_header(F, H, A0, A1);
   const size_t smem = mlp_smem_bytes(hd);
   if (smem > 227 * 1024) return (int)cudaErrorInvalidValue;
-  static size_t configured = 0;
-  if (smem > configured) {
-    cudaError_t e = cudaFuncSetAttribute(mlp_forward_kernel<TILES>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return (int)e;
-    configured = smem;
-  }
-  const long long n_tiles = (rows + kTileM - 1) / kTileM;
-  const int sm_budget = (g_mlp_max_ctas > 0 && g_mlp_max_ctas < kNumSMs) ? g_mlp_max_ctas : kNumSMs;
-  const int grid = (int)min((long long)sm_budget, n_tiles);
-  mlp_forward_kernel<TILES><<<grid, kThreads, smem, as_stream(stream)>>>(
-      reinterpret_cast<const unsigned char *>(blob), input, rows, probs0, probs1, values, 0);
-  return finish_launch();
+  const bool fast = hd.K1 == FastShape::K1 && hd.H == FastShape::H && hd.N3 == FastShape::N3;
+  return (fast ? launch_forward_shape<TILES, FastShape> : launch_forward_shape<TILES, AnyShape>)(
+      as_stream(stream), blob, smem, input, rows, probs0, probs1, values);
 }
 
 // Launch with the programmatic-stream-serialization attribute when the "pdl" option is on:
