@@ -287,6 +287,10 @@ class RolloutEngine:
     def _tensor(self, name):
         return self.dm.data_on_device_via_torch(name)
 
+    def _slot(self, t):
+        """Batch slot of timestep t of a rollout (t < 0: an evaluation step, no slot)."""
+        return t
+
     # ---- native data movement of the generic path (csrc/wdb_rollout_generic.cu) ----------
     def _ids32(self, p):
         """int32 device copy of the policy's agent ids (None: the policy covers 0..N-1)."""
@@ -322,7 +326,8 @@ class RolloutEngine:
         scatter launch per head."""
         obs = self._tensor(_OBSERVATIONS).view(self.E, self.N, -1)
         if t >= 0:
-            obs_p = {p: self._tensor(f"{_PROCESSED_OBSERVATIONS}_batch_{p}")[t]
+            s = self._slot(t)
+            obs_p = {p: self._tensor(f"{_PROCESSED_OBSERVATIONS}_batch_{p}")[s]
                      for p in self.policies}
             self._move_rows(obs, obs_p)
         else:
@@ -368,6 +373,7 @@ class RolloutEngine:
         """done / rewards / actions -> batches, running episodic sums: ONE launch
         (wdb_rollout_bookkeep), no host synchronisation (trainer_base.py:514-601 uses
         nonzero() / len())."""
+        s = self._slot(t)
         k = _lib.Bookkeep()
         k.n_envs, k.n_agents, k.n_policies = self.E, self.N, len(self.policies)
         actions = self._tensor(_ACTIONS) if self.dm.is_data_on_device_via_torch(_ACTIONS) else None
@@ -375,7 +381,7 @@ class RolloutEngine:
         k.done = _lib.ptr(self._tensor("_done_"))
         k.rewards = _lib.ptr(self._tensor(_REWARDS))
         k.actions = _lib.ptr(actions)
-        k.done_batch = _lib.ptr(self._tensor(f"{_DONE_FLAGS}_batch")[t]) if t >= 0 else None
+        k.done_batch = _lib.ptr(self._tensor(f"{_DONE_FLAGS}_batch")[s]) if t >= 0 else None
         k.step_running_sum = _lib.ptr(self.step_running_sum)
         k.episodic_step_sum = _lib.ptr(self.episodic_step_sum)
         k.num_completed_episodes = _lib.ptr(self.num_completed_episodes)
@@ -384,9 +390,9 @@ class RolloutEngine:
             io.n_agents = len(self.policy_map[p])
             io.agent_ids = _lib.ptr(self._ids32(p))
             if t >= 0:
-                io.rewards_batch = _lib.ptr(self._tensor(f"{_REWARDS}_batch_{p}")[t])
+                io.rewards_batch = _lib.ptr(self._tensor(f"{_REWARDS}_batch_{p}")[s])
                 if actions is not None:
-                    io.actions_batch = _lib.ptr(self._tensor(f"{_ACTIONS}_batch_{p}")[t])
+                    io.actions_batch = _lib.ptr(self._tensor(f"{_ACTIONS}_batch_{p}")[s])
             io.reward_running_sum = _lib.ptr(self.reward_running_sum[p])
             io.episodic_reward_sum = _lib.ptr(self.episodic_reward_sum[p])
         _lib.check(_lib.load().wdb_rollout_bookkeep(_lib.stream_ptr(), ctypes.byref(k)),
@@ -423,7 +429,7 @@ class RolloutEngine:
             return self.step_fused(t)
         if self.sa is not None and self._sa_params_ok(sample_params):
             with torch.no_grad():
-                self.sa.launch(1, t0=max(t, 0), record=t >= 0, **sample_params)
+                self.sa.launch(1, t0=max(self._slot(t), 0), record=t >= 0, **sample_params)
             return None
         with torch.no_grad():
             probs = self.evaluate_policies(t)

@@ -31,6 +31,7 @@ from warp_drive_b200.training.models.fully_connected import ModelFactory
 from warp_drive_b200.training.rollout import RolloutEngine
 from warp_drive_b200.training.utils.data_loader import (
     create_and_push_data_placeholders, validate_policy_map)
+from warp_drive_b200.training.utils.flat_adam import FlatAdam
 from warp_drive_b200.training.utils.param_scheduler import ParamScheduler
 from warp_drive_b200.utils.constants import Constants
 
@@ -98,12 +99,7 @@ class Trainer:
                  results_dir=None, verbose=True, use_cuda_graph=True):
         assert env_wrapper is not None and env_wrapper.env_backend != "cpu"
         assert config is not None
-        assert obs_dim_corresponding_to_num_agents in ("first", "last")
-        # the rollout engine views observations as [E, N, F]; 'last' ([E, ..., N]) would be
-        # silently scrambled across agents and features
-        assert obs_dim_corresponding_to_num_agents == "first", (
-            "obs_dim_corresponding_to_num_agents='last' is not supported by the native rollout "
-            "engine (observations must be [num_envs, num_agents, ...])")
+        self._check_obs_dim(obs_dim_corresponding_to_num_agents)
         assert not create_separate_placeholders_for_each_policy, (
             "separate per-policy step placeholders are not implemented in the native trainer")
         self.cuda_envs = env_wrapper
@@ -115,8 +111,7 @@ class Trainer:
         self.config = config
         config["trainer"] = recursive_merge_config_dicts(config["trainer"], default["trainer"])
         for key in config["policy"]:
-            config["policy"][key] = recursive_merge_config_dicts(config["policy"][key],
-                                                                 default["policy"])
+            self._merge_policy_defaults(config["policy"][key], default["policy"])
         config["saving"] = recursive_merge_config_dicts(config["saving"], default["saving"])
         self.sample_params_schedules = {
             k: ParamScheduler(v) for k, v in config.get("sampler", {}).get("params", {}).items()}
@@ -142,6 +137,7 @@ class Trainer:
         assert self.num_envs == env_wrapper.n_envs
         self.training_batch_size_per_env = self.training_batch_size // self.num_envs
         assert self.training_batch_size_per_env > 0
+        batch_slots_per_env = self._batch_slots_per_env(t)
 
         # first reset pushes every array to HBM
         self.cuda_envs.reset_all_envs()
@@ -150,7 +146,7 @@ class Trainer:
             env_wrapper=self.cuda_envs, action_sampler=self.cuda_sample_controller,
             policy_tag_to_agent_id_map=self.policy_tag_to_agent_id_map,
             obs_dim_corresponding_to_num_agents=obs_dim_corresponding_to_num_agents,
-            training_batch_size_per_env=self.training_batch_size_per_env)
+            training_batch_size_per_env=batch_slots_per_env)
         seed = int(t.get("seed", np.int32(time.time()))) + self.device_id
         self.seed = seed
         self.cuda_sample_controller.init_random(seed)
@@ -166,21 +162,22 @@ class Trainer:
                              "Please increase the number of episodes or reduce the training "
                              "batch size.")
 
-        self.models, self.optimizers, self.lr_schedules, self.trainers = {}, {}, {}, {}
+        self.trainers = {}
         self.clip_grad_norm, self.max_grad_norm, self.current_timestep = {}, {}, {}
+        self._create_network_dicts()
         for policy in self.policies:
             self.current_timestep[policy] = 0
             self._initialize_policy_model(policy)
         self.load_model_checkpoint()
         for policy in self.policies:
-            self.models[policy].cuda()
+            for model in self._all_networks(policy):
+                model.cuda()
         # ONE flat float32 arena for the parameters and one for the gradients of every trained
-        # policy: Adam / clipping run as flat kernels (utils/flat_adam.py) and the multi-GPU
+        # network: Adam / clipping run as flat kernels (utils/flat_adam.py) and the multi-GPU
         # gradient all-reduce is a single in-place NCCL call on `_arena_grads`
-        from warp_drive_b200.training.utils.flat_adam import FlatAdam
-
-        total = sum(FlatAdam.numel(self.models[p].parameters()) for p in self.policies)
-        dev = next(self.models[self.policies[0]].parameters()).device
+        nets = [m for p in self.policies for m in self._trained_networks(p)]
+        total = sum(FlatAdam.numel(m.parameters()) for m in nets)
+        dev = next(nets[0].parameters()).device
         self._arena_params = torch.zeros(total, dtype=torch.float32, device=dev)
         self._arena_grads = torch.zeros(total, dtype=torch.float32, device=dev)
         self._arena_off = 0
@@ -190,14 +187,56 @@ class Trainer:
             self._initialize_policy_algorithm(policy)
         if self.num_devices > 1:
             self._broadcast_parameters()
-
-        self.engine = RolloutEngine(self.cuda_envs, self.models,
-                                    self.policy_tag_to_agent_id_map,
-                                    self.cuda_sample_controller,
-                                    self.training_batch_size_per_env,
-                                    use_cuda_graph=use_cuda_graph)
+        self.engine = self._make_engine(use_cuda_graph)
         self.perf_stats = PerfStats()
-        self._flat_grad = None
+
+    # ------------------------------------------------------------------ what subclasses change
+    @staticmethod
+    def _check_obs_dim(obs_dim_corresponding_to_num_agents):
+        assert obs_dim_corresponding_to_num_agents in ("first", "last")
+        # the rollout engine views observations as [E, N, F]; 'last' ([E, ..., N]) would be
+        # silently scrambled across agents and features
+        assert obs_dim_corresponding_to_num_agents == "first", (
+            "obs_dim_corresponding_to_num_agents='last' is not supported by the native rollout "
+            "engine (observations must be [num_envs, num_agents, ...])")
+
+    @staticmethod
+    def _merge_policy_defaults(policy_config, defaults):
+        recursive_merge_config_dicts(policy_config, defaults)
+
+    def _batch_slots_per_env(self, trainer_config):
+        """Timesteps per env that the `*_batch*` arrays hold."""
+        return self.training_batch_size_per_env
+
+    def _create_network_dicts(self):
+        self.models, self.optimizers, self.lr_schedules = {}, {}, {}
+
+    def _initialize_policy_model(self, policy):
+        self.models[policy] = self._build_model(
+            policy, self._get_config(["policy", policy, "model"]))
+
+    def _trained_networks(self, policy):
+        """The networks of `policy` that an optimizer updates, in arena order."""
+        return [self.models[policy]]
+
+    def _all_networks(self, policy):
+        """Every network of `policy`: moved to the GPU and broadcast from rank 0."""
+        return self._trained_networks(policy)
+
+    def _initialize_optimizer(self, policy):
+        self.lr_schedules[policy] = ParamScheduler(self._get_config(["policy", policy, "lr"]))
+        self.optimizers[policy] = self._flat_adam(
+            self.models[policy],
+            self.lr_schedules[policy].get_param_value(self.current_timestep[policy]))
+
+    def _optimizers_of(self, policy):
+        """(metric-key suffix, FlatAdam, lr schedule) of each network `policy` trains."""
+        return [("", self.optimizers[policy], self.lr_schedules[policy])]
+
+    def _make_engine(self, use_cuda_graph):
+        return RolloutEngine(self.cuda_envs, self.models, self.policy_tag_to_agent_id_map,
+                             self.cuda_sample_controller, self.training_batch_size_per_env,
+                             use_cuda_graph=use_cuda_graph)
 
     # ------------------------------------------------------------------ setup helpers
     def _get_config(self, args):
@@ -206,28 +245,23 @@ class Trainer:
             cfg = cfg[a]
         return cfg
 
-    def _initialize_policy_model(self, policy):
-        mcfg = self._get_config(["policy", policy, "model"])
-        model = ModelFactory.create(mcfg["type"])(
-            env=self.cuda_envs, model_config=mcfg, policy=policy,
+    def _build_model(self, policy, model_config):
+        model = ModelFactory.create(model_config["type"])(
+            env=self.cuda_envs, model_config=model_config, policy=policy,
             policy_tag_to_agent_id_map=self.policy_tag_to_agent_id_map)
-        if mcfg.get("init_method") == "xavier":
+        if model_config.get("init_method") == "xavier":
             for m in model.modules():
                 if isinstance(m, nn.Linear):
                     nn.init.xavier_uniform_(m.weight)
-        self.models[policy] = model
+        return model
 
-    def _initialize_optimizer(self, policy):
-        self.lr_schedules[policy] = ParamScheduler(self._get_config(["policy", policy, "lr"]))
-        lr = self.lr_schedules[policy].get_param_value(self.current_timestep[policy])
-        from warp_drive_b200.training.utils.flat_adam import FlatAdam
-
-        n = FlatAdam.numel(self.models[policy].parameters())
+    def _flat_adam(self, model, lr):
+        """FlatAdam over `model` on the next slice of the parameter / gradient arena."""
+        n = FlatAdam.numel(model.parameters())
         lo = self._arena_off
         self._arena_off += n
-        self.optimizers[policy] = FlatAdam(
-            self.models[policy].parameters(), lr=lr,
-            arena=(self._arena_params[lo:lo + n], self._arena_grads[lo:lo + n]))
+        return FlatAdam(model.parameters(), lr=lr,
+                        arena=(self._arena_params[lo:lo + n], self._arena_grads[lo:lo + n]))
 
     def _initialize_policy_algorithm(self, policy):
         c = self._get_config(["policy", policy])
@@ -243,14 +277,16 @@ class Trainer:
 
     # ------------------------------------------------------------------ multi-GPU
     def _trained_params(self):
-        return [p for pol in self.policies_to_train for p in self.models[pol].parameters()]
+        return [p for pol in self.policies_to_train for m in self._trained_networks(pol)
+                for p in m.parameters()]
 
     def _broadcast_parameters(self):
         import torch.distributed as dist
 
         for pol in self.policies:
-            for p in self.models[pol].parameters():
-                dist.broadcast(p.data, src=0)
+            for m in self._all_networks(pol):
+                for p in m.parameters():
+                    dist.broadcast(p.data, src=0)
 
     def _allreduce_gradients(self):
         """ONE NCCL all-reduce (mean) over the gradients of every policy, in place on the flat
@@ -293,43 +329,61 @@ class Trainer:
         return params
 
     def _update_model_params(self, iteration):
-        saving = self.config["saving"]
-        logging_flag = (iteration % saving["metrics_log_freq"] == 0
-                        or iteration == self.num_iters - 1)
+        logging_flag = self._is_logging_iteration(iteration)
         dm = self.cuda_envs.cuda_data_manager
         done_flags_batch = dm.data_on_device_via_torch(f"{_DONE_FLAGS}_batch")
-        losses, metrics_dict = {}, {}
+        loss_metrics = {}
         for policy in self.policies_to_train:
             actions = dm.data_on_device_via_torch(f"{_ACTIONS}_batch_{policy}")
             rewards = dm.data_on_device_via_torch(f"{_REWARDS}_batch_{policy}")
             obs = dm.data_on_device_via_torch(f"{_PROCESSED_OBSERVATIONS}_batch_{policy}")
             probs, values = self.models[policy](obs=obs)
-            self.current_timestep[policy] += self.training_batch_size
-            loss, metrics = self.trainers[policy].compute_loss_and_metrics(
+            self._advance_timestep(policy)
+            loss, loss_metrics[policy] = self.trainers[policy].compute_loss_and_metrics(
                 self.current_timestep[policy], actions.long(), rewards, done_flags_batch,
                 probs, values, perform_logging=logging_flag,
                 negative_positive_ratio=self.config["trainer"].get("neg_pos_env_ratio", -1))
-            lr = self.lr_schedules[policy].get_param_value(self.current_timestep[policy])
-            for group in self.optimizers[policy].param_groups:
-                group["lr"] = lr
             self.optimizers[policy].zero_grad()
             loss.backward()
-            losses[policy] = (loss, metrics, lr)
-        if self.num_devices > 1 and losses:
+        return self._step_optimizers(loss_metrics, logging_flag)
+
+    def _is_logging_iteration(self, iteration):
+        return (iteration % self.config["saving"]["metrics_log_freq"] == 0
+                or iteration == self.num_iters - 1)
+
+    def _advance_timestep(self, policy):
+        """Count one training batch for `policy` and set its learning rates for that step."""
+        self.current_timestep[policy] += self.training_batch_size
+        for _, optimizer, schedule in self._optimizers_of(policy):
+            optimizer.param_groups[0]["lr"] = schedule.get_param_value(
+                self.current_timestep[policy])
+
+    def _step_optimizers(self, loss_metrics, logging_flag):
+        """The update once the gradients of the policies in `loss_metrics` are in the arena:
+        one all-reduce, then clipping + Adam per network.  On a logging iteration, returns the
+        metrics of every trained policy and restarts the episodic counters."""
+        if self.num_devices > 1 and loss_metrics:
             self._allreduce_gradients()
-        for policy, (loss, metrics, lr) in losses.items():
-            grad_norm = None
+        metrics_dict = {}
+        for policy in self.policies_to_train:
+            optimizers = self._optimizers_of(policy) if policy in loss_metrics else []
+            norms, lrs = {}, {}
             if logging_flag:
-                grad_norm = float(sum(p.grad.norm(2) for p in self.models[policy].parameters()
-                                      if p.grad is not None))
+                for suffix, opt, _ in optimizers:
+                    norms[f"Gradient norm{suffix}"] = float(sum(
+                        p.grad.norm(2) for p in opt.param_list if p.grad is not None))
+                    lrs[f"Learning rate{suffix}"] = opt.param_groups[0]["lr"]
             # clip_grad_norm_ + Adam as two flat kernels, clip factor stays on the device
-            self.optimizers[policy].step(
-                max_grad_norm=self.max_grad_norm[policy] if self.clip_grad_norm[policy] else None)
+            clip = self.max_grad_norm[policy] if self.clip_grad_norm[policy] else None
+            for _, opt, _ in optimizers:
+                opt.step(max_grad_norm=clip)
             if logging_flag:
                 n_done = int(self.engine.num_completed_episodes)
+                metrics = loss_metrics.get(policy, {})
+                metrics["Current timestep"] = self.current_timestep[policy]
+                metrics.update(norms)
+                metrics.update(lrs)
                 metrics.update({
-                    "Current timestep": self.current_timestep[policy],
-                    "Gradient norm": grad_norm, "Learning rate": lr,
                     "Mean episodic reward":
                         float(self.engine.episodic_reward_sum[policy]) / (n_done + _EPSILON),
                     "Mean episodic steps":
@@ -372,29 +426,39 @@ class Trainer:
             return
         freq = self.config["saving"]["model_params_save_freq"]
         if iteration % freq == 0 or iteration == self.num_iters - 1:
-            for policy, model in self.models.items():
+            for policy, name, model in self._checkpointed_networks():
                 path = os.path.join(
-                    self.save_dir, f"{policy}_{self.current_timestep[policy]}.state_dict")
+                    self.save_dir, f"{name}_{self.current_timestep[policy]}.state_dict")
                 if self.verbose:
-                    verbose_print(f"Saving the '{policy}' torch model to the file: '{path}'.",
+                    verbose_print(f"Saving the '{name}' torch model to the file: '{path}'.",
                                   self.device_id)
                 torch.save(model.state_dict(), path)
 
+    def _checkpointed_networks(self):
+        """(policy, file name prefix, network) of every network a checkpoint saves."""
+        return [(policy, policy, model) for policy, model in self.models.items()]
+
+    @staticmethod
+    def _checkpoint_timestep(path):
+        """The timestep encoded in a checkpoint's file name ({prefix}_{timestep}.state_dict)."""
+        return int(os.path.basename(path).split(".state_dict")[0].split("_")[-1])
+
     def load_model_checkpoint(self, ckpts_dict=None):
         if ckpts_dict is None:
-            ckpts_dict = {p: self.config["policy"][p]["model"]["model_ckpt_filepath"]
+            ckpts_dict = {p: self.config["policy"][p]["model"].get("model_ckpt_filepath", "")
                           for p in self.policies}
         for policy, path in ckpts_dict.items():
             assert policy in self.policies
-            if path:
-                assert os.path.isfile(path), "Invalid model checkpoint path!"
-                self.models[policy].load_state_dict(torch.load(path, map_location="cpu"))
-                # the timestep is encoded in the file name ({policy}_{timestep}.state_dict)
-                self.current_timestep[policy] = int(
-                    os.path.basename(path).split(".state_dict")[0].split("_")[-1])
+            self._load_policy_checkpoint(policy, path)
         # the tensor-core rollout forward keeps its own packed bf16 copy of the weights
         if getattr(self, "engine", None) is not None:
             self.engine.refresh_forward_weights()
+
+    def _load_policy_checkpoint(self, policy, path):
+        if path:
+            assert os.path.isfile(path), "Invalid model checkpoint path!"
+            self.models[policy].load_state_dict(torch.load(path, map_location="cpu"))
+            self.current_timestep[policy] = self._checkpoint_timestep(path)
 
     def graceful_close(self):
         self.cuda_sample_controller = None
@@ -419,8 +483,8 @@ class Trainer:
         done = dm.data_on_device_via_torch("_done_")
         with torch.no_grad():
             for _ in range(self.cuda_envs.episode_length):
-                probs = RolloutEngine.evaluate_policies(eng, -1)
-                RolloutEngine.sample_actions(eng, probs, -1, **sample_params)
+                probs = eng.evaluate_policies(-1)
+                eng.sample_actions(probs, -1, **sample_params)
                 self.cuda_envs.step_all_envs()
                 undone = done == 0
                 rewards = dm.data_on_device_via_torch(_REWARDS)

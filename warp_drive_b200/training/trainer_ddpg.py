@@ -27,27 +27,15 @@ Underneath:
     updates;
   * multi-GPU: one flat NCCL all-reduce over actor + critic gradients per iteration.
 """
-import json
 import os
-import random
-import time
 
-import numpy as np
 import torch
-import yaml
-from torch import nn
 
-from warp_drive_b200.managers.function_manager import CUDASampler
 from warp_drive_b200.training.algorithms.ddpg import DDPG
 from warp_drive_b200.training.algorithms.fused_ddpg import FusedDDPGUpdate, fused_ddpg_supported
-from warp_drive_b200.training.models.fully_connected import ModelFactory
 from warp_drive_b200.training.models.fully_connected_actor_critic import ActorAsPolicy
 from warp_drive_b200.training.rollout import RolloutEngine
-from warp_drive_b200.training.trainer import (
-    _CONFIG_DIR, PerfStats, Trainer, recursive_merge_config_dicts, verbose_print)
-from warp_drive_b200.training.utils.data_loader import (
-    create_and_push_data_placeholders, validate_policy_map)
-from warp_drive_b200.training.utils.flat_adam import FlatAdam
+from warp_drive_b200.training.trainer import Trainer
 from warp_drive_b200.training.utils.param_scheduler import ParamScheduler
 from warp_drive_b200.utils.constants import Constants
 
@@ -55,7 +43,6 @@ _ACTIONS = Constants.ACTIONS
 _REWARDS = Constants.REWARDS
 _DONE_FLAGS = Constants.DONE_FLAGS
 _PROCESSED_OBSERVATIONS = Constants.PROCESSED_OBSERVATIONS
-_EPSILON = 1e-10
 
 
 def soft_update(target, source, tau):
@@ -89,22 +76,6 @@ class RingRolloutEngine(RolloutEngine):
     def _slot(self, t):
         return t if t < 0 else (self.ring_cursor + t) % self.ring_capacity
 
-    def step(self, t, **sample_params):
-        if self.sa is not None and t >= 0 and self._sa_params_ok(sample_params):
-            with torch.no_grad():
-                self.sa.launch(1, t0=self._slot(t), **sample_params)
-            return None
-        return super().step(t, **sample_params)
-
-    def evaluate_policies(self, t):
-        return super().evaluate_policies(self._slot(t))
-
-    def sample_actions(self, probs, t, **sample_params):
-        return super().sample_actions(probs, self._slot(t), **sample_params)
-
-    def bookkeep(self, t):
-        return super().bookkeep(self._slot(t))
-
     def rollout(self, **sample_params):
         if self.sa is not None and self._sa_params_ok(sample_params):
             # slots cursor .. cursor + T - 1 (mod capacity): at most two launches, split at
@@ -133,119 +104,46 @@ class RingRolloutEngine(RolloutEngine):
 
 
 class TrainerDDPG(Trainer):
+    """Trainer's setup, update tail and checkpointing; what differs is an actor, a critic and
+    their target networks per policy, the replay ring and the DDPG update."""
+
     def __init__(self, env_wrapper=None, config=None, policy_tag_to_agent_id_map=None,
                  create_separate_placeholders_for_each_policy=False,
                  obs_dim_corresponding_to_num_agents="first", num_devices=1, device_id=0,
                  results_dir=None, verbose=True):
-        assert env_wrapper is not None and env_wrapper.env_backend != "cpu"
-        assert config is not None
-        assert not create_separate_placeholders_for_each_policy, (
-            "separate per-policy step placeholders are not implemented in the native trainer")
-        self.cuda_envs = env_wrapper
-        self.verbose = verbose
-        self.num_devices, self.device_id = num_devices, device_id
+        super().__init__(env_wrapper, config, policy_tag_to_agent_id_map,
+                         create_separate_placeholders_for_each_policy,
+                         obs_dim_corresponding_to_num_agents, num_devices, device_id,
+                         results_dir, verbose, use_cuda_graph=False)
 
-        with open(os.path.join(_CONFIG_DIR, "default_configs.yaml"), encoding="utf8") as fp:
-            default = yaml.safe_load(fp)
-        self.config = config
-        config["trainer"] = recursive_merge_config_dicts(config["trainer"], default["trainer"])
-        for key in config["policy"]:
-            # actor / critic sub-dicts of `model` and `lr` are kept as given
-            for k, v in default["policy"].items():
-                config["policy"][key].setdefault(k, v)
-        config["saving"] = recursive_merge_config_dicts(config["saving"], default["saving"])
-        self.sample_params_schedules = {
-            k: ParamScheduler(v) for k, v in config.get("sampler", {}).get("params", {}).items()}
+    # ------------------------------------------------------------------ setup
+    @staticmethod
+    def _check_obs_dim(obs_dim_corresponding_to_num_agents):
+        """Either layout is passed on to the step placeholders as given."""
 
-        results_dir = results_dir or f"{time.time():10.0f}"
-        s = config["saving"]
-        self.save_dir = os.path.join(s["basedir"], s["name"], s["tag"], results_dir)
-        os.makedirs(self.save_dir, exist_ok=True)
-        with open(os.path.join(self.save_dir, "run_config.json"), "a+", encoding="utf8") as fp:
-            json.dump(config, fp)
-            fp.write("\n")
+    @staticmethod
+    def _merge_policy_defaults(policy_config, defaults):
+        # actor / critic sub-dicts of `model` and `lr` are kept as given
+        for k, v in defaults.items():
+            policy_config.setdefault(k, v)
 
-        self.policy_tag_to_agent_id_map = validate_policy_map(env_wrapper,
-                                                              policy_tag_to_agent_id_map)
-        self.policies = list(config["policy"].keys())
-        assert set(self.policies) == set(self.policy_tag_to_agent_id_map.keys())
-        self.policies_to_train = [p for p in self.policies if config["policy"][p]["to_train"]]
-
-        t = config["trainer"]
-        self.num_episodes = t["num_episodes"]
-        self.training_batch_size = t["train_batch_size"]
-        self.num_envs = t["num_envs"]
-        assert self.num_envs == env_wrapper.n_envs
-        self.training_batch_size_per_env = self.training_batch_size // self.num_envs
-        assert self.training_batch_size_per_env > 0
-        self.n_step = int(t.get("n_step", 1))
+    def _batch_slots_per_env(self, trainer_config):
+        """The replay ring: one rollout plus the n_step - 1 slots the n-step target looks
+        ahead."""
+        self.n_step = int(trainer_config.get("n_step", 1))
         assert self.n_step >= 1
         self.ring_capacity = self.training_batch_size_per_env + self.n_step - 1
+        return self.ring_capacity
 
-        self.cuda_envs.reset_all_envs()
-        self.cuda_sample_controller = CUDASampler(self.cuda_envs.cuda_function_manager)
-        create_and_push_data_placeholders(
-            env_wrapper=self.cuda_envs, action_sampler=self.cuda_sample_controller,
-            policy_tag_to_agent_id_map=self.policy_tag_to_agent_id_map,
-            obs_dim_corresponding_to_num_agents=obs_dim_corresponding_to_num_agents,
-            training_batch_size_per_env=self.ring_capacity)
-        seed = int(t.get("seed", np.int32(time.time()))) + self.device_id
-        self.seed = seed
-        self.cuda_sample_controller.init_random(seed)
-        torch.manual_seed(seed)
-        random.seed(seed)
-        np.random.seed(seed)
-        self.cuda_envs.init_reset_pool(seed + random.randint(1, 10000))
-
-        self.total_steps = self.cuda_envs.episode_length * self.num_episodes
-        self.num_iters = int(self.total_steps // self.training_batch_size)
-        if self.num_iters == 0:
-            raise ValueError("Not enough steps to even perform a single training iteration!. "
-                             "Please increase the number of episodes or reduce the training "
-                             "batch size.")
-
+    def _create_network_dicts(self):
         self.actor_models, self.critic_models = {}, {}
         self.target_actor_models, self.target_critic_models = {}, {}
         self.actor_optimizers, self.critic_optimizers = {}, {}
         self.actor_lr_schedules, self.critic_lr_schedules = {}, {}
-        self.tau, self.trainers = {}, {}
-        self.clip_grad_norm, self.max_grad_norm, self.current_timestep = {}, {}, {}
-        for policy in self.policies:
-            self.current_timestep[policy] = 0
-            self._initialize_policy_model(policy)
-        self.load_model_checkpoint()
-        for policy in self.policies:
-            for group in (self.actor_models, self.critic_models, self.target_actor_models,
-                          self.target_critic_models):
-                group[policy].cuda()
-        # ONE flat float32 arena for the parameters and one for the gradients of every actor
-        # and critic (Trainer's layout): the multi-GPU all-reduce is one in-place NCCL call on
-        # `_arena_grads`
-        nets = [g[p] for p in self.policies for g in (self.actor_models, self.critic_models)]
-        total = sum(FlatAdam.numel(m.parameters()) for m in nets)
-        dev = next(nets[0].parameters()).device
-        self._arena_params = torch.zeros(total, dtype=torch.float32, device=dev)
-        self._arena_grads = torch.zeros(total, dtype=torch.float32, device=dev)
-        self._arena_off = 0
-        for policy in self.policies:
-            self._initialize_optimizer(policy)
-        self.fused_updates = {}
-        for policy in self.policies_to_train:
-            self._initialize_policy_algorithm(policy)
-        if self.num_devices > 1:
-            self._broadcast_parameters()
-
-        # names the base class' helpers use (checkpointing is overridden below)
+        self.tau, self.fused_updates = {}, {}
+        # `models`: the networks the rollout runs
         self.models = self.actor_models
-        self.engine = RingRolloutEngine(
-            self.cuda_envs, {p: ActorAsPolicy(self.actor_models[p]) for p in self.policies},
-            self.policy_tag_to_agent_id_map, self.cuda_sample_controller,
-            self.training_batch_size_per_env, ring_capacity=self.ring_capacity)
-        assert self.engine.continuous, "DDPG needs a continuous (Box) action space"
-        self.perf_stats = PerfStats()
-        self._flat_grad = None
 
-    # ------------------------------------------------------------------ setup helpers
     def _split(self, policy, key):
         """(actor part, critic part) of a config entry that may or may not be split."""
         value = self._get_config(["policy", policy, key])
@@ -255,41 +153,33 @@ class TrainerDDPG(Trainer):
 
     def _initialize_policy_model(self, policy):
         actor_cfg, critic_cfg = self._split(policy, "model")
-
-        def build(cfg):
-            model = ModelFactory.create(cfg["type"])(
-                env=self.cuda_envs, model_config=cfg, policy=policy,
-                policy_tag_to_agent_id_map=self.policy_tag_to_agent_id_map)
-            if cfg.get("init_method") == "xavier":
-                for m in model.modules():
-                    if isinstance(m, nn.Linear):
-                        nn.init.xavier_uniform_(m.weight)
-            return model
-
-        self.actor_models[policy] = build(actor_cfg)
-        self.target_actor_models[policy] = build(actor_cfg)
+        self.actor_models[policy] = self._build_model(policy, actor_cfg)
+        self.target_actor_models[policy] = self._build_model(policy, actor_cfg)
         hard_update(self.target_actor_models[policy], self.actor_models[policy])
-        self.critic_models[policy] = build(critic_cfg)
-        self.target_critic_models[policy] = build(critic_cfg)
+        self.critic_models[policy] = self._build_model(policy, critic_cfg)
+        self.target_critic_models[policy] = self._build_model(policy, critic_cfg)
         hard_update(self.target_critic_models[policy], self.critic_models[policy])
+
+    def _trained_networks(self, policy):
+        return [self.actor_models[policy], self.critic_models[policy]]
+
+    def _all_networks(self, policy):
+        return self._trained_networks(policy) + [self.target_actor_models[policy],
+                                                 self.target_critic_models[policy]]
 
     def _initialize_optimizer(self, policy):
         actor_lr, critic_lr = self._split(policy, "lr")
         self.actor_lr_schedules[policy] = ParamScheduler(actor_lr)
         self.critic_lr_schedules[policy] = ParamScheduler(critic_lr)
         ts = self.current_timestep[policy]
-
-        def flat_adam(model, lr):
-            n = FlatAdam.numel(model.parameters())
-            lo = self._arena_off
-            self._arena_off += n
-            return FlatAdam(model.parameters(), lr=lr, arena=(
-                self._arena_params[lo:lo + n], self._arena_grads[lo:lo + n]))
-
-        self.actor_optimizers[policy] = flat_adam(
+        self.actor_optimizers[policy] = self._flat_adam(
             self.actor_models[policy], self.actor_lr_schedules[policy].get_param_value(ts))
-        self.critic_optimizers[policy] = flat_adam(
+        self.critic_optimizers[policy] = self._flat_adam(
             self.critic_models[policy], self.critic_lr_schedules[policy].get_param_value(ts))
+
+    def _optimizers_of(self, policy):
+        return [(" (Actor)", self.actor_optimizers[policy], self.actor_lr_schedules[policy]),
+                (" (Critic)", self.critic_optimizers[policy], self.critic_lr_schedules[policy])]
 
     def _initialize_policy_algorithm(self, policy):
         c = self._get_config(["policy", policy])
@@ -309,82 +199,38 @@ class TrainerDDPG(Trainer):
                 actor, critic, self.target_actor_models[policy],
                 self.target_critic_models[policy], *args, gamma=c["gamma"])
 
-    # ------------------------------------------------------------------ multi-GPU
-    def _trained_params(self):
-        return [p for pol in self.policies_to_train
-                for m in (self.actor_models[pol], self.critic_models[pol])
-                for p in m.parameters()]
-
-    def _broadcast_parameters(self):
-        import torch.distributed as dist
-
-        for pol in self.policies:
-            for m in (self.actor_models[pol], self.critic_models[pol],
-                      self.target_actor_models[pol], self.target_critic_models[pol]):
-                for p in m.parameters():
-                    dist.broadcast(p.data, src=0)
+    def _make_engine(self, use_cuda_graph):
+        engine = RingRolloutEngine(
+            self.cuda_envs, {p: ActorAsPolicy(self.actor_models[p]) for p in self.policies},
+            self.policy_tag_to_agent_id_map, self.cuda_sample_controller,
+            self.training_batch_size_per_env, ring_capacity=self.ring_capacity)
+        assert engine.continuous, "DDPG needs a continuous (Box) action space"
+        return engine
 
     # ------------------------------------------------------------------ update
     def _update_model_params(self, iteration):
-        saving = self.config["saving"]
-        logging_flag = (iteration % saving["metrics_log_freq"] == 0
-                        or iteration == self.num_iters - 1)
-        eng = self.engine
-        metrics_dict = {}
-        stepped = []
-        if eng.isfull():
+        logging_flag = self._is_logging_iteration(iteration)
+        loss_metrics = {}
+        if self.engine.isfull():       # until then the rollouts only fill the replay ring
             for policy in self.policies_to_train:
-                self.current_timestep[policy] += self.training_batch_size
-                actor_lr = self.actor_lr_schedules[policy].get_param_value(
-                    self.current_timestep[policy])
-                critic_lr = self.critic_lr_schedules[policy].get_param_value(
-                    self.current_timestep[policy])
-                self.actor_optimizers[policy].param_groups[0]["lr"] = actor_lr
-                self.critic_optimizers[policy].param_groups[0]["lr"] = critic_lr
+                self._advance_timestep(policy)
                 fused = self.fused_updates.get(policy)
                 if fused is not None and self.trainers[policy].use_fused_update:
-                    metrics = self._fused_gradients(policy, fused, logging_flag)
+                    loss_metrics[policy] = self._fused_gradients(policy, fused, logging_flag)
                 else:
-                    metrics = self._torch_gradients(policy, logging_flag)
-                stepped.append((policy, metrics, actor_lr, critic_lr))
-            if self.num_devices > 1 and stepped:
-                self._allreduce_gradients()
-        for policy, metrics, actor_lr, critic_lr in stepped:
-            actor, critic = self.actor_models[policy], self.critic_models[policy]
-            if logging_flag:
-                metrics["Gradient norm (Actor)"] = float(sum(
-                    p.grad.norm(2) for p in actor.parameters() if p.grad is not None))
-                metrics["Gradient norm (Critic)"] = float(sum(
-                    p.grad.norm(2) for p in critic.parameters() if p.grad is not None))
-            # clip_grad_norm_ + Adam per network as two flat kernels each
-            clip = self.max_grad_norm[policy] if self.clip_grad_norm[policy] else None
-            self.actor_optimizers[policy].step(max_grad_norm=clip)
-            self.critic_optimizers[policy].step(max_grad_norm=clip)
-            soft_update(self.target_actor_models[policy], actor, self.tau[policy])
-            soft_update(self.target_critic_models[policy], critic, self.tau[policy])
-            if logging_flag:
-                metrics.update({"Learning rate (Actor)": actor_lr,
-                                "Learning rate (Critic)": critic_lr})
-        if logging_flag:
-            n_done = int(eng.num_completed_episodes)
+                    loss_metrics[policy] = self._torch_gradients(policy, logging_flag)
+        metrics_dict = self._step_optimizers(loss_metrics, logging_flag)
+        for policy in loss_metrics:
+            soft_update(self.target_actor_models[policy], self.actor_models[policy],
+                        self.tau[policy])
+            soft_update(self.target_critic_models[policy], self.critic_models[policy],
+                        self.tau[policy])
+        if logging_flag and self.config["trainer"].get("evaluator"):
+            reward_sum, step_sum = self.evaluate_episodes(scale=0)
             for policy in self.policies_to_train:
-                m = next((x[1] for x in stepped if x[0] == policy), {})
-                m.update({
-                    "Current timestep": self.current_timestep[policy],
-                    "Mean episodic reward":
-                        float(eng.episodic_reward_sum[policy]) / (n_done + _EPSILON),
-                    "Mean episodic steps": float(eng.episodic_step_sum) / (n_done + _EPSILON)})
-                metrics_dict[policy] = m
-            for policy in self.policies:
-                eng.episodic_reward_sum[policy].zero_()
-            eng.episodic_step_sum.zero_()
-            eng.num_completed_episodes.zero_()
-            if self.config["trainer"].get("evaluator"):
-                reward_sum, step_sum = self.evaluate_episodes(scale=0)
-                for policy in self.policies_to_train:
-                    metrics_dict[policy].update({
-                        "Mean episodic reward (test)": float(reward_sum[policy].mean()),
-                        "Mean episodic steps (test)": float(step_sum[policy].float().mean())})
+                metrics_dict[policy].update({
+                    "Mean episodic reward (test)": float(reward_sum[policy].mean()),
+                    "Mean episodic steps (test)": float(step_sum[policy].float().mean())})
         return metrics_dict
 
     def _torch_gradients(self, policy, logging_flag):
@@ -436,40 +282,21 @@ class TrainerDDPG(Trainer):
             -s[1] / fused.rows, s[0] / fused.rows, rewards, actions, values, j_values, returns)
 
     # ------------------------------------------------------------------ checkpoints
-    def save_model_checkpoint(self, iteration=0):
-        if self.device_id != 0:
-            return
-        freq = self.config["saving"]["model_params_save_freq"]
-        if iteration % freq == 0 or iteration == self.num_iters - 1:
-            for kind, models in (("actor", self.actor_models), ("critic", self.critic_models)):
-                for policy, model in models.items():
-                    path = os.path.join(
-                        self.save_dir,
-                        f"{policy}_{kind}_{self.current_timestep[policy]}.state_dict")
-                    if self.verbose:
-                        verbose_print(f"Saving the '{policy}' ({kind}) torch model to the "
-                                      f"file: '{path}'.", self.device_id)
-                    torch.save(model.state_dict(), path)
+    def _checkpointed_networks(self):
+        return [(policy, f"{policy}_{kind}", model)
+                for kind, models in (("actor", self.actor_models), ("critic", self.critic_models))
+                for policy, model in models.items()]
 
-    def load_model_checkpoint(self, ckpts_dict=None):
-        if ckpts_dict is None:
-            ckpts_dict = {}
-            for p in self.policies:
-                model_cfg = self.config["policy"][p]["model"]
-                ckpts_dict[p] = model_cfg.get("model_ckpt_filepath", "") if isinstance(
-                    model_cfg, dict) else ""
-        for policy, paths in ckpts_dict.items():
-            assert policy in self.policies
-            if not (isinstance(paths, dict) and paths.get("actor") and paths.get("critic")):
-                continue
-            assert os.path.isfile(paths["actor"]), "Invalid actor model checkpoint path!"
-            assert os.path.isfile(paths["critic"]), "Invalid critic model checkpoint path!"
-            steps = [int(os.path.basename(paths[k]).split(".state_dict")[0].split("_")[-1])
-                     for k in ("actor", "critic")]
-            assert steps[0] == steps[1], (
-                "The timestep is different between the actor model and the critic model ")
-            self.actor_models[policy].load_state_dict(torch.load(paths["actor"], map_location="cpu"))
-            self.critic_models[policy].load_state_dict(torch.load(paths["critic"], map_location="cpu"))
-            hard_update(self.target_actor_models[policy], self.actor_models[policy])
-            hard_update(self.target_critic_models[policy], self.critic_models[policy])
-            self.current_timestep[policy] = steps[0]
+    def _load_policy_checkpoint(self, policy, paths):
+        if not (isinstance(paths, dict) and paths.get("actor") and paths.get("critic")):
+            return
+        assert os.path.isfile(paths["actor"]), "Invalid actor model checkpoint path!"
+        assert os.path.isfile(paths["critic"]), "Invalid critic model checkpoint path!"
+        steps = [self._checkpoint_timestep(paths[k]) for k in ("actor", "critic")]
+        assert steps[0] == steps[1], (
+            "The timestep is different between the actor model and the critic model ")
+        self.actor_models[policy].load_state_dict(torch.load(paths["actor"], map_location="cpu"))
+        self.critic_models[policy].load_state_dict(torch.load(paths["critic"], map_location="cpu"))
+        hard_update(self.target_actor_models[policy], self.actor_models[policy])
+        hard_update(self.target_critic_models[policy], self.critic_models[policy])
+        self.current_timestep[policy] = steps[0]
