@@ -9,18 +9,19 @@
 //   * all weights (bf16, pre-packed by wdb_mlp_pack_weights into the wgmma canonical K-major
 //     no-swizzle layout) are TMA-bulk-loaded into shared memory ONCE per CTA;
 //   * every warpgroup owns 64 rows of a 128-row tile and runs the three layers on its own,
-//     with no block-wide synchronisation inside the tile loop.  Layer 1 reads its A operand
-//     from a per-warpgroup shared-memory staging buffer (the obs rows converted to bf16 in
-//     the canonical layout, or the rows of a bf16 obs tile copied as they are); layers 2 and
-//     3 take theirs from registers (wgmma register-A form): the fp32 accumulator fragment of
+//     with no block-wide synchronisation inside the tile loop.  For the config-2 shape
+//     (FastShape) every layer takes its A operand from registers (wgmma register-A form):
+//     layer 1's fragments are loaded by each thread straight from the observations (fp32
+//     rows or a bf16 obs tile).  Other shapes stage layer 1's operand in a per-warpgroup
+//     shared-memory buffer.  Layers 2 and 3 always read registers: the fp32 accumulator fragment of
 //     a hidden layer, after bias + ReLU + bf16 packing, IS the A fragment of the next layer,
 //     so hidden activations never touch shared or global memory.  B is always read from
 //     the shared-memory weights through a matrix descriptor;
-//   * a layer is computed in 32-column slices (wgmma m64n32k16).  For the config-2 shape
-//     (FastShape) the slices are pipelined: slice c + 1's MMAs run while slice c's epilogue
-//     packs it, each packed slice of layer 2 feeds its two layer-3 k-steps at once, and the
-//     next tile's observations are loaded during layer 2.  Other shapes run one slice at a
-//     time, holding both hidden layers' packed activations;
+//   * for the config-2 shape (FastShape) a hidden layer is computed in 64-column slices
+//     (wgmma m64n64k16), pipelined: slice c + 1's MMAs run while slice c's epilogue packs it,
+//     each packed slice of layer 2 feeds its four layer-3 k-steps at once, and the next
+//     tile's observations are loaded during layer 2.  Other shapes run one 32-column slice
+//     (m64n32k16) at a time, holding both hidden layers' packed activations;
 //   * final epilogue = bias + two softmaxes + value: the logits go through the staging
 //     buffer, two threads per row (head 0 | head 1 + value) compute the softmaxes, and the
 //     warpgroup's 64 rows of each output are copied to global memory with coalesced stores.
@@ -122,6 +123,25 @@ __device__ __forceinline__ void wgmma_n32(float (&d)[16], const uint32_t *a, uin
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(baddr), "r"(bsbo >> 4), "r"(accumulate)
       : "memory");
 }
+// D[64 x 64] (+)= A[64 x 16] (registers, bf16) * B[16 x 64] (shared memory, K-major)
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], const uint32_t *a, uint32_t baddr,
+                                          uint32_t bsbo, int accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .b32 lo;\n\t.reg .b64 bd;\n\tsetp.ne.b32 p, %38, 0;\n\t"
+      WGMMA_DESC_PTX("%36", "%37")
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "{%32, %33, %34, %35}, bd, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]),
+        "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]),
+        "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]),
+        "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(baddr), "r"(bsbo >> 4), "r"(accumulate)
+      : "memory");
+}
 // D[64 x 16] (+)= A[64 x 16] * B[16 x 16]
 __device__ __forceinline__ void wgmma_n16(float (&d)[8], const uint32_t *a, uint32_t baddr,
                                           uint32_t bsbo, int accumulate) {
@@ -177,7 +197,7 @@ __device__ __forceinline__ void wg_sync(int wg) {
   else asm volatile("bar.sync 1, 128;" ::: "memory");
 }
 
-// A hidden layer of a warpgroup is computed in 32-column slices (wgmma m64n32k16, one
+// A hidden layer of a warpgroup is computed in kSliceN-column slices (wgmma m64n64k16, one
 // commit group per slice) with two accumulator sets: slice c + 1's MMAs are issued before
 // the epilogue of slice c (`epi`) runs, so the tensor cores always have a slice in flight.
 // issue(c, d) issues slice c into d; its first MMA
@@ -188,14 +208,15 @@ __device__ __forceinline__ void wg_sync(int wg) {
 // 16 w + g (+ 8), columns 8 j + 2 t (+ 1); the k-step kk of the next layer's A fragment is
 // columns 16 kk .. 16 kk + 15 of the same rows in the same lanes, so the repacking is
 // register-to-register.
+constexpr int kSliceN = 64;
 template <class Issue, class Epi>
 __device__ __forceinline__ void slice_pipeline(int n_slices, Issue issue, Epi epi) {
-  float d[2][16];
+  float d[2][kSliceN / 2];
   wgmma_fence();
   issue(0, d[0]);
   wgmma_commit();
 #pragma unroll
-  for (int c = 0; c < kMaxK / 32; c++) {
+  for (int c = 0; c < kMaxK / kSliceN; c++) {
     if (c < n_slices) {
       if (c + 1 < n_slices) {
         wgmma_fence();                 // (slice c - 1's epilogue read this accumulator set)
@@ -211,13 +232,13 @@ __device__ __forceinline__ void slice_pipeline(int n_slices, Issue issue, Epi ep
 }
 
 // slice c of a hidden layer's accumulators + bias -> ReLU -> packed bf16 A fragments
-// out[8 c .. 8 c + 7] (the next layer's k-steps 2 c and 2 c + 1)
-__device__ __forceinline__ void bias_relu_slice(const float (&d)[16], const float *bias, int c,
-                                                uint32_t *out) {
+// out[0 .. kSliceN / 4) (the next layer's k-steps kSliceN / 16 * c .. + kSliceN / 16 - 1)
+__device__ __forceinline__ void bias_relu_slice(const float (&d)[kSliceN / 2], const float *bias,
+                                                int c, uint32_t *out) {
   const int t = threadIdx.x & 3;
 #pragma unroll
-  for (int j = 0; j < 4; j++) {
-    const float2 b = *reinterpret_cast<const float2 *>(bias + 32 * c + 8 * j + 2 * t);
+  for (int j = 0; j < kSliceN / 8; j++) {
+    const float2 b = *reinterpret_cast<const float2 *>(bias + kSliceN * c + 8 * j + 2 * t);
     out[2 * j] = bias_relu_pack(d[4 * j], d[4 * j + 1], b.x, b.y);
     out[2 * j + 1] = bias_relu_pack(d[4 * j + 2], d[4 * j + 3], b.x, b.y);
   }
@@ -265,83 +286,78 @@ __device__ __forceinline__ void hidden_layer(const uint32_t (&in)[kMaxK / 4], ui
   }
 }
 
-// ---- layer-1 A operand staging.  A warpgroup's operand is 64 rows x K1 bf16 in the
-// canonical K-major layout: (r, k) at (r / 8) * K1 * 16 + (k / 8) * 128 + (r % 8) * 16 +
-// (k % 8) * 2.  Task i (thread lt takes i = lt + 128 j) is one 16-byte chunk (8 consecutive
-// k) of one row; consecutive lanes take the 8 rows of a core matrix, so each shared store of
-// a warp is bank-conflict free.  A thread handles its tasks kObsBatch at a time, the loads of
-// a batch all in flight together; batch 0 of the NEXT tile is loaded during the current
-// tile's layer 2 (for K1 <= 80, e.g. the config-2 F = 71, that is the whole operand).
-constexpr int kObsBatch = 5;
+// ---- layer-1 A operand of the FastShape schedule, in register-A form: each thread loads the
+// elements of its own A fragments straight from the observations, so the operand never
+// passes through shared memory.  Fragment 4 kk + q of k-step kk (the layout of
+// bias_relu_slice's output) holds row 16 w + g (q = 0, 2) or 16 w + g + 8 (q = 1, 3),
+// columns 16 kk + 2 t (+ 1) (q = 0, 1) or 16 kk + 8 + 2 t (+ 1) (q = 2, 3), as bf16x2.
+// A thread's loads for the NEXT tile are issued during the current tile's layer 2 and packed
+// a slice later (obs_frag_pack), in two halves (part 0: fragments [0, K1 / 8), part 1 the
+// rest), so at most half of the operand is live unpacked.
+template <bool TILES, int K1> struct ObsFrag;
+template <int K1> struct ObsFrag<false, K1> { float v[K1 / 8][2]; };   // fp32 obs [rows, F]
+template <int K1> struct ObsFrag<true, K1> { uint32_t v[K1 / 8]; };    // bf16 obs tiles
 
-template <bool TILES> struct ObsBatch;
-template <> struct ObsBatch<false> { float v[kObsBatch][8]; };   // fp32 obs [rows, F]
-template <> struct ObsBatch<true> { uint4 v[kObsBatch]; };       // bf16 obs tiles, as stored
-
-struct ObsSource {
-  const void *input;
-  long long rows;
-  int F, K1;
-};
-
-// the row (within the warpgroup) and chunk of task i; false past the operand's end
-__device__ __forceinline__ bool obs_task(int i, int nchunk, int &r, int &c) {
-  const int grp = i / (8 * nchunk), in = i - grp * 8 * nchunk;
-  c = in >> 3;
-  r = 8 * grp + (in & 7);
-  return i < kWgRows * nchunk;
-}
-
-// rows beyond `rows` and k >= F read as 0
-__device__ __forceinline__ void obs_load(ObsBatch<false> &b, const ObsSource &s, long long row0,
-                                         int j0) {
-  const float *obs = reinterpret_cast<const float *>(s.input);
-  const int lt = threadIdx.x & 127, nchunk = s.K1 / 8;
+// rows beyond `rows` and columns >= F read as 0 (the zero padding of the staged operand)
+template <int K1>
+__device__ __forceinline__ void obs_frag_load(ObsFrag<false, K1> &f, int part,
+                                              const void *input, long long rows, int F,
+                                              long long row0) {
+  const int wr = (threadIdx.x >> 5) & 3, g = (threadIdx.x >> 2) & 7, t = threadIdx.x & 3;
 #pragma unroll
-  for (int j = 0; j < kObsBatch; j++) {
-    int r, c;
-    const bool ok = obs_task(lt + 128 * (j0 + j), nchunk, r, c) && row0 + r < s.rows;
-    const float *src = obs + (row0 + r) * s.F + 8 * c;
-#pragma unroll
-    for (int k = 0; k < 8; k++) b.v[j][k] = (ok && 8 * c + k < s.F) ? __ldg(src + k) : 0.0f;
+  for (int j = 0; j < K1 / 8; j++) {
+    const int i = part * (K1 / 8) + j;
+    const long long row = row0 + 16 * wr + g + 8 * (i & 1);
+    const int col = 16 * (i >> 2) + 8 * ((i >> 1) & 1) + 2 * t;
+    const float *src = reinterpret_cast<const float *>(input) + row * F + col;
+    f.v[j][0] = (row < rows && col < F) ? __ldg(src) : 0.0f;
+    f.v[j][1] = (row < rows && col + 1 < F) ? __ldg(src + 1) : 0.0f;
   }
 }
-__device__ __forceinline__ void obs_store(const ObsBatch<false> &b, const ObsSource &s,
-                                          unsigned char *s_a, int j0) {
-  const int lt = threadIdx.x & 127, nchunk = s.K1 / 8;
+// the warpgroup's 64 rows are one contiguous block of a tile in the canonical K-major layout
+// ((r, k) at (r / 8) * K1 * 16 + (k / 8) * 128 + (r % 8) * 16 + (k % 8) * 2; rows past the
+// end are the zero padding of the tile buffer), so a fragment is one aligned 4-byte word
+template <int K1>
+__device__ __forceinline__ void obs_frag_load(ObsFrag<true, K1> &f, int part,
+                                              const void *input, long long, int,
+                                              long long row0) {
+  const int wr = (threadIdx.x >> 5) & 3, g = (threadIdx.x >> 2) & 7, t = threadIdx.x & 3;
+  const unsigned char *src =
+      reinterpret_cast<const unsigned char *>(input) + row0 * (K1 * 2) + g * 16 + t * 4;
 #pragma unroll
-  for (int j = 0; j < kObsBatch; j++) {
-    int r, c;
-    if (obs_task(lt + 128 * (j0 + j), nchunk, r, c)) {
-      uint4 o4;
-      o4.x = pack_bf16(b.v[j][0], b.v[j][1]); o4.y = pack_bf16(b.v[j][2], b.v[j][3]);
-      o4.z = pack_bf16(b.v[j][4], b.v[j][5]); o4.w = pack_bf16(b.v[j][6], b.v[j][7]);
-      *reinterpret_cast<uint4 *>(s_a + (r >> 3) * (s.K1 * 16) + c * 128 + (r & 7) * 16) = o4;
-    }
+  for (int j = 0; j < K1 / 8; j++) {
+    const int i = part * (K1 / 8) + j;
+    const int grp = 2 * wr + (i & 1), chunk = 2 * (i >> 2) + ((i >> 1) & 1);
+    f.v[j] = __ldg(reinterpret_cast<const uint32_t *>(src + grp * (K1 * 16) + chunk * 128));
   }
 }
-// the warpgroup's 64 rows are one contiguous block of a tile (rows past the end are the
-// zero padding of the tile buffer), already in the staging layout
-__device__ __forceinline__ void obs_load(ObsBatch<true> &b, const ObsSource &s, long long row0,
-                                         int j0) {
-  const uint4 *src = reinterpret_cast<const uint4 *>(
-      reinterpret_cast<const unsigned char *>(s.input) + row0 * (s.K1 * 2));
-  const int lt = threadIdx.x & 127;
+template <int K1>
+__device__ __forceinline__ void obs_frag_pack(const ObsFrag<false, K1> &f, int part,
+                                              uint32_t (&a)[K1 / 4]) {
 #pragma unroll
-  for (int j = 0; j < kObsBatch; j++) {
-    const int i = lt + 128 * (j0 + j);
-    if (i < kWgRows * s.K1 / 8) b.v[j] = __ldg(src + i);
-  }
+  for (int j = 0; j < K1 / 8; j++) a[part * (K1 / 8) + j] = pack_bf16(f.v[j][0], f.v[j][1]);
 }
-__device__ __forceinline__ void obs_store(const ObsBatch<true> &b, const ObsSource &s,
-                                          unsigned char *s_a, int j0) {
-  const int lt = threadIdx.x & 127;
+template <int K1>
+__device__ __forceinline__ void obs_frag_pack(const ObsFrag<true, K1> &f, int part,
+                                              uint32_t (&a)[K1 / 4]) {
 #pragma unroll
-  for (int j = 0; j < kObsBatch; j++) {
-    const int i = lt + 128 * (j0 + j);
-    if (i < kWgRows * s.K1 / 8) reinterpret_cast<uint4 *>(s_a)[i] = b.v[j];
-  }
+  for (int j = 0; j < K1 / 8; j++) a[part * (K1 / 8) + j] = f.v[j];
 }
+
+// Profiling aid (-DWDB_PHASE_CLOCKS): thread 0 of CTA 0 of one forward launch at a time
+// records clock64 at the phase boundaries, read back by wdb_debug_mlp_clocks.  [0] = rows of
+// the recorded launch, [1] kernel start, [2] weights landed, then per tile k < 18 of the CTA,
+// [3 + 5 k + p]: p = 0 tile start, 1 layer 1 done, 2 layers 2 + 3 done, 3 softmax done,
+// 4 outputs stored.
+#ifdef WDB_PHASE_CLOCKS
+constexpr int kMlpClockSlots = 96;
+__device__ long long g_mlp_clocks[kMlpClockSlots];
+__device__ int g_mlp_clocks_busy;
+#define MLP_MARK(i)                                                                  \
+  if (rec_clocks && (i) < kMlpClockSlots) g_mlp_clocks[(i)] = clock64();
+#else
+#define MLP_MARK(i)
+#endif
 
 // TILES = false: `input` is the fp32 obs [rows, F]; TILES = true: `input` is the bf16 copy of
 // the obs already in A-operand layout (128-row tiles of the canonical K-major layout, K
@@ -358,7 +374,7 @@ template <int K1_, int H_, int N3_> struct MlpShape {
 using AnyShape = MlpShape<0, 0, 0>;
 // The config-2 policies (F = 71 -> K1 = 80, H = 256, 21 + 21 + 1 -> N3 = 48).  With every
 // MMA loop bound a constant, ptxas can follow the wgmma groups of the overlapped schedule
-// (slice_pipeline<true>, the next tile's observations prefetched during layer 2): it keeps
+// (slice_pipeline, the next tile's observations prefetched during layer 2): it keeps
 // slice c + 1's MMAs in flight across slice c's epilogue and injects no warpgroup.arrive.
 // With runtime bounds it would serialise those wgmmas (C7514) and the extra live registers
 // would spill, so every other shape runs one slice at a time and loads its observations
@@ -395,6 +411,15 @@ mlp_forward_body(const unsigned char *__restrict__ blob, const void *__restrict_
   unsigned long long *s_bar = reinterpret_cast<unsigned long long *>(
       s_w + ((w_bytes + 127) & ~127) + kWarpgroups * stage_bytes);
   const uint32_t bar_w = smem_addr(s_bar);               // weights landed
+#ifdef WDB_PHASE_CLOCKS
+  const bool rec_clocks = bid == 0 && tid == 0 && atomicCAS(&g_mlp_clocks_busy, 0, 1) == 0;
+  if (rec_clocks) {
+    for (int i = 0; i < kMlpClockSlots; i++) g_mlp_clocks[i] = 0;
+    g_mlp_clocks[0] = rows;
+  }
+  int clock_tile = 0;
+#endif
+  MLP_MARK(1);
   if (tid == 0) {
     mbar_init(bar_w, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -417,76 +442,84 @@ mlp_forward_body(const unsigned char *__restrict__ blob, const void *__restrict_
   if (flags & kMlpWeightsStable) griddep_wait();
   griddep_launch_dependents();
 
-  const ObsSource obs_src = {input, rows, F, K1};
   const int lt = tid & 127;
-  // kOverlap: layer-1 operand tasks per thread, in batches of kObsBatch
-  const int n_batches = ((kWgRows * K1 / 8 + 127) / 128 + kObsBatch - 1) / kObsBatch;
   const long long n_tiles = (rows + kTileM - 1) / kTileM;
-  ObsBatch<TILES> next;           // kOverlap: batch 0 of the warpgroup's next tile, prefetched
-  if (kOverlap && bid < n_tiles && bid * kTileM + wg * kWgRows < rows)   // (overlaps the weight load)
-    obs_load(next, obs_src, bid * kTileM + wg * kWgRows, 0);
+  // kOverlap: layer 1's A fragments of the warpgroup's current tile (a1), and the loads of its
+  // next tile (next), issued during layer 2
+  constexpr int kFragK1 = kOverlap ? Shape::K1 : 16;
+  ObsFrag<TILES, kFragK1> next;
+  uint32_t a1[kFragK1 / 4];
+  const bool have_first = bid < n_tiles && bid * kTileM + wg * kWgRows < rows;
+  if (kOverlap && have_first)                              // (overlaps the weight load)
+    obs_frag_load(next, 0, input, rows, F, bid * kTileM + wg * kWgRows);
   mbar_wait(bar_w, 0);
+  MLP_MARK(2);
+  if (kOverlap && have_first) {
+    obs_frag_pack(next, 0, a1);
+    obs_frag_load(next, 1, input, rows, F, bid * kTileM + wg * kWgRows);
+    obs_frag_pack(next, 1, a1);
+  }
 
   const uint32_t sbo_a = (uint32_t)(K1 / 8) * 128u;       // W1: K1/8 core matrices per row group
   const uint32_t sbo_h = (uint32_t)(H / 8) * 128u;        // W2 / W3: H/8 core matrices per row group
   for (long long tile = bid; tile < n_tiles; tile += gdim) {
     const long long row0 = tile * kTileM + wg * kWgRows;  // first row of the warpgroup
     if (row0 >= rows) continue;                           // (warpgroup-uniform; so are all later tiles)
+#ifdef WDB_PHASE_CLOCKS
+    const int mark0 = 3 + 5 * (clock_tile < 18 ? clock_tile : kMlpClockSlots);
+    clock_tile++;
+#endif
+    MLP_MARK(mark0);
 
     float o[kMaxN3 / 16][8];   // layer-3 logits
     if constexpr (kOverlap) {
-      // ---- layer 1 A operand -> this warpgroup's staging buffer.  The previous tile's
-      // output copy, the last reader of the buffer, is done in every warp.
-      wg_sync(wg);
-      obs_store(next, obs_src, s_a, 0);
-      for (int b = 1; b < n_batches; b++) {                 // (K1 > 80 only)
-        ObsBatch<TILES> rest;
-        obs_load(rest, obs_src, row0, b * kObsBatch);
-        obs_store(rest, obs_src, s_a, b * kObsBatch);
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // visible to wgmma
-      wg_sync(wg);
-
-      // ---- layer 1 (A from the staging buffer) -> h: packed bf16 A fragments of layer 2
+      // ---- layer 1 (A = a1, in registers) -> h: packed bf16 A fragments of layer 2
       uint32_t h[kMaxK / 4];
-      const uint32_t a_smem = smem_addr(s_a);
       slice_pipeline(
-          H / 32,
-          [&](int c, float(&d)[16]) {
+          H / kSliceN,
+          [&](int c, float(&d)[kSliceN / 2]) {
+#pragma unroll
             for (int kk = 0; kk < K1 / 16; kk++)
-              wgmma_n32_ss(d, make_desc(a_smem + kk * 256, sbo_a),
-                           make_desc(s_w1 + 4 * c * sbo_a + kk * 256, sbo_a), kk);
+              wgmma_n64(d, &a1[4 * kk], s_w1 + kSliceN / 8 * c * sbo_a + kk * 256, sbo_a, kk);
           },
-          [&](int c, const float(&d)[16]) { bias_relu_slice(d, s_b1, c, &h[8 * c]); });
+          [&](int c, const float(&d)[kSliceN / 2]) {
+            bias_relu_slice(d, s_b1, c, &h[kSliceN / 4 * c]);
+          });
+      MLP_MARK(mark0 + 1);
 
       // ---- layer 2 (A = h) streamed into layer 3 ([head0 | head1 | value | pad] in
-      // 16-column slices, accumulated in o): as soon as a 32-column slice of layer 2 is packed,
-      // the two layer-3 k-steps it feeds are issued, so layer 2's output is never held whole.
+      // 16-column slices, accumulated in o): as soon as a 64-column slice of layer 2 is packed,
+      // the four layer-3 k-steps it feeds are issued, so layer 2's output is never held whole.
       // Every layer-3 output still accumulates its k-steps 0, 1, ..., H / 16 - 1 in order, the
-      // first with scale-d = 0.  The next tile's observations load meanwhile.
+      // first with scale-d = 0.  The next tile's observations load meanwhile, half after
+      // slice 0 and half after slice 1, each packed into a1 (which layer 1 no longer reads)
+      // one slice after its loads were issued.
+      const bool have_next = row0 + (long long)gdim * kTileM < rows;
       slice_pipeline(
-          H / 32,
-          [&](int c, float(&d)[16]) {
+          H / kSliceN,
+          [&](int c, float(&d)[kSliceN / 2]) {
 #pragma unroll
             for (int kk = 0; kk < kMaxK / 16; kk++)
-              if (kk < H / 16) wgmma_n32(d, &h[4 * kk], s_w2 + 4 * c * sbo_h + kk * 256, sbo_h, kk);
+              if (kk < H / 16)
+                wgmma_n64(d, &h[4 * kk], s_w2 + kSliceN / 8 * c * sbo_h + kk * 256, sbo_h, kk);
           },
-          [&](int c, const float(&d)[16]) {
-            uint32_t a[8];
+          [&](int c, const float(&d)[kSliceN / 2]) {
+            uint32_t a[kSliceN / 4];
             bias_relu_slice(d, s_b2, c, a);
             wgmma_fence();
 #pragma unroll
             for (int n = 0; n < kMaxN3 / 16; n++) {
               if (n < N3 / 16) {
 #pragma unroll
-                for (int k = 0; k < 2; k++)
-                  wgmma_n16(o[n], &a[4 * k], s_w3 + 2 * n * sbo_h + (2 * c + k) * 256, sbo_h,
-                            2 * c + k);
+                for (int k = 0; k < kSliceN / 16; k++)
+                  wgmma_n16(o[n], &a[4 * k], s_w3 + 2 * n * sbo_h + (kSliceN / 16 * c + k) * 256,
+                            sbo_h, kSliceN / 16 * c + k);
               }
             }
             wgmma_commit();
-            if (c == 0 && row0 + (long long)gdim * kTileM < rows)
-              obs_load(next, obs_src, row0 + (long long)gdim * kTileM, 0);
+            if (have_next && (c == 1 || c == 2)) obs_frag_pack(next, c - 1, a1);
+            if (have_next && (c == 0 || c == 1))
+              obs_frag_load(next, c, input, rows, F, row0 + (long long)gdim * kTileM);
           });
       wgmma_wait<0>();
     } else {
@@ -539,11 +572,18 @@ mlp_forward_body(const unsigned char *__restrict__ blob, const void *__restrict_
       wgmma_commit();
       wgmma_wait<0>();
     }
+    MLP_MARK(mark0 + 2);
 
     // ---- output epilogue.  Logits (+ bias) -> staging [64 rows x N3]: o[c][4 j + 0/1] is
-    // row 16 wr + g, o[c][4 j + 2/3] row + 8, columns 16 c + 8 j + 2 t (+1).  (The layer-1
-    // MMAs that read the staging buffer have completed in every warp.)
+    // row 16 wr + g, o[c][4 j + 2/3] row + 8, columns 16 c + 8 j + 2 t (+1).  (The previous
+    // tile's output copy and, for other shapes, the layer-1 MMAs that read the staging buffer
+    // have completed in every warp.)  Column col of row r is stored at col ^ (r & 14):
+    // the softmax below reads one column of 32 consecutive rows per warp, which with N3 = 48
+    // would otherwise fall into two shared-memory banks (16-way conflicts; 2-way with it).
+    // The swizzle stays inside the column's 16-column group (N3 is a multiple of 16) and
+    // keeps the pairs (col, col + 1) of even col together, so they are still float2 stores.
     wg_sync(wg);
+    auto logit_at = [&](int r, int col) { return r * N3 + (col ^ (r & 14)); };
     const int lr = wr * 16 + g;
 #pragma unroll
     for (int c = 0; c < kMaxN3 / 16; c++) {
@@ -552,9 +592,9 @@ mlp_forward_body(const unsigned char *__restrict__ blob, const void *__restrict_
         for (int j = 0; j < 2; j++) {
           const int col = 16 * c + 8 * j + 2 * t;
           const float2 b = *reinterpret_cast<const float2 *>(s_b3 + col);
-          *reinterpret_cast<float2 *>(s_o + lr * N3 + col) =
+          *reinterpret_cast<float2 *>(s_o + logit_at(lr, col)) =
               make_float2(o[c][4 * j] + b.x, o[c][4 * j + 1] + b.y);
-          *reinterpret_cast<float2 *>(s_o + (lr + 8) * N3 + col) =
+          *reinterpret_cast<float2 *>(s_o + logit_at(lr + 8, col)) =
               make_float2(o[c][4 * j + 2] + b.x, o[c][4 * j + 3] + b.y);
         }
       }
@@ -570,7 +610,7 @@ mlp_forward_body(const unsigned char *__restrict__ blob, const void *__restrict_
     float value = 0.0f;
 #pragma unroll
     for (int i = 0; i < 32; i++) {
-      const float x = s_o[row * N3 + min(cbase + i, N3 - 1)];
+      const float x = s_o[logit_at(row, min(cbase + i, N3 - 1))];
       lg[i] = i < cnt ? x * kLog2e : -CUDART_INF_F;
       mx[i & 3] = fmaxf(mx[i & 3], lg[i]);
       value = (i == cnt) ? x : value;
@@ -583,6 +623,7 @@ mlp_forward_body(const unsigned char *__restrict__ blob, const void *__restrict_
       zz[i & 3] += lg[i];
     }
     const float inv = 1.0f / ((zz[0] + zz[1]) + (zz[2] + zz[3]));
+    MLP_MARK(mark0 + 3);
     wg_sync(wg);
     // staging = [probs0 64 x A0 | probs1 64 x A1 | values 64]: the warpgroup's rows of each
     // output are contiguous in global memory
@@ -598,7 +639,14 @@ mlp_forward_body(const unsigned char *__restrict__ blob, const void *__restrict_
     for (int i = lt; i < valid * A0; i += 128) probs0[rb * A0 + i] = s_p0[i];
     for (int i = lt; i < valid * A1; i += 128) probs1[rb * A1 + i] = s_p1[i];
     if (values && lt < valid) values[rb + lt] = s_v[lt];
+    MLP_MARK(mark0 + 4);
   }
+#ifdef WDB_PHASE_CLOCKS
+  if (rec_clocks) {
+    __threadfence();
+    atomicExch(&g_mlp_clocks_busy, 0);
+  }
+#endif
 }
 
 template <bool TILES, class Shape>
@@ -886,6 +934,14 @@ WDB_API int wdb_mlp_policy_forward_pair(void *stream, const wdb_mlp_pair *pair) 
   if (!pair) return (int)cudaErrorInvalidValue;
   return launch_forward_pair(stream, *pair);
 }
+
+#ifdef WDB_PHASE_CLOCKS
+// the phase clocks of the last recorded forward launch (see MLP_MARK)
+WDB_API int wdb_debug_mlp_clocks(long long *out) {
+  if (!out) return (int)cudaErrorInvalidValue;
+  return (int)cudaMemcpyFromSymbol(out, g_mlp_clocks, sizeof(g_mlp_clocks));
+}
+#endif
 
 WDB_API int wdb_mlp_policy_forward_tiles(void *stream, const void *blob, int F, int H, int A0,
                                          int A1, const void *obs_tiles, long long rows,
