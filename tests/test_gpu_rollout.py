@@ -119,6 +119,11 @@ def test_fused_step_equals_separate_calls(full_obs, tc_variant):
         # ---- B: one fused launch
         slot = t % T
         ab = {p: dmb.data_on_device_via_torch(f"sampled_actions_batch_{p}")[slot] for p in pm}
+        # one step with the first policy's action slot NULL: that disables the action push for
+        # every policy, so the second policy's slot must stay untouched
+        null_push = t == 1
+        if null_push:
+            ab = {p: None if i == 0 else torch.full_like(ab[p], -3) for i, p in enumerate(pm)}
         rb = {p: dmb.data_on_device_via_torch(f"rewards_batch_{p}")[slot] for p in pm}
         ob = {p: torch.full((E, len(v), F), -7.0, device="cuda") for p, v in pm.items()}
         db = dmb.data_on_device_via_torch("done_flags_batch")[slot]
@@ -137,7 +142,10 @@ def test_fused_step_equals_separate_calls(full_obs, tc_variant):
         assert torch.equal(db, done_a)
         obs_post = dma.data_on_device_via_torch("observations").view(E, N, -1)
         for p in pm:
-            assert torch.equal(ab[p], acts_a[:, ids[p]]), (t, p)
+            if null_push:
+                assert ab[p] is None or bool((ab[p] == -3).all()), (t, p)
+            else:
+                assert torch.equal(ab[p], acts_a[:, ids[p]]), (t, p)
             assert torch.equal(rb[p], rew_a[:, ids[p]]), (t, p)
             assert torch.equal(ob[p], obs_post[:, ids[p]]), (t, p)      # post-reset obs
             assert torch.allclose(run[p], ref_run[p], atol=1e-5)

@@ -49,7 +49,8 @@ def test_library_is_sm90a_only(wdb_lib):
 def test_kernel_resource_usage_matches_the_residency_the_design_assumes(wdb_lib):
     """The launch geometry assumes: fused env kernel 96 registers x 320 threads ->
     two CTAs per SM (register file 65536); its 1024-thread instance (BASELINE config 4) must
-    fit one CTA; the persistent MLP kernel (two warpgroups, 256 threads) must fit one CTA per SM,
+    fit one CTA; the second-generation kernel's <MAXT, MINB> instances must fit MINB CTAs and
+    the cluster kernel one 1024-thread CTA per SM; the persistent MLP kernel (two warpgroups, 256 threads) must fit one CTA per SM,
     where shared memory binds: the [256, 256] policy of config 2 (F = 71, two 21-way heads) must
     fit the 227 KB a block may use (wdb_mlp_blob_bytes returns -1 when it does not).
     A compiler or source change that silently breaks this shows up here, without a GPU."""
@@ -73,6 +74,13 @@ def test_kernel_resource_usage_matches_the_residency_the_design_assumes(wdb_lib)
     for u in find("tag_continuous_kernel", "Li320E"):
         assert u["REG"] * 320 * 2 <= 65536 and u["STACK"] <= 128, u
     for u in find("tag_continuous_kernel", "Li1024E"):
+        assert u["REG"] * 1024 <= 65536, u
+    # the second-generation kernel, built for MINB CTAs of MAXT threads per SM
+    for maxt, minb in ((320, 3), (224, 4), (128, 7)):
+        for u in find("tc_small_v2_kernel", f"Li{maxt}ELi{minb}E"):
+            assert u["REG"] * maxt * minb <= 65536, (maxt, minb, u)
+    # the cluster kernel: one CTA of up to 1024 threads per SM
+    for u in find("tc_wide_kernel"):
         assert u["REG"] * 1024 <= 65536, u
     for u in find("mlp_forward_kernel"):
         assert u["REG"] * 256 <= 65536 and u["STACK"] <= 32, u

@@ -1,9 +1,10 @@
-// wdb_tc_common.cuh -- parameter blocks and device helpers shared by the two TagContinuous
+// wdb_tc_common.cuh -- parameter blocks and device helpers shared by the three TagContinuous
 // kernels: wdb_tag_continuous.cu (whole env replicas packed into one CTA, N <= 320 and the
-// single-CTA large-env variant) and wdb_tc_wide.cu (one env spread over a thread-block
-// cluster: blocks_per_env > 1, BASELINE config 4).  Everything here is exactness-critical:
-// both kernels must rank, divide and sample with the SAME expressions (see the header of
-// wdb_tag_continuous.cu for what "parity" means).
+// single-CTA large-env variant), wdb_tc_small_v2.cu (the second-generation small-env kernel)
+// and wdb_tc_wide.cu (one env spread over a thread-block cluster: blocks_per_env > 1,
+// BASELINE config 4).  Everything here is exactness-critical: all kernels must rank, divide
+// and sample with the SAME expressions (see the header of wdb_tag_continuous.cu for what
+// "parity" means).
 #pragma once
 #include <math_constants.h>
 
@@ -552,6 +553,111 @@ __device__ __forceinline__ float div_by_two_pi(float x, float c, float r) {
   const float q0 = x * r;
   const float rem = __fmaf_rn(-q0, c, x);
   return __fmaf_rn(rem, r, q0);
+}
+
+// ---- per-agent phases of the step, shared by the packed, second-generation and cluster
+// kernels.  Every float expression here is the one parity depends on: keep operand order,
+// double promotions and the __f*_rn intrinsics as they are.
+
+// Philox draw of both heads' uniforms (core/random.cu:51-85): one block of agent gi's stream.
+// `seed` and `off` are loaded by the caller (in its phase 0); the offset is advanced here.
+__device__ __forceinline__ void tc_draw_uniforms(const FusedParams &Q, int gi,
+                                                 unsigned long long seed, unsigned long long off,
+                                                 float &u0, float &u1) {
+  RngHeader h;
+  h.seed = seed; h.n_streams = 0;
+  const uint4 d = rng_draw4(h, (unsigned long long)gi, off);
+  rng_offsets(Q.rng)[gi] = off + 1;
+  u0 = u32_to_uniform(d.x);
+  u1 = u32_to_uniform(d.y);
+}
+
+// The sampled actions of agent gi (slot `slot` of policy `pol`, np agents per env) to every
+// output that is set.  A NULL actions_batch[0] disables the push to the batch for every policy.
+__device__ __forceinline__ void tc_push_actions(const FusedParams &Q, int gi, int env, int pol,
+                                                int np, int slot, int act0, int act1) {
+  if (Q.actions_out) *reinterpret_cast<int2 *>(Q.actions_out + 2ll * gi) = make_int2(act0, act1);
+  if (Q.actions_head0) Q.actions_head0[gi] = act0;
+  if (Q.actions_head1) Q.actions_head1[gi] = act1;
+  if (Q.actions_batch[0]) {
+#pragma unroll
+    for (int p = 0; p < kMaxPolicies; p++)
+      if (p == pol && Q.actions_batch[p])
+        *reinterpret_cast<int2 *>(Q.actions_batch[p] + 2ll * ((long long)env * np + slot)) =
+            make_int2(act0, act1);
+  }
+}
+
+struct TcMove { float x, y, sp, dir, acc, ep; bool crossed; };
+
+// :402-465 kinematics of agent gi, same float32 expression forms as the reference, and the
+// state written back.  d_acc / d_turn: the acceleration / turn table entries of its actions.
+__device__ __forceinline__ TcMove tc_move_agent(const TcParams &P, int gi, float x, float y,
+                                                float sp, float dir, float acc, float skill,
+                                                int alive, float d_acc, float d_turn) {
+  const float L = P.grid_length;
+  acc += d_acc;
+  dir = fmod(dir + d_turn, kTwoPi) * alive;
+  if (dir < 0) dir = kTwoPi + dir;
+  const float cap = P.max_speed * skill;
+  sp = min(cap, max(0.0, sp + acc)) * alive;
+  if ((sp <= 0.0) || (sp >= cap)) acc = 0.0;
+  x += sp * cos(dir);
+  y += sp * sin(dir);
+  const bool crossed = (x < 0) | (x > L) | (y < 0) | (y > L);
+  float ep = 0.0f;
+  if (crossed) {
+    if (x < 0) x = 0.0; else if (x > L) x = L;
+    if (y < 0) y = 0.0; else if (y > L) y = L;
+    ep = P.edge_hit_penalty;
+  }
+  P.loc_x[gi] = x; P.loc_y[gi] = y; P.speed[gi] = sp;
+  P.direction[gi] = dir; P.acceleration[gi] = acc; P.edge_pen[gi] = ep;
+  return {x, y, sp, dir, acc, ep, crossed};
+}
+
+// Tagger ids in id order (agent_types is shared by all envs), built by one warp; returns
+// their count.
+template <typename T>
+__device__ __forceinline__ int tc_build_tagger_list(const int *stype, int N, T *stag, int lane) {
+  int cnt = 0;
+  for (int base = 0; base < N; base += kWarp) {
+    const int j = base + lane;
+    const bool is_t = (j < N) && (stype[j] == 1);
+    const unsigned m = __ballot_sync(0xffffffffu, is_t);
+    if (is_t) stag[cnt + __popc(m & ((1u << lane) - 1))] = (T)j;
+    cnt += __popc(m);
+  }
+  return cnt;
+}
+
+// :296-338 the tagger that tags the runner at `pa`: the nearest of the `ntag` taggers
+// stag[] within the margin, or -1.  A float32 pre-test with a guard band; only candidates
+// near the margin need the reference's float64 expression.
+template <typename T>
+__device__ __forceinline__ int tc_tagging_tagger(const TcParams &P, float2 pa, const float2 *pos,
+                                                 const T *stag, int ntag) {
+  float min_dist = P.grid_length * sqrt(2.0);
+  int nearest_tagger = -1;
+  float min_s = CUDART_INF_F;
+  for (int q = 0; q < ntag; q++) {
+    const float2 pb = pos[stag[q]];
+    const float dx = pa.x - pb.x, dy = pa.y - pb.y;
+    min_s = fminf(min_s, dx * dx + dy * dy);
+  }
+  const float guard = P.margin * 1.001f;
+  if (min_s > guard * guard) return -1;
+  // a tagger outside the guard band is farther than the margin, so it can only be the arg-min
+  // when nobody is within the margin -- and then the arg-min is not used
+  for (int q = 0; q < ntag; q++) {
+    const int b = stag[q];
+    const float2 pb = pos[b];
+    const float dx = pa.x - pb.x, dy = pa.y - pb.y;
+    if (dx * dx + dy * dy > guard * guard) continue;
+    const float dist = exact_distance(pa.x, pa.y, pb.x, pb.y);
+    if (dist < min_dist) { min_dist = dist; nearest_tagger = b; }
+  }
+  return min_dist < P.margin ? nearest_tagger : -1;
 }
 
 }  // namespace

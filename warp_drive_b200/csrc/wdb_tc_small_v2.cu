@@ -205,44 +205,19 @@ tc_small_v2_kernel(const __grid_constant__ TcParams P, const __grid_constant__ F
   }
   __syncthreads();     // barrier 0: tables / types / counters staged
 
-  // tagger id list in id order (agent_types is shared by all envs), built by warp 0; read
-  // after barrier 1
+  // tagger id list, built by warp 0; read after barrier 1
   if (warp == 0) {
-    int cnt = 0;
-    for (int base = 0; base < N; base += kWarp) {
-      const int j = base + lane;
-      const bool is_t = (j < N) && (stype[j] == 1);
-      const unsigned m = __ballot_sync(0xffffffffu, is_t);
-      if (is_t) stag[cnt + __popc(m & ((1u << lane) - 1))] = j;
-      cnt += __popc(m);
-    }
+    const int cnt = tc_build_tagger_list(stype, N, stag, lane);
     if (lane == 0) *s_ntag = cnt;
   }
 
   int act0 = 0, act1 = 0;
   if (FUSED) {
     if (active) {
-      if (!Q.uniforms) {
-        RngHeader h;
-        h.seed = rng_seed; h.n_streams = 0;
-        const uint4 d = rng_draw4(h, (unsigned long long)gi, rng_off);
-        rng_offsets(Q.rng)[gi] = rng_off + 1;
-        u0 = u32_to_uniform(d.x);
-        u1 = u32_to_uniform(d.y);
-      }
+      if (!Q.uniforms) tc_draw_uniforms(Q, gi, rng_seed, rng_off, u0, u1);
       act0 = sample_row_regs(g0, Q.A0, u0);
       act1 = sample_row_regs(g1, Q.A1, u1);
-      if (Q.actions_out) *reinterpret_cast<int2 *>(Q.actions_out + 2ll * gi) = make_int2(act0, act1);
-      if (Q.actions_head0) Q.actions_head0[gi] = act0;
-      if (Q.actions_head1) Q.actions_head1[gi] = act1;
-      if (Q.actions_batch[0]) {
-#pragma unroll
-        for (int p = 0; p < kMaxPolicies; p++)
-          if (p == my_pol && Q.actions_batch[p])
-            *reinterpret_cast<int2 *>(Q.actions_batch[p] +
-                                      2ll * ((long long)env * np_mine + my_slot)) =
-                make_int2(act0, act1);
-      }
+      tc_push_actions(Q, gi, env, my_pol, np_mine, my_slot, act0, act1);
     }
   } else if (active) {
     const int2 act = *reinterpret_cast<const int2 *>(P.actions + 2ll * gi);
@@ -250,46 +225,27 @@ tc_small_v2_kernel(const __grid_constant__ TcParams P, const __grid_constant__ F
   }
 
   int alive = 0;
-  float cap = 0.f;
   if (active) {
-    // :402-465 kinematics, same float32 expression forms as the reference
-    float x = st_x, y = st_y, sp = st_sp;
-    float dir = st_dir, acc = st_acc;
     alive = st_alive;
-    acc += tab_ok ? s_tab[act0] : P.acc_actions[act0];
-    dir = fmod(dir + (tab_ok ? s_tab[Q.A0 + act1] : P.turn_actions[act1]), kTwoPi) * alive;
-    if (dir < 0) dir = kTwoPi + dir;
-    cap = P.max_speed * st_skill;
-    sp = min(cap, max(0.0, sp + acc)) * alive;
-    if ((sp <= 0.0) || (sp >= cap)) acc = 0.0;
-    x += sp * cos(dir);
-    y += sp * sin(dir);
-    const bool crossed = (x < 0) | (x > L) | (y < 0) | (y > L);
-    float ep = 0.0f;
-    if (crossed) {
-      if (x < 0) x = 0.0; else if (x > L) x = L;
-      if (y < 0) y = 0.0; else if (y > L) y = L;
-      ep = P.edge_hit_penalty;
-    }
-    P.loc_x[gi] = x; P.loc_y[gi] = y; P.speed[gi] = sp;
-    P.direction[gi] = dir; P.acceleration[gi] = acc; P.edge_pen[gi] = ep;
-    spos[li] = make_float2(x, y);
+    const TcMove mv = tc_move_agent(P, gi, st_x, st_y, st_sp, st_dir, st_acc, st_skill, alive,
+                                    tab_ok ? s_tab[act0] : P.acc_actions[act0],
+                                    tab_ok ? s_tab[Q.A0 + act1] : P.turn_actions[act1]);
+    spos[li] = make_float2(mv.x, mv.y);
     // alive agents take the env's first slots, dead ones the last (any order inside each
     // group: results do not depend on which thread works on which agent)
     const int slot = alive ? atomicAdd(&s_nalive[le], 1) : N - 1 - atomicAdd(&s_ndead[le], 1);
     s_perm[le * N + slot] = (unsigned char)a;
-    skx[le * Ne + slot] = alive ? x : CUDART_INF_F;
-    sky[le * Ne + slot] = alive ? y : CUDART_INF_F;
-    ssp[li] = sp; sacc[li] = acc; sdir[li] = dir;
+    skx[le * Ne + slot] = alive ? mv.x : CUDART_INF_F;
+    sky[le * Ne + slot] = alive ? mv.y : CUDART_INF_F;
+    ssp[li] = mv.sp; sacc[li] = mv.acc; sdir[li] = mv.dir;
     salive[li] = alive;
     float r = 0.0f;          // :283-291 reward initialisation (0 + edge + step)
-    if (alive) { r += ep; r += P.step_rewards[a]; }
+    if (alive) { r += mv.ep; r += P.step_rewards[a]; }
     srew[li] = r;
   }
   __syncthreads();   // barrier 1: state staged; the scratch head (action tables) is dead
 
   // ------------------------------------------------------------------ k-nearest selection
-  // (verbatim the selection of tag_continuous_kernel: history scan / network / exact path)
   const int t_env = active ? s_t[le] : 0;
   const float2 *epos = spos + le * N;
   const int *ealive = salive + le * N;
@@ -576,35 +532,15 @@ tc_small_v2_kernel(const __grid_constant__ TcParams P, const __grid_constant__ F
   float r = active ? srew[liw] : 0.0f;
   const bool is_runner = active && (stype[aw] == 0);
   if (is_runner && alive_w) {                                // :296-338
-    float min_dist = L * sqrt(2.0);
-    int nearest_tagger = -1;
-    const float2 pa = epos[aw];
-    const int ntag = *s_ntag;
-    float min_s = CUDART_INF_F;
-    for (int q = 0; q < ntag; q++) {
-      const float2 pb = epos[stag[q]];
-      const float dx = pa.x - pb.x, dy = pa.y - pb.y;
-      min_s = fminf(min_s, dx * dx + dy * dy);
-    }
-    const float guard = P.margin * 1.001f;
-    if (min_s <= guard * guard) {
-      for (int q = 0; q < ntag; q++) {
-        const int b = stag[q];
-        const float2 pb = epos[b];
-        const float dx = pa.x - pb.x, dy = pa.y - pb.y;
-        if (dx * dx + dy * dy > guard * guard) continue;
-        const float dist = exact_distance(pa.x, pa.y, pb.x, pb.y);
-        if (dist < min_dist) { min_dist = dist; nearest_tagger = b; }
+    const int tagger = tc_tagging_tagger(P, epos[aw], epos, stag, *s_ntag);
+    if (tagger >= 0) {
+      r += P.tag_penalty;
+      atomicAdd(&srew[le * N + tagger], P.tag_reward);
+      if (P.runner_exits) {
+        P.alive[giw] = 0;
+        atomicSub(&s_nrun[le], 1);
       }
-      if (min_dist < P.margin) {
-        r += P.tag_penalty;
-        atomicAdd(&srew[le * N + nearest_tagger], P.tag_reward);
-        if (P.runner_exits) {
-          P.alive[giw] = 0;
-          atomicSub(&s_nrun[le], 1);
-        }
-        if (P.stats) atomicAdd(&P.stats[1], 1);
-      }
+      if (P.stats) atomicAdd(&P.stats[1], 1);
     }
     if (t_env == P.episode_length) r += P.end_reward;        // :334-337
   }

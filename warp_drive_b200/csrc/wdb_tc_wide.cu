@@ -202,14 +202,8 @@ tc_wide_kernel(const __grid_constant__ TcParams P, const __grid_constant__ Fused
         u0 = Q.uniforms[2ll * gi];
         u1 = Q.uniforms[2ll * gi + 1];
       } else {
-        RngHeader h;
-        h.seed = reinterpret_cast<const RngHeader *>(Q.rng)->seed;
-        h.n_streams = 0;
-        const unsigned long long off = rng_offsets(Q.rng)[gi];
-        const uint4 d = rng_draw4(h, (unsigned long long)gi, off);
-        rng_offsets(Q.rng)[gi] = off + 1;
-        u0 = u32_to_uniform(d.x);
-        u1 = u32_to_uniform(d.y);
+        tc_draw_uniforms(Q, gi, reinterpret_cast<const RngHeader *>(Q.rng)->seed,
+                         rng_offsets(Q.rng)[gi], u0, u1);
       }
       int np = 0;
       const float *g0 = nullptr, *g1 = nullptr;
@@ -227,41 +221,19 @@ tc_wide_kernel(const __grid_constant__ TcParams P, const __grid_constant__ Fused
       float *row = reinterpret_cast<float *>(s_scr) + lane;
       act0 = sample_row_strided(row, g0, Q.A0, u0);
       act1 = sample_row_strided(row, g1, Q.A1, u1);
-      if (Q.actions_out) *reinterpret_cast<int2 *>(Q.actions_out + 2ll * gi) = make_int2(act0, act1);
-      if (Q.actions_head0) Q.actions_head0[gi] = act0;
-      if (Q.actions_head1) Q.actions_head1[gi] = act1;
-#pragma unroll
-      for (int p = 0; p < kMaxPolicies; p++)
-        if (p == my_pol && Q.actions_batch[p])
-          *reinterpret_cast<int2 *>(Q.actions_batch[p] + 2ll * ((long long)env * np + my_slot)) =
-              make_int2(act0, act1);
+      tc_push_actions(Q, gi, env, my_pol, np, my_slot, act0, act1);
     }
     __syncthreads();   // s_tab staged
   }
 
   cluster_wait();     // all peers are running: their shared memory may be written
   if (own) {
-    // :402-465 kinematics, same float32 expression forms as the reference
-    float x = st_x, y = st_y, sp = st_sp;
-    float dir = st_dir, acc = st_acc;
     const int alive = st_alive;
-    acc += FUSED ? s_tab[act0] : P.acc_actions[act0];
-    dir = fmod(dir + (FUSED ? s_tab[Q.A0 + act1] : P.turn_actions[act1]), kTwoPi) * alive;
-    if (dir < 0) dir = kTwoPi + dir;
-    const float cap = P.max_speed * st_skill;
-    sp = min(cap, max(0.0, sp + acc)) * alive;
-    if ((sp <= 0.0) || (sp >= cap)) acc = 0.0;
-    x += sp * cos(dir);
-    y += sp * sin(dir);
-    const bool crossed = (x < 0) | (x > L) | (y < 0) | (y > L);
-    float ep = 0.0f;
-    if (crossed) {
-      if (x < 0) x = 0.0; else if (x > L) x = L;
-      if (y < 0) y = 0.0; else if (y > L) y = L;
-      ep = P.edge_hit_penalty;
-    }
-    P.loc_x[gi] = x; P.loc_y[gi] = y; P.speed[gi] = sp;
-    P.direction[gi] = dir; P.acceleration[gi] = acc; P.edge_pen[gi] = ep;
+    const TcMove mv = tc_move_agent(P, gi, st_x, st_y, st_sp, st_dir, st_acc, st_skill, alive,
+                                    FUSED ? s_tab[act0] : P.acc_actions[act0],
+                                    FUSED ? s_tab[Q.A0 + act1] : P.turn_actions[act1]);
+    const float x = mv.x, y = mv.y, sp = mv.sp, dir = mv.dir, acc = mv.acc;
+    const bool crossed = mv.crossed;
     // the whole env on chip in EVERY CTA of the cluster: local store + DSMEM push to the peers
     pos[a] = make_float2(x, y);
     ssp[a] = sp; sacc[a] = acc; sdir[a] = dir;
@@ -286,16 +258,9 @@ tc_wide_kernel(const __grid_constant__ TcParams P, const __grid_constant__ Fused
   const int g_nrun = misc[M_NRUN];
   const int done_prev = misc[M_DONEPREV];
 
-  // tagger id list in id order, built by warp 0 (agent_types is shared by all envs)
+  // tagger id list, built by warp 0
   if (warp == 0) {
-    int cnt = 0;
-    for (int base = 0; base < N; base += kWarp) {
-      const int j = base + lane;
-      const bool is_t = (j < N) && (stype[j] == 1);
-      const unsigned m = __ballot_sync(full, is_t);
-      if (is_t) stag[cnt + __popc(m & ((1u << lane) - 1))] = (uint16_t)j;
-      cnt += __popc(m);
-    }
+    const int cnt = tc_build_tagger_list(stype, N, stag, lane);
     if (lane == 0) misc[M_NTAG] = cnt;
   }
 
@@ -795,35 +760,15 @@ tc_wide_kernel(const __grid_constant__ TcParams P, const __grid_constant__ Fused
     r += P.step_rewards[a2];
   }
   if (is_runner && is_alive_now) {                          // :296-338
-    float min_dist = L * sqrt(2.0);
-    int nearest_tagger = -1;
-    const float2 pa = pos[a2];
-    const int ntag = misc[M_NTAG];
-    float min_s = CUDART_INF_F;
-    for (int i = 0; i < ntag; i++) {
-      const float2 pb = pos[stag[i]];
-      const float dx = pa.x - pb.x, dy = pa.y - pb.y;
-      min_s = fminf(min_s, dx * dx + dy * dy);
-    }
-    const float guard = P.margin * 1.001f;
-    if (min_s <= guard * guard) {
-      for (int i = 0; i < ntag; i++) {
-        const int b = stag[i];
-        const float2 pb = pos[b];
-        const float dx = pa.x - pb.x, dy = pa.y - pb.y;
-        if (dx * dx + dy * dy > guard * guard) continue;
-        const float dist = exact_distance(pa.x, pa.y, pb.x, pb.y);
-        if (dist < min_dist) { min_dist = dist; nearest_tagger = b; }
+    const int tagger = tc_tagging_tagger(P, pos[a2], pos, stag, misc[M_NTAG]);
+    if (tagger >= 0) {
+      r += P.tag_penalty;
+      atomicAdd(&tagcnt[tagger], 1);
+      if (P.runner_exits) {
+        P.alive[gi2] = 0;
+        atomicAdd(&misc[M_EXITS], 1);
       }
-      if (min_dist < P.margin) {
-        r += P.tag_penalty;
-        atomicAdd(&tagcnt[nearest_tagger], 1);
-        if (P.runner_exits) {
-          P.alive[gi2] = 0;
-          atomicAdd(&misc[M_EXITS], 1);
-        }
-        if (P.stats) atomicAdd(&P.stats[1], 1);
-      }
+      if (P.stats) atomicAdd(&P.stats[1], 1);
     }
     if (t_env == P.episode_length) r += P.end_reward;        // :334-337
   }
