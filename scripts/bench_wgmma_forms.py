@@ -8,7 +8,7 @@
 Builds a small stand-alone CUDA program with nvcc (sm_90a) in a temporary directory and runs
 it.  Every CTA (one per SM) has one or two warpgroups; each warpgroup issues `iters` groups of
 8 back-to-back MMAs into one of two accumulator sets (one for N = 128; wait_group 1 between groups, as the
-forward's slice pipeline does).  Per N in {16, 32, 64, 128}, form and warpgroup count it
+forward's slice pipeline does).  Per N in {16, 32, 48, 64, 128}, form and warpgroup count it
 reports the SM clocks per MMA (clock64 of CTA 0, so one SM's view), the tensor-core share
 (the dense rate of 2048 bf16 FMA per clock per SM, i.e. N / 2 clocks per m64nNk16, over the
 measured clocks) and TFLOP/s over all SMs from CUDA events.  The card's name and power limit
@@ -20,7 +20,7 @@ import os
 import subprocess
 import tempfile
 
-NS = (16, 32, 64, 128)
+NS = (16, 32, 48, 64, 128)
 GROUP = 8        # MMAs per commit group
 
 

@@ -19,9 +19,10 @@
 //     the shared-memory weights through a matrix descriptor;
 //   * for the config-2 shape (FastShape) a hidden layer is computed in 64-column slices
 //     (wgmma m64n64k16), pipelined: slice c + 1's MMAs run while slice c's epilogue packs it,
-//     each packed slice of layer 2 feeds its four layer-3 k-steps at once, and the next
-//     tile's observations are loaded during layer 2.  Other shapes run one 32-column slice
-//     (m64n32k16) at a time, holding both hidden layers' packed activations;
+//     each packed slice of layer 2 feeds its four layer-3 k-steps (one m64n48k16 each) at
+//     once, and the next tile's observations are loaded during layer 2.  Other shapes run
+//     one 32-column slice (m64n32k16) at a time, holding both hidden layers' packed
+//     activations;
 //   * final epilogue = bias + two softmaxes + value: the logits go through the staging
 //     buffer, two threads per row (head 0 | head 1 + value) compute the softmaxes, and the
 //     warpgroup's 64 rows of each output are copied to global memory with coalesced stores.
@@ -59,6 +60,15 @@ struct MlpHeader {            // start of the packed weight blob (device memory)
   int F, K1, H, A0, A1, N3;   // input features, padded K of layer 1, hidden width, heads, padded N3
   int off_w1, off_w2, off_w3, off_b, total_bytes, pad;
 };
+// Where the blob's parts start: header | W1 | W2 | W3 | biases.  A function of K1, H and N3
+// alone, so a kernel compiled for one shape (FastShape) has them as constants.
+struct MlpLayout {
+  int off_w1, off_w2, off_w3, off_b, total_bytes;
+};
+__host__ __device__ constexpr MlpLayout mlp_layout(int K1, int H, int N3) {
+  const int w1 = 128, w2 = w1 + H * K1 * 2, w3 = w2 + H * H * 2, b = w3 + N3 * H * 2;
+  return {w1, w2, w3, b, (b + (2 * H + N3) * 4 + 15) / 16 * 16};
+}
 
 __device__ __forceinline__ uint32_t smem_addr(const void *p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -142,6 +152,23 @@ __device__ __forceinline__ void wgmma_n64(float (&d)[32], const uint32_t *a, uin
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(baddr), "r"(bsbo >> 4), "r"(accumulate)
       : "memory");
 }
+// D[64 x 48] (+)= A[64 x 16] (registers, bf16) * B[16 x 48] (shared memory, K-major)
+__device__ __forceinline__ void wgmma_n48(float (&d)[24], const uint32_t *a, uint32_t baddr,
+                                          uint32_t bsbo, int accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .b32 lo;\n\t.reg .b64 bd;\n\tsetp.ne.b32 p, %30, 0;\n\t"
+      WGMMA_DESC_PTX("%28", "%29")
+      "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23}, "
+      "{%24, %25, %26, %27}, bd, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]),
+        "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]),
+        "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(baddr), "r"(bsbo >> 4), "r"(accumulate)
+      : "memory");
+}
 // D[64 x 16] (+)= A[64 x 16] * B[16 x 16]
 __device__ __forceinline__ void wgmma_n16(float (&d)[8], const uint32_t *a, uint32_t baddr,
                                           uint32_t bsbo, int accumulate) {
@@ -195,6 +222,19 @@ __device__ __forceinline__ uint32_t bias_relu_pack(float lo, float hi, float b_l
 __device__ __forceinline__ void wg_sync(int wg) {
   if (wg) asm volatile("bar.sync 2, 128;" ::: "memory");
   else asm volatile("bar.sync 1, 128;" ::: "memory");
+}
+
+// dst[0 .. n) = src[0 .. n) by the 128 threads of a warpgroup (lt = thread in it); src is
+// 16-byte aligned, so when dst is too the bulk moves as float4
+__device__ __forceinline__ void copy_out(float *__restrict__ dst, const float *src, int n,
+                                         int lt) {
+  int done = 0;
+  if ((reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
+    done = n & ~3;
+    for (int i = lt; i < n / 4; i += 128)
+      reinterpret_cast<float4 *>(dst)[i] = reinterpret_cast<const float4 *>(src)[i];
+  }
+  for (int i = done + lt; i < n; i += 128) dst[i] = src[i];
 }
 
 // A hidden layer of a warpgroup is computed in kSliceN-column slices (wgmma m64n64k16, one
@@ -393,12 +433,17 @@ mlp_forward_body(const unsigned char *__restrict__ blob, const void *__restrict_
   const int K1 = Shape::K1 ? Shape::K1 : hd.K1, H = Shape::H ? Shape::H : hd.H,
             N3 = Shape::N3 ? Shape::N3 : hd.N3;
   constexpr bool kOverlap = Shape::H != 0;
-  const int w_bytes = hd.total_bytes - hd.off_w1;        // W1 | W2 | W3 | biases, contiguous
+  // FastShape: constant offsets, so the wgmma descriptors fold to constants (computed from
+  // the header they take registers, and the fp32-observation kernel spills)
+  const MlpLayout lay = kOverlap ? mlp_layout(Shape::K1, Shape::H, Shape::N3)
+                                 : MlpLayout{hd.off_w1, hd.off_w2, hd.off_w3, hd.off_b,
+                                             hd.total_bytes};
+  const int w_bytes = lay.total_bytes - lay.off_w1;      // W1 | W2 | W3 | biases, contiguous
   unsigned char *s_w = smem;                             // packed weights + biases
   const uint32_t s_w1 = smem_addr(s_w);
-  const uint32_t s_w2 = s_w1 + (hd.off_w2 - hd.off_w1);
-  const uint32_t s_w3 = s_w1 + (hd.off_w3 - hd.off_w1);
-  const float *s_b1 = reinterpret_cast<const float *>(s_w + (hd.off_b - hd.off_w1));
+  const uint32_t s_w2 = s_w1 + (lay.off_w2 - lay.off_w1);
+  const uint32_t s_w3 = s_w1 + (lay.off_w3 - lay.off_w1);
+  const float *s_b1 = reinterpret_cast<const float *>(s_w + (lay.off_b - lay.off_w1));
   const float *s_b2 = s_b1 + H;
   const float *s_b3 = s_b2 + H;
   const int tid = threadIdx.x, lane = tid & 31;
@@ -435,7 +480,7 @@ mlp_forward_body(const unsigned char *__restrict__ blob, const void *__restrict_
     uint32_t off = 0;
     while (off < (uint32_t)w_bytes) {
       const uint32_t n = min((uint32_t)w_bytes - off, 65536u);
-      tma_load(s_w1 + off, blob + hd.off_w1 + off, n, bar_w);
+      tma_load(s_w1 + off, blob + lay.off_w1 + off, n, bar_w);
       off += n;
     }
   }
@@ -487,13 +532,17 @@ mlp_forward_body(const unsigned char *__restrict__ blob, const void *__restrict_
           });
       MLP_MARK(mark0 + 1);
 
-      // ---- layer 2 (A = h) streamed into layer 3 ([head0 | head1 | value | pad] in
-      // 16-column slices, accumulated in o): as soon as a 64-column slice of layer 2 is packed,
-      // the four layer-3 k-steps it feeds are issued, so layer 2's output is never held whole.
-      // Every layer-3 output still accumulates its k-steps 0, 1, ..., H / 16 - 1 in order, the
-      // first with scale-d = 0.  The next tile's observations load meanwhile, half after
-      // slice 0 and half after slice 1, each packed into a1 (which layer 1 no longer reads)
-      // one slice after its loads were issued.
+      // ---- layer 2 (A = h) streamed into layer 3 ([head0 | head1 | value | pad], one
+      // m64n48k16 per k-step, accumulated in o): as soon as a 64-column slice of layer 2 is
+      // packed, the four layer-3 k-steps it feeds are issued, so layer 2's output is never held
+      // whole.  Every layer-3 output still accumulates its k-steps 0, 1, ..., H / 16 - 1 in
+      // order, the first with scale-d = 0.  The n48 accumulator fragment holds columns
+      // 8 j + 2 t (+ 1) at [4 j ..], so it is o[n][4 j' ..] (columns 16 n + 8 j' + 2 t) laid
+      // out flat.  The next tile's observations load meanwhile, half after slice 0 and half
+      // after slice 1, each packed into a1 (which layer 1 no longer reads) one slice after its
+      // loads were issued.
+      static_assert(Shape::N3 == 48, "layer 3 of the overlapped schedule is one m64n48k16");
+      float(&o48)[48 / 2] = *reinterpret_cast<float(*)[48 / 2]>(&o[0][0]);
       const bool have_next = row0 + (long long)gdim * kTileM < rows;
       slice_pipeline(
           H / kSliceN,
@@ -508,14 +557,9 @@ mlp_forward_body(const unsigned char *__restrict__ blob, const void *__restrict_
             bias_relu_slice(d, s_b2, c, a);
             wgmma_fence();
 #pragma unroll
-            for (int n = 0; n < kMaxN3 / 16; n++) {
-              if (n < N3 / 16) {
-#pragma unroll
-                for (int k = 0; k < kSliceN / 16; k++)
-                  wgmma_n16(o[n], &a[4 * k], s_w3 + 2 * n * sbo_h + (kSliceN / 16 * c + k) * 256,
-                            sbo_h, kSliceN / 16 * c + k);
-              }
-            }
+            for (int k = 0; k < kSliceN / 16; k++)
+              wgmma_n48(o48, &a[4 * k], s_w3 + (kSliceN / 16 * c + k) * 256, sbo_h,
+                        kSliceN / 16 * c + k);
             wgmma_commit();
             if (have_next && (c == 1 || c == 2)) obs_frag_pack(next, c - 1, a1);
             if (have_next && (c == 0 || c == 1))
@@ -636,8 +680,8 @@ mlp_forward_body(const unsigned char *__restrict__ blob, const void *__restrict_
     wg_sync(wg);
     const long long rb = tile * kTileM + wg * kWgRows;   // first row of the warpgroup
     const int valid = (int)min((long long)kWgRows, rows - rb);
-    for (int i = lt; i < valid * A0; i += 128) probs0[rb * A0 + i] = s_p0[i];
-    for (int i = lt; i < valid * A1; i += 128) probs1[rb * A1 + i] = s_p1[i];
+    copy_out(probs0 + rb * A0, s_p0, valid * A0, lt);
+    copy_out(probs1 + rb * A1, s_p1, valid * A1, lt);
     if (values && lt < valid) values[rb + lt] = s_v[lt];
     MLP_MARK(mark0 + 4);
   }
@@ -716,11 +760,12 @@ MlpHeader make_header(int F, int H, int A0, int A1) {
   MlpHeader hd;
   hd.F = F; hd.K1 = round_up(F, 16); hd.H = H; hd.A0 = A0; hd.A1 = A1;
   hd.N3 = round_up(A0 + A1 + 1, 16);
-  hd.off_w1 = 128;
-  hd.off_w2 = hd.off_w1 + H * hd.K1 * 2;
-  hd.off_w3 = hd.off_w2 + H * H * 2;
-  hd.off_b = hd.off_w3 + hd.N3 * H * 2;
-  hd.total_bytes = round_up(hd.off_b + (2 * H + hd.N3) * 4, 16);
+  const MlpLayout l = mlp_layout(hd.K1, H, hd.N3);
+  hd.off_w1 = l.off_w1;
+  hd.off_w2 = l.off_w2;
+  hd.off_w3 = l.off_w3;
+  hd.off_b = l.off_b;
+  hd.total_bytes = l.total_bytes;
   hd.pad = 0;
   return hd;
 }
