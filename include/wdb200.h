@@ -321,7 +321,9 @@ typedef struct wdb_sa_rollout {
   float *rewards;                    /* [E] */
   void *sampled_actions;             /* [E]: int32 (discrete kinds) or float32 (continuous) */
   int n_hidden;                      /* hidden Linear + ReLU layers (0..3), then the head */
-  int dims[5];                       /* F, H1, ..., A (continuous kinds: A = 1) */
+  int dims[5];                       /* F, H1, ..., A: F = the kind's observation width, A =
+                                      * its action count (CartPole 2, MountainCar 3, Acrobot
+                                      * 3; continuous kinds 1); hidden widths 1..64 */
   const float *w[4], *b[4];          /* nn.Linear weights [out, in] and biases, fp32 */
   void *rng_state;
   const float *uniforms;             /* test hook [n_steps, E]; NULL = device RNG */

@@ -288,6 +288,9 @@ static __device__ __noinline__ float4 acrobot_physics(float4 s4, int action, flo
 // one float2 / float4, and an observation row as one too where it is as wide as the state
 constexpr int kSaStateDim[] = {4, 2, 4, 2, 2};
 constexpr int kSaObsDim[] = {4, 2, 6, 2, 3};
+// policy head width per kind: the discrete action count (CartPole push left / right,
+// MountainCar and Acrobot -1 / 0 / +1), one tanh output for the continuous kinds
+constexpr int kSaNActions[] = {2, 3, 3, 1, 1};
 
 template <int Kind>
 using SaAction = std::conditional_t<(Kind >= WDB_SA_CONTINUOUS_MOUNTAIN_CAR), float, int>;

@@ -333,15 +333,17 @@ WDB_API int wdb_single_agent_rollout(void *stream, const wdb_sa_rollout *r) {
   for (int l = 0; l <= r->n_hidden; l++)
     if (!r->w[l] || !r->b[l]) return (int)cudaErrorInvalidValue;
   if (continuous) {
-    // one tanh action; the OU state and a normal source unless the bypass (scale < 1e-8)
-    // draws nothing
-    if (r->dims[r->n_hidden + 1] != 1) return (int)cudaErrorInvalidValue;
+    // the OU state and a normal source unless the bypass (scale < 1e-8) draws nothing
     if (!(r->ou_scale < 1.0e-8f) && (!r->ou_state || (!r->normals && !r->rng_state)))
       return (int)cudaErrorInvalidValue;
   } else if (!r->use_argmax && !r->uniforms && !r->rng_state) {
     return (int)cudaErrorInvalidValue;
   }
-  if (r->state_dim != kSaStateDim[r->env_kind] || r->dims[0] != kSaObsDim[r->env_kind])
+  // the observation feeds the first layer, and the head is one logit per discrete action
+  // (one tanh output for the continuous kinds): a wider head would step the env with actions
+  // it does not have
+  if (r->state_dim != kSaStateDim[r->env_kind] || r->dims[0] != kSaObsDim[r->env_kind] ||
+      r->dims[r->n_hidden + 1] != kSaNActions[r->env_kind])
     return (int)cudaErrorInvalidValue;
   if (r->reset_done_envs && r->n_reset_arrays > 0 && !r->reset_table)
     return (int)cudaErrorInvalidValue;
