@@ -373,16 +373,27 @@ int wdb_gather_policy_rows(void *stream, const wdb_gather *gather);
  * in one launch.  Field f of agent agent_ids[j] lands, converted to float32, at columns
  * [col, col + width) of row (e, j) of destination `dst` of the policy: destination 0 is the
  * processed observation [E, Np, dst_width[0]] (the non-mask keys concatenated), destination 1
- * the action-mask rows [E, Np, dst_width[1]].  A NULL destination is skipped. */
+ * the action-mask rows [E, Np, dst_width[1]].  A NULL destination is skipped.
+ * Heterogeneous agents (a zero-initialised extension keeps the behaviour above):
+ *   policy_mask  bit p set: the field feeds policy p only; 0 = every policy;
+ *   own_rows     1: src holds only its policy's agents, in slot order (Ns = Np, agent_ids
+ *                unused; policy_mask must name exactly one policy); 0: every agent (Ns = N);
+ *   agents_last  1: src is [E, *F, Ns] with width = prod(F): column c of agent a of env e is
+ *                src[(e * width + c) * Ns + a] (C order over F, numpy.moveaxis(x, 0, -1) of
+ *                [Ns, *F]); moved through a shared-memory tile so that reads and writes are
+ *                both coalesced;
+ *   policy[p].dst_width[d] > 0 overrides dst_width[d] for that policy. */
 #define WDB_GATHER_MAX_FIELDS 16
 typedef struct wdb_gather_field {
-  const void *src;                   /* [E, N, width] */
+  const void *src;                   /* [E, Ns, width] or [E, width, Ns] */
   int width, is_int32, dst, col;
+  int policy_mask, own_rows, agents_last;
 } wdb_gather_field;
 typedef struct wdb_gather_fields_policy {
   int n_agents;                      /* Np */
   const int *agent_ids;              /* device [Np] or NULL (agents 0..Np-1) */
   float *rows[2];                    /* [E, Np, dst_width[d]] or NULL */
+  int dst_width[2];                  /* 0: the descriptor's dst_width[d] */
 } wdb_gather_fields_policy;
 typedef struct wdb_gather_fields {
   int n_envs, n_agents, n_policies, n_fields;
@@ -397,7 +408,11 @@ int wdb_gather_policy_fields(void *stream, const wdb_gather_fields *gather);
  * agents' rewards -> rewards_batch, sampled actions -> actions_batch, reward_running_sum += r,
  * and for done envs episodic_reward_sum += the running sums, which are then cleared;
  * step_running_sum += 1, for done envs episodic_step_sum += it, cleared, num_completed += 1.
- * Any pointer may be NULL (that piece is skipped); ONE launch, no host synchronisation. */
+ * Any pointer may be NULL (that piece is skipped); ONE launch, no host synchronisation.
+ * A policy with its own step arrays (separate placeholders) sets policy[p].rewards [E, Np]
+ * and / or policy[p].actions [E, Np, policy[p].n_heads]; those are read in slot order instead
+ * of the shared rewards / actions through agent_ids.  The shared rewards may be NULL when
+ * every policy has its own. */
 typedef struct wdb_bookkeep_policy {
   int n_agents;
   const int *agent_ids;              /* device [Np] or NULL (agents 0..Np-1) */
@@ -405,11 +420,14 @@ typedef struct wdb_bookkeep_policy {
   int *actions_batch;                /* [E, Np, n_heads] slot t */
   float *reward_running_sum;         /* [E, Np] */
   float *episodic_reward_sum;        /* scalar */
+  const float *rewards;              /* [E, Np] or NULL (the shared rewards) */
+  const int *actions;                /* [E, Np, n_heads] or NULL (the shared actions) */
+  int n_heads;                       /* heads of `actions` (ignored when it is NULL) */
 } wdb_bookkeep_policy;
 typedef struct wdb_bookkeep {
   int n_envs, n_agents, n_policies, n_heads;
   const int *done;                   /* [E] */
-  const float *rewards;              /* [E, N] */
+  const float *rewards;              /* [E, N] or NULL */
   const int *actions;                /* [E, N, n_heads] or NULL */
   int *done_batch;                   /* [E] slot t */
   int *step_running_sum;             /* [E] */

@@ -91,11 +91,12 @@ GATHER_MAX_FIELDS = 16
 
 
 class GatherField(ctypes.Structure):
-    _fields_ = [("src", _fp), ("width", _i), ("is_int32", _i), ("dst", _i), ("col", _i)]
+    _fields_ = [("src", _fp), ("width", _i), ("is_int32", _i), ("dst", _i), ("col", _i),
+                ("policy_mask", _i), ("own_rows", _i), ("agents_last", _i)]
 
 
 class GatherFieldsPolicy(ctypes.Structure):
-    _fields_ = [("n_agents", _i), ("agent_ids", _fp), ("rows", _fp * 2)]
+    _fields_ = [("n_agents", _i), ("agent_ids", _fp), ("rows", _fp * 2), ("dst_width", _i * 2)]
 
 
 class GatherFields(ctypes.Structure):
@@ -112,6 +113,7 @@ class BookkeepPolicy(ctypes.Structure):
     _fields_ = [
         ("n_agents", _i), ("agent_ids", _fp), ("rewards_batch", _fp), ("actions_batch", _fp),
         ("reward_running_sum", _fp), ("episodic_reward_sum", _fp),
+        ("rewards", _fp), ("actions", _fp), ("n_heads", _i),
     ]
 
 

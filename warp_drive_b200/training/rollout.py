@@ -27,8 +27,16 @@ class RolloutEngine:
     def __init__(self, env_wrapper, models, policy_tag_to_agent_id_map, sampler,
                  batch_size_per_env, use_cuda_graph=True, forward_dtype=None,
                  use_fused_step=True, write_observations=True, stats=None,
-                 use_fused_forward=True, use_obs_tiles=False, use_pair_forward=False):
+                 use_fused_forward=True, use_obs_tiles=False, use_pair_forward=False,
+                 create_separate_placeholders_for_each_policy=False,
+                 obs_dim_corresponding_to_num_agents="first"):
         self.env_wrapper = env_wrapper
+        # heterogeneous agents: every policy steps through its own observations_{p}[_{key}],
+        # sampled_actions[_{k}]_{p} and rewards_{p} arrays, and / or the env writes its
+        # observations agent-last ([E, *F, N]); both are read by the fields gather
+        self.separate = bool(create_separate_placeholders_for_each_policy)
+        assert obs_dim_corresponding_to_num_agents in ("first", "last")
+        self.agents_last = obs_dim_corresponding_to_num_agents == "last"
         self.use_pair_forward = bool(use_pair_forward)
         # A/B switch: with one forward launch per policy, launch the env step programmatically
         # dependent on the main-stream forward (option "pdl" must be on as well)
@@ -48,20 +56,32 @@ class RolloutEngine:
                     for p, ids in self.policy_map.items()}
         self.covers_all = {p: len(ids) == self.N and list(ids) == list(range(self.N))
                            for p, ids in self.policy_map.items()}
-        first = self.policy_map[self.policies[0]][0]
         from warp_drive_b200.training.utils.data_loader import (
             action_head_sizes, dict_observation_keys)
 
-        self.heads, self.continuous = action_head_sizes(env_wrapper.env.action_space[first])
+        # per policy: action heads, Dict observation keys (None for a Box space) and whether an
+        # action mask rides along (a masked policy samples with the selection that never
+        # returns a zero-probability action).  With shared placeholders every agent has the
+        # same spaces, so these are the same for every policy.
+        self.heads_of, self.continuous_of, self.obs_keys_of, self.masked_of = {}, {}, {}, {}
+        for p, ids in self.policy_map.items():
+            self.heads_of[p], self.continuous_of[p] = action_head_sizes(
+                env_wrapper.env.action_space[ids[0]])
+            self.obs_keys_of[p], self.masked_of[p] = dict_observation_keys(
+                env_wrapper.env.observation_space[ids[0]])
+            assert not (self.masked_of[p] and self.continuous_of[p]), (
+                "an action mask needs discrete actions")
+        p0 = self.policies[0]
+        self.heads, self.obs_keys = self.heads_of[p0], self.obs_keys_of[p0]
         self.n_heads = len(self.heads)
-        # Dict observations: the keys the policies see (None for a Box space) and whether an
-        # action mask rides along; a masked policy samples with the selection that never
-        # returns a zero-probability action
-        self.obs_keys, self.masked = dict_observation_keys(
-            env_wrapper.env.observation_space[first])
-        assert not (self.masked and self.continuous), "an action mask needs discrete actions"
+        self.continuous = any(self.continuous_of.values())
+        self.masked = any(self.masked_of.values())
+        # observations reach the policies through wdb_gather_policy_fields unless they are one
+        # shared [E, N, F] Box array (wdb_gather_policy_rows)
+        self.gather_fields = (self.separate or self.agents_last
+                              or any(k is not None for k in self.obs_keys_of.values()))
         self.combined = None
-        if len(self.policies) > 1:
+        if len(self.policies) > 1 and not self.separate:
             self.combined = [torch.zeros((self.E, self.N, h), device=dev) for h in self.heads]
         # episodic statistics (device scalars: no host sync while rolling out)
         self.reward_running_sum = {p: torch.zeros((self.E, len(ids)), device=dev)
@@ -91,7 +111,9 @@ class RolloutEngine:
         # ---- whole-rollout single launch (single-agent classic control, small FullyConnected
         #      policy or actor)
         self.sa = None
-        if use_fused_step and self.fused is None:
+        # (one agent: agent-last and agent-first observations are the same memory)
+        if (use_fused_step and self.fused is None and not self.separate
+                and (not self.agents_last or self.N == 1)):
             from warp_drive_b200.training.fused_single_agent import FusedSingleAgentRollout
 
             if (self.T >= 1
@@ -113,7 +135,7 @@ class RolloutEngine:
             if all(FusedPolicyForward.supported(m) for m in self.models.values()):
                 self.fused_forward = {p: FusedPolicyForward(self.models[p]) for p in self.policies}
                 self._probs = {p: [torch.empty((self.E, len(self.policy_map[p]), h), device=dev)
-                                   for h in self.heads] for p in self.policies}
+                                   for h in self.heads_of[p]] for p in self.policies}
                 # bf16 MMA-ready mirror of the observations the next forward reads: written by
                 # the fused env step itself (and by pack_obs whenever cur_obs changes outside it)
                 # (off by default: at config 2 the env step's extra pass costs about what the
@@ -135,6 +157,8 @@ class RolloutEngine:
         from warp_drive_b200.utils.spaces import Box, MultiDiscrete
 
         env = self.env_wrapper.env
+        if self.separate or self.agents_last:
+            return False
         if getattr(env, "name", "") != "TagContinuous" or len(self.policies) > 4:
             return False
         if self.continuous or self.n_heads != 2:
@@ -328,41 +352,72 @@ class RolloutEngine:
         _lib.check(_lib.load().wdb_gather_policy_rows(_lib.stream_ptr(), ctypes.byref(g)),
                    "gather_policy_rows")
 
-    def _gather_dict_fields(self, obs_rows, mask_rows):
-        """Every key of a Dict observation -> obs_rows {policy: [E, Np, F]} (the non-mask keys
-        concatenated, converted to float32) and its action mask -> mask_rows {policy:
-        [E, Np, sum A]}, ONE launch for all policies (wdb_gather_policy_fields)."""
-        if not hasattr(self, "_dict_fields"):
-            fields, col = [], 0
-            for key in self.obs_keys + ([_ACTION_MASK] if self.masked else []):
-                src = self._tensor(f"{_OBSERVATIONS}_{key}")
-                assert src.dtype in (torch.float32, torch.int32), (
-                    f"observation key {key!r}: only float32 / int32 arrays are gathered")
-                assert src.is_contiguous()
-                width = src.numel() // (self.E * self.N)
-                if key == _ACTION_MASK:
-                    assert width == sum(self.heads), "action_mask must cover every head's actions"
-                    fields.append((src, width, 1, 0))
-                else:
-                    fields.append((src, width, 0, col))
-                    col += width
+    def _field_plan(self):
+        """The fields wdb_gather_policy_fields moves: (source, width, destination, column,
+        index of the policy whose own array it is or None) per key, and per policy the widths
+        (F_p, sum of its head sizes) of its two destinations."""
+        if not hasattr(self, "_fields"):
+            owners = (list(enumerate(self.policies)) if self.separate
+                      else [(None, self.policies[0])])
+            fields = []
+            for i, p in owners:
+                prefix = f"{_OBSERVATIONS}_{p}" if self.separate else _OBSERVATIONS
+                n_src = len(self.policy_map[p]) if self.separate else self.N
+                keys = self.obs_keys_of[p]
+                names = ([(prefix, False)] if keys is None
+                         else [(f"{prefix}_{k}", False) for k in keys])
+                if self.masked_of[p]:
+                    names.append((f"{prefix}_{_ACTION_MASK}", True))
+                col = 0
+                for name, is_mask in names:
+                    src = self._tensor(name)
+                    assert src.dtype in (torch.float32, torch.int32), (
+                        f"observation array {name!r}: only float32 / int32 arrays are gathered")
+                    assert src.is_contiguous()
+                    width = src.numel() // (self.E * n_src)
+                    if is_mask:
+                        assert width == sum(self.heads_of[p]), (
+                            "action_mask must cover every head's actions")
+                        fields.append((src, width, 1, 0, i))
+                    else:
+                        fields.append((src, width, 0, col, i))
+                        col += width
             assert len(fields) <= _lib.GATHER_MAX_FIELDS
-            self._dict_fields = (fields, col)
-        fields, F = self._dict_fields
+            widths = {p: (self._tensor(f"{_PROCESSED_OBSERVATIONS}_batch_{p}").shape[-1],
+                          sum(self.heads_of[p])) for p in self.policies}
+            for src, width, dst, col, i in fields:
+                owned = self.policies if i is None else [self.policies[i]]
+                assert all(col + width <= widths[p][dst] for p in owned), (
+                    "observation widths differ from the processed observation batch")
+            self._fields = (fields, widths)
+        return self._fields
+
+    def _gather_fields(self, obs_rows, mask_rows):
+        """Every observation array of every policy -> obs_rows {policy: [E, Np, F_p]} (the
+        non-mask keys concatenated, converted to float32) and its action mask -> mask_rows
+        {policy: [E, Np, sum A_p]}, ONE launch for all policies (wdb_gather_policy_fields).
+        Sources are the shared [E, N, ...] arrays or, with separate placeholders, each
+        policy's own [E, Np, ...] ones; agent-last sources ([E, *F, Ns]) are transposed on
+        the way."""
+        fields, widths = self._field_plan()
+        p0 = self.policies[0]
         g = _lib.GatherFields()
         g.n_envs, g.n_agents = self.E, self.N
-        g.n_policies, g.n_fields = len(obs_rows), len(fields)
-        g.dst_width[0], g.dst_width[1] = F, sum(self.heads)
-        for i, (src, width, dst, col) in enumerate(fields):
-            f = g.field[i]
+        g.n_policies, g.n_fields = len(self.policies), len(fields)
+        g.dst_width[0], g.dst_width[1] = widths[p0]
+        for j, (src, width, dst, col, i) in enumerate(fields):
+            f = g.field[j]
             f.src, f.width, f.is_int32 = _lib.ptr(src), width, int(src.dtype == torch.int32)
             f.dst, f.col = dst, col
-        for i, p in enumerate(obs_rows):
+            f.policy_mask, f.own_rows = (0, 0) if i is None else (1 << i, 1)
+            f.agents_last = int(self.agents_last)
+        for i, p in enumerate(self.policies):
             io = g.policy[i]
             io.n_agents = len(self.policy_map[p])
-            io.agent_ids = _lib.ptr(self._ids32(p))
+            io.agent_ids = None if self.separate else _lib.ptr(self._ids32(p))
             io.rows[0] = _lib.ptr(obs_rows[p])
-            io.rows[1] = _lib.ptr(mask_rows[p]) if self.masked else None
+            io.rows[1] = _lib.ptr(mask_rows[p]) if mask_rows[p] is not None else None
+            io.dst_width[0], io.dst_width[1] = widths[p]
         _lib.check(_lib.load().wdb_gather_policy_fields(_lib.stream_ptr(), ctypes.byref(g)),
                    "gather_policy_fields")
 
@@ -370,10 +425,11 @@ class RolloutEngine:
         """obs -> per-head probabilities [E, N, A_k] (trainer_a2c.py:159-216).  The per-policy
         observation rows go to the batch slot in one gather launch and the forward reads the
         slot; the per-policy probabilities return to the sampler's [E, N, A] arrays in one
-        scatter launch per head."""
+        scatter launch per head.  With separate placeholders: {policy: per-head probabilities
+        [E, Np, A_k]}, which the sampler reads as they are."""
         mask_p = {p: None for p in self.policies}
-        if self.obs_keys is not None:
-            obs_p, mask_p = self._dict_slots(t)
+        if self.gather_fields:
+            obs_p, mask_p = self._field_slots(t)
         elif t >= 0:
             obs = self._tensor(_OBSERVATIONS).view(self.E, self.N, -1)
             s = self._slot(t)
@@ -402,6 +458,8 @@ class RolloutEngine:
             else:
                 per_policy[p] = self._forward(self.models[p], obs_p[p].view(
                     self.E, len(self.policy_map[p]), -1), mask_p[p])
+        if self.separate:
+            return per_policy
         if self.combined is None:
             return per_policy[self.policies[0]]
         for k in range(self.n_heads):
@@ -409,42 +467,55 @@ class RolloutEngine:
                             scatter=True)
         return self.combined
 
-    def _dict_slots(self, t):
-        """Per-policy observation and mask rows of a Dict env for timestep t, filled by one
-        gather launch: the batch slots of t (t >= 0), or scratch rows (an evaluation step)."""
+    def _field_slots(self, t):
+        """Per-policy observation and mask rows for timestep t, filled by one gather launch:
+        the batch slots of t (t >= 0), or scratch rows (an evaluation step)."""
         if t >= 0:
             s = self._slot(t)
             obs_p = {p: self._tensor(f"{_PROCESSED_OBSERVATIONS}_batch_{p}")[s]
                      for p in self.policies}
-            mask_p = {p: (self._tensor(f"{_ACTION_MASK}_batch_{p}")[s] if self.masked else None)
-                      for p in self.policies}
+            mask_p = {p: (self._tensor(f"{_ACTION_MASK}_batch_{p}")[s] if self.masked_of[p]
+                          else None) for p in self.policies}
         else:
-            if not hasattr(self, "_dict_scratch"):
+            if not hasattr(self, "_field_scratch"):
                 dev = self.dm.device
-                F = self._tensor(f"{_PROCESSED_OBSERVATIONS}_batch_{self.policies[0]}").shape[-1]
-                self._dict_scratch = (
-                    {p: torch.empty((self.E, len(self.policy_map[p]), F), device=dev)
+                _, widths = self._field_plan()
+                self._field_scratch = (
+                    {p: torch.empty((self.E, len(self.policy_map[p]), widths[p][0]), device=dev)
                      for p in self.policies},
-                    {p: (torch.empty((self.E, len(self.policy_map[p]), sum(self.heads)),
-                                     device=dev) if self.masked else None)
+                    {p: (torch.empty((self.E, len(self.policy_map[p]), widths[p][1]),
+                                     device=dev) if self.masked_of[p] else None)
                      for p in self.policies})
-            obs_p, mask_p = self._dict_scratch
-        self._gather_dict_fields(obs_p, mask_p)
+            obs_p, mask_p = self._field_scratch
+        self._gather_fields(obs_p, mask_p)
         return obs_p, mask_p
+
+    def _sample(self, probs, suffix, heads, masked, sample_params):
+        """probs [per head] -> sampled_actions{suffix} (one head) or sampled_actions_{k}{suffix},
+        combined into sampled_actions{suffix} (several)."""
+        dm = self.dm
+        if masked:
+            sample_params = dict(sample_params, nonzero=True)
+        if len(heads) == 1:
+            self.sampler.sample(dm, probs[0], f"{_ACTIONS}{suffix}", write_cum_distr=False,
+                                **sample_params)
+        else:
+            actions = self._tensor(f"{_ACTIONS}{suffix}")
+            for k in range(len(heads)):
+                self.sampler.sample(dm, probs[k], f"{_ACTIONS}_{k}{suffix}",
+                                    write_cum_distr=False,
+                                    combined=(actions, len(heads), k), **sample_params)
 
     def sample_actions(self, probs, t, **sample_params):
         """probs -> sampled_actions (trainer_base.py:466-512); the per-policy batch push of the
-        actions happens in bookkeep()."""
-        dm = self.dm
-        if self.masked:
-            sample_params = dict(sample_params, nonzero=True)
-        if self.n_heads == 1:
-            self.sampler.sample(dm, probs[0], _ACTIONS, write_cum_distr=False, **sample_params)
+        actions happens in bookkeep().  With separate placeholders, each policy's
+        probabilities go to its own sampled_actions[_{k}]_{p}."""
+        if self.separate:
+            for p in self.policies:
+                self._sample(probs[p], f"_{p}", self.heads_of[p], self.masked_of[p],
+                             sample_params)
         else:
-            actions = self._tensor(_ACTIONS)
-            for k in range(self.n_heads):
-                self.sampler.sample(dm, probs[k], f"{_ACTIONS}_{k}", write_cum_distr=False,
-                                    combined=(actions, self.n_heads, k), **sample_params)
+            self._sample(probs, "", self.heads, self.masked, sample_params)
 
     def bookkeep(self, t):
         """done / rewards / actions -> batches, running episodic sums: ONE launch
@@ -453,11 +524,15 @@ class RolloutEngine:
         s = self._slot(t)
         k = _lib.Bookkeep()
         k.n_envs, k.n_agents, k.n_policies = self.E, self.N, len(self.policies)
-        actions = self._tensor(_ACTIONS) if self.dm.is_data_on_device_via_torch(_ACTIONS) else None
-        k.n_heads = (actions.numel() // (self.E * self.N)) if actions is not None else 0
         k.done = _lib.ptr(self._tensor("_done_"))
-        k.rewards = _lib.ptr(self._tensor(_REWARDS))
-        k.actions = _lib.ptr(actions)
+        if self.separate:
+            k.n_heads = 0
+        else:
+            actions = (self._tensor(_ACTIONS) if self.dm.is_data_on_device_via_torch(_ACTIONS)
+                       else None)
+            k.n_heads = (actions.numel() // (self.E * self.N)) if actions is not None else 0
+            k.rewards = _lib.ptr(self._tensor(_REWARDS))
+            k.actions = _lib.ptr(actions)
         k.done_batch = _lib.ptr(self._tensor(f"{_DONE_FLAGS}_batch")[s]) if t >= 0 else None
         k.step_running_sum = _lib.ptr(self.step_running_sum)
         k.episodic_step_sum = _lib.ptr(self.episodic_step_sum)
@@ -465,32 +540,45 @@ class RolloutEngine:
         for i, p in enumerate(self.policies):
             io = k.policy[i]
             io.n_agents = len(self.policy_map[p])
-            io.agent_ids = _lib.ptr(self._ids32(p))
+            if self.separate:
+                own = self._tensor(f"{_ACTIONS}_{p}")
+                io.rewards = _lib.ptr(self._tensor(f"{_REWARDS}_{p}"))
+                io.actions = _lib.ptr(own)
+                io.n_heads = own.numel() // (self.E * io.n_agents)
+                has_actions = True
+            else:
+                io.agent_ids = _lib.ptr(self._ids32(p))
+                has_actions = actions is not None
             if t >= 0:
                 io.rewards_batch = _lib.ptr(self._tensor(f"{_REWARDS}_batch_{p}")[s])
-                if actions is not None:
+                if has_actions:
                     io.actions_batch = _lib.ptr(self._tensor(f"{_ACTIONS}_batch_{p}")[s])
             io.reward_running_sum = _lib.ptr(self.reward_running_sum[p])
             io.episodic_reward_sum = _lib.ptr(self.episodic_reward_sum[p])
         _lib.check(_lib.load().wdb_rollout_bookkeep(_lib.stream_ptr(), ctypes.byref(k)),
                    "rollout_bookkeep")
 
+    def policy_step_arrays(self, p):
+        """(rewards [E, Np], sampled actions [E, Np, n_heads]) of policy p's agents."""
+        if self.separate:
+            return self._tensor(f"{_REWARDS}_{p}"), self._tensor(f"{_ACTIONS}_{p}")
+        rewards, actions = self._tensor(_REWARDS), self._tensor(_ACTIONS)
+        if self.covers_all[p]:
+            return rewards, actions
+        return rewards.index_select(1, self.ids[p]), actions.index_select(1, self.ids[p])
+
     def bookkeep_torch(self, t):
         """The same bookkeeping in plain torch ops (the parity reference of bookkeep() in
         tests/test_gpu_rollout.py; not used by the engine)."""
         raw_done = self._tensor("_done_")
-        rewards = self._tensor(_REWARDS)
         if t >= 0:
             self._tensor(f"{_DONE_FLAGS}_batch")[t].copy_(raw_done)
-            actions = self._tensor(_ACTIONS)
-            for p in self.policies:
-                self._tensor(f"{_ACTIONS}_batch_{p}")[t].copy_(
-                    actions if self.covers_all[p] else actions.index_select(1, self.ids[p]))
         done = (raw_done > 0).to(torch.int32)
         donef = done.to(torch.float32)
         for p in self.policies:
-            r_p = rewards if self.covers_all[p] else rewards.index_select(1, self.ids[p])
+            r_p, a_p = self.policy_step_arrays(p)
             if t >= 0:
+                self._tensor(f"{_ACTIONS}_batch_{p}")[t].copy_(a_p)
                 self._tensor(f"{_REWARDS}_batch_{p}")[t].copy_(r_p)
             run = self.reward_running_sum[p]
             run.add_(r_p)

@@ -101,8 +101,11 @@ class Trainer:
         assert env_wrapper is not None and env_wrapper.env_backend != "cpu"
         assert config is not None
         self._check_obs_dim(obs_dim_corresponding_to_num_agents)
-        assert not create_separate_placeholders_for_each_policy, (
-            "separate per-policy step placeholders are not implemented in the native trainer")
+        # heterogeneous agents: each policy steps through its own observation / action /
+        # reward arrays, and / or the env writes observations agent-last ([E, *F, N])
+        self.create_separate_placeholders_for_each_policy = bool(
+            create_separate_placeholders_for_each_policy)
+        self.obs_dim_corresponding_to_num_agents = obs_dim_corresponding_to_num_agents
         self.cuda_envs = env_wrapper
         self.verbose = verbose
         self.num_devices, self.device_id = num_devices, device_id
@@ -146,6 +149,8 @@ class Trainer:
         create_and_push_data_placeholders(
             env_wrapper=self.cuda_envs, action_sampler=self.cuda_sample_controller,
             policy_tag_to_agent_id_map=self.policy_tag_to_agent_id_map,
+            create_separate_placeholders_for_each_policy=(
+                self.create_separate_placeholders_for_each_policy),
             obs_dim_corresponding_to_num_agents=obs_dim_corresponding_to_num_agents,
             training_batch_size_per_env=batch_slots_per_env)
         seed = int(t.get("seed", np.int32(time.time()))) + self.device_id
@@ -194,12 +199,9 @@ class Trainer:
     # ------------------------------------------------------------------ what subclasses change
     @staticmethod
     def _check_obs_dim(obs_dim_corresponding_to_num_agents):
-        assert obs_dim_corresponding_to_num_agents in ("first", "last")
-        # the rollout engine views observations as [E, N, F]; 'last' ([E, ..., N]) would be
-        # silently scrambled across agents and features
-        assert obs_dim_corresponding_to_num_agents == "first", (
-            "obs_dim_corresponding_to_num_agents='last' is not supported by the native rollout "
-            "engine (observations must be [num_envs, num_agents, ...])")
+        assert obs_dim_corresponding_to_num_agents in ("first", "last"), (
+            "obs_dim_corresponding_to_num_agents must be 'first' ([E, N, *F] observations) or "
+            "'last' ([E, *F, N])")
 
     @staticmethod
     def _merge_policy_defaults(policy_config, defaults):
@@ -235,9 +237,13 @@ class Trainer:
         return [("", self.optimizers[policy], self.lr_schedules[policy])]
 
     def _make_engine(self, use_cuda_graph):
-        return RolloutEngine(self.cuda_envs, self.models, self.policy_tag_to_agent_id_map,
-                             self.cuda_sample_controller, self.training_batch_size_per_env,
-                             use_cuda_graph=use_cuda_graph)
+        return RolloutEngine(
+            self.cuda_envs, self.models, self.policy_tag_to_agent_id_map,
+            self.cuda_sample_controller, self.training_batch_size_per_env,
+            use_cuda_graph=use_cuda_graph,
+            create_separate_placeholders_for_each_policy=(
+                self.create_separate_placeholders_for_each_policy),
+            obs_dim_corresponding_to_num_agents=self.obs_dim_corresponding_to_num_agents)
 
     # ------------------------------------------------------------------ setup helpers
     def _get_config(self, args):
@@ -249,7 +255,10 @@ class Trainer:
     def _build_model(self, policy, model_config):
         model = ModelFactory.create(model_config["type"])(
             env=self.cuda_envs, model_config=model_config, policy=policy,
-            policy_tag_to_agent_id_map=self.policy_tag_to_agent_id_map)
+            policy_tag_to_agent_id_map=self.policy_tag_to_agent_id_map,
+            create_separate_placeholders_for_each_policy=(
+                self.create_separate_placeholders_for_each_policy),
+            obs_dim_corresponding_to_num_agents=self.obs_dim_corresponding_to_num_agents)
         if model_config.get("init_method") == "xavier":
             for m in model.modules():
                 if isinstance(m, nn.Linear):
@@ -493,9 +502,8 @@ class Trainer:
                 eng.sample_actions(probs, -1, **sample_params)
                 self.cuda_envs.step_all_envs()
                 undone = done == 0
-                rewards = dm.data_on_device_via_torch(_REWARDS)
                 for p in self.policies:
-                    r_p = rewards if eng.covers_all[p] else rewards.index_select(1, eng.ids[p])
+                    r_p, _ = eng.policy_step_arrays(p)
                     reward_sum[p] += r_p * undone[:, None]
                     step_sum[p] += undone.to(torch.int32)
                 # done envs restart but keep their flag: one episode per env is counted
@@ -507,9 +515,12 @@ class Trainer:
 
     # ------------------------------------------------------------------ episode states
     def fetch_episode_states(self, list_of_states=None, env_id=0, include_rewards_actions=False,
-                             include_probabilities=False):
+                             include_probabilities=False, policy=""):
         """Play one episode of env `env_id` with the current policies and return the
         per-timestep values of the requested device arrays (trainer_base.py:689-792).
+        With separate placeholders, `policy` names the policy whose `sampled_actions_{policy}`
+        / `rewards_{policy}` (include_rewards_actions) and probabilities
+        (include_probabilities) are logged.
 
         The episode is logged ON THE DEVICE: every requested array has a [T + 1, ...] ring in
         HBM that `wdb_log_one_step` (the CUDALogController kernel, function_manager.py:295-422)
@@ -534,9 +545,15 @@ class Trainer:
         rings = {name: ring(name, T + 1) for name in list_of_states}
         for name in list_of_states:
             logger.log_tensor_one_step(rings[name], dm.data_on_device_via_torch(name), 0, env_id)
+        suffix = f"_{policy}" if policy else ""
+        if self.create_separate_placeholders_for_each_policy and (
+                include_rewards_actions or include_probabilities):
+            assert policy in self.policies, (
+                "with separate placeholders, name the policy whose actions, rewards or "
+                "probabilities to log")
         extra = {}
         if include_rewards_actions:
-            extra = {_ACTIONS: ring(_ACTIONS, T), _REWARDS: ring(_REWARDS, T)}
+            extra = {name: ring(name, T) for name in (_ACTIONS + suffix, _REWARDS + suffix)}
         done_ring = torch.zeros(T, dtype=torch.int32, device=dm.device)
         prob_rings = None
         fused, self.engine.fused = self.engine.fused, None
@@ -555,6 +572,8 @@ class Trainer:
                 logger.log_tensor_one_step(done_ring, dm.data_on_device_via_torch("_done_"), t,
                                            env_id)
                 if include_probabilities:
+                    if self.create_separate_placeholders_for_each_policy:
+                        probs = probs[policy]
                     if prob_rings is None:
                         prob_rings = [torch.zeros((T,) + tuple(p.shape[1:]), device=p.device)
                                       for p in probs]

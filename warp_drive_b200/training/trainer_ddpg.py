@@ -111,6 +111,9 @@ class TrainerDDPG(Trainer):
                  create_separate_placeholders_for_each_policy=False,
                  obs_dim_corresponding_to_num_agents="first", num_devices=1, device_id=0,
                  results_dir=None, verbose=True):
+        assert not create_separate_placeholders_for_each_policy, (
+            "TrainerDDPG steps every policy through the shared observation / action / reward "
+            "arrays: separate per-policy placeholders are not supported")
         super().__init__(env_wrapper, config, policy_tag_to_agent_id_map,
                          create_separate_placeholders_for_each_policy,
                          obs_dim_corresponding_to_num_agents, num_devices, device_id,
