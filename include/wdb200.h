@@ -559,7 +559,8 @@ int wdb_relu_backward_bias(void *stream, float *grad_hidden, const float *hidden
  * every head, the loss sums and the gradients of
  *     loss = mean(-logp * adv) + vf_coeff * mean((V - R)^2) - entropy_coeff * sum_k mean(H_k)
  * with respect to the probabilities and the values (PPO's clipped surrogate has the same
- * gradient at ratio == 1, the reference's single-epoch case, ppo.py:127-136).
+ * gradient at ratio == 1, the reference's single-epoch case, ppo.py:127-136; several epochs
+ * over minibatches go through wdb_gae and wdb_ppo_loss_and_grads).
  * sums (double[4], zeroed by the caller): sum(-logp*adv), sum((V-R)^2), sum_k sum(H_k), sum(adv). */
 typedef struct wdb_pg_loss {
   int T, n_envs, n_agents, n_heads;
@@ -612,6 +613,92 @@ int wdb_pg_gaussian_loss_and_grads(void *stream, const wdb_pg_gaussian_loss *los
 /* 1 if wdb_pg_gaussian_loss_and_grads takes this action dimension (1..WDB_PG_GAUSSIAN_MAX_DIM:
  * a row's dimensions are held in registers), else 0.  No CUDA call. */
 int wdb_pg_gaussian_loss_supported(int action_dim);
+
+/* Multi-epoch PPO over shuffled minibatches (no reference counterpart: the reference's PPO
+ * takes one step per batch at ratio == 1).
+ *
+ * wdb_gae: advantages and value targets of GAE(lambda), one backward-in-time scan per (env,
+ * agent), with d = done[t, e] > 0 and the bootstrapping of wdb_discounted_returns:
+ *   t = T-1:  A = d ? r - V : 0
+ *   t < T-1:  delta = r + (d ? 0 : gamma * V[t+1]) - V ;  A = delta + (d ? 0 : gamma*lambda*A[t+1])
+ *   value_target = A + V
+ * (lambda = 1: value_target is the discounted return; lambda = 0: one-step TD). */
+typedef struct wdb_gae_args {
+  int T, n_envs, n_agents;
+  const float *rewards;              /* [T, E, Np] */
+  const float *values;               /* [T, E, Np] */
+  const int *done;                   /* [T, E] (> 0 = done) */
+  float gamma, gae_lambda;
+  float *advantages;                 /* out [T, E, Np] */
+  float *value_targets;              /* out [T, E, Np] */
+} wdb_gae_args;
+int wdb_gae(void *stream, const wdb_gae_args *gae);
+
+/* The loss of one minibatch of B rows of the flat [R = T * E * Np] batch and its gradients with
+ * respect to the model outputs.  Row b of the minibatch is flat row rows[b] (rows == NULL: row
+ * b); the model outputs (probs / mean, values) are in minibatch order, everything else is read
+ * through rows.  With l = the row's log-prob (Categorical over every head, as
+ * wdb_pg_loss_and_grads, or the diagonal Normal of wdb_pg_gaussian_loss_and_grads),
+ * rho = exp(l - old_log_prob), A = advantages and eps = clip_param:
+ *   policy = ppo ? -(1/B) sum min(rho * A, clamp(rho, 1 - eps, 1 + eps) * A)
+ *                : -(1/B) sum l * A
+ *   loss   = policy + vf_coeff * (1/B) sum (V - value_target)^2 - entropy_coeff * (1/B) sum H
+ * The gradients are torch autograd's for that expression: torch.minimum gives half to each side
+ * of a tie, clamp passes the gradient on the closed interval [1 - eps, 1 + eps].
+ * sums (double[5], zeroed by the caller): sum of the policy terms, sum (V - value_target)^2,
+ * sum H, sum (old_log_prob - l) (approximate KL), count of |rho - 1| > eps.
+ * log_prob (optional out [B]): l in minibatch order.  old_log_prob == NULL is the log-prob
+ * pre-pass: only log_prob is written (required), no gradient output may be given, and values,
+ * advantages, value_targets and sums are not read. */
+typedef struct wdb_ppo_loss {
+  int B, n_heads;
+  int n_actions[4];
+  const float *probs[4];             /* [B, A_k] */
+  const float *values;               /* [B] */
+  const int *rows;                   /* [B] into [R], or NULL */
+  const int *actions;                /* [R, n_heads] */
+  const float *advantages;           /* [R] */
+  const float *value_targets;        /* [R] */
+  const float *old_log_prob;         /* [R], or NULL: the pre-pass */
+  int ppo;                           /* 0: the A2C policy term */
+  float clip_param, vf_coeff, entropy_coeff;
+  float *grad_probs[4];              /* out [B, A_k] (or NULL) */
+  float *grad_values;                /* out [B] (or NULL) */
+  float *log_prob;                   /* out [B] (or NULL) */
+  double *sums;                      /* out [5], accumulated atomically */
+} wdb_ppo_loss;
+int wdb_ppo_loss_and_grads(void *stream, const wdb_ppo_loss *loss);
+/* 1 if wdb_ppo_loss_and_grads takes these heads (those of wdb_pg_loss_supported), else 0.
+ * No CUDA call. */
+int wdb_ppo_loss_supported(int n_heads, const int *n_actions);
+
+/* The same for a diagonal Gaussian policy.  The log_std gradient,
+ *   -(1/B) sum_b w_b (z_bk^2 - 1) - entropy_coeff  with w_b = -B * d policy / d l_b,
+ * is summed from per-CTA float64 partials in a fixed order by a second launch, so it is
+ * bit-identical on relaunch. */
+typedef struct wdb_ppo_gaussian_loss {
+  int B, action_dim;                 /* action_dim A: 1..WDB_PG_GAUSSIAN_MAX_DIM */
+  const float *mean;                 /* [B, A] */
+  const float *log_std;              /* [A] */
+  const float *values;               /* [B] */
+  const int *rows;                   /* [B] into [R], or NULL */
+  const float *actions;              /* [R, A] */
+  const float *advantages;           /* [R] */
+  const float *value_targets;        /* [R] */
+  const float *old_log_prob;         /* [R], or NULL: the pre-pass */
+  int ppo;
+  float clip_param, vf_coeff, entropy_coeff;
+  float *grad_mean;                  /* out [B, A] (or NULL) */
+  float *grad_log_std;               /* out [A] (or NULL) */
+  float *grad_values;                /* out [B] (or NULL) */
+  float *log_prob;                   /* out [B] (or NULL) */
+  double *sums;                      /* out [5] as wdb_ppo_loss */
+  double *partials;                  /* workspace [ceil(B / ROWS_PER_CTA), A] doubles;
+                                      * required with grad_log_std */
+} wdb_ppo_gaussian_loss;
+int wdb_ppo_gaussian_loss_and_grads(void *stream, const wdb_ppo_gaussian_loss *loss);
+/* 1 if wdb_ppo_gaussian_loss_and_grads takes this action dimension, else 0.  No CUDA call. */
+int wdb_ppo_gaussian_loss_supported(int action_dim);
 
 /* Gradient-norm clipping + Adam over one flat float32 arena (torch.optim.Adam semantics, no
  * weight decay; torch.nn.utils.clip_grad_norm_ semantics for the clip factor, which the Adam

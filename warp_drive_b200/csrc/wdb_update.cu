@@ -12,6 +12,10 @@
 // (1b) pg_gaussian_loss_kernel: the same scan for a diagonal Gaussian policy (mean per row,
 //     state-independent log_std), whose log_std gradient is reduced in a fixed order by
 //     pg_gaussian_log_std_grad_kernel (no reference counterpart).
+// (1c) gae_kernel + ppo_loss_kernel / ppo_gaussian_loss_kernel: PPO over several epochs of
+//     shuffled minibatches (no reference counterpart): GAE(lambda) once per batch, then per
+//     minibatch the clipped loss against the rollout policy's log-probs and its gradients,
+//     row-parallel, with the batch-side inputs read through an int32 row list.
 // (2) sumsq_kernel + adam_kernel: gradient-norm clipping and Adam over ONE flat parameter
 //     arena (every trained tensor of a policy is a view into it), no host synchronisation:
 //     the clip factor is read from device memory by the Adam kernel.
@@ -260,6 +264,236 @@ __global__ void pg_gaussian_log_std_grad_kernel(const double *__restrict__ parti
   double acc = 0.0;
   for (int c = 0; c < n_ctas; c++) acc += partials[(long long)c * A + k];
   grad_log_std[k] = (float)(-acc * inv_m - (double)entropy_coeff);
+}
+
+// ---- multi-epoch PPO over minibatches: GAE once per batch, then a row-parallel loss ---------
+// GAE(lambda) with this repo's bootstrapping convention: one thread per (env, agent) walks T
+// backwards; consecutive threads read consecutive rows of a timestep (coalesced).
+__global__ void __launch_bounds__(kPgThreads) gae_kernel(const __grid_constant__ wdb_gae_args G) {
+  const long long per_t = (long long)G.n_envs * G.n_agents;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= per_t) return;
+  const int env = (int)(i / G.n_agents);
+  const float gl = G.gamma * G.gae_lambda;
+  float adv = 0.0f, v_next = 0.0f;
+  for (int t = G.T - 1; t >= 0; t--) {
+    const long long idx = (long long)t * per_t + i;
+    const int d = G.done[(long long)t * G.n_envs + env] > 0;
+    const float r = G.rewards[idx], v = G.values[idx];
+    if (t == G.T - 1) {
+      adv = d ? r - v : 0.0f;
+    } else {
+      const float delta = r + (d ? 0.0f : G.gamma * v_next) - v;
+      adv = delta + (d ? 0.0f : gl * adv);
+    }
+    G.advantages[idx] = adv;
+    G.value_targets[idx] = adv + v;
+    v_next = v;
+  }
+}
+
+// d loss / d logp of one row, times -B: the weight that replaces `adv` in the A2C gradient.
+// PPO: d/d rho of min(rho * A, clamp(rho, 1 - eps, 1 + eps) * A) (torch.minimum splits a tie
+// half and half; clamp passes the gradient on its closed interval), times d rho / d logp = rho.
+__device__ __forceinline__ float ppo_weight(int ppo, float adv, float rho, float eps) {
+  if (!ppo) return adv;
+  const float lo = 1.0f - eps, hi = 1.0f + eps;
+  const float inside = (rho >= lo && rho <= hi) ? 1.0f : 0.0f;
+  const float x = rho * adv, y = fminf(fmaxf(rho, lo), hi) * adv;
+  const float g = x < y ? adv : (x > y ? adv * inside : 0.5f * adv + 0.5f * (adv * inside));
+  return g * rho;
+}
+
+// sums[0..4] of one row into the thread's float64 accumulators (shared by both PPO kernels)
+__device__ __forceinline__ void ppo_row_sums(double *s, int ppo, float logp, float old, float rho,
+                                             float adv, float eps, float dv, float ent) {
+  if (ppo) {
+    const float lo = 1.0f - eps, hi = 1.0f + eps;
+    s[0] -= (double)fminf(rho * adv, fminf(fmaxf(rho, lo), hi) * adv);
+  } else {
+    s[0] -= (double)(logp * adv);
+  }
+  s[1] += (double)dv * (double)dv;
+  s[2] += (double)ent;
+  s[3] += (double)(old - logp);
+  s[4] += fabsf(rho - 1.0f) > eps ? 1.0 : 0.0;
+}
+
+// block reduction of the five sums -> 5 double atomics per CTA
+template <int kThreads>
+__device__ __forceinline__ void ppo_reduce_sums(double *s, double *out) {
+  __shared__ double red[5][kThreads / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int k = 0; k < 5; k++) {
+    const double v = warp_sum(s[k]);
+    if (lane == 0) red[k][warp] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x < 5) {
+    double acc = 0.0;
+    for (int w = 0; w < kThreads / 32; w++) acc += red[threadIdx.x][w];
+    atomicAdd(&out[threadIdx.x], acc);
+  }
+}
+
+// The Categorical minibatch loss: thread b owns minibatch row b; the warp's 32 probability rows
+// are one contiguous block (minibatch order) staged through shared memory like pg_loss_kernel.
+// Pass 1 over the heads: log-prob and entropy.  Pass 2 (when gradients are asked for): the
+// gradient of every head with the row's weight w = -B * d loss / d logp.
+__global__ void __launch_bounds__(kPgThreads)
+ppo_loss_kernel(const __grid_constant__ wdb_ppo_loss L, int tile_pitch) {
+  extern __shared__ float pg_tiles[];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  float *tile = pg_tiles + (size_t)warp * 32 * tile_pitch;
+  const long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long b0 = b - lane;
+  const bool live = b < L.B;
+  const int n_rows = (int)max(0ll, min(32ll, (long long)L.B - b0));
+  const bool loss = L.old_log_prob != nullptr;
+  const float inv_bf = (float)(1.0 / (double)L.B);
+  double s[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
+  if (n_rows > 0) {
+    const long long row = live ? (L.rows ? (long long)L.rows[b] : b) : 0;
+    float logp = 0.0f, ent = 0.0f;
+    for (int k = 0; k < L.n_heads; k++) {
+      const int A = L.n_actions[k];
+      __syncwarp();
+      warp_block_load(tile, tile_pitch, L.probs[k] + b0 * A, A, n_rows, lane);
+      __syncwarp();
+      if (live) {
+        // torch.distributions.Categorical(probs=p), as pg_loss_kernel
+        const float *p = tile + lane * tile_pitch;
+        const int a = L.actions[row * L.n_heads + k];
+        float z = 0.0f;
+        for (int j = 0; j < A; j++) z += p[j];
+        const float inv_z = 1.0f / z;
+        for (int j = 0; j < A; j++) {
+          const float lq = logf(fminf(fmaxf(p[j] * inv_z, kProbEps), 1.0f - kProbEps));
+          ent -= lq * (p[j] * inv_z);
+          if (j == a) logp += lq;
+        }
+      }
+    }
+    if (live && L.log_prob) L.log_prob[b] = logp;
+    float w = 0.0f;
+    if (loss && live) {
+      const float old = L.old_log_prob[row], adv = L.advantages[row];
+      const float rho = expf(logp - old);
+      const float dv = L.values[b] - L.value_targets[row];
+      w = ppo_weight(L.ppo, adv, rho, L.clip_param);
+      ppo_row_sums(s, L.ppo, logp, old, rho, adv, L.clip_param, dv, ent);
+      if (L.grad_values) L.grad_values[b] = 2.0f * L.vf_coeff * dv * inv_bf;
+    }
+    for (int k = 0; k < L.n_heads; k++) {
+      if (!L.grad_probs[k]) continue;
+      const int A = L.n_actions[k];
+      if (L.n_heads > 1) {               // one head: the tile still holds its rows
+        __syncwarp();
+        warp_block_load(tile, tile_pitch, L.probs[k] + b0 * A, A, n_rows, lane);
+        __syncwarp();
+      }
+      if (live) {
+        float *p = tile + lane * tile_pitch;
+        const int a = L.actions[row * L.n_heads + k];
+        float z = 0.0f;
+        for (int j = 0; j < A; j++) z += p[j];
+        const float inv_z = 1.0f / z;
+        float S = 0.0f;
+        for (int j = 0; j < A; j++) {
+          const float q = p[j] * inv_z;
+          const bool inside = q >= kProbEps && q <= 1.0f - kProbEps;
+          const float lq = logf(fminf(fmaxf(q, kProbEps), 1.0f - kProbEps));
+          float gq = L.entropy_coeff * (lq + (inside ? 1.0f : 0.0f));
+          if (j == a && inside) gq -= w / q;
+          S += gq * q;
+        }
+        for (int j = 0; j < A; j++) {
+          const float q = p[j] * inv_z;
+          const bool inside = q >= kProbEps && q <= 1.0f - kProbEps;
+          const float lq = logf(fminf(fmaxf(q, kProbEps), 1.0f - kProbEps));
+          float gq = L.entropy_coeff * (lq + (inside ? 1.0f : 0.0f));
+          if (j == a && inside) gq -= w / q;
+          p[j] = (gq - S) * inv_bf * inv_z;
+        }
+      }
+      __syncwarp();
+      warp_block_store(L.grad_probs[k] + b0 * A, tile, tile_pitch, A, n_rows, lane);
+    }
+  }
+  if (loss) ppo_reduce_sums<kPgThreads>(s, L.sums);
+}
+
+// The diagonal-Gaussian minibatch loss: thread b owns minibatch row b, its A dimensions in
+// registers.  partials[blockIdx.x, k] = sum over the CTA's rows of w * (z_k^2 - 1), reduced in
+// a fixed order; pg_gaussian_log_std_grad_kernel turns them into the log_std gradient.
+__global__ void __launch_bounds__(kGaussThreads)
+ppo_gaussian_loss_kernel(const __grid_constant__ wdb_ppo_gaussian_loss L) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int A = L.action_dim;
+  const long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const bool live = b < L.B;
+  const bool loss = L.old_log_prob != nullptr;
+  const float inv_bf = (float)(1.0 / (double)L.B);
+  float ls[kGaussMaxA], inv_std[kGaussMaxA];
+  double g_ls[kGaussMaxA];
+  float ent = 0.0f;
+#pragma unroll
+  for (int k = 0; k < kGaussMaxA; k++) {
+    ls[k] = k < A ? L.log_std[k] : 0.0f;
+    inv_std[k] = expf(-ls[k]);
+    g_ls[k] = 0.0;
+    if (k < A) ent += ls[k] + (0.5f + kHalfLog2Pi);
+  }
+  double s[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
+  if (live) {
+    const long long row = L.rows ? (long long)L.rows[b] : b;
+    const float *mu = L.mean + b * A;
+    const float *a = L.actions + row * A;
+    float z[kGaussMaxA];
+    float logp = 0.0f;
+#pragma unroll
+    for (int k = 0; k < kGaussMaxA; k++) {
+      if (k < A) {
+        z[k] = (a[k] - mu[k]) * inv_std[k];
+        logp += -0.5f * z[k] * z[k] - ls[k] - kHalfLog2Pi;
+      }
+    }
+    if (L.log_prob) L.log_prob[b] = logp;
+    if (loss) {
+      const float old = L.old_log_prob[row], adv = L.advantages[row];
+      const float rho = expf(logp - old);
+      const float dv = L.values[b] - L.value_targets[row];
+      const float w = ppo_weight(L.ppo, adv, rho, L.clip_param);
+      ppo_row_sums(s, L.ppo, logp, old, rho, adv, L.clip_param, dv, ent);
+      if (L.grad_values) L.grad_values[b] = 2.0f * L.vf_coeff * dv * inv_bf;
+      float *gm = L.grad_mean ? L.grad_mean + b * A : nullptr;
+#pragma unroll
+      for (int k = 0; k < kGaussMaxA; k++) {
+        if (k < A) {
+          // d(-logp * w) / d mu_k = -w * z / std;  / d ls_k = -w * (z^2 - 1)
+          if (gm) gm[k] = -w * z[k] * inv_std[k] * inv_bf;
+          g_ls[k] += (double)(w * (z[k] * z[k] - 1.0f));
+        }
+      }
+    }
+  }
+  if (!loss) return;
+  ppo_reduce_sums<kGaussThreads>(s, L.sums);
+  __shared__ double red[kGaussMaxA][kGaussThreads / 32];
+#pragma unroll
+  for (int k = 0; k < kGaussMaxA; k++) {
+    if (k < A) {
+      const double v = warp_sum(g_ls[k]);
+      if (lane == 0) red[k][warp] = v;
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x < A && L.partials) {
+    double acc = 0.0;
+    for (int w = 0; w < kGaussThreads / 32; w++) acc += red[threadIdx.x][w];
+    L.partials[(long long)blockIdx.x * A + threadIdx.x] = acc;
+  }
 }
 
 // sum of squares of a flat float buffer -> *out (double, zeroed by the caller)
@@ -587,6 +821,77 @@ WDB_API int wdb_pg_gaussian_loss_and_grads(void *stream, const wdb_pg_gaussian_l
   pg_gaussian_log_std_grad_kernel<<<1, 32, 0, as_stream(stream)>>>(
       l->partials, grid, l->action_dim, 1.0 / ((double)l->T * (double)n), l->entropy_coeff,
       l->grad_log_std);
+  return finish_launch();
+}
+
+WDB_API int wdb_gae(void *stream, const wdb_gae_args *g) {
+  if (!g || g->T < 1 || g->n_envs < 1 || g->n_agents < 1 || !g->rewards || !g->values ||
+      !g->done || !g->advantages || !g->value_targets)
+    return (int)cudaErrorInvalidValue;
+  const long long n = (long long)g->n_envs * g->n_agents;
+  gae_kernel<<<(unsigned)((n + kPgThreads - 1) / kPgThreads), kPgThreads, 0,
+               as_stream(stream)>>>(*g);
+  return finish_launch();
+}
+
+WDB_API int wdb_ppo_loss_supported(int n_heads, const int *n_actions) {
+  return pg_loss_smem(n_heads, n_actions, nullptr) > 0;
+}
+
+WDB_API int wdb_ppo_gaussian_loss_supported(int action_dim) {
+  return action_dim >= 1 && action_dim <= kGaussMaxA;
+}
+
+// The loss mode (old_log_prob given) needs every per-row input and the sums; the log-prob
+// pre-pass (old_log_prob NULL) needs log_prob and takes no gradient outputs.
+static bool ppo_common_ok(int B, const void *old_log_prob, const float *log_prob,
+                          const float *values, const float *advantages,
+                          const float *value_targets, const double *sums, bool any_grad) {
+  if (B < 1) return false;
+  if (!old_log_prob) return log_prob && !any_grad;
+  return values && advantages && value_targets && sums;
+}
+
+WDB_API int wdb_ppo_loss_and_grads(void *stream, const wdb_ppo_loss *l) {
+  if (!l) return (int)cudaErrorInvalidValue;
+  int pitch = 0;
+  const size_t smem = pg_loss_smem(l->n_heads, l->n_actions, &pitch);
+  if (!smem || !l->actions) return (int)cudaErrorInvalidValue;
+  bool any_grad = l->grad_values != nullptr;
+  for (int k = 0; k < l->n_heads; k++) {
+    if (!l->probs[k]) return (int)cudaErrorInvalidValue;
+    any_grad = any_grad || l->grad_probs[k];
+  }
+  if (!ppo_common_ok(l->B, l->old_log_prob, l->log_prob, l->values, l->advantages,
+                     l->value_targets, l->sums, any_grad))
+    return (int)cudaErrorInvalidValue;
+  static size_t configured = 48 * 1024;
+  if (smem > configured) {
+    cudaError_t e = cudaFuncSetAttribute(ppo_loss_kernel,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return (int)e;
+    configured = smem;
+  }
+  ppo_loss_kernel<<<(unsigned)(((long long)l->B + kPgThreads - 1) / kPgThreads), kPgThreads, smem,
+                    as_stream(stream)>>>(*l, pitch);
+  return finish_launch();
+}
+
+WDB_API int wdb_ppo_gaussian_loss_and_grads(void *stream, const wdb_ppo_gaussian_loss *l) {
+  if (!l || !wdb_ppo_gaussian_loss_supported(l->action_dim) || !l->mean || !l->log_std ||
+      !l->actions)
+    return (int)cudaErrorInvalidValue;
+  const bool any_grad = l->grad_mean || l->grad_log_std || l->grad_values;
+  if (!ppo_common_ok(l->B, l->old_log_prob, l->log_prob, l->values, l->advantages,
+                     l->value_targets, l->sums, any_grad) ||
+      (l->grad_log_std && !l->partials))
+    return (int)cudaErrorInvalidValue;
+  const int grid = (int)(((long long)l->B + kGaussThreads - 1) / kGaussThreads);
+  ppo_gaussian_loss_kernel<<<grid, kGaussThreads, 0, as_stream(stream)>>>(*l);
+  int err = finish_launch();
+  if (err || !l->grad_log_std) return err;
+  pg_gaussian_log_std_grad_kernel<<<1, 32, 0, as_stream(stream)>>>(
+      l->partials, grid, l->action_dim, 1.0 / (double)l->B, l->entropy_coeff, l->grad_log_std);
   return finish_launch();
 }
 

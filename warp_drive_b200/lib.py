@@ -191,6 +191,40 @@ class PgGaussianLoss(ctypes.Structure):
     ]
 
 
+class GaeArgs(ctypes.Structure):
+    """struct wdb_gae_args (include/wdb200.h)."""
+
+    _fields_ = [
+        ("T", _i), ("n_envs", _i), ("n_agents", _i), ("rewards", _fp), ("values", _fp),
+        ("done", _fp), ("gamma", _f), ("gae_lambda", _f), ("advantages", _fp),
+        ("value_targets", _fp),
+    ]
+
+
+class PpoLoss(ctypes.Structure):
+    """struct wdb_ppo_loss (include/wdb200.h)."""
+
+    _fields_ = [
+        ("B", _i), ("n_heads", _i), ("n_actions", _i * 4), ("probs", _fp * 4), ("values", _fp),
+        ("rows", _fp), ("actions", _fp), ("advantages", _fp), ("value_targets", _fp),
+        ("old_log_prob", _fp), ("ppo", _i), ("clip_param", _f), ("vf_coeff", _f),
+        ("entropy_coeff", _f), ("grad_probs", _fp * 4), ("grad_values", _fp),
+        ("log_prob", _fp), ("sums", _fp),
+    ]
+
+
+class PpoGaussianLoss(ctypes.Structure):
+    """struct wdb_ppo_gaussian_loss (include/wdb200.h)."""
+
+    _fields_ = [
+        ("B", _i), ("action_dim", _i), ("mean", _fp), ("log_std", _fp), ("values", _fp),
+        ("rows", _fp), ("actions", _fp), ("advantages", _fp), ("value_targets", _fp),
+        ("old_log_prob", _fp), ("ppo", _i), ("clip_param", _f), ("vf_coeff", _f),
+        ("entropy_coeff", _f), ("grad_mean", _fp), ("grad_log_std", _fp),
+        ("grad_values", _fp), ("log_prob", _fp), ("sums", _fp), ("partials", _fp),
+    ]
+
+
 class DdpgNet(ctypes.Structure):
     """struct wdb_ddpg_net (include/wdb200.h)."""
 
@@ -262,6 +296,11 @@ _SIGNATURES = {
     "wdb_pg_loss_supported": (_i, [_i, ctypes.POINTER(_i)]),
     "wdb_pg_gaussian_loss_and_grads": (_i, [_vp, ctypes.POINTER(PgGaussianLoss)]),
     "wdb_pg_gaussian_loss_supported": (_i, [_i]),
+    "wdb_gae": (_i, [_vp, ctypes.POINTER(GaeArgs)]),
+    "wdb_ppo_loss_and_grads": (_i, [_vp, ctypes.POINTER(PpoLoss)]),
+    "wdb_ppo_loss_supported": (_i, [_i, ctypes.POINTER(_i)]),
+    "wdb_ppo_gaussian_loss_and_grads": (_i, [_vp, ctypes.POINTER(PpoGaussianLoss)]),
+    "wdb_ppo_gaussian_loss_supported": (_i, [_i]),
     "wdb_heads_softmax": (_i, [_vp, _vp, _ll, _i, _i, _i, _vp, _vp, _vp]),
     "wdb_heads_softmax_masked": (_i, [_vp, _vp, _ll, _i, _i, _i, _vp, _i, _vp, _vp, _vp]),
     "wdb_heads_softmax_backward": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _ll, _i, _i, _i, _vp]),

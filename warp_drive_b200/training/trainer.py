@@ -191,9 +191,11 @@ class Trainer:
             self._initialize_optimizer(policy)
         for policy in self.policies_to_train:
             self._initialize_policy_algorithm(policy)
+        self._minibatch_steps = self._minibatch_schedule()
         if self.num_devices > 1:
             self._broadcast_parameters()
         self.engine = self._make_engine(use_cuda_graph)
+        self._perm_generator = None
         self.perf_stats = PerfStats()
 
     # ------------------------------------------------------------------ what subclasses change
@@ -282,8 +284,35 @@ class Trainer:
         kw = dict(discount_factor_gamma=c["gamma"], normalize_advantage=c["normalize_advantage"],
                   normalize_return=c["normalize_return"], vf_loss_coeff=c["vf_loss_coeff"],
                   entropy_coeff=c["entropy_coeff"])
+        # several epochs over shuffled minibatches / GAE (absent keys: the single-step update)
+        kw.update(num_epochs=c.get("num_epochs", 1), num_mini_batches=c.get("num_mini_batches", 1),
+                  gae_lambda=c.get("gae_lambda"))
         self.trainers[policy] = A2C(**kw) if c["algorithm"] == "A2C" else PPO(
             clip_param=c["clip_param"], **kw)
+        if (self.trainers[policy].minibatch_path
+                and self.config["trainer"].get("neg_pos_env_ratio", -1) > 0):
+            raise ValueError("neg_pos_env_ratio is not supported with num_epochs, "
+                             "num_mini_batches or gae_lambda")
+
+    def _minibatch_schedule(self):
+        """Optimizer steps per iteration (num_epochs x num_mini_batches) when the trained
+        policies take the minibatch update, None when they all take the single-step update.
+        Every optimizer step all-reduces the whole gradient arena once, so the policies must
+        agree on that product; each still runs its own epochs and minibatch split."""
+        on = {p: getattr(self.trainers.get(p), "minibatch_path", False)
+              for p in self.policies_to_train}
+        if not any(on.values()):
+            return None
+        if not all(on.values()):
+            raise ValueError("either every trained policy sets num_epochs / num_mini_batches / "
+                             f"gae_lambda or none does: {on}")
+        steps = {p: (self.trainers[p].num_epochs, self.trainers[p].num_mini_batches)
+                 for p in self.policies_to_train}
+        if len({e * m for e, m in steps.values()}) != 1:
+            raise ValueError("the trained policies must agree on num_epochs x num_mini_batches: "
+                             f"{steps}")
+        e, m = next(iter(steps.values()))
+        return e * m
 
     # ------------------------------------------------------------------ multi-GPU
     def _trained_params(self):
@@ -339,6 +368,8 @@ class Trainer:
         return params
 
     def _update_model_params(self, iteration):
+        if self._minibatch_steps is not None:
+            return self._update_model_params_minibatches(iteration)
         logging_flag = self._is_logging_iteration(iteration)
         dm = self.cuda_envs.cuda_data_manager
         done_flags_batch = dm.data_on_device_via_torch(f"{_DONE_FLAGS}_batch")
@@ -368,6 +399,73 @@ class Trainer:
             loss.backward()
         return self._step_optimizers(loss_metrics, logging_flag)
 
+    def _update_model_params_minibatches(self, iteration):
+        """num_epochs x num_mini_batches optimizer steps on one batch: the batch is prepared
+        once per policy (advantages, value targets and old log-probs at the rollout's
+        parameters), then every step is forward + fused loss + backward for every policy, one
+        all-reduce and clipping + Adam.  Step s of a policy with m minibatches is chunk s % m of
+        its epoch s // m; each epoch draws a fresh permutation of that policy's rows.  The bf16
+        rollout weights are repacked once, after the last step."""
+        logging_flag = self._is_logging_iteration(iteration)
+        dm = self.cuda_envs.cuda_data_manager
+        done_flags_batch = dm.data_on_device_via_torch(f"{_DONE_FLAGS}_batch")
+        batches = {}
+        for policy in self.policies_to_train:
+            mask_name = f"{_ACTION_MASK}_batch_{policy}"
+            mask = (dm.data_on_device_via_torch(mask_name)
+                    if dm.is_data_on_device_via_torch(mask_name) else None)
+            self._advance_timestep(policy)
+            batches[policy] = self.trainers[policy].prepare_batch(
+                self.models[policy],
+                dm.data_on_device_via_torch(f"{_PROCESSED_OBSERVATIONS}_batch_{policy}"),
+                dm.data_on_device_via_torch(f"{_ACTIONS}_batch_{policy}"),
+                dm.data_on_device_via_torch(f"{_REWARDS}_batch_{policy}"), done_flags_batch,
+                mask)
+        if self._perm_generator is None:
+            self._perm_generator = torch.Generator(device=done_flags_batch.device)
+            self._perm_generator.manual_seed(self.seed)
+        n_steps = self._minibatch_steps
+        sums = {p: torch.zeros(5, dtype=torch.float64, device=done_flags_batch.device)
+                for p in self.policies_to_train}
+        chunks = {}
+        step_info = None
+        for step in range(n_steps):
+            for policy in self.policies_to_train:
+                n_mini = self.trainers[policy].num_mini_batches
+                if step % n_mini == 0:         # a new epoch of this policy
+                    chunks[policy] = torch.tensor_split(
+                        self.minibatch_permutation(batches[policy].R), n_mini)
+                rows = chunks[policy][step % n_mini]
+                loss, s = self.trainers[policy].minibatch_loss(
+                    self.models[policy], batches[policy], rows, self.current_timestep[policy])
+                self.optimizers[policy].zero_grad()
+                loss.backward()
+                if logging_flag:
+                    sums[policy] += s / rows.numel()
+            info = self._optimizer_step(self.policies_to_train, logging_flag)
+            step_info = info if step_info is None else self._add_step_info(step_info, info)
+        loss_metrics = {}
+        if logging_flag:
+            for policy, (norms, lrs) in step_info.items():
+                norms.update({k: v / n_steps for k, v in norms.items()})
+            for policy in self.policies_to_train:
+                loss_metrics[policy] = self.trainers[policy].minibatch_metrics(
+                    batches[policy], sums[policy] / n_steps, self.current_timestep[policy])
+        return self._finish_update(loss_metrics, step_info, logging_flag)
+
+    def minibatch_permutation(self, n_rows):
+        """The next epoch's order of a policy's n_rows batch rows (int32, on the device), drawn
+        from the trainer's seeded generator: a run is reproducible."""
+        return torch.randperm(n_rows, generator=self._perm_generator,
+                              device=self._perm_generator.device).to(torch.int32)
+
+    @staticmethod
+    def _add_step_info(total, info):
+        for policy, (norms, _) in info.items():
+            for k, v in norms.items():
+                total[policy][0][k] = total[policy][0][k] + v
+        return total
+
     def _is_logging_iteration(self, iteration):
         return (iteration % self.config["saving"]["metrics_log_freq"] == 0
                 or iteration == self.num_iters - 1)
@@ -383,26 +481,43 @@ class Trainer:
         """The update once the gradients of the policies in `loss_metrics` are in the arena:
         one all-reduce, then clipping + Adam per network.  On a logging iteration, returns the
         metrics of every trained policy and restarts the episodic counters."""
-        if self.num_devices > 1 and loss_metrics:
+        step_info = self._optimizer_step(loss_metrics, logging_flag)
+        return self._finish_update(loss_metrics, step_info, logging_flag)
+
+    def _optimizer_step(self, stepped, logging_flag):
+        """One optimizer step of the policies in `stepped`: one all-reduce of the gradient
+        arena, then clipping + Adam per network.  Returns {policy: (gradient norms as device
+        tensors, learning rates)}, filled on a logging iteration."""
+        if self.num_devices > 1 and stepped:
             self._allreduce_gradients()
-        metrics_dict = {}
+        step_info = {}
         for policy in self.policies_to_train:
-            optimizers = self._optimizers_of(policy) if policy in loss_metrics else []
+            optimizers = self._optimizers_of(policy) if policy in stepped else []
             norms, lrs = {}, {}
             if logging_flag:
                 for suffix, opt, _ in optimizers:
-                    norms[f"Gradient norm{suffix}"] = float(sum(
-                        p.grad.norm(2) for p in opt.param_list if p.grad is not None))
+                    norms[f"Gradient norm{suffix}"] = sum(
+                        p.grad.norm(2) for p in opt.param_list if p.grad is not None)
                     lrs[f"Learning rate{suffix}"] = opt.param_groups[0]["lr"]
             # clip_grad_norm_ + Adam as two flat kernels, clip factor stays on the device
             clip = self.max_grad_norm[policy] if self.clip_grad_norm[policy] else None
             for _, opt, _ in optimizers:
                 opt.step(max_grad_norm=clip)
+            step_info[policy] = (norms, lrs)
+        return step_info
+
+    def _finish_update(self, loss_metrics, step_info, logging_flag):
+        """Once per iteration after the last optimizer step: repack the rollout weights and, on
+        a logging iteration, collect every trained policy's metrics and restart the episodic
+        counters."""
+        metrics_dict = {}
+        for policy in self.policies_to_train:
             if logging_flag:
+                norms, lrs = step_info[policy]
                 n_done = int(self.engine.num_completed_episodes)
                 metrics = loss_metrics.get(policy, {})
                 metrics["Current timestep"] = self.current_timestep[policy]
-                metrics.update(norms)
+                metrics.update({k: float(v) for k, v in norms.items()})
                 metrics.update(lrs)
                 metrics.update({
                     "Mean episodic reward":
