@@ -752,6 +752,50 @@ long long wdb_ddpg_update_workspace_bytes(const wdb_ddpg_update_args *update);  
 /* cudaErrorInvalidValue without launching if unsupported or a required pointer is NULL. */
 int wdb_ddpg_update(void *stream, const wdb_ddpg_update_args *update);
 
+/* One TD3 update of one policy (Fujimoto et al. 2018) over the same ring and the same M loss
+ * rows as wdb_ddpg_update, as two passes of two launches each (a tile kernel and the
+ * fixed-order reduction: bit-reproducible).
+ * Critic pass (wdb_td3_critic_update): per loss row g (window i, agent row n) and action dim c,
+ *   a'[c] = clamp(pi'[c] + clamp(sigma * scale * noise[g][c], -clip * scale, clip * scale),
+ *                 bias - scale, bias + scale),   pi' = target_actor(obs') as in DDPG,
+ *   R = the n-step return of DDPG bootstrapped with min(target_critic(obs', a'),
+ *       target_critic2(obs', a')) at DDPG's bootstrap slot,
+ *   gradients of mse(Q1(obs, actions), R) + mse(Q2(obs, actions), R) into critic.gw / gb and
+ *   critic2.gw / gb (nothing else reaches them).
+ * Actor pass (wdb_td3_actor_update): the gradient of -mean Q1(obs, actor(obs)) into
+ *   actor.gw / gb (the critic's weights carry it to the action inputs; no critic gradient).
+ * The critic pass reads critic, critic2, both target critics and target_actor; the actor pass
+ * reads actor and critic. */
+typedef struct wdb_td3_update_args {
+  int n_envs, n_agents, obs_dim, action_dim;   /* E, Np, F, A */
+  int capacity, cursor, n_step;      /* as wdb_ddpg_update_args */
+  float gamma, action_scale, action_bias;
+  float target_noise, target_noise_clip;       /* sigma, clip >= 0: units of action_scale */
+  const float *obs;                  /* [C, E, Np, F] */
+  const float *actions;              /* [C, E, Np, A] */
+  const float *rewards;              /* [C, E, Np] */
+  const int *done;                   /* [C, E] */
+  const float *noise;                /* [valid, E * Np, A] standard normal, logical window order */
+  wdb_ddpg_net actor, critic, critic2;          /* gradients: actor (actor pass), critics */
+  wdb_ddpg_net target_actor, target_critic, target_critic2;   /* the online shapes */
+  float *q1_values, *q2_values, *returns;       /* critic pass out [valid, E * Np], or NULL */
+  float *j_values;                   /* actor pass out [valid, E * Np], or NULL */
+  double *sums;                      /* out [4]: sum (Q1 - R)^2, sum (Q2 - R)^2 (critic pass),
+                                        sum J, 0 (actor pass) */
+  void *workspace;                   /* the pass's _workspace_bytes() bytes */
+} wdb_td3_update_args;
+/* 1 if a pass takes the shapes: those of wdb_ddpg_update_supported, both critics (and all
+ * three targets) shaped alike, sigma, clip >= 0, and the pass's networks, gradient
+ * accumulators and row tiles in one CTA's shared memory -- the critic pass holds five
+ * networks and two critic gradient blocks.  No CUDA call. */
+int wdb_td3_critic_update_supported(const wdb_td3_update_args *update);
+long long wdb_td3_critic_update_workspace_bytes(const wdb_td3_update_args *update);  /* -1: unsupported */
+int wdb_td3_actor_update_supported(const wdb_td3_update_args *update);
+long long wdb_td3_actor_update_workspace_bytes(const wdb_td3_update_args *update);   /* -1: unsupported */
+/* cudaErrorInvalidValue without launching if unsupported or a required pointer is NULL. */
+int wdb_td3_critic_update(void *stream, const wdb_td3_update_args *update);
+int wdb_td3_actor_update(void *stream, const wdb_td3_update_args *update);
+
 #ifdef __cplusplus
 }
 #endif

@@ -23,6 +23,16 @@
 // Thread layout (256 threads, 16-row tiles): forward and input-gradient steps give each
 // thread one output column and four rows (one float4 weight load feeds sixteen FMAs);
 // weight-gradient steps give each thread one input column and sixteen output rows.
+//
+// TD3 (wdb_td3_critic_update / wdb_td3_actor_update) runs on the same tile primitives, Plan
+// layout and reduction, as two passes of two launches each:
+//   critic pass, per tile: target actor on obs' -> a' = clamp(pi' + clamp(sigma scale eps,
+//     -c scale, c scale), bias - scale, bias + scale); both target critics on (obs', a') ->
+//     min -> the n-step return R; Q1 and Q2 on (obs, actions); dL/dQk = 2 (Qk - R) / M; back
+//     through each critic into its own gradient block (no actor-loss term).
+//   actor pass, per tile: actor on obs -> pi; Q1 on (obs, pi) -> J; dL/dJ = -1 / M back
+//     through Q1 to its action inputs only (no critic weight gradient), the tanh head and the
+//     actor.
 #include "wdb_common.cuh"
 
 using namespace wdb;
@@ -50,22 +60,27 @@ struct Plan {
   long long smem_floats;
 };
 
-bool make_plan(const wdb_ddpg_update_args *u, Plan *p) {
-  if (!u) return false;
-  const int F = u->obs_dim, A = u->action_dim;
-  if (u->n_envs < 1 || u->n_agents < 1 || F < 1 || A < 1 || F + A > kMaxWidth) return false;
-  if (u->n_step < 1 || u->capacity < 2 || u->capacity < u->n_step || u->cursor < 0 || u->cursor >= u->capacity)
-    return false;
-  const wdb_ddpg_net *nets[2] = {&u->actor, &u->critic};
-  const wdb_ddpg_net *targets[2] = {&u->target_actor, &u->target_critic};
+// Shape checks and the shared-memory layout of the actor shape (k = 0: F -> A) and the critic
+// shape (k = 1: F + A -> 1).  nets[k][0] sets the shape; nets[k][1 .. count[k] - 1] (targets,
+// the second critic) must have the same.
+bool plan_layout(int E, int Np, int F, int A, int C, int cursor, int ns,
+                 const wdb_ddpg_net *const *const nets[2], const int count[2], Plan *p) {
+  if (E < 1 || Np < 1 || F < 1 || A < 1 || F + A > kMaxWidth) return false;
+  if (ns < 1 || C < 2 || C < ns || cursor < 0 || cursor >= C) return false;
   for (int k = 0; k < 2; k++) {
-    const wdb_ddpg_net &n = *nets[k], &t = *targets[k];
-    if (n.n_hidden < 0 || n.n_hidden > 3 || t.n_hidden != n.n_hidden) return false;
+    const wdb_ddpg_net &n = *nets[k][0];
+    if (n.n_hidden < 0 || n.n_hidden > 3) return false;
+    for (int t = 1; t < count[k]; t++)
+      if (nets[k][t]->n_hidden != n.n_hidden) return false;
     int prev = k == 0 ? F : F + A, woff = 0, goff = 0;
     p->L[k] = n.n_hidden + 1;
     for (int l = 0; l <= n.n_hidden; l++) {
       const int out = l < n.n_hidden ? n.widths[l] : (k == 0 ? A : 1);
-      if (l < n.n_hidden && (out < 1 || out > kMaxWidth || t.widths[l] != out)) return false;
+      if (l < n.n_hidden) {
+        if (out < 1 || out > kMaxWidth) return false;
+        for (int t = 1; t < count[k]; t++)
+          if (nets[k][t]->widths[l] != out) return false;
+      }
       int pw = round_up(prev, 4);
       if (pw % 8 == 0) pw += 4;               // float4 rows of 8 lanes hit distinct banks
       p->in[k][l] = prev;
@@ -80,17 +95,34 @@ bool make_plan(const wdb_ddpg_update_args *u, Plan *p) {
     p->wfloats[k] = woff;
     p->gfloats[k] = goff;
   }
-  p->valid = u->capacity - u->n_step + 1;
-  p->EN = (long long)u->n_envs * u->n_agents;
+  p->valid = C - ns + 1;
+  p->EN = (long long)E * Np;
   p->M = p->valid * p->EN;
-  if (p->M > (1ll << 31)) return false;
-  p->n_buf = 6 + 2 * (p->L[1] - 1) + (p->L[0] - 1);
-  p->smem_floats = 2ll * (p->wfloats[0] + p->wfloats[1]) +
-                   round_up(p->gfloats[0] + p->gfloats[1], 4) + (long long)p->n_buf * kTile;
+  return p->M <= (1ll << 31);
+}
+
+// A kernel's activation buffers, shared-memory floats (weights, gradient accumulators, row
+// tiles) and grid; false if they do not fit one CTA.
+bool plan_smem(Plan *p, int n_buf, long long weight_floats, int grad_floats) {
+  p->n_buf = n_buf;
+  p->smem_floats = weight_floats + round_up(grad_floats, 4) + (long long)n_buf * kTile;
   if (p->smem_floats * 4 > kMaxDynSmem) return false;
   const long long tiles = (p->M + kRows - 1) / kRows;
   p->grid = (int)(tiles < kNumSMs ? tiles : kNumSMs);
   return true;
+}
+
+bool make_plan(const wdb_ddpg_update_args *u, Plan *p) {
+  if (!u) return false;
+  const wdb_ddpg_net *actors[2] = {&u->actor, &u->target_actor};
+  const wdb_ddpg_net *critics[2] = {&u->critic, &u->target_critic};
+  const wdb_ddpg_net *const *nets[2] = {actors, critics};
+  const int count[2] = {2, 2};
+  if (!plan_layout(u->n_envs, u->n_agents, u->obs_dim, u->action_dim, u->capacity, u->cursor,
+                   u->n_step, nets, count, p))
+    return false;
+  return plan_smem(p, 6 + 2 * (p->L[1] - 1) + (p->L[0] - 1),
+                   2ll * (p->wfloats[0] + p->wfloats[1]), p->gfloats[0] + p->gfloats[1]);
 }
 
 __device__ __forceinline__ float4 ld4(const float *p) {
@@ -209,10 +241,11 @@ __device__ __forceinline__ void net_forward(const float *W, const Plan &P, int k
   }
 }
 
-// Back-propagates the head delta Dh through net k, adding every weight gradient to G;
-// inbuf(l) is layer l's input.  i_lo >= 0 also forms the input gradient of columns
-// [i_lo, in) of layer 0; the buffer that holds it (D0 or D1) is returned.
-template <class InBuf>
+// Back-propagates the head delta Dh through net k, adding every weight gradient to G (unless
+// kWeightGrads is false: G is not touched); inbuf(l) is layer l's input.  i_lo >= 0 also
+// forms the input gradient of columns [i_lo, in) of layer 0; the buffer that holds it (D0 or
+// D1) is returned.
+template <bool kWeightGrads = true, class InBuf>
 __device__ __forceinline__ const float *net_backward(const float *W, const Plan &P, int k,
                                                      float *G, const float *Dh, InBuf inbuf,
                                                      float *D0, float *D1, int i_lo) {
@@ -220,7 +253,7 @@ __device__ __forceinline__ const float *net_backward(const float *W, const Plan 
   float *nxt = Dh == D0 ? D1 : D0;
   for (int l = P.L[k] - 1; l >= 0; l--) {
     const float *x = inbuf(l);
-    layer_grad(G + P.goff[k][l], P.in[k][l], P.out[k][l], d, x);
+    if (kWeightGrads) layer_grad(G + P.goff[k][l], P.in[k][l], P.out[k][l], d, x);
     const float *Wl = W + P.woff[k][l];
     if (l > 0)
       layer_backward(Wl, P.pw[k][l], P.in[k][l], P.out[k][l], d, nxt, x, 0);
@@ -429,8 +462,328 @@ __global__ void ddpg_reduce_kernel(const __grid_constant__ Reduce R, const float
   }
 }
 
+// ---------------------------------------------------------------------------- TD3
+// The n-step return of loss row g (logical window i, agent row n) from the bootstrap value qt:
+// ddpg.py:62-79's recursion in the same float32 operations as ddpg_update_kernel.
+__device__ __forceinline__ float td3_return(const wdb_td3_update_args &U, const Plan &P, int i,
+                                            long long n, float qt) {
+  const int C = U.capacity, ns = U.n_step;
+  auto phys = [&](int k) { const int s = U.cursor + k; return s >= C ? s - C : s; };
+  const long long EN = P.EN, E = U.n_envs, env = n / U.n_agents;
+  const int pl = phys(i + ns - 1);
+  const float rl = U.rewards[(long long)pl * EN + n];
+  const float dl = (float)U.done[(long long)pl * E + env];
+  const float om = __fsub_rn(1.0f, dl);
+  float ret = i < P.valid - 1 ? __fadd_rn(rl, __fmul_rn(__fmul_rn(om, U.gamma), qt))
+                              : __fadd_rn(__fmul_rn(dl, rl), __fmul_rn(om, qt));
+  for (int j = 1; j < ns; j++) {
+    const int pk = phys(ns - 1 - j + i);
+    const float dk = (float)U.done[(long long)pk * E + env];
+    ret = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(1.0f, dk), U.gamma), ret),
+                    U.rewards[(long long)pk * EN + n]);
+  }
+  return ret;
+}
+
+// Critic pass: the gradients of mse(Q1, R) + mse(Q2, R) into per-CTA partials [G1 | G2].
+__global__ void __launch_bounds__(kThreads, 1)
+td3_critic_kernel(const __grid_constant__ wdb_td3_update_args U, const __grid_constant__ Plan Pg,
+                  float *partials, double *psums) {
+  extern __shared__ __align__(16) float smem[];
+  __shared__ Plan P;
+  __shared__ double s_e1[kRows], s_e2[kRows];
+  if (threadIdx.x == 0) P = Pg;
+  __syncthreads();
+  const int tid = threadIdx.x;
+  float *Wta = smem, *Wc1 = Wta + P.wfloats[0], *Wc2 = Wc1 + P.wfloats[1];
+  float *Wt1 = Wc2 + P.wfloats[1], *Wt2 = Wt1 + P.wfloats[1];
+  float *G1 = Wt2 + P.wfloats[1], *G2 = G1 + P.gfloats[1];
+  const int g_total = 2 * P.gfloats[1];
+  float *XQ = G1 + ((g_total + 3) / 4) * 4;      // obs ++ actions
+  float *XS = XQ + kTile;                      // scratch of the target forwards
+  float *V = XS + kTile;                       // columns: 0 Q1', 1 Q2', 2 Q1, 3 Q2, 4 dQ1, 8 dQ2
+  float *Z = V + kTile;                        // target actor head pre-activation
+  float *D0 = Z + kTile, *D1 = D0 + kTile;     // deltas (target path: obs' ++ a' and scratch)
+  float *H1 = D1 + kTile;                      // Q1 hidden outputs
+  float *H2 = H1 + (P.L[1] - 1) * kTile;       // Q2 hidden outputs
+
+  load_net(Wta, U.target_actor, P, 0);
+  load_net(Wc1, U.critic, P, 1);
+  load_net(Wc2, U.critic2, P, 1);
+  load_net(Wt1, U.target_critic, P, 1);
+  load_net(Wt2, U.target_critic2, P, 1);
+  for (int e = tid; e < g_total; e += kThreads) G1[e] = 0.0f;
+  for (int e = tid; e < P.n_buf * kTile; e += kThreads) XQ[e] = 0.0f;
+  __syncthreads();
+
+  const int F = U.obs_dim, A = U.action_dim, FA = F + A;
+  const int C = U.capacity, cursor = U.cursor, ns = U.n_step, valid = P.valid;
+  const long long EN = P.EN, M = P.M;
+  const float scale = U.action_scale, bias = U.action_bias;
+  const float sd = __fmul_rn(U.target_noise, scale), clip = __fmul_rn(U.target_noise_clip, scale);
+  const float lo = __fsub_rn(bias, scale), hi = __fadd_rn(bias, scale);
+  const float norm_q = (float)(2.0 / (double)M);
+  auto phys = [&](int k) { const int s = cursor + k; return s >= C ? s - C : s; };
+  auto target_slot = [&](int i) { return i < valid - 1 ? i + ns : C - 1; };
+  double e1_acc = 0.0, e2_acc = 0.0;
+
+  for (long long g0 = (long long)blockIdx.x * kRows; g0 < M; g0 += (long long)gridDim.x * kRows) {
+    // ---- inputs: XQ = obs ++ actions at slot i, D0 = obs at the bootstrap slot
+    for (int e = tid; e < kRows * FA; e += kThreads) {
+      const int r = e / FA, c = e - r * FA;
+      const long long g = g0 + r;
+      float xq = 0.0f, xt = 0.0f;
+      if (g < M) {
+        const int i = (int)(g / EN);
+        const long long n = g - (long long)i * EN;
+        const long long row = (long long)phys(i) * EN + n;
+        if (c < F) {
+          xq = U.obs[row * F + c];
+          xt = U.obs[((long long)phys(target_slot(i)) * EN + n) * F + c];
+        } else {
+          xq = U.actions[row * A + (c - F)];
+        }
+      }
+      XQ[r * kPitch + c] = xq;
+      if (c < F) D0[r * kPitch + c] = xt;
+    }
+    __syncthreads();
+    // ---- target actor + clipped noise -> a' into D0's action columns
+    net_forward(Wta, P, 0, D0,
+                [&](int l) { return l == P.L[0] - 1 ? Z : (l % 2 == 0 ? D1 : XS); });
+    for (int e = tid; e < kRows * A; e += kThreads) {
+      const int r = e / A, c = e - r * A;
+      const long long g = g0 + r;
+      const float pi = __fadd_rn(__fmul_rn(scale, tanhf(Z[r * kPitch + c])), bias);
+      const float eps = g < M ? U.noise[g * A + c] : 0.0f;
+      const float nz = fminf(fmaxf(__fmul_rn(eps, sd), -clip), clip);
+      D0[r * kPitch + F + c] = fminf(fmaxf(__fadd_rn(pi, nz), lo), hi);
+    }
+    __syncthreads();
+    // ---- target critics -> V[., 0], V[., 1]; critics on (obs, actions) -> V[., 2], V[., 3]
+    net_forward(Wt1, P, 1, D0,
+                [&](int l) { return l == P.L[1] - 1 ? V : (l % 2 == 0 ? D1 : XS); });
+    net_forward(Wt2, P, 1, D0,
+                [&](int l) { return l == P.L[1] - 1 ? V + 1 : (l % 2 == 0 ? D1 : XS); });
+    net_forward(Wc1, P, 1, XQ,
+                [&](int l) { return l == P.L[1] - 1 ? V + 2 : H1 + l * kTile; });
+    net_forward(Wc2, P, 1, XQ,
+                [&](int l) { return l == P.L[1] - 1 ? V + 3 : H2 + l * kTile; });
+    // ---- the n-step return from min(Q1', Q2') and the loss gradients
+    if (tid < kRows) {
+      const int r = tid;
+      const long long g = g0 + r;
+      float d1 = 0.0f, d2 = 0.0f;
+      if (g < M) {
+        const int i = (int)(g / EN);
+        const long long n = g - (long long)i * EN;
+        const float qt = fminf(V[r * kPitch], V[r * kPitch + 1]);
+        const float q1 = V[r * kPitch + 2], q2 = V[r * kPitch + 3];
+        const float ret = td3_return(U, P, i, n, qt);
+        const float e1 = __fsub_rn(q1, ret), e2 = __fsub_rn(q2, ret);
+        d1 = __fmul_rn(e1, norm_q);
+        d2 = __fmul_rn(e2, norm_q);
+        e1_acc += (double)e1 * (double)e1;
+        e2_acc += (double)e2 * (double)e2;
+        if (U.q1_values) U.q1_values[g] = q1;
+        if (U.q2_values) U.q2_values[g] = q2;
+        if (U.returns) U.returns[g] = ret;
+      }
+      V[r * kPitch + 4] = d1;
+      V[r * kPitch + 8] = d2;
+    }
+    __syncthreads();
+    // ---- backward: each critic on (obs, actions) into its own gradient block
+    net_backward(Wc1, P, 1, G1, V + 4,
+                 [&](int l) { return l == 0 ? XQ : H1 + (l - 1) * kTile; }, D0, D1, -1);
+    net_backward(Wc2, P, 1, G2, V + 8,
+                 [&](int l) { return l == 0 ? XQ : H2 + (l - 1) * kTile; }, D0, D1, -1);
+  }
+
+  float *part = partials + (long long)blockIdx.x * g_total;
+  for (int e = tid; e < g_total; e += kThreads) part[e] = G1[e];
+  if (tid < kRows) {
+    s_e1[tid] = e1_acc;
+    s_e2[tid] = e2_acc;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    double a = 0.0, b = 0.0;
+    for (int r = 0; r < kRows; r++) {
+      a += s_e1[r];
+      b += s_e2[r];
+    }
+    psums[2 * blockIdx.x] = a;
+    psums[2 * blockIdx.x + 1] = b;
+  }
+}
+
+// Actor pass: the gradient of -mean Q1(obs, actor(obs)) into per-CTA actor partials; the
+// critic's weights only carry the gradient to its action inputs.
+__global__ void __launch_bounds__(kThreads, 1)
+td3_actor_kernel(const __grid_constant__ wdb_td3_update_args U, const __grid_constant__ Plan Pg,
+                 float *partials, double *psums) {
+  extern __shared__ __align__(16) float smem[];
+  __shared__ Plan P;
+  __shared__ double s_j[kRows];
+  if (threadIdx.x == 0) P = Pg;
+  __syncthreads();
+  const int tid = threadIdx.x;
+  float *Wa = smem, *Wc = Wa + P.wfloats[0];
+  float *Ga = Wc + P.wfloats[1];
+  const int g_total = P.gfloats[0];
+  float *XJ = Ga + ((g_total + 3) / 4) * 4;      // obs ++ pi
+  float *V = XJ + kTile;                       // columns: 0 J, 8 dJ
+  float *Z = V + kTile;                        // actor head pre-activation
+  float *D0 = Z + kTile, *D1 = D0 + kTile;     // deltas
+  float *HJ = D1 + kTile;                      // Q1 hidden outputs on (obs, pi)
+  float *HA = HJ + (P.L[1] - 1) * kTile;       // actor hidden outputs
+
+  load_net(Wa, U.actor, P, 0);
+  load_net(Wc, U.critic, P, 1);
+  for (int e = tid; e < g_total; e += kThreads) Ga[e] = 0.0f;
+  for (int e = tid; e < P.n_buf * kTile; e += kThreads) XJ[e] = 0.0f;
+  __syncthreads();
+
+  const int F = U.obs_dim, A = U.action_dim;
+  const int C = U.capacity, cursor = U.cursor;
+  const long long EN = P.EN, M = P.M;
+  const float scale = U.action_scale, bias = U.action_bias;
+  const float d_j = -1.0f / (float)M;
+  auto phys = [&](int k) { const int s = cursor + k; return s >= C ? s - C : s; };
+  double j_acc = 0.0;
+
+  for (long long g0 = (long long)blockIdx.x * kRows; g0 < M; g0 += (long long)gridDim.x * kRows) {
+    for (int e = tid; e < kRows * F; e += kThreads) {
+      const int r = e / F, c = e - r * F;
+      const long long g = g0 + r;
+      float x = 0.0f;
+      if (g < M) {
+        const int i = (int)(g / EN);
+        const long long n = g - (long long)i * EN;
+        x = U.obs[((long long)phys(i) * EN + n) * F + c];
+      }
+      XJ[r * kPitch + c] = x;
+    }
+    __syncthreads();
+    // ---- actor -> pi into XJ's action columns; Q1 on (obs, pi) -> V[., 0]
+    net_forward(Wa, P, 0, XJ, [&](int l) { return l == P.L[0] - 1 ? Z : HA + l * kTile; });
+    for (int e = tid; e < kRows * A; e += kThreads) {
+      const int r = e / A, c = e - r * A;
+      XJ[r * kPitch + F + c] = __fadd_rn(__fmul_rn(scale, tanhf(Z[r * kPitch + c])), bias);
+    }
+    __syncthreads();
+    net_forward(Wc, P, 1, XJ, [&](int l) { return l == P.L[1] - 1 ? V : HJ + l * kTile; });
+    if (tid < kRows) {
+      const int r = tid;
+      const long long g = g0 + r;
+      float dj = 0.0f;
+      if (g < M) {
+        const float jv = V[r * kPitch];
+        dj = d_j;
+        j_acc += (double)jv;
+        if (U.j_values) U.j_values[g] = jv;
+      }
+      V[r * kPitch + 8] = dj;
+    }
+    __syncthreads();
+    // ---- backward: Q1 to its action inputs, the tanh head, the actor
+    const float *dpi = net_backward<false>(
+        Wc, P, 1, nullptr, V + 8, [&](int l) { return l == 0 ? XJ : HJ + (l - 1) * kTile; },
+        D0, D1, F);
+    float *dz = dpi == D0 ? D1 : D0;
+    for (int e = tid; e < kRows * A; e += kThreads) {
+      const int r = e / A, c = e - r * A;
+      const float y = tanhf(Z[r * kPitch + c]);
+      dz[r * kPitch + c] = __fmul_rn(__fmul_rn(dpi[r * kPitch + F + c], scale),
+                                     __fsub_rn(1.0f, __fmul_rn(y, y)));
+    }
+    __syncthreads();
+    net_backward(Wa, P, 0, Ga, dz, [&](int l) { return l == 0 ? XJ : HA + (l - 1) * kTile; },
+                 D0, D1, -1);
+  }
+
+  float *part = partials + (long long)blockIdx.x * g_total;
+  for (int e = tid; e < g_total; e += kThreads) part[e] = Ga[e];
+  if (tid < kRows) s_j[tid] = j_acc;
+  __syncthreads();
+  if (tid == 0) {
+    double a = 0.0;
+    for (int r = 0; r < kRows; r++) a += s_j[r];
+    psums[2 * blockIdx.x] = a;
+    psums[2 * blockIdx.x + 1] = 0.0;
+  }
+}
+
+// ---------------------------------------------------------------------------- host side
 long long workspace_bytes(const Plan &P) {
   return 16ll * P.grid + 4ll * P.grid * (P.gfloats[0] + P.gfloats[1]);
+}
+
+// Opts `kernel` into `smem` bytes of dynamic shared memory (once per size it grows to).
+int allow_smem(const void *kernel, size_t smem, size_t *configured) {
+  if (smem > 48 * 1024 && smem > *configured) {
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem);
+    if (e != cudaSuccess) return (int)e;
+    *configured = smem;
+  }
+  return cudaSuccess;
+}
+
+// Adds the weight and bias segments of net k, packed from `base` in a CTA partial, to R.
+void add_segments(Reduce *R, const Plan &P, int k, int base, const wdb_ddpg_net &net,
+                  int *widest) {
+  for (int l = 0; l < P.L[k]; l++) {
+    const int nw = P.in[k][l] * P.out[k][l];
+    R->off[R->nseg] = base + P.goff[k][l];
+    R->n[R->nseg] = nw;
+    R->dst[R->nseg++] = net.gw[l];
+    R->off[R->nseg] = base + P.goff[k][l] + nw;
+    R->n[R->nseg] = P.out[k][l];
+    R->dst[R->nseg++] = net.gb[l];
+    *widest = nw > *widest ? nw : *widest;
+  }
+}
+
+int launch_reduce(void *stream, const Reduce &R, int widest, const float *partials,
+                  const double *psums, double *sums) {
+  const dim3 grid((widest + 255) / 256, R.nseg);
+  ddpg_reduce_kernel<<<grid, 256, 0, as_stream(stream)>>>(R, partials, psums, sums);
+  return finish_launch();
+}
+
+// TD3's plan of one pass: the actor shape (actor, target actor) and the critic shape (both
+// critics and their targets) as in DDPG; the critic pass holds the target actor, four critics
+// and both critic gradient blocks, the actor pass the actor, Q1 and the actor gradients.
+bool td3_plan(const wdb_td3_update_args *u, bool actor_pass, Plan *p) {
+  if (!u) return false;
+  if (!(u->target_noise >= 0.0f) || !(u->target_noise_clip >= 0.0f)) return false;
+  const wdb_ddpg_net *actors[2] = {&u->actor, &u->target_actor};
+  const wdb_ddpg_net *critics[4] = {&u->critic, &u->critic2, &u->target_critic,
+                                    &u->target_critic2};
+  const wdb_ddpg_net *const *nets[2] = {actors, critics};
+  const int count[2] = {2, 4};
+  if (!plan_layout(u->n_envs, u->n_agents, u->obs_dim, u->action_dim, u->capacity, u->cursor,
+                   u->n_step, nets, count, p))
+    return false;
+  if (actor_pass)
+    return plan_smem(p, 5 + (p->L[1] - 1) + (p->L[0] - 1), p->wfloats[0] + p->wfloats[1],
+                     p->gfloats[0]);
+  return plan_smem(p, 6 + 2 * (p->L[1] - 1), p->wfloats[0] + 4ll * p->wfloats[1],
+                   2 * p->gfloats[1]);
+}
+
+long long td3_workspace_bytes(const Plan &P, bool actor_pass) {
+  return 16ll * P.grid + 4ll * P.grid * (actor_pass ? P.gfloats[0] : 2 * P.gfloats[1]);
+}
+
+bool net_ok(const wdb_ddpg_net &net, int layers, bool grads) {
+  for (int l = 0; l < layers; l++) {
+    if (!net.w[l] || !net.b[l]) return false;
+    if (grads && (!net.gw[l] || !net.gb[l])) return false;
+  }
+  return true;
 }
 
 bool nets_ok(const wdb_ddpg_update_args *u, const Plan &P) {
@@ -462,37 +815,91 @@ WDB_API int wdb_ddpg_update(void *stream, const wdb_ddpg_update_args *u) {
     return (int)cudaErrorInvalidValue;
   const size_t smem = (size_t)P.smem_floats * sizeof(float);
   static size_t configured = 0;
-  if (smem > 48 * 1024 && smem > configured) {
-    cudaError_t e = cudaFuncSetAttribute(ddpg_update_kernel,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return (int)e;
-    configured = smem;
-  }
+  int rc = allow_smem((const void *)ddpg_update_kernel, smem, &configured);
+  if (rc != cudaSuccess) return rc;
   double *psums = static_cast<double *>(u->workspace);
   float *partials = reinterpret_cast<float *>(psums + 2 * P.grid);
   ddpg_update_kernel<<<P.grid, kThreads, smem, as_stream(stream)>>>(*u, P, partials, psums);
-  int rc = finish_launch();
+  rc = finish_launch();
   if (rc != cudaSuccess) return rc;
 
   Reduce R = {};
   R.grid = P.grid;
   R.g_total = P.gfloats[0] + P.gfloats[1];
   int widest = 1;
-  for (int k = 0; k < 2; k++) {
-    const wdb_ddpg_net &net = k == 0 ? u->actor : u->critic;
-    const int base = k == 0 ? 0 : P.gfloats[0];
-    for (int l = 0; l < P.L[k]; l++) {
-      const int nw = P.in[k][l] * P.out[k][l];
-      R.off[R.nseg] = base + P.goff[k][l];
-      R.n[R.nseg] = nw;
-      R.dst[R.nseg++] = net.gw[l];
-      R.off[R.nseg] = base + P.goff[k][l] + nw;
-      R.n[R.nseg] = P.out[k][l];
-      R.dst[R.nseg++] = net.gb[l];
-      widest = nw > widest ? nw : widest;
-    }
-  }
-  const dim3 grid((widest + 255) / 256, R.nseg);
-  ddpg_reduce_kernel<<<grid, 256, 0, as_stream(stream)>>>(R, partials, psums, u->sums);
-  return finish_launch();
+  add_segments(&R, P, 0, 0, u->actor, &widest);
+  add_segments(&R, P, 1, P.gfloats[0], u->critic, &widest);
+  return launch_reduce(stream, R, widest, partials, psums, u->sums);
+}
+
+WDB_API int wdb_td3_critic_update_supported(const wdb_td3_update_args *update) {
+  Plan P;
+  return td3_plan(update, false, &P) ? 1 : 0;
+}
+
+WDB_API long long wdb_td3_critic_update_workspace_bytes(const wdb_td3_update_args *update) {
+  Plan P;
+  return td3_plan(update, false, &P) ? td3_workspace_bytes(P, false) : -1;
+}
+
+WDB_API int wdb_td3_critic_update(void *stream, const wdb_td3_update_args *u) {
+  Plan P;
+  if (!td3_plan(u, false, &P)) return (int)cudaErrorInvalidValue;
+  if (!net_ok(u->target_actor, P.L[0], false) || !net_ok(u->critic, P.L[1], true) ||
+      !net_ok(u->critic2, P.L[1], true) || !net_ok(u->target_critic, P.L[1], false) ||
+      !net_ok(u->target_critic2, P.L[1], false))
+    return (int)cudaErrorInvalidValue;
+  if (!u->obs || !u->actions || !u->rewards || !u->done || !u->noise || !u->workspace)
+    return (int)cudaErrorInvalidValue;
+  const size_t smem = (size_t)P.smem_floats * sizeof(float);
+  static size_t configured = 0;
+  int rc = allow_smem((const void *)td3_critic_kernel, smem, &configured);
+  if (rc != cudaSuccess) return rc;
+  double *psums = static_cast<double *>(u->workspace);
+  float *partials = reinterpret_cast<float *>(psums + 2 * P.grid);
+  td3_critic_kernel<<<P.grid, kThreads, smem, as_stream(stream)>>>(*u, P, partials, psums);
+  rc = finish_launch();
+  if (rc != cudaSuccess) return rc;
+
+  Reduce R = {};
+  R.grid = P.grid;
+  R.g_total = 2 * P.gfloats[1];
+  int widest = 1;
+  add_segments(&R, P, 1, 0, u->critic, &widest);
+  add_segments(&R, P, 1, P.gfloats[1], u->critic2, &widest);
+  return launch_reduce(stream, R, widest, partials, psums, u->sums);
+}
+
+WDB_API int wdb_td3_actor_update_supported(const wdb_td3_update_args *update) {
+  Plan P;
+  return td3_plan(update, true, &P) ? 1 : 0;
+}
+
+WDB_API long long wdb_td3_actor_update_workspace_bytes(const wdb_td3_update_args *update) {
+  Plan P;
+  return td3_plan(update, true, &P) ? td3_workspace_bytes(P, true) : -1;
+}
+
+WDB_API int wdb_td3_actor_update(void *stream, const wdb_td3_update_args *u) {
+  Plan P;
+  if (!td3_plan(u, true, &P)) return (int)cudaErrorInvalidValue;
+  if (!net_ok(u->actor, P.L[0], true) || !net_ok(u->critic, P.L[1], false))
+    return (int)cudaErrorInvalidValue;
+  if (!u->obs || !u->workspace) return (int)cudaErrorInvalidValue;
+  const size_t smem = (size_t)P.smem_floats * sizeof(float);
+  static size_t configured = 0;
+  int rc = allow_smem((const void *)td3_actor_kernel, smem, &configured);
+  if (rc != cudaSuccess) return rc;
+  double *psums = static_cast<double *>(u->workspace);
+  float *partials = reinterpret_cast<float *>(psums + 2 * P.grid);
+  td3_actor_kernel<<<P.grid, kThreads, smem, as_stream(stream)>>>(*u, P, partials, psums);
+  rc = finish_launch();
+  if (rc != cudaSuccess) return rc;
+
+  Reduce R = {};
+  R.grid = P.grid;
+  R.g_total = P.gfloats[0];
+  int widest = 1;
+  add_segments(&R, P, 0, 0, u->actor, &widest);
+  return launch_reduce(stream, R, widest, partials, psums, u->sums ? u->sums + 2 : nullptr);
 }

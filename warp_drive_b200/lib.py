@@ -247,6 +247,22 @@ class DdpgUpdate(ctypes.Structure):
     ]
 
 
+class Td3Update(ctypes.Structure):
+    """struct wdb_td3_update_args (include/wdb200.h)."""
+
+    _fields_ = [
+        ("n_envs", _i), ("n_agents", _i), ("obs_dim", _i), ("action_dim", _i),
+        ("capacity", _i), ("cursor", _i), ("n_step", _i),
+        ("gamma", _f), ("action_scale", _f), ("action_bias", _f),
+        ("target_noise", _f), ("target_noise_clip", _f),
+        ("obs", _fp), ("actions", _fp), ("rewards", _fp), ("done", _fp), ("noise", _fp),
+        ("actor", DdpgNet), ("critic", DdpgNet), ("critic2", DdpgNet),
+        ("target_actor", DdpgNet), ("target_critic", DdpgNet), ("target_critic2", DdpgNet),
+        ("q1_values", _fp), ("q2_values", _fp), ("returns", _fp), ("j_values", _fp),
+        ("sums", _fp), ("workspace", _fp),
+    ]
+
+
 _SIGNATURES = {
     "wdb_abi_version": (_i, []),
     "wdb_error_string": (ctypes.c_char_p, [_i]),
@@ -313,6 +329,12 @@ _SIGNATURES = {
     "wdb_ddpg_update_supported": (_i, [ctypes.POINTER(DdpgUpdate)]),
     "wdb_ddpg_update_workspace_bytes": (_ll, [ctypes.POINTER(DdpgUpdate)]),
     "wdb_ddpg_update": (_i, [_vp, ctypes.POINTER(DdpgUpdate)]),
+    "wdb_td3_critic_update_supported": (_i, [ctypes.POINTER(Td3Update)]),
+    "wdb_td3_critic_update_workspace_bytes": (_ll, [ctypes.POINTER(Td3Update)]),
+    "wdb_td3_critic_update": (_i, [_vp, ctypes.POINTER(Td3Update)]),
+    "wdb_td3_actor_update_supported": (_i, [ctypes.POINTER(Td3Update)]),
+    "wdb_td3_actor_update_workspace_bytes": (_ll, [ctypes.POINTER(Td3Update)]),
+    "wdb_td3_actor_update": (_i, [_vp, ctypes.POINTER(Td3Update)]),
     "wdb_single_agent_rollout_supported": (_i, [_i, ctypes.POINTER(_i)]),
     "wdb_single_agent_rollout": (_i, [_vp, ctypes.POINTER(SaRollout)]),
     "wdb_mountain_car_step": (

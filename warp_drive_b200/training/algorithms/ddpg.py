@@ -34,6 +34,13 @@ class DDPG:
     def n_step_returns(self, rewards, done_flags, next_values):
         """rewards [T, E, Np], done_flags [T, E] (0/1), next_values [T-1, E, Np] (detached)
         -> returns [T - n_step + 1, E, Np]  (ddpg.py:62-79)."""
+        return self.window_returns(rewards, done_flags, next_values[self.n_step - 1:],
+                                   next_values[-1])
+
+    def window_returns(self, rewards, done_flags, boot, boot_last):
+        """The n-step returns [T - n_step + 1, E, Np] from each window's bootstrap value:
+        `boot` [T - n_step, E, Np] for the windows whose last step has a successor inside the
+        batch, `boot_last` [E, Np] for the last window (ddpg.py:62-79)."""
         T, n, gamma = rewards.shape[0], self.n_step, self.discount_factor_gamma
         valid = T - n + 1
         assert valid >= 1, "the batch is shorter than n_step"
@@ -42,8 +49,8 @@ class DDPG:
         last_r, last_d = rewards[n - 1:], done[n - 1:]
         r = torch.empty_like(last_r)
         if valid > 1:       # windows whose last step has a successor inside the batch
-            r[:-1] = last_r[:-1] + (1 - last_d[:-1]) * gamma * next_values[n - 1:]
-        r[-1] = last_d[-1] * last_r[-1] + (1 - last_d[-1]) * next_values[-1]
+            r[:-1] = last_r[:-1] + (1 - last_d[:-1]) * gamma * boot
+        r[-1] = last_d[-1] * last_r[-1] + (1 - last_d[-1]) * boot_last
         for j in range(1, n):
             lo = n - 1 - j
             r = (1 - done[lo:lo + valid]) * gamma * r + rewards[lo:lo + valid]

@@ -49,6 +49,15 @@ def fused_ddpg_supported(algo, actor, critic, n_envs, n_agents, capacity, n_step
     """True if `wdb_ddpg_update` takes this policy: a FullyConnectedActor (tanh head, Box
     observation, no action mask) and a FullyConnectedActionValueCritic of 0..3 hidden layers of
     width <= 64, obs + action width <= 64, and no return normalisation."""
+    if not fused_models_supported(algo, actor, critic):
+        return False
+    u = _shape_struct(actor, critic, n_envs, n_agents, capacity, n_step)
+    return bool(_lib.load().wdb_ddpg_update_supported(ctypes.byref(u)))
+
+
+def fused_models_supported(algo, actor, critic):
+    """The model and algorithm checks of the fused actor-critic updates (DDPG, TD3); the
+    kernels' own support calls check the shapes."""
     from warp_drive_b200.training.models.fully_connected_actor_critic import (
         FullyConnectedActionValueCritic, FullyConnectedActor)
 
@@ -64,10 +73,7 @@ def fused_ddpg_supported(algo, actor, critic, n_envs, n_agents, capacity, n_step
         return False
     if len(actor.fc_dims) > 3 or len(critic.fc_dims) > 3:
         return False
-    if critic.flattened_obs_size != actor.flattened_obs_size:
-        return False
-    u = _shape_struct(actor, critic, n_envs, n_agents, capacity, n_step)
-    return bool(_lib.load().wdb_ddpg_update_supported(ctypes.byref(u)))
+    return critic.flattened_obs_size == actor.flattened_obs_size
 
 
 class FusedDDPGUpdate:

@@ -178,7 +178,11 @@ class TrainerDDPG(Trainer):
         self.actor_optimizers[policy] = self._flat_adam(
             self.actor_models[policy], self.actor_lr_schedules[policy].get_param_value(ts))
         self.critic_optimizers[policy] = self._flat_adam(
-            self.critic_models[policy], self.critic_lr_schedules[policy].get_param_value(ts))
+            self._critic_optimized(policy), self.critic_lr_schedules[policy].get_param_value(ts))
+
+    def _critic_optimized(self, policy):
+        """The module whose parameters the critic's optimizer steps (and clips together)."""
+        return self.critic_models[policy]
 
     def _optimizers_of(self, policy):
         return [(" (Actor)", self.actor_optimizers[policy], self.actor_lr_schedules[policy]),
@@ -228,13 +232,17 @@ class TrainerDDPG(Trainer):
                         self.tau[policy])
             soft_update(self.target_critic_models[policy], self.critic_models[policy],
                         self.tau[policy])
+        self._add_test_metrics(metrics_dict, logging_flag)
+        return metrics_dict
+
+    def _add_test_metrics(self, metrics_dict, logging_flag):
+        """On a logging iteration with the evaluator on: noise-free test episodes' metrics."""
         if logging_flag and self.config["trainer"].get("evaluator"):
             reward_sum, step_sum = self.evaluate_episodes(scale=0)
             for policy in self.policies_to_train:
                 metrics_dict[policy].update({
                     "Mean episodic reward (test)": float(reward_sum[policy].mean()),
                     "Mean episodic steps (test)": float(step_sum[policy].float().mean())})
-        return metrics_dict
 
     def _torch_gradients(self, policy, logging_flag):
         """Actor / critic gradients by torch autograd over the unrolled ring (accumulated into
