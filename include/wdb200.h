@@ -257,6 +257,12 @@ typedef struct wdb_tc_rollout {
                                       * launch is programmatically dependent on it -- the state
                                       * prologue overlaps the forward's tail, the probabilities
                                       * are read after griddepcontrol.wait.  0: plain launch. */
+  int actions_in;                    /* 1: the actions were already sampled (by
+                                      * wdb_mlp_policy_forward_sampled) into every policy's
+                                      * actions_batch, which is then required and only read;
+                                      * probs0 / probs1 and the RNG are not used.  Only the packed
+                                      * kernel of up to 320 threads per CTA takes this mode
+                                      * (wdb_tag_continuous_rollout_supported reads this field). */
 } wdb_tc_rollout;
 
 int wdb_tag_continuous_rollout_step(void *stream, const wdb_tc_env *env,
@@ -495,6 +501,28 @@ int wdb_mlp_policy_forward(void *stream, const void *blob, int F, int H, int A0,
 int wdb_mlp_policy_forward_masked(void *stream, const void *blob, int F, int H, int A0, int A1,
                                   const float *obs, long long rows, const float *mask,
                                   float *probs0, float *probs1, float *values /* may be NULL */);
+/* The same forward, which also samples both heads of every row as the fused TagContinuous
+ * step samples them (wdb_sample_actions): row r = env * Np + slot is agent
+ * gi = env * N + agent_of_slot[slot]; its uniforms are draws x (head 0) and y (head 1) of
+ * Philox stream gi at that stream's offset, which advances by one (or uniforms[2 gi + head]
+ * when `uniforms` is set; the offsets are then left alone).  actions[r] = (head 0, head 1)
+ * is the index the reference's CDF search picks from the stored probabilities.  Only the
+ * config-2 shape samples (F in [65, 80], H = 256, two heads with A0 + A1 + 1 in [33, 48]):
+ * wdb_mlp_forward_samples says whether a shape does.  input_is_tiles: `input` is the bf16
+ * tile copy of wdb_mlp_policy_forward_tiles instead of fp32 obs [rows, F]. */
+typedef struct wdb_mlp_sampling {
+  int *actions;                      /* [rows, 2] (8-byte aligned) */
+  void *rng_state;                   /* wdb_rng_init state of E * N streams; may be NULL with uniforms */
+  const float *uniforms;             /* [E, N, 2] or NULL */
+  const int *agent_of_slot;          /* [Np] */
+  int n_agents;                      /* N */
+  int n_policy_agents;               /* Np; rows must be a multiple of it */
+} wdb_mlp_sampling;
+int wdb_mlp_forward_samples(int F, int H, int A0, int A1);
+int wdb_mlp_policy_forward_sampled(void *stream, const void *blob, int F, int H, int A0, int A1,
+                                   const void *input, int input_is_tiles, long long rows,
+                                   float *probs0, float *probs1, float *values /* may be NULL */,
+                                   const wdb_mlp_sampling *sampling);
 /* Two policies in ONE launch (the rollout of a two-policy env: tag_continuous runners and
  * taggers): CTAs [0, grid - ctas_b) run policy 0, the last ctas_b CTAs policy 1, each
  * persistent over its own 128-row tiles.  ctas_b = 0 picks the split from the row counts.

@@ -107,6 +107,37 @@ __device__ __forceinline__ int search_index(const float *cdf, int stride, float 
   return left > r ? r : left;
 }
 
+// Categorical draw from one probability row held in registers, p[0 .. A) with A <= kMax <=
+// 32: the float32 CDF of the same left-to-right additions (never contracted into an FMA with
+// whatever produced p) searched exactly as search_index(cdf, 1, u, A - 1) searches it.  That
+// search only asks two things of an entry it probes, |cdf - u| < 1e-8 and cdf < u, so both
+// are evaluated for every entry as bit masks first and the search then runs on the masks:
+// no dynamically indexed register array.  The packed TagContinuous step and the policy
+// forward (wdb_mlp_policy_forward_sampled) both sample through this, so they draw the same
+// action from the same probabilities and uniform.
+template <int kMax>
+__device__ __forceinline__ int sample_cdf_regs(const float (&p)[kMax], int A, float u) {
+  static_assert(kMax <= 32, "one bit per action");
+  uint32_t near = 0, below = 0;
+  float c = 0.0f;
+#pragma unroll
+  for (int i = 0; i < kMax; i++) {
+    c = i ? __fadd_rn(p[i], c) : p[i];
+    if (i < A) {
+      near |= (fabsf(__fsub_rn(c, u)) < 1.0e-8f ? 1u : 0u) << i;
+      below |= (c < u ? 1u : 0u) << i;
+    }
+  }
+  const int r = A - 1;
+  int left = 0, right = r;
+  while (left <= right) {
+    const int mid = left + (right - left) / 2;
+    if ((near >> mid) & 1u) return mid;
+    if ((below >> mid) & 1u) left = mid + 1; else right = mid - 1;
+  }
+  return left > r ? r : left;
+}
+
 // Index selection for masked policies: p[0 .. A) becomes the same float32 CDF the reference
 // sampler builds, and the result is the first index with p_i > 0 whose CDF reaches u, or,
 // when u lies above the float32 total, the last index with p_i > 0.  search_index can return

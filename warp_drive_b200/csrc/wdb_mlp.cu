@@ -423,12 +423,25 @@ using AnyShape = MlpShape<0, 0, 0>;
 // at the top of the tile.
 using FastShape = MlpShape<80, 256, 48>;
 
-template <bool TILES, class Shape, bool MASK = false>
+// SAMPLE (FastShape only, wdb_mlp_policy_forward_sampled): the epilogue also draws both
+// heads' actions of every row, as the fused TagContinuous step would from the stored
+// probabilities.  Row r = env * Np + slot of the policy is agent gi = env * N + agent[slot].
+struct MlpSampling {
+  int *actions;               // [rows, 2]
+  void *rng;                  // RNG state of E * N streams (NULL with uniforms)
+  const float *uniforms;      // [E * N * 2] or NULL
+  const int *agent;           // [Np]
+  int N, Np;
+};
+
+template <bool TILES, class Shape, bool MASK = false, bool SAMPLE = false>
 __device__ __forceinline__ void
 mlp_forward_body(const unsigned char *__restrict__ blob, const void *__restrict__ input,
                  long long rows, float *__restrict__ probs0, float *__restrict__ probs1,
                  float *__restrict__ values, const unsigned bid, const unsigned gdim,
-                 const int flags, const float *__restrict__ mask = nullptr) {
+                 const int flags, const float *__restrict__ mask = nullptr,
+                 const MlpSampling &smp = MlpSampling{}) {
+  static_assert(!SAMPLE || (Shape::H != 0 && !MASK), "sampling is a FastShape epilogue");
   extern __shared__ __align__(128) unsigned char smem[];
   const MlpHeader hd = *reinterpret_cast<const MlpHeader *>(blob);
   const int F = hd.F, A0 = hd.A0, A1 = hd.A1;
@@ -620,6 +633,28 @@ mlp_forward_body(const unsigned char *__restrict__ blob, const void *__restrict_
     }
     MLP_MARK(mark0 + 2);
 
+    // SAMPLE: thread lt draws head lt / 64 of row lt % 64, the head its softmax below
+    // computes.  Its uniform's inputs are requested here, so that the loads overlap the
+    // epilogue; both threads of a row read the RNG offset before the wg_sync after the softmax,
+    // the head-0 thread advances it after that barrier.
+    const long long s_row = tile * kTileM + wg * kWgRows + (lt & 63);
+    const bool s_valid = SAMPLE && s_row < rows;
+    long long s_gi = 0;
+    unsigned long long s_seed = 0, s_off = 0;
+    float s_u = 0.0f;
+    if constexpr (SAMPLE) {
+      if (s_valid) {
+        const long long env = s_row / smp.Np;
+        s_gi = env * smp.N + __ldg(smp.agent + (int)(s_row - env * smp.Np));
+        if (smp.uniforms) {
+          s_u = __ldg(smp.uniforms + 2 * s_gi + (lt >> 6));
+        } else {
+          s_seed = reinterpret_cast<const RngHeader *>(smp.rng)->seed;
+          s_off = rng_offsets(smp.rng)[s_gi];
+        }
+      }
+    }
+
     // ---- output epilogue.  Logits (+ bias) -> staging [64 rows x N3]: o[c][4 j + 0/1] is
     // row 16 wr + g, o[c][4 j + 2/3] row + 8, columns 16 c + 8 j + 2 t (+1).  (The previous
     // tile's output copy and, for other shapes, the layer-1 MMAs that read the staging buffer
@@ -685,13 +720,28 @@ mlp_forward_body(const unsigned char *__restrict__ blob, const void *__restrict_
     const float inv = 1.0f / ((zz[0] + zz[1]) + (zz[2] + zz[3]));
     MLP_MARK(mark0 + 3);
     wg_sync(wg);
+    if constexpr (SAMPLE) {
+      // the probabilities exactly as they are stored below, sampled in registers
+#pragma unroll
+      for (int i = 0; i < 32; i++) lg[i] = lg[i] * inv;
+      if (s_valid) {
+        if (!smp.uniforms) {
+          RngHeader h;
+          h.seed = s_seed; h.n_streams = 0;
+          const uint4 d = rng_draw4(h, (unsigned long long)s_gi, s_off);
+          s_u = u32_to_uniform(part ? d.y : d.x);
+          if (!part) rng_offsets(smp.rng)[s_gi] = s_off + 1;
+        }
+        smp.actions[2 * s_row + part] = sample_cdf_regs(lg, cnt, s_u);
+      }
+    }
     // staging = [probs0 64 x A0 | probs1 64 x A1 | values 64]: the warpgroup's rows of each
     // output are contiguous in global memory
     float *s_p0 = s_o, *s_p1 = s_o + kWgRows * A0, *s_v = s_p1 + kWgRows * A1;
     float *dst = (part ? s_p1 : s_p0) + row * cnt;
 #pragma unroll
     for (int i = 0; i < 32; i++)
-      if (i < cnt) dst[i] = lg[i] * inv;
+      if (i < cnt) dst[i] = SAMPLE ? lg[i] : lg[i] * inv;
     if (part) s_v[row] = value;
     wg_sync(wg);
     const long long rb = tile * kTileM + wg * kWgRows;   // first row of the warpgroup
@@ -715,6 +765,15 @@ mlp_forward_kernel(const unsigned char *__restrict__ blob, const void *__restric
                    long long rows, float *__restrict__ probs0, float *__restrict__ probs1,
                    float *__restrict__ values, int flags) {
   mlp_forward_body<TILES, Shape>(blob, input, rows, probs0, probs1, values, blockIdx.x, gridDim.x, flags);
+}
+
+template <bool TILES>
+__global__ void __launch_bounds__(kThreads, 1)
+mlp_forward_sampled_kernel(const unsigned char *__restrict__ blob, const void *__restrict__ input,
+                           long long rows, float *__restrict__ probs0, float *__restrict__ probs1,
+                           float *__restrict__ values, const __grid_constant__ MlpSampling smp) {
+  mlp_forward_body<TILES, FastShape, false, true>(blob, input, rows, probs0, probs1, values,
+                                                  blockIdx.x, gridDim.x, 0, nullptr, smp);
 }
 
 template <class Shape>
@@ -902,6 +961,43 @@ int launch_forward(void *stream, const void *blob, int F, int H, int A0, int A1,
       as_stream(stream), blob, smem, input, rows, mask, probs0, probs1, values);
 }
 
+bool mlp_samples(int F, int H, int A0, int A1) {
+  if (!mlp_shape_ok(F, H, A0, A1) || A1 < 1) return false;
+  const MlpHeader hd = make_header(F, H, A0, A1);
+  return hd.K1 == FastShape::K1 && hd.H == FastShape::H && hd.N3 == FastShape::N3;
+}
+
+template <bool TILES>
+int launch_forward_sampled(void *stream, const void *blob, int F, int H, int A0, int A1,
+                           const void *input, long long rows, float *probs0, float *probs1,
+                           float *values, const wdb_mlp_sampling *s) {
+  if (!blob || !input || !probs0 || !probs1 || rows <= 0 || !s) return (int)cudaErrorInvalidValue;
+  if (!mlp_samples(F, H, A0, A1)) return (int)cudaErrorInvalidValue;
+  if (TILES && (reinterpret_cast<uintptr_t>(input) & 15)) return (int)cudaErrorInvalidValue;
+  if (!s->actions || !s->agent_of_slot || (!s->rng_state && !s->uniforms))
+    return (int)cudaErrorInvalidValue;
+  if (reinterpret_cast<uintptr_t>(s->actions) & 7) return (int)cudaErrorMisalignedAddress;
+  if (s->n_policy_agents < 1 || s->n_agents < s->n_policy_agents || rows % s->n_policy_agents)
+    return (int)cudaErrorInvalidValue;
+  const size_t smem = mlp_smem_bytes(make_header(F, H, A0, A1));
+  static size_t configured = 0;
+  if (smem > configured) {
+    const cudaError_t e = cudaFuncSetAttribute(mlp_forward_sampled_kernel<TILES>,
+                                               cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               (int)smem);
+    if (e != cudaSuccess) return (int)e;
+    configured = smem;
+  }
+  const MlpSampling smp = {s->actions, s->rng_state, s->uniforms, s->agent_of_slot, s->n_agents,
+                           s->n_policy_agents};
+  const long long n_tiles = (rows + kTileM - 1) / kTileM;
+  const int sm_budget = (g_mlp_max_ctas > 0 && g_mlp_max_ctas < kNumSMs) ? g_mlp_max_ctas : kNumSMs;
+  const int grid = (int)min((long long)sm_budget, n_tiles);
+  mlp_forward_sampled_kernel<TILES><<<grid, kThreads, smem, as_stream(stream)>>>(
+      reinterpret_cast<const unsigned char *>(blob), input, rows, probs0, probs1, values, smp);
+  return finish_launch();
+}
+
 // Launch with the programmatic-stream-serialization attribute when the "pdl" option is on:
 // the grid may start while the previous kernel of the stream drains; the kernels order
 // themselves with griddepcontrol.wait (under stream capture this becomes a programmatic edge
@@ -1021,6 +1117,18 @@ WDB_API int wdb_mlp_policy_forward_masked(void *stream, const void *blob, int F,
   if (!mask) return (int)cudaErrorInvalidValue;
   return launch_forward<false>(stream, blob, F, H, A0, A1, obs, rows, probs0, probs1, values,
                                mask);
+}
+
+WDB_API int wdb_mlp_forward_samples(int F, int H, int A0, int A1) {
+  return mlp_samples(F, H, A0, A1) ? 1 : 0;
+}
+
+WDB_API int wdb_mlp_policy_forward_sampled(void *stream, const void *blob, int F, int H, int A0,
+                                           int A1, const void *input, int input_is_tiles,
+                                           long long rows, float *probs0, float *probs1,
+                                           float *values, const wdb_mlp_sampling *sampling) {
+  return (input_is_tiles ? launch_forward_sampled<true> : launch_forward_sampled<false>)(
+      stream, blob, F, H, A0, A1, input, rows, probs0, probs1, values, sampling);
 }
 
 WDB_API int wdb_mlp_policy_forward_pair(void *stream, const wdb_mlp_pair *pair) {

@@ -50,9 +50,13 @@
 
 namespace {
 
-template <bool FUSED, int MAXT>
+// ACTS_IN (fused only): the policy forward already sampled this step's actions into
+// Q.actions_batch (wdb_mlp_policy_forward_sampled); they are read instead of sampled, so no
+// probability tile, no TMA and no RNG.
+template <bool FUSED, int MAXT, bool ACTS_IN = false>
 __global__ void __launch_bounds__(MAXT, MAXT == 320 ? 2 : 1)
 tag_continuous_kernel(const __grid_constant__ TcParams P, const __grid_constant__ FusedParams Q) {
+  static_assert(FUSED || !ACTS_IN, "actions in the batch is a mode of the fused step");
   extern __shared__ __align__(16) unsigned char smem_raw[];
 #ifdef WDB_PHASE_CLOCKS
   const long long wdb_t0 = clock64();
@@ -175,7 +179,7 @@ tag_continuous_kernel(const __grid_constant__ TcParams P, const __grid_constant_
   };
   uint32_t tma_mask = 0;   // bit 2p / 2p+1: block (p, head) travels by TMA
   const uint32_t mbar = smem_u32(s_mbar);
-  if (FUSED) {
+  if (FUSED && !ACTS_IN) {
 #pragma unroll
     for (int q = 0; q < 2 * kMaxPolicies; q++)
       if (prob_block(q).tma) tma_mask |= 1u << q;
@@ -209,7 +213,7 @@ tag_continuous_kernel(const __grid_constant__ TcParams P, const __grid_constant_
   if (active && a == 0) { g_t = P.timestep[env]; g_nrun = P.num_runners[env]; }
   unsigned long long rng_seed = 0, rng_off = 0;
   float u0 = 0.f, u1 = 0.f;
-  if (FUSED && active) {
+  if (FUSED && !ACTS_IN && active) {
     if (Q.uniforms) {
       u0 = Q.uniforms[2ll * gi];
       u1 = Q.uniforms[2ll * gi + 1];
@@ -226,12 +230,24 @@ tag_continuous_kernel(const __grid_constant__ TcParams P, const __grid_constant_
   if (tab_ok && tid < Q.A0 + Q.A1)
     g_tab = tid < Q.A0 ? P.acc_actions[tid] : P.turn_actions[tid - Q.A0];
 
+  int act0 = 0, act1 = 0;
   if (FUSED) {
     // Programmatic dependent launch (option "pdl"): this grid may have started while the policy
     // forward was still running.  Everything above read only what the PREVIOUS env step wrote
     // (complete: the forward released us after its own griddepcontrol.wait); the probabilities
-    // are requested only now.  A no-op when launched without the attribute.
+    // (or the actions the forward sampled) are requested only now.  A no-op when launched
+    // without the attribute.
     griddep_wait();
+    if (ACTS_IN && active) {
+#pragma unroll
+      for (int p = 0; p < kMaxPolicies; p++) {
+        if (p == my_pol) {
+          const int2 v = *reinterpret_cast<const int2 *>(
+              Q.actions_batch[p] + 2ll * ((long long)env * Q.policy_size[p] + my_slot));
+          act0 = v.x; act1 = v.y;
+        }
+      }
+    }
     if (tid == 0 && tma_mask) {
       uint32_t total = 0;
 #pragma unroll
@@ -285,15 +301,16 @@ tag_continuous_kernel(const __grid_constant__ TcParams P, const __grid_constant_
   // has its barrier in the sampling phase)
   if (!FUSED) __syncthreads();
 
-  int act0 = 0, act1 = 0;
   if (FUSED) {
     // random draw for both heads (independent of the probabilities: overlaps the copies)
-    if (active && !Q.uniforms) tc_draw_uniforms(Q, gi, rng_seed, rng_off, u0, u1);
+    if (!ACTS_IN && active && !Q.uniforms) tc_draw_uniforms(Q, gi, rng_seed, rng_off, u0, u1);
     __syncthreads();                      // mbarrier initialised; tables / phase-0 arrays staged
     WDB_MARK(0)   // rng drawn, state requested
     if (tma_mask) mbar_wait(mbar, 0);      // TMA blocks landed
     WDB_MARK(1)   // probabilities landed
-    if (active) {
+    if (ACTS_IN) {
+      if (active) tc_push_actions(Q, gi, env, my_pol, 0, my_slot, act0, act1, false);
+    } else if (active) {
       const int pol = my_pol, slot = my_slot;
       int np = 0, o0 = 0, o1 = 0;
       const float *g0 = nullptr, *g1 = nullptr;   // global rows of blocks that did not go by TMA
@@ -886,8 +903,8 @@ int plan_packed(TcParams &P, const FusedParams *Q, TcPlan &plan) {
   warp_bytes = (warp_bytes + 15) & ~(size_t)15;
   const size_t scr = warp_bytes * nwarps;
   size_t tile_obs = P.use_full_obs ? 0 : sizeof(float) * (size_t)epb * N * F;
-  size_t tile_probs = 0;
-  if (Q) {
+  size_t tile_probs = 0;   // (no probability tile when the actions come in sampled)
+  if (Q && !Q->actions_in) {
     for (int p = 0; p < Q->n_policies; p++)
       tile_probs += ((sizeof(float) * (size_t)epb * Q->policy_size[p] * Q->A0 + 15) & ~(size_t)15) +
                     ((sizeof(float) * (size_t)epb * Q->policy_size[p] * Q->A1 + 15) & ~(size_t)15) + 64;
@@ -947,16 +964,16 @@ int plan_packed(TcParams &P, const FusedParams *Q, TcPlan &plan) {
   return 0;
 }
 
-template <bool FUSED, int MAXT>
+template <bool FUSED, int MAXT, bool ACTS_IN = false>
 int launch_t(const TcParams &P, const FusedParams &Q, const TcPlan &plan, cudaStream_t st) {
   static size_t configured = 0;
   if (plan.smem > 48 * 1024 && plan.smem > configured) {
-    cudaError_t e = cudaFuncSetAttribute(tag_continuous_kernel<FUSED, MAXT>,
+    cudaError_t e = cudaFuncSetAttribute(tag_continuous_kernel<FUSED, MAXT, ACTS_IN>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          (int)plan.smem);
     if (e != cudaSuccess) return (int)e;
     // all of the SM's unified L1 as shared memory: the CTAs are sized to fill it
-    cudaFuncSetAttribute(tag_continuous_kernel<FUSED, MAXT>,
+    cudaFuncSetAttribute(tag_continuous_kernel<FUSED, MAXT, ACTS_IN>,
                          cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     configured = plan.smem;
   }
@@ -970,7 +987,7 @@ int launch_t(const TcParams &P, const FusedParams &Q, const TcPlan &plan, cudaSt
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = (FUSED && Q.pdl && g_pdl) ? 1 : 0;
-  const cudaError_t e = cudaLaunchKernelEx(&cfg, tag_continuous_kernel<FUSED, MAXT>, P, Q);
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, tag_continuous_kernel<FUSED, MAXT, ACTS_IN>, P, Q);
   if (e != cudaSuccess) return (int)e;
   return finish_launch();
 }
@@ -1013,8 +1030,11 @@ int tc_plan(TcParams &P, const FusedParams *Q, bool obs_next, bool obs_tiles, in
   // blocks_per_env > 1: the env is spread over that many CTAs, launched as one thread-block
   // cluster (wdb_tc_wide.cu) -- the reference's multi-block mode, env_dim_mapper.h:22-31.
   // Observation tiles come from the packed kernel's staged tile only.
+  // The actions-in mode (Q->actions_in) is a mode of the packed kernel alone: the
+  // second-generation and cluster kernels always sample from the probabilities.
+  const bool acts_in = Q && Q->actions_in;
   if (blocks_per_env > 1) {
-    if (obs_tiles) return (int)cudaErrorInvalidValue;
+    if (obs_tiles || acts_in) return (int)cudaErrorInvalidValue;
     return tc_wide_plan(P, Q, blocks_per_env, plan);
   }
   if (P.N > 1024) return (int)cudaErrorInvalidValue;   // one CTA per env: <= 1024 threads
@@ -1022,12 +1042,17 @@ int tc_plan(TcParams &P, const FusedParams *Q, bool obs_next, bool obs_tiles, in
   // whole env in ONE CTA (a cluster of 1); wdb_set_option("tc_wide_single", 0) keeps the
   // first-generation single-CTA path for A/B runs
   if (g_tc_wide_single && P.N > 320 && !P.use_full_obs && P.K + 2 <= kListLen) {
-    if (obs_tiles) return (int)cudaErrorInvalidValue;
+    if (obs_tiles || acts_in) return (int)cudaErrorInvalidValue;
     return tc_wide_plan(P, Q, 1, plan);
   }
-  if (tc_v2_eligible(P, Q, obs_tiles)) return tc_v2_plan(P, plan);
+  if (tc_v2_eligible(P, Q, obs_tiles)) {
+    if (acts_in) return (int)cudaErrorInvalidValue;
+    return tc_v2_plan(P, plan);
+  }
   const int err = plan_packed(P, Q, plan);
   if (err) return err;
+  // the actions-in instance is built for the two-CTAs-per-SM geometry only
+  if (acts_in && plan.block > 320) return (int)cudaErrorInvalidValue;
   // the per-policy observation push needs the shared-memory tile
   if (!P.stage_obs && !P.use_full_obs && (obs_next || obs_tiles))
     return (int)cudaErrorInvalidValue;
@@ -1042,6 +1067,7 @@ int tc_launch(const TcParams &P, const FusedParams *Q, const TcPlan &plan, cudaS
   if (!Q)
     return plan.block <= 320 ? launch_t<false, 320>(P, none, plan, st)
                              : launch_t<false, 1024>(P, none, plan, st);
+  if (Q->actions_in) return launch_t<true, 320, true>(P, *Q, plan, st);   // (tc_plan: block <= 320)
   return plan.block <= 320 ? launch_t<true, 320>(P, *Q, plan, st)
                            : launch_t<true, 1024>(P, *Q, plan, st);
 }
@@ -1057,9 +1083,10 @@ int plan_rollout(const wdb_tc_env *env, const wdb_tc_rollout *ro, bool shapes_on
   if (ro->n_policies < 1 || ro->n_policies > kMaxPolicies || ro->n_actions0 < 1 ||
       ro->n_actions1 < 1)
     return (int)cudaErrorInvalidValue;
+  const bool acts_in = ro->actions_in != 0;
   if (!shapes_only) {
     if (!ro->agent_policy || !ro->agent_slot) return (int)cudaErrorInvalidValue;
-    if (!ro->uniforms && !ro->rng_state) return (int)cudaErrorInvalidValue;
+    if (!acts_in && !ro->uniforms && !ro->rng_state) return (int)cudaErrorInvalidValue;
     if (ro->sampled_actions && ((uintptr_t)ro->sampled_actions & 7))
       return (int)cudaErrorMisalignedAddress;
   }
@@ -1073,7 +1100,8 @@ int plan_rollout(const wdb_tc_env *env, const wdb_tc_rollout *ro, bool shapes_on
     const wdb_tc_policy_io &io = ro->policy[p];
     if (io.n_agents < 1) return (int)cudaErrorInvalidValue;
     if (!shapes_only) {
-      if (!io.probs0 || !io.probs1) return (int)cudaErrorInvalidValue;
+      if (acts_in ? !io.actions_batch : (!io.probs0 || !io.probs1))
+        return (int)cudaErrorInvalidValue;
       if (io.actions_batch && ((uintptr_t)io.actions_batch & 7))
         return (int)cudaErrorMisalignedAddress;
       if (io.obs_next_tiles && ((uintptr_t)io.obs_next_tiles & 15))
@@ -1098,6 +1126,7 @@ int plan_rollout(const wdb_tc_env *env, const wdb_tc_rollout *ro, bool shapes_on
   Q.reset_table = ro->reset_table; Q.n_reset = ro->n_reset_arrays;
   Q.obs_at_reset = ro->obs_at_reset; Q.do_reset = ro->reset_done_envs;
   Q.pdl = ro->launch_after_forward;
+  Q.actions_in = acts_in;
   if (!shapes_only && Q.do_reset && Q.n_reset > 0 && !Q.reset_table)
     return (int)cudaErrorInvalidValue;
   return tc_plan(P, &Q, obs_next, obs_tiles, env->blocks_per_env, plan);

@@ -89,6 +89,8 @@ struct FusedParams {
   const float *obs_at_reset;        // [E, N, F] (for obs_next of envs that reset)
   int do_reset;
   int pdl;                          // host only: launch programmatically dependent on the forward
+  int actions_in;                   // host only: actions_batch already holds the actions (the
+                                    // packed kernel's ACTS_IN instance reads them)
 };
 
 struct V2Params {
@@ -287,8 +289,8 @@ __device__ __forceinline__ float div_by_const_f64(float d, double c, double inv_
 
 // Inclusive float32 prefix sum of one probability row (same left-to-right additions as
 // core/random.cu:62-72) followed by the reference's binary search.  Rows of <= 32 actions
-// are summed in registers (independent loads, one dependent FADD chain) instead of a
-// load-add-store chain through shared memory.
+// are loaded into registers and sampled there (sample_cdf_regs, which the policy forward's
+// sampling epilogue calls too); longer rows build their CDF in shared memory.
 __device__ __noinline__ void cdf_long_row(float *row, const float *src, int A) {
   float c = src[0];
   row[0] = c;
@@ -297,18 +299,14 @@ __device__ __noinline__ void cdf_long_row(float *row, const float *src, int A) {
 __device__ __forceinline__ int sample_row(float *row, const float *src, int A, float u) {
   // src: where the probabilities are (the staged shared-memory row itself, or the global row
   // of a block that could not travel by TMA); row: shared-memory row that receives the CDF
+  // of a row longer than 32
   if (A <= 32) {
     float v[32];
 #pragma unroll
     for (int i = 0; i < 32; i++) v[i] = i < A ? src[i] : 0.0f;
-#pragma unroll
-    for (int i = 1; i < 32; i++) v[i] = v[i] + v[i - 1];
-#pragma unroll
-    for (int i = 0; i < 32; i++)
-      if (i < A) row[i] = v[i];
-  } else {
-    cdf_long_row(row, src, A);
+    return sample_cdf_regs(v, A, u);
   }
+  cdf_long_row(row, src, A);
   return search_index(row, 1, u, A - 1);
 }
 
@@ -573,13 +571,15 @@ __device__ __forceinline__ void tc_draw_uniforms(const FusedParams &Q, int gi,
 }
 
 // The sampled actions of agent gi (slot `slot` of policy `pol`, np agents per env) to every
-// output that is set.  A NULL actions_batch[0] disables the push to the batch for every policy.
+// output that is set.  A NULL actions_batch[0] disables the push to the batch for every policy;
+// so does to_batch = false (the actions came from the batch).
 __device__ __forceinline__ void tc_push_actions(const FusedParams &Q, int gi, int env, int pol,
-                                                int np, int slot, int act0, int act1) {
+                                                int np, int slot, int act0, int act1,
+                                                bool to_batch = true) {
   if (Q.actions_out) *reinterpret_cast<int2 *>(Q.actions_out + 2ll * gi) = make_int2(act0, act1);
   if (Q.actions_head0) Q.actions_head0[gi] = act0;
   if (Q.actions_head1) Q.actions_head1[gi] = act1;
-  if (Q.actions_batch[0]) {
+  if (to_batch && Q.actions_batch[0]) {
 #pragma unroll
     for (int p = 0; p < kMaxPolicies; p++)
       if (p == pol && Q.actions_batch[p])

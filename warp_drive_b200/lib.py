@@ -70,7 +70,7 @@ class TcRollout(ctypes.Structure):
         ("done_batch", _fp), ("step_running_sum", _fp),
         ("episodic_step_sum", _fp), ("num_completed_episodes", _fp),
         ("reset_table", _fp), ("n_reset_arrays", _i), ("obs_at_reset", _fp),
-        ("reset_done_envs", _i), ("launch_after_forward", _i),
+        ("reset_done_envs", _i), ("launch_after_forward", _i), ("actions_in", _i),
     ]
 
 
@@ -140,6 +140,15 @@ class MlpPair(ctypes.Structure):
 
 
 MLP_WEIGHTS_STABLE = 1
+
+
+class MlpSampling(ctypes.Structure):
+    """struct wdb_mlp_sampling (include/wdb200.h)."""
+
+    _fields_ = [
+        ("actions", _fp), ("rng_state", _fp), ("uniforms", _fp), ("agent_of_slot", _fp),
+        ("n_agents", _i), ("n_policy_agents", _i),
+    ]
 
 
 class SaRollout(ctypes.Structure):
@@ -320,6 +329,9 @@ _SIGNATURES = {
     "wdb_mlp_policy_forward_masked": (
         _i, [_vp, _vp, _i, _i, _i, _i, _vp, _ll, _vp, _vp, _vp, _vp]),
     "wdb_mlp_policy_forward_pair": (_i, [_vp, ctypes.POINTER(MlpPair)]),
+    "wdb_mlp_forward_samples": (_i, [_i, _i, _i, _i]),
+    "wdb_mlp_policy_forward_sampled": (
+        _i, [_vp, _vp, _i, _i, _i, _i, _vp, _i, _ll, _vp, _vp, _vp, ctypes.POINTER(MlpSampling)]),
     "wdb_gather_policy_rows": (_i, [_vp, ctypes.POINTER(Gather)]),
     "wdb_gather_policy_fields": (_i, [_vp, ctypes.POINTER(GatherFields)]),
     "wdb_rollout_bookkeep": (_i, [_vp, ctypes.POINTER(Bookkeep)]),

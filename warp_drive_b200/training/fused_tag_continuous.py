@@ -57,10 +57,12 @@ def fill_tc_env(dm, stats=None, with_scratch=False, write_observations=True):
 
 class FusedTagContinuousStep:
     @staticmethod
-    def eligible(env_wrapper, policy_map, obs_tiles=False):
-        """Whether the library runs the fused step for this env, these policies and (with
-        obs_tiles) the bf16 observation tiles; it applies the same launch plan as the step."""
+    def eligible(env_wrapper, policy_map, obs_tiles=False, actions_in=False):
+        """Whether the library runs the fused step for this env, these policies, (with
+        obs_tiles) the bf16 observation tiles and (with actions_in) actions sampled by the
+        forward; it applies the same launch plan as the step."""
         ro = _lib.TcRollout()
+        ro.actions_in = int(bool(actions_in))
         ro.n_policies = len(policy_map)
         heads = env_wrapper.env.action_space[0].nvec
         ro.n_actions0, ro.n_actions1 = int(heads[0]), int(heads[1])
@@ -122,13 +124,15 @@ class FusedTagContinuousStep:
 
     def launch(self, probs, actions_batch=None, rewards_batch=None, obs_next=None,
                done_batch=None, uniforms=None, reset_done_envs=True, obs_next_tiles=None,
-               after_forward=False):
+               after_forward=False, actions_in=False):
         """probs: {policy: [probs_head0 [E,Np,A0], probs_head1 [E,Np,A1]]}; the *_batch /
-        obs_next dicts hold this timestep's slots (tensors) per policy, or None."""
+        obs_next dicts hold this timestep's slots (tensors) per policy, or None.
+        actions_in: the forward already sampled the actions into `actions_batch` (required),
+        which the step then reads instead of sampling from `probs` (may be None)."""
         ro = self.ro
         for pi, p in enumerate(self.policies):
             io = ro.policy[pi]
-            io.probs0, io.probs1 = _p(probs[p][0]), _p(probs[p][1])
+            io.probs0, io.probs1 = (_p(probs[p][0]), _p(probs[p][1])) if probs else (None, None)
             io.actions_batch = _p(actions_batch[p]) if actions_batch else None
             io.rewards_batch = _p(rewards_batch[p]) if rewards_batch else None
             io.obs_next = _p(obs_next[p]) if obs_next else None
@@ -137,5 +141,6 @@ class FusedTagContinuousStep:
         ro.uniforms = _p(uniforms)
         ro.reset_done_envs = int(bool(reset_done_envs))
         ro.launch_after_forward = int(bool(after_forward))
+        ro.actions_in = int(bool(actions_in))
         _lib.check(self.lib.wdb_tag_continuous_rollout_step(
             _lib.stream_ptr(), self._env_ref, self._ro_ref), "tag_continuous_rollout_step")

@@ -40,6 +40,8 @@ class FusedPolicyForward:
         nbytes = int(self.lib.wdb_mlp_blob_bytes(self.F, self.H, self.A0, self.A1))
         dev = next(model.parameters()).device
         self.blob = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
+        # whether this shape's forward can also sample both heads (wdb_mlp_policy_forward_sampled)
+        self.samples = bool(self.lib.wdb_mlp_forward_samples(self.F, self.H, self.A0, self.A1))
         self.refresh()
 
     def refresh(self):
@@ -57,12 +59,33 @@ class FusedPolicyForward:
             self.F, self.H, self.A0, self.A1), "mlp_pack_weights")
         self._keep = ts
 
-    def __call__(self, obs, probs0, probs1, values=None, max_ctas=0, mask=None):
+    def sampling(self, actions, agent_of_slot, n_agents, rng_state=None, uniforms=None):
+        """The sampling arguments of a forward (see `__call__`): both heads' actions of every
+        row go to `actions` [E, Np, 2] int32; row env * Np + slot is agent
+        env * n_agents + agent_of_slot[slot] of the RNG state (or of `uniforms` [E, N, 2])."""
+        s = _lib.MlpSampling()
+        s.actions, s.rng_state, s.uniforms = _lib.ptr(actions), _lib.ptr(rng_state), _lib.ptr(uniforms)
+        s.agent_of_slot = _lib.ptr(agent_of_slot)
+        s.n_agents, s.n_policy_agents = int(n_agents), int(agent_of_slot.numel())
+        return s
+
+    def _sampled(self, input_, tiles, rows, probs0, probs1, values, sampling):
+        _lib.check(self.lib.wdb_mlp_policy_forward_sampled(
+            _lib.stream_ptr(), _lib.ptr(self.blob), self.F, self.H, self.A0, self.A1,
+            _lib.ptr(input_), int(tiles), int(rows), _lib.ptr(probs0), _lib.ptr(probs1),
+            _lib.ptr(values), ctypes.byref(sampling)), "mlp_policy_forward_sampled")
+
+    def __call__(self, obs, probs0, probs1, values=None, max_ctas=0, mask=None, sampling=None):
         """obs [..., F] float32 contiguous -> probs0 [..., A0], probs1 [..., A1] (written).
         max_ctas > 0 restricts the launch to that many SMs (side-by-side forwards).
-        mask [..., A0 + A1] float32 contiguous (1 = valid): the masked forward."""
+        mask [..., A0 + A1] float32 contiguous (1 = valid): the masked forward.
+        sampling (from `sampling()`, shapes with `samples` only): also sample both heads."""
         rows = obs.numel() // self.F
         _lib.check(self.lib.wdb_set_option(b"mlp_max_ctas", int(max_ctas)), "set_option")
+        if sampling is not None:
+            assert mask is None
+            self._sampled(obs, False, rows, probs0, probs1, values, sampling)
+            return
         if mask is not None:
             assert mask.dtype == torch.float32 and mask.numel() == rows * (self.A0 + self.A1)
             _lib.check(self.lib.wdb_mlp_policy_forward_masked(
@@ -85,9 +108,12 @@ class FusedPolicyForward:
         _lib.check(self.lib.wdb_mlp_pack_obs(_lib.stream_ptr(), _lib.ptr(obs), rows, self.F,
                                              _lib.ptr(tiles)), "mlp_pack_obs")
 
-    def forward_tiles(self, tiles, rows, probs0, probs1, values=None, max_ctas=0):
+    def forward_tiles(self, tiles, rows, probs0, probs1, values=None, max_ctas=0, sampling=None):
         """The forward fed from the bf16 tiles (written by pack_obs or by the fused env step)."""
         _lib.check(self.lib.wdb_set_option(b"mlp_max_ctas", int(max_ctas)), "set_option")
+        if sampling is not None:
+            self._sampled(tiles, True, rows, probs0, probs1, values, sampling)
+            return
         _lib.check(self.lib.wdb_mlp_policy_forward_tiles(
             _lib.stream_ptr(), _lib.ptr(self.blob), self.F, self.H, self.A0, self.A1,
             _lib.ptr(tiles), int(rows), _lib.ptr(probs0), _lib.ptr(probs1), _lib.ptr(values)),

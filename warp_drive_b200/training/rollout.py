@@ -139,6 +139,7 @@ class RolloutEngine:
         # ---- tensor-core forward (wgmma MLP kernel) for the fused path
         self.fused_forward = {}
         self.obs_tiles = {}
+        self.sample_in_forward = False
         if self.sa is None and use_fused_forward and forward_dtype is None and not self.continuous:
             from warp_drive_b200.training.models.fused_forward import FusedPolicyForward
 
@@ -157,6 +158,23 @@ class RolloutEngine:
                     self.obs_tiles = {
                         p: torch.zeros(self.fused_forward[p].tiles_bytes(
                             self.E * len(self.policy_map[p])), dtype=torch.uint8, device=dev)
+                        for p in self.policies}
+                # The forwards also sample both heads, straight into the step's action batch
+                # slot, and the fused step reads those actions instead of the probabilities
+                # (no probability round trip, no sampling phase in the env kernel): when every
+                # policy's shape samples and the step's launch plan takes its actions in.  The
+                # same uniforms and CDF search, so the same actions as sampling in the step.
+                self.sample_in_forward = (
+                    self.fused is not None and not self.use_pair_forward
+                    and all(f.samples for f in self.fused_forward.values())
+                    and self.fused.eligible(env_wrapper, self.policy_map,
+                                            obs_tiles=bool(self.obs_tiles), actions_in=True))
+                if self.sample_in_forward:
+                    self._agent_of_slot = {
+                        p: torch.as_tensor(self.policy_map[p], dtype=torch.int32, device=dev)
+                        for p in self.policies}
+                    self._sampling = {
+                        p: self.fused_forward[p].sampling(None, self._agent_of_slot[p], self.N)
                         for p in self.policies}
 
     def refresh_forward_weights(self):
@@ -221,16 +239,18 @@ class RolloutEngine:
         probs, _ = model(obs_p, **kw)
         return [q.contiguous() for q in probs]
 
-    def _forward_side_by_side(self, obs_in, probs, weights_stable=False):
+    def _forward_side_by_side(self, obs_in, probs, weights_stable=False, sampling=None):
         """Every policy's fused forward, concurrently: the persistent MLP kernel uses one CTA
         per SM, so the SMs are split between the policies in proportion to their rows and the
         smaller policies run on side streams (fork/join by events, also under graph capture).
         Sequential launches would each pay the 195 KB weight load and leave most SMs idle
-        during the small policy's single wave."""
+        during the small policy's single wave.  sampling: {policy: MlpSampling}, the forwards
+        also sample (see sample_in_forward)."""
         if len(self.policies) == 1:
-            self._one_forward(self.policies[0], obs_in, probs)
+            self._one_forward(self.policies[0], obs_in, probs, sampling=sampling)
             return False
         if len(self.policies) == 2 and not self.obs_tiles and self.use_pair_forward:
+            assert sampling is None, "the pair forward does not sample"
             # both policies in ONE launch (CTAs split by tile counts), no fork / join
             from warp_drive_b200.training.models.fused_forward import forward_pair
 
@@ -270,23 +290,25 @@ class RolloutEngine:
         for p, st in zip(order[1:], self._fwd_streams):
             st.wait_event(fork)
             with torch.cuda.stream(st):
-                self._one_forward(p, obs_in, probs, share[p])
+                self._one_forward(p, obs_in, probs, share[p], sampling)
                 ev = torch.cuda.Event()
                 ev.record(st)
             joins.append(ev)
         p = order[0]
-        self._one_forward(p, obs_in, probs, share[p])
+        self._one_forward(p, obs_in, probs, share[p], sampling)
         for ev in joins:
             cur.wait_event(ev)
         return self.pdl_after_fork
 
-    def _one_forward(self, p, obs_in, probs, max_ctas=0):
+    def _one_forward(self, p, obs_in, probs, max_ctas=0, sampling=None):
+        smp = sampling[p] if sampling else None
         if self.obs_tiles:
             rows = obs_in[p].numel() // obs_in[p].shape[-1]
             self.fused_forward[p].forward_tiles(self.obs_tiles[p], rows, probs[p][0], probs[p][1],
-                                                max_ctas=max_ctas)
+                                                max_ctas=max_ctas, sampling=smp)
         else:
-            self.fused_forward[p](obs_in[p], probs[p][0], probs[p][1], max_ctas=max_ctas)
+            self.fused_forward[p](obs_in[p], probs[p][0], probs[p][1], max_ctas=max_ctas,
+                                  sampling=smp)
 
     def step_fused(self, t, uniforms=None):
         """One timestep = policy forwards + ONE libwdb200 launch."""
@@ -314,16 +336,35 @@ class RolloutEngine:
                 obs_next = self._scratch_obs
                 actions_batch = rewards_batch = done_batch = None
             paired = False
+            sampling = None
+            if self.sample_in_forward:
+                # the forwards sample into the batch slot (t < 0: into a scratch buffer), with
+                # the RNG state the step would have sampled with
+                if actions_batch is None:
+                    if not hasattr(self, "_scratch_actions"):
+                        self._scratch_actions = {
+                            p: torch.empty((self.E, len(self.policy_map[p]), 2),
+                                           dtype=torch.int32, device=self.dm.device)
+                            for p in self.policies}
+                    actions_batch = self._scratch_actions
+                sampling = self._sampling
+                for p in self.policies:
+                    s = sampling[p]
+                    s.actions = _lib.ptr(actions_batch[p])
+                    s.rng_state = self.fused.ro.rng_state
+                    s.uniforms = _lib.ptr(uniforms)
             if self.fused_forward:
                 probs = self._probs
                 # t > 0: the kernel before this forward is the previous env step, not a weight
                 # re-pack -> the weight load may overlap its tail (programmatic launch)
-                paired = self._forward_side_by_side(obs_in, probs, weights_stable=t > 0)
+                paired = self._forward_side_by_side(obs_in, probs, weights_stable=t > 0,
+                                                    sampling=sampling)
             else:
                 probs = {p: self._forward(self.models[p], obs_in[p]) for p in self.policies}
             self.fused.launch(probs, actions_batch=actions_batch, rewards_batch=rewards_batch,
                               obs_next=obs_next, done_batch=done_batch, uniforms=uniforms,
-                              obs_next_tiles=self.obs_tiles or None, after_forward=paired)
+                              obs_next_tiles=self.obs_tiles or None, after_forward=paired,
+                              actions_in=sampling is not None)
             if t < 0:
                 for p in self.policies:
                     self.cur_obs[p].copy_(self._scratch_obs[p])
