@@ -889,6 +889,61 @@ long long wdb_sac_actor_update_workspace_bytes(const wdb_sac_update_args *update
 int wdb_sac_critic_update(void *stream, const wdb_sac_update_args *update);
 int wdb_sac_actor_update(void *stream, const wdb_sac_update_args *update);
 
+/* Replay buffer: the same ring made long (capacity >= n_step + 1 slots of which `filled` hold
+ * data, the oldest at physical slot `oldest`), and each of the five passes above over B
+ * uniformly sampled n-step windows instead of every window of the ring.
+ *
+ * wdb_replay_sample_windows writes, for g < n_windows, windows[g] = {(oldest + k) mod capacity,
+ * n}: a logical window start k uniform in [0, filled - n_step - 1] and an agent row n uniform
+ * in [0, n_rows), n_rows = E * Np.  A window is the logical slots k .. k + n_step, so none
+ * crosses the seam between the newest and the oldest data.  The draws are Philox4x32-10 with
+ * key `seed` and counter (counter, g): no RNG state, the same (seed, counter) gives the same
+ * windows.  A 32-bit draw x is reduced to [0, range) as the high word of x * range, so a value's
+ * probability differs from 1 / range by less than 2^-32 (relative bias <= range / 2^32).
+ * cudaErrorInvalidValue without launching unless n_step >= 1, n_step + 1 <= filled <= capacity,
+ * 0 <= oldest < capacity, n_rows >= 1 and n_windows >= 1.  One launch. */
+int wdb_replay_sample_windows(void *stream, int *windows /* out [n_windows][2] */, int n_windows,
+                              unsigned long long seed, unsigned long long counter, int oldest,
+                              int filled, int capacity, int n_step, int n_rows);
+
+/* The loss rows of a *_sampled pass: row g is the window of agent row windows[g][1] that starts
+ * at physical slot s = windows[g][0]; slot(j) = (s + j) mod capacity.  Observation and action
+ * at slot(0), rewards and done flags at slot(0 .. n_step - 1), the bootstrap observation at
+ * slot(n_step), and
+ *   R = r_0 + (1 - d_0) gamma (r_1 + ... (1 - d_{n_step - 1}) gamma * bootstrap)
+ * in the float32 operation order of a regular (not the last) window of the ring passes; there
+ * is no last-window rule.  M = B = n_windows: the means, 2 / M, -1 / M, `sums` and the optional
+ * per-row outputs ([B]) are those of the ring passes with that M, the noise inputs are [B, A],
+ * and `cursor` of the args struct is not read.  A window may appear more than once; each
+ * appearance is a loss row.  Every windows[g][0] must lie in [0, capacity) and windows[g][1] in
+ * [0, E * Np): they are not checked on the device.  Bit-reproducible as the ring passes. */
+typedef struct wdb_replay_windows {
+  const int *windows;                /* device [B][2] */
+  int n_windows;                     /* B >= 1 */
+} wdb_replay_windows;
+/* _sampled_supported: the ring pass's conditions without the one on cursor, capacity >= n_step
+ * + 1 and n_windows >= 1.  The workspace depends on n_windows. */
+int wdb_ddpg_update_sampled_supported(const wdb_ddpg_update_args *update, int n_windows);
+long long wdb_ddpg_update_sampled_workspace_bytes(const wdb_ddpg_update_args *update, int n_windows);
+int wdb_ddpg_update_sampled(void *stream, const wdb_ddpg_update_args *update,
+                            const wdb_replay_windows *windows);
+int wdb_td3_critic_update_sampled_supported(const wdb_td3_update_args *update, int n_windows);
+long long wdb_td3_critic_update_sampled_workspace_bytes(const wdb_td3_update_args *update, int n_windows);
+int wdb_td3_critic_update_sampled(void *stream, const wdb_td3_update_args *update,
+                                  const wdb_replay_windows *windows);
+int wdb_td3_actor_update_sampled_supported(const wdb_td3_update_args *update, int n_windows);
+long long wdb_td3_actor_update_sampled_workspace_bytes(const wdb_td3_update_args *update, int n_windows);
+int wdb_td3_actor_update_sampled(void *stream, const wdb_td3_update_args *update,
+                                 const wdb_replay_windows *windows);
+int wdb_sac_critic_update_sampled_supported(const wdb_sac_update_args *update, int n_windows);
+long long wdb_sac_critic_update_sampled_workspace_bytes(const wdb_sac_update_args *update, int n_windows);
+int wdb_sac_critic_update_sampled(void *stream, const wdb_sac_update_args *update,
+                                  const wdb_replay_windows *windows);
+int wdb_sac_actor_update_sampled_supported(const wdb_sac_update_args *update, int n_windows);
+long long wdb_sac_actor_update_sampled_workspace_bytes(const wdb_sac_update_args *update, int n_windows);
+int wdb_sac_actor_update_sampled(void *stream, const wdb_sac_update_args *update,
+                                 const wdb_replay_windows *windows);
+
 #ifdef __cplusplus
 }
 #endif

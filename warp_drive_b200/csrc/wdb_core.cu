@@ -478,3 +478,34 @@ WDB_API int wdb_discounted_returns(void *stream, const float *rewards, const int
       rewards, done, values, returns, T, n_envs, n_agents, gamma);
   return finish_launch();
 }
+
+// =================================================================== replay window sampling
+// windows[g] = {physical start slot, agent row} of a uniformly drawn n-step window (wdb200.h):
+// Philox keyed by the seed at counter (counter, g), so the draw needs no state array and an
+// update's windows are a function of (seed, counter) alone.  __umulhi(x, range) maps a 32-bit
+// draw to [0, range) with each value's probability within 2^-32 of 1 / range.
+__global__ void replay_sample_windows_kernel(int2 *__restrict__ windows, int n_windows,
+                                             unsigned long long seed, unsigned long long counter,
+                                             int oldest, int n_starts, int capacity, int n_rows) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= n_windows) return;
+  const RngHeader h = {seed, 0ull};
+  const uint4 x = rng_draw4(h, (unsigned long long)g, counter);
+  const int s = oldest + (int)__umulhi(x.x, (uint32_t)n_starts);
+  windows[g] = make_int2(s >= capacity ? s - capacity : s, (int)__umulhi(x.y, (uint32_t)n_rows));
+}
+
+WDB_API int wdb_replay_sample_windows(void *stream, int *windows, int n_windows,
+                                      unsigned long long seed, unsigned long long counter,
+                                      int oldest, int filled, int capacity, int n_step,
+                                      int n_rows) {
+  if (!windows || n_windows < 1 || n_rows < 1 || n_step < 1 || capacity < 1)
+    return (int)cudaErrorInvalidValue;
+  if (filled > capacity || filled - n_step < 1 || oldest < 0 || oldest >= capacity)
+    return (int)cudaErrorInvalidValue;
+  const int block = 256;
+  replay_sample_windows_kernel<<<(n_windows + block - 1) / block, block, 0, as_stream(stream)>>>(
+      reinterpret_cast<int2 *>(windows), n_windows, seed, counter, oldest, filled - n_step,
+      capacity, n_rows);
+  return finish_launch();
+}

@@ -33,6 +33,10 @@
 //   actor pass, per tile: actor on obs -> pi; Q1 on (obs, pi) -> J; dL/dJ = -1 / M back
 //     through Q1 to its action inputs only (no critic weight gradient), the tanh head and the
 //     actor.
+//
+// Replay buffer (wdb_*_update_sampled): each of the five passes also exists over B sampled
+// windows of a long ring, row g = windows[g] instead of (g / EN, g % EN) -- the *_sampled
+// kernels after the ring kernels.
 #include "wdb_common.cuh"
 
 using namespace wdb;
@@ -60,14 +64,18 @@ struct Plan {
   long long smem_floats;
 };
 
+// The loss rows are every window of the ring (w NULL: valid * E * Np rows from `cursor`) or w's
+// sampled windows (n_windows rows of n_step + 1 slots each; `cursor` is not read).
 // Shape checks and the shared-memory layout of the actor shape (k = 0: F -> head, head = A, or
 // 2A for SAC's mean ++ log-std) and the critic shape (k = 1: F + A -> 1).  nets[k][0] sets the
 // shape; nets[k][1 .. count[k] - 1] (targets, the second critic) must have the same.
 bool plan_layout(int E, int Np, int F, int A, int head, int C, int cursor, int ns,
-                 const wdb_ddpg_net *const *const nets[2], const int count[2], Plan *p) {
+                 const wdb_replay_windows *w, const wdb_ddpg_net *const *const nets[2],
+                 const int count[2], Plan *p) {
   if (E < 1 || Np < 1 || F < 1 || A < 1 || F + A > kMaxWidth) return false;
   if (head < A || head > kMaxWidth) return false;
-  if (ns < 1 || C < 2 || C < ns || cursor < 0 || cursor >= C) return false;
+  if (ns < 1 || C < 2 || C < ns) return false;
+  if (w ? (C < ns + 1 || w->n_windows < 1) : (cursor < 0 || cursor >= C)) return false;
   for (int k = 0; k < 2; k++) {
     const wdb_ddpg_net &n = *nets[k][0];
     if (n.n_hidden < 0 || n.n_hidden > 3) return false;
@@ -98,7 +106,7 @@ bool plan_layout(int E, int Np, int F, int A, int head, int C, int cursor, int n
   }
   p->valid = C - ns + 1;
   p->EN = (long long)E * Np;
-  p->M = p->valid * p->EN;
+  p->M = w ? w->n_windows : p->valid * p->EN;
   return p->M <= (1ll << 31);
 }
 
@@ -113,14 +121,14 @@ bool plan_smem(Plan *p, int n_buf, long long weight_floats, int grad_floats) {
   return true;
 }
 
-bool make_plan(const wdb_ddpg_update_args *u, Plan *p) {
+bool make_plan(const wdb_ddpg_update_args *u, const wdb_replay_windows *w, Plan *p) {
   if (!u) return false;
   const wdb_ddpg_net *actors[2] = {&u->actor, &u->target_actor};
   const wdb_ddpg_net *critics[2] = {&u->critic, &u->target_critic};
   const wdb_ddpg_net *const *nets[2] = {actors, critics};
   const int count[2] = {2, 2};
   if (!plan_layout(u->n_envs, u->n_agents, u->obs_dim, u->action_dim, u->action_dim,
-                   u->capacity, u->cursor, u->n_step, nets, count, p))
+                   u->capacity, u->cursor, u->n_step, w, nets, count, p))
     return false;
   return plan_smem(p, 6 + 2 * (p->L[1] - 1) + (p->L[0] - 1),
                    2ll * (p->wfloats[0] + p->wfloats[1]), p->gfloats[0] + p->gfloats[1]);
@@ -1021,6 +1029,682 @@ sac_actor_kernel(const __grid_constant__ wdb_sac_update_args U, const __grid_con
   }
 }
 
+// ---------------------------------------------------------------------------- sampled rows
+// The five passes over B sampled windows (wdb_replay_windows) instead of every window of the
+// ring: the kernels above with a different row source, M = B and no last-window rule, on the
+// same tile primitives, Plan layout and reduction.  They are separate kernels because the ring
+// kernels' machine code is pinned (tests/test_td3_cpu.py) and does not survive being
+// instantiated from a shared template.
+
+// A sampled loss row: the n-step window of agent row n (env * Np + agent) whose step 0 is at
+// physical ring slot s.
+struct Row {
+  int s;
+  long long n;
+};
+
+// The row source of the *_sampled kernels: row g = windows[g] = {s, n}, any n_step + 1
+// consecutive slots (mod C) of the ring, in any order, duplicates allowed.  slot(w, j) is the
+// physical slot of the window's step j; step n_step holds the bootstrap observation.  Unlike the
+// ring kernels' last window, every window bootstraps discounted.
+struct SampledRows {
+  const int2 *windows;
+  int C;
+  __device__ __forceinline__ Row at(long long g) const {
+    const int2 w = windows[g];
+    return {w.x, w.y};
+  }
+  __device__ __forceinline__ int slot(const Row &w, int j) const {
+    const int s = w.s + j;
+    return s >= C ? s - C : s;
+  }
+};
+
+// The n-step return of sampled window w from its bootstrap value qt: the recursion of a
+// regular window of the ring kernels in the same float32 operations, for all three algorithms'
+// argument structs.
+template <class Args>
+__device__ __forceinline__ float sampled_return(const Args &U, const Plan &P,
+                                                const SampledRows &rows, const Row &w, float qt) {
+  const int ns = U.n_step;
+  const long long EN = P.EN, E = U.n_envs, n = w.n, env = n / U.n_agents;
+  float ret = qt;
+  for (int j = ns - 1; j >= 0; j--) {
+    const int pk = rows.slot(w, j);
+    const float dk = (float)U.done[(long long)pk * E + env];
+    const float rk = U.rewards[(long long)pk * EN + n];
+    ret = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(1.0f, dk), U.gamma), ret), rk);
+  }
+  return ret;
+}
+
+// ddpg_update_kernel over sampled windows.
+__global__ void __launch_bounds__(kThreads, 1)
+ddpg_update_sampled(const __grid_constant__ wdb_ddpg_update_args U, const __grid_constant__ Plan Pg,
+                    float *partials, double *psums, const int2 *windows) {
+  extern __shared__ __align__(16) float smem[];
+  __shared__ Plan P;                           // dynamic indexing of the kernel parameter goes
+  __shared__ double s_err[kRows], s_j[kRows];  // through local memory: copy it once
+  if (threadIdx.x == 0) P = Pg;
+  __syncthreads();
+  const int tid = threadIdx.x;
+  float *Wa = smem, *Wc = Wa + P.wfloats[0], *Wta = Wc + P.wfloats[1], *Wtc = Wta + P.wfloats[0];
+  float *Ga = Wtc + P.wfloats[1], *Gc = Ga + P.gfloats[0];
+  const int g_total = P.gfloats[0] + P.gfloats[1];
+  float *XQ = Ga + ((g_total + 3) / 4) * 4;      // obs ++ actions
+  float *XJ = XQ + kTile;                      // obs ++ pi (target path: scratch)
+  float *V = XJ + kTile;                       // columns: 0 target Q, 1 Q, 2 J, 4 dQ, 8 dJ
+  float *Z = V + kTile;                        // actor head pre-activation
+  float *D0 = Z + kTile, *D1 = D0 + kTile;     // deltas (target path: obs' and scratch)
+  float *HQ = D1 + kTile;                      // critic hidden outputs, (obs, actions) path
+  float *HJ = HQ + (P.L[1] - 1) * kTile;       // critic hidden outputs, (obs, pi) path
+  float *HA = HJ + (P.L[1] - 1) * kTile;       // actor hidden outputs
+
+  load_net(Wa, U.actor, P, 0);
+  load_net(Wc, U.critic, P, 1);
+  load_net(Wta, U.target_actor, P, 0);
+  load_net(Wtc, U.target_critic, P, 1);
+  for (int e = tid; e < g_total; e += kThreads) Ga[e] = 0.0f;
+  for (int e = tid; e < P.n_buf * kTile; e += kThreads) XQ[e] = 0.0f;
+  __syncthreads();
+
+  const int F = U.obs_dim, A = U.action_dim, FA = F + A;
+  const SampledRows rows = {windows, U.capacity};
+  const long long EN = P.EN, M = P.M;
+  const float scale = U.action_scale, bias = U.action_bias;
+  const float norm_q = (float)(2.0 / (double)M);         // mse_loss backward: 2 / numel
+  const float d_j = -1.0f / (float)M;                    // -mean backward
+  double err_acc = 0.0, j_acc = 0.0;
+
+  for (long long g0 = (long long)blockIdx.x * kRows; g0 < M; g0 += (long long)gridDim.x * kRows) {
+    // ---- inputs: XQ = obs ++ actions at slot i, D0 = obs at the bootstrap slot
+    for (int e = tid; e < kRows * FA; e += kThreads) {
+      const int r = e / FA, c = e - r * FA;
+      const long long g = g0 + r;
+      float xq = 0.0f, xt = 0.0f;
+      if (g < M) {
+        const Row w = rows.at(g);
+        const long long row = (long long)rows.slot(w, 0) * EN + w.n;
+        if (c < F) {
+          xq = U.obs[row * F + c];
+          xt = U.obs[((long long)rows.slot(w, U.n_step) * EN + w.n) * F + c];
+        } else {
+          xq = U.actions[row * A + (c - F)];
+        }
+      }
+      XQ[r * kPitch + c] = xq;
+      if (c < F) D0[r * kPitch + c] = xt;
+    }
+    __syncthreads();
+    // ---- target actor -> a' = scale * tanh(z) + bias into D0's action columns
+    net_forward(Wta, P, 0, D0,
+                [&](int l) { return l == P.L[0] - 1 ? Z : (l % 2 == 0 ? D1 : XJ); });
+    for (int e = tid; e < kRows * A; e += kThreads) {
+      const int r = e / A, c = e - r * A;
+      D0[r * kPitch + F + c] = __fadd_rn(__fmul_rn(scale, tanhf(Z[r * kPitch + c])), bias);
+    }
+    __syncthreads();
+    // ---- target critic -> V[., 0]; critic on (obs, actions) -> V[., 1]; actor -> Z
+    net_forward(Wtc, P, 1, D0,
+                [&](int l) { return l == P.L[1] - 1 ? V : (l % 2 == 0 ? D1 : XJ); });
+    net_forward(Wc, P, 1, XQ,
+                [&](int l) { return l == P.L[1] - 1 ? V + 1 : HQ + l * kTile; });
+    net_forward(Wa, P, 0, XQ,
+                [&](int l) { return l == P.L[0] - 1 ? Z : HA + l * kTile; });
+    // ---- critic on (obs, pi) -> V[., 2]
+    for (int e = tid; e < kRows * FA; e += kThreads) {
+      const int r = e / FA, c = e - r * FA;
+      XJ[r * kPitch + c] = c < F ? XQ[r * kPitch + c]
+                                 : __fadd_rn(__fmul_rn(scale, tanhf(Z[r * kPitch + c - F])), bias);
+    }
+    __syncthreads();
+    net_forward(Wc, P, 1, XJ,
+                [&](int l) { return l == P.L[1] - 1 ? V + 2 : HJ + l * kTile; });
+    // ---- n-step return (ddpg.py:62-79, same float32 operations) and the loss gradients
+    if (tid < kRows) {
+      const int r = tid;
+      const long long g = g0 + r;
+      float dq = 0.0f, dj = 0.0f;
+      if (g < M) {
+        const float qt = V[r * kPitch], q = V[r * kPitch + 1], jv = V[r * kPitch + 2];
+        const float ret = sampled_return(U, P, rows, rows.at(g), qt);
+        const float diff = __fsub_rn(q, ret);
+        dq = __fmul_rn(diff, norm_q);
+        dj = d_j;
+        err_acc += (double)diff * (double)diff;
+        j_acc += (double)jv;
+        if (U.values) U.values[g] = q;
+        if (U.j_values) U.j_values[g] = jv;
+        if (U.returns) U.returns[g] = ret;
+      }
+      V[r * kPitch + 4] = dq;
+      V[r * kPitch + 8] = dj;
+    }
+    __syncthreads();
+    // ---- backward: critic on both paths, then the tanh head and the actor
+    net_backward(Wc, P, 1, Gc, V + 4,
+                 [&](int l) { return l == 0 ? XQ : HQ + (l - 1) * kTile; }, D0, D1, -1);
+    const float *dpi = net_backward(
+        Wc, P, 1, Gc, V + 8, [&](int l) { return l == 0 ? XJ : HJ + (l - 1) * kTile; }, D0, D1, F);
+    float *dz = dpi == D0 ? D1 : D0;
+    for (int e = tid; e < kRows * A; e += kThreads) {
+      const int r = e / A, c = e - r * A;
+      const float y = tanhf(Z[r * kPitch + c]);
+      dz[r * kPitch + c] = __fmul_rn(__fmul_rn(dpi[r * kPitch + F + c], scale),
+                                     __fsub_rn(1.0f, __fmul_rn(y, y)));
+    }
+    __syncthreads();
+    net_backward(Wa, P, 0, Ga, dz, [&](int l) { return l == 0 ? XQ : HA + (l - 1) * kTile; },
+                 D0, D1, -1);
+  }
+
+  // ---- this CTA's partials
+  float *part = partials + (long long)blockIdx.x * g_total;
+  for (int e = tid; e < g_total; e += kThreads) part[e] = Ga[e];
+  if (tid < kRows) {
+    s_err[tid] = err_acc;
+    s_j[tid] = j_acc;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    double a = 0.0, b = 0.0;
+    for (int r = 0; r < kRows; r++) {
+      a += s_err[r];
+      b += s_j[r];
+    }
+    psums[2 * blockIdx.x] = a;
+    psums[2 * blockIdx.x + 1] = b;
+  }
+}
+
+// td3_critic_kernel over sampled windows.
+__global__ void __launch_bounds__(kThreads, 1)
+td3_critic_sampled(const __grid_constant__ wdb_td3_update_args U, const __grid_constant__ Plan Pg,
+                   float *partials, double *psums, const int2 *windows) {
+  extern __shared__ __align__(16) float smem[];
+  __shared__ Plan P;
+  __shared__ double s_e1[kRows], s_e2[kRows];
+  if (threadIdx.x == 0) P = Pg;
+  __syncthreads();
+  const int tid = threadIdx.x;
+  float *Wta = smem, *Wc1 = Wta + P.wfloats[0], *Wc2 = Wc1 + P.wfloats[1];
+  float *Wt1 = Wc2 + P.wfloats[1], *Wt2 = Wt1 + P.wfloats[1];
+  float *G1 = Wt2 + P.wfloats[1], *G2 = G1 + P.gfloats[1];
+  const int g_total = 2 * P.gfloats[1];
+  float *XQ = G1 + ((g_total + 3) / 4) * 4;      // obs ++ actions
+  float *XS = XQ + kTile;                      // scratch of the target forwards
+  float *V = XS + kTile;                       // columns: 0 Q1', 1 Q2', 2 Q1, 3 Q2, 4 dQ1, 8 dQ2
+  float *Z = V + kTile;                        // target actor head pre-activation
+  float *D0 = Z + kTile, *D1 = D0 + kTile;     // deltas (target path: obs' ++ a' and scratch)
+  float *H1 = D1 + kTile;                      // Q1 hidden outputs
+  float *H2 = H1 + (P.L[1] - 1) * kTile;       // Q2 hidden outputs
+
+  load_net(Wta, U.target_actor, P, 0);
+  load_net(Wc1, U.critic, P, 1);
+  load_net(Wc2, U.critic2, P, 1);
+  load_net(Wt1, U.target_critic, P, 1);
+  load_net(Wt2, U.target_critic2, P, 1);
+  for (int e = tid; e < g_total; e += kThreads) G1[e] = 0.0f;
+  for (int e = tid; e < P.n_buf * kTile; e += kThreads) XQ[e] = 0.0f;
+  __syncthreads();
+
+  const int F = U.obs_dim, A = U.action_dim, FA = F + A;
+  const SampledRows rows = {windows, U.capacity};
+  const long long EN = P.EN, M = P.M;
+  const float scale = U.action_scale, bias = U.action_bias;
+  const float sd = __fmul_rn(U.target_noise, scale), clip = __fmul_rn(U.target_noise_clip, scale);
+  const float lo = __fsub_rn(bias, scale), hi = __fadd_rn(bias, scale);
+  const float norm_q = (float)(2.0 / (double)M);
+  double e1_acc = 0.0, e2_acc = 0.0;
+
+  for (long long g0 = (long long)blockIdx.x * kRows; g0 < M; g0 += (long long)gridDim.x * kRows) {
+    // ---- inputs: XQ = obs ++ actions at slot i, D0 = obs at the bootstrap slot
+    for (int e = tid; e < kRows * FA; e += kThreads) {
+      const int r = e / FA, c = e - r * FA;
+      const long long g = g0 + r;
+      float xq = 0.0f, xt = 0.0f;
+      if (g < M) {
+        const Row w = rows.at(g);
+        const long long row = (long long)rows.slot(w, 0) * EN + w.n;
+        if (c < F) {
+          xq = U.obs[row * F + c];
+          xt = U.obs[((long long)rows.slot(w, U.n_step) * EN + w.n) * F + c];
+        } else {
+          xq = U.actions[row * A + (c - F)];
+        }
+      }
+      XQ[r * kPitch + c] = xq;
+      if (c < F) D0[r * kPitch + c] = xt;
+    }
+    __syncthreads();
+    // ---- target actor + clipped noise -> a' into D0's action columns
+    net_forward(Wta, P, 0, D0,
+                [&](int l) { return l == P.L[0] - 1 ? Z : (l % 2 == 0 ? D1 : XS); });
+    for (int e = tid; e < kRows * A; e += kThreads) {
+      const int r = e / A, c = e - r * A;
+      const long long g = g0 + r;
+      const float pi = __fadd_rn(__fmul_rn(scale, tanhf(Z[r * kPitch + c])), bias);
+      const float eps = g < M ? U.noise[g * A + c] : 0.0f;
+      const float nz = fminf(fmaxf(__fmul_rn(eps, sd), -clip), clip);
+      D0[r * kPitch + F + c] = fminf(fmaxf(__fadd_rn(pi, nz), lo), hi);
+    }
+    __syncthreads();
+    // ---- target critics -> V[., 0], V[., 1]; critics on (obs, actions) -> V[., 2], V[., 3]
+    net_forward(Wt1, P, 1, D0,
+                [&](int l) { return l == P.L[1] - 1 ? V : (l % 2 == 0 ? D1 : XS); });
+    net_forward(Wt2, P, 1, D0,
+                [&](int l) { return l == P.L[1] - 1 ? V + 1 : (l % 2 == 0 ? D1 : XS); });
+    net_forward(Wc1, P, 1, XQ,
+                [&](int l) { return l == P.L[1] - 1 ? V + 2 : H1 + l * kTile; });
+    net_forward(Wc2, P, 1, XQ,
+                [&](int l) { return l == P.L[1] - 1 ? V + 3 : H2 + l * kTile; });
+    // ---- the n-step return from min(Q1', Q2') and the loss gradients
+    if (tid < kRows) {
+      const int r = tid;
+      const long long g = g0 + r;
+      float d1 = 0.0f, d2 = 0.0f;
+      if (g < M) {
+        const float qt = fminf(V[r * kPitch], V[r * kPitch + 1]);
+        const float q1 = V[r * kPitch + 2], q2 = V[r * kPitch + 3];
+        const float ret = sampled_return(U, P, rows, rows.at(g), qt);
+        const float e1 = __fsub_rn(q1, ret), e2 = __fsub_rn(q2, ret);
+        d1 = __fmul_rn(e1, norm_q);
+        d2 = __fmul_rn(e2, norm_q);
+        e1_acc += (double)e1 * (double)e1;
+        e2_acc += (double)e2 * (double)e2;
+        if (U.q1_values) U.q1_values[g] = q1;
+        if (U.q2_values) U.q2_values[g] = q2;
+        if (U.returns) U.returns[g] = ret;
+      }
+      V[r * kPitch + 4] = d1;
+      V[r * kPitch + 8] = d2;
+    }
+    __syncthreads();
+    // ---- backward: each critic on (obs, actions) into its own gradient block
+    net_backward(Wc1, P, 1, G1, V + 4,
+                 [&](int l) { return l == 0 ? XQ : H1 + (l - 1) * kTile; }, D0, D1, -1);
+    net_backward(Wc2, P, 1, G2, V + 8,
+                 [&](int l) { return l == 0 ? XQ : H2 + (l - 1) * kTile; }, D0, D1, -1);
+  }
+
+  float *part = partials + (long long)blockIdx.x * g_total;
+  for (int e = tid; e < g_total; e += kThreads) part[e] = G1[e];
+  if (tid < kRows) {
+    s_e1[tid] = e1_acc;
+    s_e2[tid] = e2_acc;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    double a = 0.0, b = 0.0;
+    for (int r = 0; r < kRows; r++) {
+      a += s_e1[r];
+      b += s_e2[r];
+    }
+    psums[2 * blockIdx.x] = a;
+    psums[2 * blockIdx.x + 1] = b;
+  }
+}
+
+// td3_actor_kernel over sampled windows.
+__global__ void __launch_bounds__(kThreads, 1)
+td3_actor_sampled(const __grid_constant__ wdb_td3_update_args U, const __grid_constant__ Plan Pg,
+                  float *partials, double *psums, const int2 *windows) {
+  extern __shared__ __align__(16) float smem[];
+  __shared__ Plan P;
+  __shared__ double s_j[kRows];
+  if (threadIdx.x == 0) P = Pg;
+  __syncthreads();
+  const int tid = threadIdx.x;
+  float *Wa = smem, *Wc = Wa + P.wfloats[0];
+  float *Ga = Wc + P.wfloats[1];
+  const int g_total = P.gfloats[0];
+  float *XJ = Ga + ((g_total + 3) / 4) * 4;      // obs ++ pi
+  float *V = XJ + kTile;                       // columns: 0 J, 8 dJ
+  float *Z = V + kTile;                        // actor head pre-activation
+  float *D0 = Z + kTile, *D1 = D0 + kTile;     // deltas
+  float *HJ = D1 + kTile;                      // Q1 hidden outputs on (obs, pi)
+  float *HA = HJ + (P.L[1] - 1) * kTile;       // actor hidden outputs
+
+  load_net(Wa, U.actor, P, 0);
+  load_net(Wc, U.critic, P, 1);
+  for (int e = tid; e < g_total; e += kThreads) Ga[e] = 0.0f;
+  for (int e = tid; e < P.n_buf * kTile; e += kThreads) XJ[e] = 0.0f;
+  __syncthreads();
+
+  const int F = U.obs_dim, A = U.action_dim;
+  const SampledRows rows = {windows, U.capacity};
+  const long long EN = P.EN, M = P.M;
+  const float scale = U.action_scale, bias = U.action_bias;
+  const float d_j = -1.0f / (float)M;
+  double j_acc = 0.0;
+
+  for (long long g0 = (long long)blockIdx.x * kRows; g0 < M; g0 += (long long)gridDim.x * kRows) {
+    for (int e = tid; e < kRows * F; e += kThreads) {
+      const int r = e / F, c = e - r * F;
+      const long long g = g0 + r;
+      float x = 0.0f;
+      if (g < M) {
+        const Row w = rows.at(g);
+        x = U.obs[((long long)rows.slot(w, 0) * EN + w.n) * F + c];
+      }
+      XJ[r * kPitch + c] = x;
+    }
+    __syncthreads();
+    // ---- actor -> pi into XJ's action columns; Q1 on (obs, pi) -> V[., 0]
+    net_forward(Wa, P, 0, XJ, [&](int l) { return l == P.L[0] - 1 ? Z : HA + l * kTile; });
+    for (int e = tid; e < kRows * A; e += kThreads) {
+      const int r = e / A, c = e - r * A;
+      XJ[r * kPitch + F + c] = __fadd_rn(__fmul_rn(scale, tanhf(Z[r * kPitch + c])), bias);
+    }
+    __syncthreads();
+    net_forward(Wc, P, 1, XJ, [&](int l) { return l == P.L[1] - 1 ? V : HJ + l * kTile; });
+    if (tid < kRows) {
+      const int r = tid;
+      const long long g = g0 + r;
+      float dj = 0.0f;
+      if (g < M) {
+        const float jv = V[r * kPitch];
+        dj = d_j;
+        j_acc += (double)jv;
+        if (U.j_values) U.j_values[g] = jv;
+      }
+      V[r * kPitch + 8] = dj;
+    }
+    __syncthreads();
+    // ---- backward: Q1 to its action inputs, the tanh head, the actor
+    const float *dpi = net_backward<false>(
+        Wc, P, 1, nullptr, V + 8, [&](int l) { return l == 0 ? XJ : HJ + (l - 1) * kTile; },
+        D0, D1, F);
+    float *dz = dpi == D0 ? D1 : D0;
+    for (int e = tid; e < kRows * A; e += kThreads) {
+      const int r = e / A, c = e - r * A;
+      const float y = tanhf(Z[r * kPitch + c]);
+      dz[r * kPitch + c] = __fmul_rn(__fmul_rn(dpi[r * kPitch + F + c], scale),
+                                     __fsub_rn(1.0f, __fmul_rn(y, y)));
+    }
+    __syncthreads();
+    net_backward(Wa, P, 0, Ga, dz, [&](int l) { return l == 0 ? XJ : HA + (l - 1) * kTile; },
+                 D0, D1, -1);
+  }
+
+  float *part = partials + (long long)blockIdx.x * g_total;
+  for (int e = tid; e < g_total; e += kThreads) part[e] = Ga[e];
+  if (tid < kRows) s_j[tid] = j_acc;
+  __syncthreads();
+  if (tid == 0) {
+    double a = 0.0;
+    for (int r = 0; r < kRows; r++) a += s_j[r];
+    psums[2 * blockIdx.x] = a;
+    psums[2 * blockIdx.x + 1] = 0.0;
+  }
+}
+
+// sac_critic_kernel over sampled windows.
+__global__ void __launch_bounds__(kThreads, 1)
+sac_critic_sampled(const __grid_constant__ wdb_sac_update_args U, const __grid_constant__ Plan Pg,
+                   float *partials, double *psums, const int2 *windows) {
+  extern __shared__ __align__(16) float smem[];
+  __shared__ Plan P;
+  __shared__ double s_e1[kRows], s_e2[kRows];
+  if (threadIdx.x == 0) P = Pg;
+  __syncthreads();
+  const int tid = threadIdx.x;
+  float *Wa = smem, *Wc1 = Wa + P.wfloats[0], *Wc2 = Wc1 + P.wfloats[1];
+  float *Wt1 = Wc2 + P.wfloats[1], *Wt2 = Wt1 + P.wfloats[1];
+  float *G1 = Wt2 + P.wfloats[1], *G2 = G1 + P.gfloats[1];
+  const int g_total = 2 * P.gfloats[1];
+  float *XQ = G1 + ((g_total + 3) / 4) * 4;      // obs ++ actions
+  float *XS = XQ + kTile;                      // scratch of the bootstrap forwards
+  float *V = XS + kTile;                       // columns: 0 Q1', 1 Q2', 2 Q1, 3 Q2, 4 dQ1, 8 dQ2
+  float *Z = V + kTile;                        // actor head on obs'; then [0, A): log-prob terms
+  float *D0 = Z + kTile, *D1 = D0 + kTile;     // deltas (bootstrap path: obs' ++ a' and scratch)
+  float *H1 = D1 + kTile;                      // Q1 hidden outputs
+  float *H2 = H1 + (P.L[1] - 1) * kTile;       // Q2 hidden outputs
+
+  load_net(Wa, U.actor, P, 0);
+  load_net(Wc1, U.critic, P, 1);
+  load_net(Wc2, U.critic2, P, 1);
+  load_net(Wt1, U.target_critic, P, 1);
+  load_net(Wt2, U.target_critic2, P, 1);
+  for (int e = tid; e < g_total; e += kThreads) G1[e] = 0.0f;
+  for (int e = tid; e < P.n_buf * kTile; e += kThreads) XQ[e] = 0.0f;
+  __syncthreads();
+
+  const int F = U.obs_dim, A = U.action_dim, FA = F + A;
+  const SampledRows rows = {windows, U.capacity};
+  const long long EN = P.EN, M = P.M;
+  const float scale = U.action_scale, bias = U.action_bias;
+  const float lo = U.log_std_min, hi = U.log_std_max;
+  const float alpha = expf(*U.log_alpha);
+  const float norm_q = (float)(2.0 / (double)M);
+  double e1_acc = 0.0, e2_acc = 0.0;
+
+  for (long long g0 = (long long)blockIdx.x * kRows; g0 < M; g0 += (long long)gridDim.x * kRows) {
+    // ---- inputs: XQ = obs ++ actions at slot i, D0 = obs at the bootstrap slot
+    for (int e = tid; e < kRows * FA; e += kThreads) {
+      const int r = e / FA, c = e - r * FA;
+      const long long g = g0 + r;
+      float xq = 0.0f, xt = 0.0f;
+      if (g < M) {
+        const Row w = rows.at(g);
+        const long long row = (long long)rows.slot(w, 0) * EN + w.n;
+        if (c < F) {
+          xq = U.obs[row * F + c];
+          xt = U.obs[((long long)rows.slot(w, U.n_step) * EN + w.n) * F + c];
+        } else {
+          xq = U.actions[row * A + (c - F)];
+        }
+      }
+      XQ[r * kPitch + c] = xq;
+      if (c < F) D0[r * kPitch + c] = xt;
+    }
+    __syncthreads();
+    // ---- actor on obs' -> a' ~ pi(. | obs') into D0's action columns, log-prob terms into Z
+    net_forward(Wa, P, 0, D0,
+                [&](int l) { return l == P.L[0] - 1 ? Z : (l % 2 == 0 ? D1 : XS); });
+    for (int e = tid; e < kRows * A; e += kThreads) {
+      const int r = e / A, c = e - r * A;
+      const long long g = g0 + r;
+      const float eps = g < M ? U.critic_noise[g * A + c] : 0.0f;
+      const SquashedDim s = squashed_dim(Z + r * kPitch, A, c, eps, lo, hi);
+      D0[r * kPitch + F + c] = __fadd_rn(__fmul_rn(scale, s.y), bias);
+      Z[r * kPitch + c] = s.term;
+    }
+    __syncthreads();
+    // ---- target critics -> V[., 0], V[., 1]; critics on (obs, actions) -> V[., 2], V[., 3]
+    net_forward(Wt1, P, 1, D0,
+                [&](int l) { return l == P.L[1] - 1 ? V : (l % 2 == 0 ? D1 : XS); });
+    net_forward(Wt2, P, 1, D0,
+                [&](int l) { return l == P.L[1] - 1 ? V + 1 : (l % 2 == 0 ? D1 : XS); });
+    net_forward(Wc1, P, 1, XQ,
+                [&](int l) { return l == P.L[1] - 1 ? V + 2 : H1 + l * kTile; });
+    net_forward(Wc2, P, 1, XQ,
+                [&](int l) { return l == P.L[1] - 1 ? V + 3 : H2 + l * kTile; });
+    // ---- the n-step return from min(Q1', Q2') - alpha log pi' and the loss gradients
+    if (tid < kRows) {
+      const int r = tid;
+      const long long g = g0 + r;
+      float d1 = 0.0f, d2 = 0.0f;
+      if (g < M) {
+        float lp = 0.0f;
+        for (int c = 0; c < A; c++) lp += Z[r * kPitch + c];
+        const float qt = __fsub_rn(fminf(V[r * kPitch], V[r * kPitch + 1]), __fmul_rn(alpha, lp));
+        const float q1 = V[r * kPitch + 2], q2 = V[r * kPitch + 3];
+        const float ret = sampled_return(U, P, rows, rows.at(g), qt);
+        const float e1 = __fsub_rn(q1, ret), e2 = __fsub_rn(q2, ret);
+        d1 = __fmul_rn(e1, norm_q);
+        d2 = __fmul_rn(e2, norm_q);
+        e1_acc += (double)e1 * (double)e1;
+        e2_acc += (double)e2 * (double)e2;
+        if (U.q1_values) U.q1_values[g] = q1;
+        if (U.q2_values) U.q2_values[g] = q2;
+        if (U.returns) U.returns[g] = ret;
+      }
+      V[r * kPitch + 4] = d1;
+      V[r * kPitch + 8] = d2;
+    }
+    __syncthreads();
+    // ---- backward: each critic on (obs, actions) into its own gradient block
+    net_backward(Wc1, P, 1, G1, V + 4,
+                 [&](int l) { return l == 0 ? XQ : H1 + (l - 1) * kTile; }, D0, D1, -1);
+    net_backward(Wc2, P, 1, G2, V + 8,
+                 [&](int l) { return l == 0 ? XQ : H2 + (l - 1) * kTile; }, D0, D1, -1);
+  }
+
+  float *part = partials + (long long)blockIdx.x * g_total;
+  for (int e = tid; e < g_total; e += kThreads) part[e] = G1[e];
+  if (tid < kRows) {
+    s_e1[tid] = e1_acc;
+    s_e2[tid] = e2_acc;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    double a = 0.0, b = 0.0;
+    for (int r = 0; r < kRows; r++) {
+      a += s_e1[r];
+      b += s_e2[r];
+    }
+    psums[2 * blockIdx.x] = a;
+    psums[2 * blockIdx.x + 1] = b;
+  }
+}
+
+// sac_actor_kernel over sampled windows.
+__global__ void __launch_bounds__(kThreads, 1)
+sac_actor_sampled(const __grid_constant__ wdb_sac_update_args U, const __grid_constant__ Plan Pg,
+                  float *partials, double *psums, const int2 *windows) {
+  extern __shared__ __align__(16) float smem[];
+  __shared__ Plan P;
+  __shared__ double s_q[kRows], s_lp[kRows];
+  if (threadIdx.x == 0) P = Pg;
+  __syncthreads();
+  const int tid = threadIdx.x;
+  float *Wa = smem, *Wc1 = Wa + P.wfloats[0], *Wc2 = Wc1 + P.wfloats[1];
+  float *Ga = Wc2 + P.wfloats[1];
+  const int g_total = P.gfloats[0];
+  float *XJ = Ga + ((g_total + 3) / 4) * 4;      // obs ++ a
+  float *V = XJ + kTile;                       // columns: 0 Q1, 1 Q2, 8 dQ1, 12 dQ2
+  float *Z = V + kTile;                        // actor head: mu ++ raw log-std
+  float *D0 = Z + kTile, *D1 = D0 + kTile;     // deltas
+  float *DA = D1 + kTile;                      // log-prob terms, then Q1's action gradient
+  float *H1 = DA + kTile;                      // Q1 hidden outputs on (obs, a)
+  float *H2 = H1 + (P.L[1] - 1) * kTile;       // Q2 hidden outputs on (obs, a)
+  float *HA = H2 + (P.L[1] - 1) * kTile;       // actor hidden outputs
+
+  load_net(Wa, U.actor, P, 0);
+  load_net(Wc1, U.critic, P, 1);
+  load_net(Wc2, U.critic2, P, 1);
+  for (int e = tid; e < g_total; e += kThreads) Ga[e] = 0.0f;
+  for (int e = tid; e < P.n_buf * kTile; e += kThreads) XJ[e] = 0.0f;
+  __syncthreads();
+
+  const int F = U.obs_dim, A = U.action_dim;
+  const SampledRows rows = {windows, U.capacity};
+  const long long EN = P.EN, M = P.M;
+  const float scale = U.action_scale, bias = U.action_bias;
+  const float lo = U.log_std_min, hi = U.log_std_max;
+  const float alpha = expf(*U.log_alpha);
+  const float d_q = -1.0f / (float)M;                    // d loss / d min(Q1, Q2)
+  const float d_lp = alpha / (float)M;                   // d loss / d log pi
+  double q_acc = 0.0, lp_acc = 0.0;
+
+  for (long long g0 = (long long)blockIdx.x * kRows; g0 < M; g0 += (long long)gridDim.x * kRows) {
+    for (int e = tid; e < kRows * F; e += kThreads) {
+      const int r = e / F, c = e - r * F;
+      const long long g = g0 + r;
+      float x = 0.0f;
+      if (g < M) {
+        const Row w = rows.at(g);
+        x = U.obs[((long long)rows.slot(w, 0) * EN + w.n) * F + c];
+      }
+      XJ[r * kPitch + c] = x;
+    }
+    __syncthreads();
+    // ---- actor -> a into XJ's action columns (log-prob terms into DA); Q1, Q2 on (obs, a)
+    net_forward(Wa, P, 0, XJ, [&](int l) { return l == P.L[0] - 1 ? Z : HA + l * kTile; });
+    for (int e = tid; e < kRows * A; e += kThreads) {
+      const int r = e / A, c = e - r * A;
+      const long long g = g0 + r;
+      const float eps = g < M ? U.actor_noise[g * A + c] : 0.0f;
+      const SquashedDim s = squashed_dim(Z + r * kPitch, A, c, eps, lo, hi);
+      XJ[r * kPitch + F + c] = __fadd_rn(__fmul_rn(scale, s.y), bias);
+      DA[r * kPitch + c] = s.term;
+    }
+    __syncthreads();
+    net_forward(Wc1, P, 1, XJ, [&](int l) { return l == P.L[1] - 1 ? V : H1 + l * kTile; });
+    net_forward(Wc2, P, 1, XJ, [&](int l) { return l == P.L[1] - 1 ? V + 1 : H2 + l * kTile; });
+    if (tid < kRows) {
+      const int r = tid;
+      const long long g = g0 + r;
+      float d1 = 0.0f, d2 = 0.0f;
+      if (g < M) {
+        const float q1 = V[r * kPitch], q2 = V[r * kPitch + 1];
+        const bool first = q1 <= q2;
+        float lp = 0.0f;
+        for (int c = 0; c < A; c++) lp += DA[r * kPitch + c];
+        d1 = first ? d_q : 0.0f;
+        d2 = first ? 0.0f : d_q;
+        q_acc += (double)(first ? q1 : q2);
+        lp_acc += (double)lp;
+        if (U.log_probs) U.log_probs[g] = lp;
+      }
+      V[r * kPitch + 8] = d1;
+      V[r * kPitch + 12] = d2;
+    }
+    __syncthreads();
+    // ---- backward: Q1 to its action inputs (kept in DA), Q2 likewise
+    const float *da1 = net_backward<false>(
+        Wc1, P, 1, nullptr, V + 8, [&](int l) { return l == 0 ? XJ : H1 + (l - 1) * kTile; },
+        D0, D1, F);
+    for (int e = tid; e < kRows * A; e += kThreads) {
+      const int r = e / A, c = e - r * A;
+      DA[r * kPitch + c] = da1[r * kPitch + F + c];
+    }
+    __syncthreads();
+    const float *da2 = net_backward<false>(
+        Wc2, P, 1, nullptr, V + 12, [&](int l) { return l == 0 ? XJ : H2 + (l - 1) * kTile; },
+        D0, D1, F);
+    // ---- the tanh, the reparameterisation, the log-prob's own terms and the clamp
+    float *dz = da2 == D0 ? D1 : D0;
+    for (int e = tid; e < kRows * A; e += kThreads) {
+      const int r = e / A, c = e - r * A;
+      const long long g = g0 + r;
+      float dmu = 0.0f, dls = 0.0f;
+      if (g < M) {
+        const float eps = U.actor_noise[g * A + c];
+        const SquashedDim s = squashed_dim(Z + r * kPitch, A, c, eps, lo, hi);
+        const float da = __fadd_rn(DA[r * kPitch + c], da2[r * kPitch + F + c]);
+        const float du = fmaf(__fmul_rn(da, scale), __fsub_rn(1.0f, __fmul_rn(s.y, s.y)),
+                              __fmul_rn(d_lp, 2.0f * s.y));
+        dmu = du;
+        dls = s.in_range ? fmaf(__fmul_rn(du, s.sigma), eps, -d_lp) : 0.0f;
+      }
+      dz[r * kPitch + c] = dmu;
+      dz[r * kPitch + A + c] = dls;
+    }
+    __syncthreads();
+    net_backward(Wa, P, 0, Ga, dz, [&](int l) { return l == 0 ? XJ : HA + (l - 1) * kTile; },
+                 D0, D1, -1);
+  }
+
+  float *part = partials + (long long)blockIdx.x * g_total;
+  for (int e = tid; e < g_total; e += kThreads) part[e] = Ga[e];
+  if (tid < kRows) {
+    s_q[tid] = q_acc;
+    s_lp[tid] = lp_acc;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    double a = 0.0, b = 0.0;
+    for (int r = 0; r < kRows; r++) {
+      a += s_q[r];
+      b += s_lp[r];
+    }
+    psums[2 * blockIdx.x] = a;
+    psums[2 * blockIdx.x + 1] = b;
+  }
+}
+
 // ---------------------------------------------------------------------------- host side
 long long workspace_bytes(const Plan &P) {
   return 16ll * P.grid + 4ll * P.grid * (P.gfloats[0] + P.gfloats[1]);
@@ -1062,7 +1746,8 @@ int launch_reduce(void *stream, const Reduce &R, int widest, const float *partia
 // TD3's plan of one pass: the actor shape (actor, target actor) and the critic shape (both
 // critics and their targets) as in DDPG; the critic pass holds the target actor, four critics
 // and both critic gradient blocks, the actor pass the actor, Q1 and the actor gradients.
-bool td3_plan(const wdb_td3_update_args *u, bool actor_pass, Plan *p) {
+bool td3_plan(const wdb_td3_update_args *u, const wdb_replay_windows *w, bool actor_pass,
+              Plan *p) {
   if (!u) return false;
   if (!(u->target_noise >= 0.0f) || !(u->target_noise_clip >= 0.0f)) return false;
   const wdb_ddpg_net *actors[2] = {&u->actor, &u->target_actor};
@@ -1071,7 +1756,7 @@ bool td3_plan(const wdb_td3_update_args *u, bool actor_pass, Plan *p) {
   const wdb_ddpg_net *const *nets[2] = {actors, critics};
   const int count[2] = {2, 4};
   if (!plan_layout(u->n_envs, u->n_agents, u->obs_dim, u->action_dim, u->action_dim,
-                   u->capacity, u->cursor, u->n_step, nets, count, p))
+                   u->capacity, u->cursor, u->n_step, w, nets, count, p))
     return false;
   if (actor_pass)
     return plan_smem(p, 5 + (p->L[1] - 1) + (p->L[0] - 1), p->wfloats[0] + p->wfloats[1],
@@ -1102,121 +1787,11 @@ bool nets_ok(const wdb_ddpg_update_args *u, const Plan &P) {
   return true;
 }
 
-}  // namespace
-
-WDB_API int wdb_ddpg_update_supported(const wdb_ddpg_update_args *update) {
-  Plan P;
-  return make_plan(update, &P) ? 1 : 0;
-}
-
-WDB_API long long wdb_ddpg_update_workspace_bytes(const wdb_ddpg_update_args *update) {
-  Plan P;
-  return make_plan(update, &P) ? workspace_bytes(P) : -1;
-}
-
-WDB_API int wdb_ddpg_update(void *stream, const wdb_ddpg_update_args *u) {
-  Plan P;
-  if (!make_plan(u, &P) || !nets_ok(u, P)) return (int)cudaErrorInvalidValue;
-  if (!u->obs || !u->actions || !u->rewards || !u->done || !u->workspace)
-    return (int)cudaErrorInvalidValue;
-  const size_t smem = (size_t)P.smem_floats * sizeof(float);
-  static size_t configured = 0;
-  int rc = allow_smem((const void *)ddpg_update_kernel, smem, &configured);
-  if (rc != cudaSuccess) return rc;
-  double *psums = static_cast<double *>(u->workspace);
-  float *partials = reinterpret_cast<float *>(psums + 2 * P.grid);
-  ddpg_update_kernel<<<P.grid, kThreads, smem, as_stream(stream)>>>(*u, P, partials, psums);
-  rc = finish_launch();
-  if (rc != cudaSuccess) return rc;
-
-  Reduce R = {};
-  R.grid = P.grid;
-  R.g_total = P.gfloats[0] + P.gfloats[1];
-  int widest = 1;
-  add_segments(&R, P, 0, 0, u->actor, &widest);
-  add_segments(&R, P, 1, P.gfloats[0], u->critic, &widest);
-  return launch_reduce(stream, R, widest, partials, psums, u->sums);
-}
-
-WDB_API int wdb_td3_critic_update_supported(const wdb_td3_update_args *update) {
-  Plan P;
-  return td3_plan(update, false, &P) ? 1 : 0;
-}
-
-WDB_API long long wdb_td3_critic_update_workspace_bytes(const wdb_td3_update_args *update) {
-  Plan P;
-  return td3_plan(update, false, &P) ? td3_workspace_bytes(P, false) : -1;
-}
-
-WDB_API int wdb_td3_critic_update(void *stream, const wdb_td3_update_args *u) {
-  Plan P;
-  if (!td3_plan(u, false, &P)) return (int)cudaErrorInvalidValue;
-  if (!net_ok(u->target_actor, P.L[0], false) || !net_ok(u->critic, P.L[1], true) ||
-      !net_ok(u->critic2, P.L[1], true) || !net_ok(u->target_critic, P.L[1], false) ||
-      !net_ok(u->target_critic2, P.L[1], false))
-    return (int)cudaErrorInvalidValue;
-  if (!u->obs || !u->actions || !u->rewards || !u->done || !u->noise || !u->workspace)
-    return (int)cudaErrorInvalidValue;
-  const size_t smem = (size_t)P.smem_floats * sizeof(float);
-  static size_t configured = 0;
-  int rc = allow_smem((const void *)td3_critic_kernel, smem, &configured);
-  if (rc != cudaSuccess) return rc;
-  double *psums = static_cast<double *>(u->workspace);
-  float *partials = reinterpret_cast<float *>(psums + 2 * P.grid);
-  td3_critic_kernel<<<P.grid, kThreads, smem, as_stream(stream)>>>(*u, P, partials, psums);
-  rc = finish_launch();
-  if (rc != cudaSuccess) return rc;
-
-  Reduce R = {};
-  R.grid = P.grid;
-  R.g_total = 2 * P.gfloats[1];
-  int widest = 1;
-  add_segments(&R, P, 1, 0, u->critic, &widest);
-  add_segments(&R, P, 1, P.gfloats[1], u->critic2, &widest);
-  return launch_reduce(stream, R, widest, partials, psums, u->sums);
-}
-
-WDB_API int wdb_td3_actor_update_supported(const wdb_td3_update_args *update) {
-  Plan P;
-  return td3_plan(update, true, &P) ? 1 : 0;
-}
-
-WDB_API long long wdb_td3_actor_update_workspace_bytes(const wdb_td3_update_args *update) {
-  Plan P;
-  return td3_plan(update, true, &P) ? td3_workspace_bytes(P, true) : -1;
-}
-
-WDB_API int wdb_td3_actor_update(void *stream, const wdb_td3_update_args *u) {
-  Plan P;
-  if (!td3_plan(u, true, &P)) return (int)cudaErrorInvalidValue;
-  if (!net_ok(u->actor, P.L[0], true) || !net_ok(u->critic, P.L[1], false))
-    return (int)cudaErrorInvalidValue;
-  if (!u->obs || !u->workspace) return (int)cudaErrorInvalidValue;
-  const size_t smem = (size_t)P.smem_floats * sizeof(float);
-  static size_t configured = 0;
-  int rc = allow_smem((const void *)td3_actor_kernel, smem, &configured);
-  if (rc != cudaSuccess) return rc;
-  double *psums = static_cast<double *>(u->workspace);
-  float *partials = reinterpret_cast<float *>(psums + 2 * P.grid);
-  td3_actor_kernel<<<P.grid, kThreads, smem, as_stream(stream)>>>(*u, P, partials, psums);
-  rc = finish_launch();
-  if (rc != cudaSuccess) return rc;
-
-  Reduce R = {};
-  R.grid = P.grid;
-  R.g_total = P.gfloats[0];
-  int widest = 1;
-  add_segments(&R, P, 0, 0, u->actor, &widest);
-  return launch_reduce(stream, R, widest, partials, psums, u->sums ? u->sums + 2 : nullptr);
-}
-
-// ---------------------------------------------------------------------------- SAC host side
-namespace {
-
 // SAC's plan of one pass: the actor shape (head 2A) and the critic shape (both critics and
 // their targets); the critic pass holds the actor, four critics and both critic gradient
 // blocks, the actor pass the actor, both critics and the actor gradients.
-bool sac_plan(const wdb_sac_update_args *u, bool actor_pass, Plan *p) {
+bool sac_plan(const wdb_sac_update_args *u, const wdb_replay_windows *w, bool actor_pass,
+              Plan *p) {
   if (!u) return false;
   if (!(u->log_std_min <= u->log_std_max)) return false;
   const wdb_ddpg_net *actors[1] = {&u->actor};
@@ -1225,7 +1800,7 @@ bool sac_plan(const wdb_sac_update_args *u, bool actor_pass, Plan *p) {
   const wdb_ddpg_net *const *nets[2] = {actors, critics};
   const int count[2] = {1, 4};
   if (!plan_layout(u->n_envs, u->n_agents, u->obs_dim, u->action_dim, 2 * u->action_dim,
-                   u->capacity, u->cursor, u->n_step, nets, count, p))
+                   u->capacity, u->cursor, u->n_step, w, nets, count, p))
     return false;
   if (actor_pass)
     return plan_smem(p, 6 + 2 * (p->L[1] - 1) + (p->L[0] - 1),
@@ -1234,79 +1809,163 @@ bool sac_plan(const wdb_sac_update_args *u, bool actor_pass, Plan *p) {
                    2 * p->gfloats[1]);
 }
 
-}  // namespace
 
-WDB_API int wdb_sac_critic_update_supported(const wdb_sac_update_args *update) {
-  Plan P;
-  return sac_plan(update, false, &P) ? 1 : 0;
-}
-
-WDB_API long long wdb_sac_critic_update_workspace_bytes(const wdb_sac_update_args *update) {
-  Plan P;
-  return sac_plan(update, false, &P) ? td3_workspace_bytes(P, false) : -1;
-}
-
-WDB_API int wdb_sac_critic_update(void *stream, const wdb_sac_update_args *u) {
-  Plan P;
-  if (!sac_plan(u, false, &P)) return (int)cudaErrorInvalidValue;
-  if (!net_ok(u->actor, P.L[0], false) || !net_ok(u->critic, P.L[1], true) ||
-      !net_ok(u->critic2, P.L[1], true) || !net_ok(u->target_critic, P.L[1], false) ||
-      !net_ok(u->target_critic2, P.L[1], false))
-    return (int)cudaErrorInvalidValue;
-  if (!u->obs || !u->actions || !u->rewards || !u->done || !u->critic_noise || !u->log_alpha ||
-      !u->workspace)
-    return (int)cudaErrorInvalidValue;
+// Launches one pass (`ring` over every window of the ring, or `sampled` over w's windows) and
+// the reduction R of its per-CTA partials into the gradient arena and `sums`.
+template <class Args>
+int launch_pass(void *stream, const Args *u, const Plan &P, const wdb_replay_windows *w,
+                void (*ring)(const Args, const Plan, float *, double *),
+                void (*sampled)(const Args, const Plan, float *, double *, const int2 *),
+                size_t *configured, Reduce *R, int widest, double *sums) {
+  if (!u->workspace || (w && !w->windows)) return (int)cudaErrorInvalidValue;
   const size_t smem = (size_t)P.smem_floats * sizeof(float);
-  static size_t configured = 0;
-  int rc = allow_smem((const void *)sac_critic_kernel, smem, &configured);
+  int rc = allow_smem(w ? (const void *)sampled : (const void *)ring, smem,
+                      &configured[w ? 1 : 0]);
   if (rc != cudaSuccess) return rc;
   double *psums = static_cast<double *>(u->workspace);
   float *partials = reinterpret_cast<float *>(psums + 2 * P.grid);
-  sac_critic_kernel<<<P.grid, kThreads, smem, as_stream(stream)>>>(*u, P, partials, psums);
+  if (w)
+    sampled<<<P.grid, kThreads, smem, as_stream(stream)>>>(
+        *u, P, partials, psums, reinterpret_cast<const int2 *>(w->windows));
+  else
+    ring<<<P.grid, kThreads, smem, as_stream(stream)>>>(*u, P, partials, psums);
   rc = finish_launch();
   if (rc != cudaSuccess) return rc;
+  R->grid = P.grid;
+  return launch_reduce(stream, *R, widest, partials, psums, sums);
+}
 
+int ddpg_update(void *stream, const wdb_ddpg_update_args *u, const wdb_replay_windows *w) {
+  Plan P;
+  if (!make_plan(u, w, &P) || !nets_ok(u, P)) return (int)cudaErrorInvalidValue;
+  if (!u->obs || !u->actions || !u->rewards || !u->done) return (int)cudaErrorInvalidValue;
   Reduce R = {};
-  R.grid = P.grid;
+  R.g_total = P.gfloats[0] + P.gfloats[1];
+  int widest = 1;
+  add_segments(&R, P, 0, 0, u->actor, &widest);
+  add_segments(&R, P, 1, P.gfloats[0], u->critic, &widest);
+  static size_t configured[2] = {0, 0};
+  return launch_pass(stream, u, P, w, ddpg_update_kernel, ddpg_update_sampled, configured, &R,
+                     widest, u->sums);
+}
+
+int td3_critic_update(void *stream, const wdb_td3_update_args *u, const wdb_replay_windows *w) {
+  Plan P;
+  if (!td3_plan(u, w, false, &P)) return (int)cudaErrorInvalidValue;
+  if (!net_ok(u->target_actor, P.L[0], false) || !net_ok(u->critic, P.L[1], true) ||
+      !net_ok(u->critic2, P.L[1], true) || !net_ok(u->target_critic, P.L[1], false) ||
+      !net_ok(u->target_critic2, P.L[1], false))
+    return (int)cudaErrorInvalidValue;
+  if (!u->obs || !u->actions || !u->rewards || !u->done || !u->noise)
+    return (int)cudaErrorInvalidValue;
+  Reduce R = {};
   R.g_total = 2 * P.gfloats[1];
   int widest = 1;
   add_segments(&R, P, 1, 0, u->critic, &widest);
   add_segments(&R, P, 1, P.gfloats[1], u->critic2, &widest);
-  return launch_reduce(stream, R, widest, partials, psums, u->sums);
+  static size_t configured[2] = {0, 0};
+  return launch_pass(stream, u, P, w, td3_critic_kernel, td3_critic_sampled, configured, &R,
+                     widest, u->sums);
 }
 
-WDB_API int wdb_sac_actor_update_supported(const wdb_sac_update_args *update) {
+int td3_actor_update(void *stream, const wdb_td3_update_args *u, const wdb_replay_windows *w) {
   Plan P;
-  return sac_plan(update, true, &P) ? 1 : 0;
-}
-
-WDB_API long long wdb_sac_actor_update_workspace_bytes(const wdb_sac_update_args *update) {
-  Plan P;
-  return sac_plan(update, true, &P) ? td3_workspace_bytes(P, true) : -1;
-}
-
-WDB_API int wdb_sac_actor_update(void *stream, const wdb_sac_update_args *u) {
-  Plan P;
-  if (!sac_plan(u, true, &P)) return (int)cudaErrorInvalidValue;
-  if (!net_ok(u->actor, P.L[0], true) || !net_ok(u->critic, P.L[1], false) ||
-      !net_ok(u->critic2, P.L[1], false))
+  if (!td3_plan(u, w, true, &P)) return (int)cudaErrorInvalidValue;
+  if (!net_ok(u->actor, P.L[0], true) || !net_ok(u->critic, P.L[1], false))
     return (int)cudaErrorInvalidValue;
-  if (!u->obs || !u->actor_noise || !u->log_alpha || !u->workspace)
-    return (int)cudaErrorInvalidValue;
-  const size_t smem = (size_t)P.smem_floats * sizeof(float);
-  static size_t configured = 0;
-  int rc = allow_smem((const void *)sac_actor_kernel, smem, &configured);
-  if (rc != cudaSuccess) return rc;
-  double *psums = static_cast<double *>(u->workspace);
-  float *partials = reinterpret_cast<float *>(psums + 2 * P.grid);
-  sac_actor_kernel<<<P.grid, kThreads, smem, as_stream(stream)>>>(*u, P, partials, psums);
-  rc = finish_launch();
-  if (rc != cudaSuccess) return rc;
-
+  if (!u->obs) return (int)cudaErrorInvalidValue;
   Reduce R = {};
-  R.grid = P.grid;
   R.g_total = P.gfloats[0];
   int widest = 1;
   add_segments(&R, P, 0, 0, u->actor, &widest);
-  return launch_reduce(stream, R, widest, partials, psums, u->sums ? u->sums + 2 : nullptr);
+  static size_t configured[2] = {0, 0};
+  return launch_pass(stream, u, P, w, td3_actor_kernel, td3_actor_sampled, configured, &R,
+                     widest, u->sums ? u->sums + 2 : nullptr);
 }
+
+int sac_critic_update(void *stream, const wdb_sac_update_args *u, const wdb_replay_windows *w) {
+  Plan P;
+  if (!sac_plan(u, w, false, &P)) return (int)cudaErrorInvalidValue;
+  if (!net_ok(u->actor, P.L[0], false) || !net_ok(u->critic, P.L[1], true) ||
+      !net_ok(u->critic2, P.L[1], true) || !net_ok(u->target_critic, P.L[1], false) ||
+      !net_ok(u->target_critic2, P.L[1], false))
+    return (int)cudaErrorInvalidValue;
+  if (!u->obs || !u->actions || !u->rewards || !u->done || !u->critic_noise || !u->log_alpha)
+    return (int)cudaErrorInvalidValue;
+  Reduce R = {};
+  R.g_total = 2 * P.gfloats[1];
+  int widest = 1;
+  add_segments(&R, P, 1, 0, u->critic, &widest);
+  add_segments(&R, P, 1, P.gfloats[1], u->critic2, &widest);
+  static size_t configured[2] = {0, 0};
+  return launch_pass(stream, u, P, w, sac_critic_kernel, sac_critic_sampled, configured, &R,
+                     widest, u->sums);
+}
+
+int sac_actor_update(void *stream, const wdb_sac_update_args *u, const wdb_replay_windows *w) {
+  Plan P;
+  if (!sac_plan(u, w, true, &P)) return (int)cudaErrorInvalidValue;
+  if (!net_ok(u->actor, P.L[0], true) || !net_ok(u->critic, P.L[1], false) ||
+      !net_ok(u->critic2, P.L[1], false))
+    return (int)cudaErrorInvalidValue;
+  if (!u->obs || !u->actor_noise || !u->log_alpha) return (int)cudaErrorInvalidValue;
+  Reduce R = {};
+  R.g_total = P.gfloats[0];
+  int widest = 1;
+  add_segments(&R, P, 0, 0, u->actor, &widest);
+  static size_t configured[2] = {0, 0};
+  return launch_pass(stream, u, P, w, sac_actor_kernel, sac_actor_sampled, configured, &R,
+                     widest, u->sums ? u->sums + 2 : nullptr);
+}
+
+}  // namespace
+
+// ---------------------------------------------------------------------------- entry points
+// Each pass has a ring form and a _sampled form; the latter's _supported / _workspace_bytes
+// take the number of windows B.
+#define WDB_PASS_API(name, Args, plan, bytes)                                                  \
+  WDB_API int wdb_##name##_supported(const Args *u) {                                          \
+    Plan P;                                                                                    \
+    return plan(u, nullptr, &P) ? 1 : 0;                                                       \
+  }                                                                                            \
+  WDB_API long long wdb_##name##_workspace_bytes(const Args *u) {                              \
+    Plan P;                                                                                    \
+    return plan(u, nullptr, &P) ? bytes(P) : -1;                                               \
+  }                                                                                            \
+  WDB_API int wdb_##name(void *stream, const Args *u) { return name(stream, u, nullptr); }     \
+  WDB_API int wdb_##name##_sampled_supported(const Args *u, int n_windows) {                   \
+    const wdb_replay_windows w = {nullptr, n_windows};                                         \
+    Plan P;                                                                                    \
+    return plan(u, &w, &P) ? 1 : 0;                                                            \
+  }                                                                                            \
+  WDB_API long long wdb_##name##_sampled_workspace_bytes(const Args *u, int n_windows) {       \
+    const wdb_replay_windows w = {nullptr, n_windows};                                         \
+    Plan P;                                                                                    \
+    return plan(u, &w, &P) ? bytes(P) : -1;                                                    \
+  }                                                                                            \
+  WDB_API int wdb_##name##_sampled(void *stream, const Args *u, const wdb_replay_windows *w) { \
+    return w ? name(stream, u, w) : (int)cudaErrorInvalidValue;                                \
+  }
+
+namespace {
+bool td3_critic_plan(const wdb_td3_update_args *u, const wdb_replay_windows *w, Plan *p) {
+  return td3_plan(u, w, false, p);
+}
+bool td3_actor_plan(const wdb_td3_update_args *u, const wdb_replay_windows *w, Plan *p) {
+  return td3_plan(u, w, true, p);
+}
+bool sac_critic_plan(const wdb_sac_update_args *u, const wdb_replay_windows *w, Plan *p) {
+  return sac_plan(u, w, false, p);
+}
+bool sac_actor_plan(const wdb_sac_update_args *u, const wdb_replay_windows *w, Plan *p) {
+  return sac_plan(u, w, true, p);
+}
+long long critic_bytes(const Plan &P) { return td3_workspace_bytes(P, false); }
+long long actor_bytes(const Plan &P) { return td3_workspace_bytes(P, true); }
+}  // namespace
+
+WDB_PASS_API(ddpg_update, wdb_ddpg_update_args, make_plan, workspace_bytes)
+WDB_PASS_API(td3_critic_update, wdb_td3_update_args, td3_critic_plan, critic_bytes)
+WDB_PASS_API(td3_actor_update, wdb_td3_update_args, td3_actor_plan, actor_bytes)
+WDB_PASS_API(sac_critic_update, wdb_sac_update_args, sac_critic_plan, critic_bytes)
+WDB_PASS_API(sac_actor_update, wdb_sac_update_args, sac_actor_plan, actor_bytes)

@@ -289,6 +289,12 @@ class SacUpdate(ctypes.Structure):
     ]
 
 
+class ReplayWindows(ctypes.Structure):
+    """struct wdb_replay_windows (include/wdb200.h)."""
+
+    _fields_ = [("windows", _fp), ("n_windows", _i)]
+
+
 _SIGNATURES = {
     "wdb_abi_version": (_i, []),
     "wdb_error_string": (ctypes.c_char_p, [_i]),
@@ -372,6 +378,27 @@ _SIGNATURES = {
     "wdb_sac_actor_update_supported": (_i, [ctypes.POINTER(SacUpdate)]),
     "wdb_sac_actor_update_workspace_bytes": (_ll, [ctypes.POINTER(SacUpdate)]),
     "wdb_sac_actor_update": (_i, [_vp, ctypes.POINTER(SacUpdate)]),
+    "wdb_ddpg_update_sampled_supported": (_i, [ctypes.POINTER(DdpgUpdate), _i]),
+    "wdb_ddpg_update_sampled_workspace_bytes": (_ll, [ctypes.POINTER(DdpgUpdate), _i]),
+    "wdb_ddpg_update_sampled": (
+        _i, [_vp, ctypes.POINTER(DdpgUpdate), ctypes.POINTER(ReplayWindows)]),
+    "wdb_td3_critic_update_sampled_supported": (_i, [ctypes.POINTER(Td3Update), _i]),
+    "wdb_td3_critic_update_sampled_workspace_bytes": (_ll, [ctypes.POINTER(Td3Update), _i]),
+    "wdb_td3_critic_update_sampled": (
+        _i, [_vp, ctypes.POINTER(Td3Update), ctypes.POINTER(ReplayWindows)]),
+    "wdb_td3_actor_update_sampled_supported": (_i, [ctypes.POINTER(Td3Update), _i]),
+    "wdb_td3_actor_update_sampled_workspace_bytes": (_ll, [ctypes.POINTER(Td3Update), _i]),
+    "wdb_td3_actor_update_sampled": (
+        _i, [_vp, ctypes.POINTER(Td3Update), ctypes.POINTER(ReplayWindows)]),
+    "wdb_sac_critic_update_sampled_supported": (_i, [ctypes.POINTER(SacUpdate), _i]),
+    "wdb_sac_critic_update_sampled_workspace_bytes": (_ll, [ctypes.POINTER(SacUpdate), _i]),
+    "wdb_sac_critic_update_sampled": (
+        _i, [_vp, ctypes.POINTER(SacUpdate), ctypes.POINTER(ReplayWindows)]),
+    "wdb_sac_actor_update_sampled_supported": (_i, [ctypes.POINTER(SacUpdate), _i]),
+    "wdb_sac_actor_update_sampled_workspace_bytes": (_ll, [ctypes.POINTER(SacUpdate), _i]),
+    "wdb_sac_actor_update_sampled": (
+        _i, [_vp, ctypes.POINTER(SacUpdate), ctypes.POINTER(ReplayWindows)]),
+    "wdb_replay_sample_windows": (_i, [_vp, _vp, _i, _ull, _ull, _i, _i, _i, _i, _i]),
     "wdb_single_agent_rollout_supported": (_i, [_i, ctypes.POINTER(_i)]),
     "wdb_single_agent_rollout": (_i, [_vp, ctypes.POINTER(SaRollout)]),
     "wdb_mountain_car_step": (

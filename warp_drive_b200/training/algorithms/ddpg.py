@@ -56,6 +56,16 @@ class DDPG:
             r = (1 - done[lo:lo + valid]) * gamma * r + rewards[lo:lo + valid]
         return r
 
+    def sampled_returns(self, rewards, done, boot):
+        """The n-step returns [B] of B sampled windows: rewards and done flags [n_step, B] of
+        each window's steps and its bootstrap value `boot` [B].  Every window is a regular one:
+        R = r_0 + (1 - d_0) gamma (r_1 + ... (1 - d_{n-1}) gamma boot), with no last-window
+        rule, in window_returns' operation order."""
+        r = boot
+        for j in reversed(range(self.n_step)):
+            r = (1 - done[j]) * self.discount_factor_gamma * r + rewards[j]
+        return r
+
     def compute_loss_and_metrics(self, timestep=None, actions_batch=None, rewards_batch=None,
                                  done_flags_batch=None, value_functions_batch=None,
                                  next_value_functions_batch=None, j_functions_batch=None,

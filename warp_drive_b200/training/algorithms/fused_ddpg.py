@@ -45,14 +45,27 @@ def _shape_struct(actor, critic, n_envs, n_agents, capacity, n_step):
     return u
 
 
-def fused_ddpg_supported(algo, actor, critic, n_envs, n_agents, capacity, n_step):
+def fused_ddpg_supported(algo, actor, critic, n_envs, n_agents, capacity, n_step,
+                         replay_rows=None):
     """True if `wdb_ddpg_update` takes this policy: a FullyConnectedActor (tanh head, Box
     observation, no action mask) and a FullyConnectedActionValueCritic of 0..3 hidden layers of
-    width <= 64, obs + action width <= 64, and no return normalisation."""
+    width <= 64, obs + action width <= 64, and no return normalisation.  replay_rows: asks
+    `wdb_ddpg_update_sampled` with that many sampled windows per update instead."""
     if not fused_models_supported(algo, actor, critic):
         return False
     u = _shape_struct(actor, critic, n_envs, n_agents, capacity, n_step)
+    if replay_rows is not None:
+        return bool(_lib.load().wdb_ddpg_update_sampled_supported(ctypes.byref(u), replay_rows))
     return bool(_lib.load().wdb_ddpg_update_supported(ctypes.byref(u)))
+
+
+def replay_windows(windows):
+    """struct wdb_replay_windows of a device int32 tensor [B, 2] (physical start slot, agent
+    row), as wdb_replay_sample_windows writes it."""
+    assert windows.dtype == torch.int32 and windows.dim() == 2 and windows.shape[1] == 2
+    w = _lib.ReplayWindows()
+    w.windows, w.n_windows = _lib.ptr(windows), int(windows.shape[0])
+    return w
 
 
 def fused_models_supported(algo, actor, critic, actor_type=None):
@@ -81,25 +94,32 @@ class FusedDDPGUpdate:
     sums (device double[2]: sum (Q - R)^2, sum J)."""
 
     def __init__(self, actor, critic, target_actor, target_critic, n_envs, n_agents,
-                 capacity, n_step, gamma):
+                 capacity, n_step, gamma, replay_rows=None):
         self.models = (actor, critic, target_actor, target_critic)
         u = self.u = _shape_struct(actor, critic, n_envs, n_agents, capacity, n_step)
         u.gamma = float(gamma)
         u.action_scale, u.action_bias = float(actor.action_scale), float(actor.action_bias)
         self.lib = _lib.load()
-        nbytes = int(self.lib.wdb_ddpg_update_workspace_bytes(ctypes.byref(u)))
+        if replay_rows is None:
+            nbytes = int(self.lib.wdb_ddpg_update_workspace_bytes(ctypes.byref(u)))
+        else:
+            nbytes = int(self.lib.wdb_ddpg_update_sampled_workspace_bytes(
+                ctypes.byref(u), replay_rows))
         assert nbytes > 0, "shapes not supported by wdb_ddpg_update"
         dev = next(actor.parameters()).device
         self.workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         self.sums = torch.zeros(2, dtype=torch.float64, device=dev)
         self.valid = int(capacity) - int(n_step) + 1
-        self.rows = self.valid * int(n_envs) * int(n_agents)
+        # loss rows per update: every window of the ring, or replay_rows sampled windows
+        self.rows = self.valid * int(n_envs) * int(n_agents) if replay_rows is None else int(
+            replay_rows)
 
-    def launch(self, obs, actions, rewards, done, cursor, outputs=None):
+    def launch(self, obs, actions, rewards, done, cursor, outputs=None, windows=None):
         """Gradients of the update into the actor's and the critic's `.grad`.  obs [C, E, Np,
         F], actions [C, E, Np, A], rewards [C, E, Np], done [C, E] are the ring in physical slot
         order, `cursor` its oldest slot.  outputs: optional (values, j_values, returns) tensors
-        [valid, E, Np] for the metrics."""
+        [valid, E, Np] for the metrics.  windows: int32 [rows, 2] sampled windows -- the update
+        runs over them (wdb_ddpg_update_sampled; `cursor` is not read, outputs are [rows])."""
         u = self.u
         actor, critic, target_actor, target_critic = self.models
         # parameters may have been re-allocated (load_state_dict keeps storage; .to() does not)
@@ -114,5 +134,12 @@ class FusedDDPGUpdate:
         u.values, u.j_values, u.returns = _lib.ptr(values), _lib.ptr(j_values), _lib.ptr(returns)
         u.sums = _lib.ptr(self.sums)
         u.workspace = _lib.ptr(self.workspace)
-        _lib.check(self.lib.wdb_ddpg_update(_lib.stream_ptr(), ctypes.byref(u)), "ddpg_update")
+        if windows is not None:
+            assert windows.shape[0] == self.rows
+            _lib.check(self.lib.wdb_ddpg_update_sampled(
+                _lib.stream_ptr(), ctypes.byref(u), ctypes.byref(replay_windows(windows))),
+                "ddpg_update_sampled")
+        else:
+            _lib.check(self.lib.wdb_ddpg_update(_lib.stream_ptr(), ctypes.byref(u)),
+                       "ddpg_update")
         return self.sums

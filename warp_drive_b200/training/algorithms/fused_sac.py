@@ -10,7 +10,8 @@ import torch
 
 from warp_drive_b200 import lib as _lib
 from warp_drive_b200.training.algorithms.fused_ddpg import (_set_pointers, _set_shape,
-                                                            fused_models_supported)
+                                                            fused_models_supported,
+                                                            replay_windows)
 
 
 def _shape_struct(actor, critic, n_envs, n_agents, capacity, n_step):
@@ -26,7 +27,8 @@ def _shape_struct(actor, critic, n_envs, n_agents, capacity, n_step):
     return u
 
 
-def fused_sac_supported(algo, actor, critic, critic2, n_envs, n_agents, capacity, n_step):
+def fused_sac_supported(algo, actor, critic, critic2, n_envs, n_agents, capacity, n_step,
+                        replay_rows=None):
     """True if both SAC passes take this policy: a FullyConnectedSACActor (Box observation, no
     action mask), two FullyConnectedActionValueCritics of one shape, 0..3 hidden layers of width
     <= 64, a head of 2A <= 64, and the actor, four critics and two critic gradient blocks in
@@ -42,6 +44,9 @@ def fused_sac_supported(algo, actor, critic, critic2, n_envs, n_agents, capacity
         return False
     u = _shape_struct(actor, critic, n_envs, n_agents, capacity, n_step)
     lib = _lib.load()
+    if replay_rows is not None:     # the passes over that many sampled windows per update
+        return bool(lib.wdb_sac_critic_update_sampled_supported(ctypes.byref(u), replay_rows)
+                    and lib.wdb_sac_actor_update_sampled_supported(ctypes.byref(u), replay_rows))
     return bool(lib.wdb_sac_critic_update_supported(ctypes.byref(u))
                 and lib.wdb_sac_actor_update_supported(ctypes.byref(u)))
 
@@ -52,21 +57,40 @@ class FusedSACUpdate:
     sum min(Q1, Q2), sum log pi)."""
 
     def __init__(self, actor, critic, critic2, target_critic, target_critic2, log_alpha, n_envs,
-                 n_agents, capacity, n_step, gamma):
+                 n_agents, capacity, n_step, gamma, replay_rows=None):
         self.models = (actor, critic, critic2, target_critic, target_critic2)
         self.log_alpha = log_alpha
         u = self.u = _shape_struct(actor, critic, n_envs, n_agents, capacity, n_step)
         u.gamma = float(gamma)
         u.action_scale, u.action_bias = float(actor.action_scale), float(actor.action_bias)
         self.lib = _lib.load()
-        nbytes = max(int(self.lib.wdb_sac_critic_update_workspace_bytes(ctypes.byref(u))),
-                     int(self.lib.wdb_sac_actor_update_workspace_bytes(ctypes.byref(u))))
+        if replay_rows is None:
+            nbytes = max(int(self.lib.wdb_sac_critic_update_workspace_bytes(ctypes.byref(u))),
+                         int(self.lib.wdb_sac_actor_update_workspace_bytes(ctypes.byref(u))))
+        else:
+            nbytes = max(int(self.lib.wdb_sac_critic_update_sampled_workspace_bytes(
+                ctypes.byref(u), replay_rows)), int(
+                    self.lib.wdb_sac_actor_update_sampled_workspace_bytes(
+                        ctypes.byref(u), replay_rows)))
         assert nbytes > 0, "shapes not supported by wdb_sac_*_update"
         dev = next(actor.parameters()).device
         self.workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         self.sums = torch.zeros(4, dtype=torch.float64, device=dev)
         self.valid = int(capacity) - int(n_step) + 1
-        self.rows = self.valid * int(n_envs) * int(n_agents)
+        # loss rows per update: every window of the ring, or replay_rows sampled windows
+        self.rows = self.valid * int(n_envs) * int(n_agents) if replay_rows is None else int(
+            replay_rows)
+
+    def _launch(self, name, windows):
+        """Pass `name` over the ring, or over `windows` (int32 [rows, 2]: the _sampled pass;
+        the cursor is not read, noise and outputs are per sampled row)."""
+        if windows is None:
+            rc = getattr(self.lib, f"wdb_{name}")(_lib.stream_ptr(), ctypes.byref(self.u))
+        else:
+            assert windows.shape[0] == self.rows
+            rc = getattr(self.lib, f"wdb_{name}_sampled")(
+                _lib.stream_ptr(), ctypes.byref(self.u), ctypes.byref(replay_windows(windows)))
+        _lib.check(rc, name)
 
     def _ring(self, obs, cursor):
         u = self.u
@@ -76,7 +100,8 @@ class FusedSACUpdate:
         u.sums = _lib.ptr(self.sums)
         u.workspace = _lib.ptr(self.workspace)
 
-    def critic_launch(self, obs, actions, rewards, done, cursor, noise, outputs=None):
+    def critic_launch(self, obs, actions, rewards, done, cursor, noise, outputs=None,
+                      windows=None):
         """Both critics' gradients into their `.grad`.  obs [C, E, Np, F], actions [C, E, Np,
         A], rewards [C, E, Np], done [C, E]: the ring in physical slot order, `cursor` its
         oldest slot; noise [valid, E, Np, A] standard normal (eps') in window order.  outputs:
@@ -94,11 +119,10 @@ class FusedSACUpdate:
         u.critic_noise = _lib.ptr(noise)
         q1, q2, returns = outputs if outputs is not None else (None, None, None)
         u.q1_values, u.q2_values, u.returns = _lib.ptr(q1), _lib.ptr(q2), _lib.ptr(returns)
-        _lib.check(self.lib.wdb_sac_critic_update(_lib.stream_ptr(), ctypes.byref(u)),
-                   "sac_critic_update")
+        self._launch("sac_critic_update", windows)
         return self.sums
 
-    def actor_launch(self, obs, cursor, noise, log_probs=None):
+    def actor_launch(self, obs, cursor, noise, log_probs=None, windows=None):
         """The actor's gradient into its `.grad`, through both critics as they are now; noise
         [valid, E, Np, A] (eps).  log_probs: optional [valid, E, Np] output."""
         u = self.u
@@ -109,6 +133,5 @@ class FusedSACUpdate:
         self._ring(obs, cursor)
         u.actor_noise = _lib.ptr(noise)
         u.log_probs = _lib.ptr(log_probs)
-        _lib.check(self.lib.wdb_sac_actor_update(_lib.stream_ptr(), ctypes.byref(u)),
-                   "sac_actor_update")
+        self._launch("sac_actor_update", windows)
         return self.sums

@@ -80,6 +80,20 @@ def torch_critic_loss(algo, actor, target_critic, target_critic2, critic, critic
     return l1, l2, q1, q2, returns
 
 
+def torch_sampled_critic_loss(algo, actor, target_critic, target_critic2, critic, critic2,
+                              log_alpha, obs, actions, rewards, done, boot_obs, noise):
+    """torch_critic_loss over B sampled windows gathered from the replay buffer: obs and
+    boot_obs [B, F], actions [B, A], rewards and done [n_step, B], noise [B, A] (eps')."""
+    with torch.no_grad():
+        a_t, log_pi = actor.sample(boot_obs, noise)
+        q_t = torch.minimum(target_critic(obs=boot_obs, action=a_t),
+                            target_critic2(obs=boot_obs, action=a_t))
+        returns = algo.sampled_returns(rewards, done, q_t - log_alpha.exp() * log_pi)
+    q1, q2 = critic(obs=obs, action=actions), critic2(obs=obs, action=actions)
+    l1, l2 = algo.critic_losses(q1, q2, returns)
+    return l1, l2, q1, q2, returns
+
+
 def torch_actor_loss(algo, actor, critic, critic2, log_alpha, obs_rows, noise):
     """mean(alpha log pi - min(Q1, Q2)) over the loss rows' observations [valid, E, Np, F] with
     eps = noise [valid, E, Np, A]; returns (loss, min Q, log pi).  Call

@@ -120,6 +120,22 @@ def torch_critic_loss(algo, target_actor, target_critic, target_critic2, critic,
     return l1, l2, q1, q2, returns
 
 
+def torch_sampled_critic_loss(algo, target_actor, target_critic, target_critic2, critic, critic2,
+                              obs, actions, rewards, done, boot_obs, noise):
+    """torch_critic_loss over B sampled windows gathered from the replay buffer: obs and
+    boot_obs [B, F], actions [B, A], rewards and done [n_step, B], noise [B, A]."""
+    with torch.no_grad():
+        pi = torch.cat(list(target_actor(obs=boot_obs)), dim=-1)
+        a_t = algo.target_actions(pi, noise, float(target_actor.action_scale),
+                                  float(target_actor.action_bias))
+        boot = torch.minimum(target_critic(obs=boot_obs, action=a_t),
+                             target_critic2(obs=boot_obs, action=a_t))
+        returns = algo.sampled_returns(rewards, done, boot)
+    q1, q2 = critic(obs=obs, action=actions), critic2(obs=obs, action=actions)
+    l1, l2 = algo.critic_losses(q1, q2, returns)
+    return l1, l2, q1, q2, returns
+
+
 def torch_actor_loss(algo, actor, critic, obs_rows):
     """-mean Q1(s, pi(s)) over the loss rows' observations [valid, E, Np, F]; returns (loss,
     J).  Call .backward(inputs=actor parameters) to keep the critic's gradient out."""

@@ -26,11 +26,19 @@ Underneath:
     own norm as clip_grad_norm_ does; target networks are tracked with fused `torch._foreach`
     updates;
   * multi-GPU: one flat NCCL all-reduce over actor + critic gradients per iteration.
+
+Replay buffer (trainer key `replay_slots_per_env`, see `replay_settings`): the same ring made
+that many timesteps long, and `updates_per_iteration` updates after each rollout, each over
+`replay_batch_rows` uniformly sampled n-step windows (wdb_replay_sample_windows) that the
+*_sampled passes read in place.  The buffer is per GPU (each rank samples its own store with
+its own seed) and is not checkpointed.
 """
+import math
 import os
 
 import torch
 
+from warp_drive_b200 import lib as _lib
 from warp_drive_b200.training.algorithms.ddpg import DDPG
 from warp_drive_b200.training.algorithms.fused_ddpg import FusedDDPGUpdate, fused_ddpg_supported
 from warp_drive_b200.training.models.fully_connected_actor_critic import ActorAsPolicy
@@ -55,6 +63,36 @@ def soft_update(target, source, tau):
 
 def hard_update(target, source):
     target.load_state_dict(source.state_dict())
+
+
+_REPLAY_KEYS = ("replay_batch_rows", "updates_per_iteration", "replay_warmup_slots")
+
+
+def replay_settings(trainer_config, batch_slots, n_step):
+    """The validated replay-buffer keys of a trainer config, or None without
+    `replay_slots_per_env` (the ring of one rollout, updated over every window).  Returns
+    {"slots", "batch_rows" (None: one rollout's rows of the policy), "updates", "warmup"}."""
+    slots = trainer_config.get("replay_slots_per_env")
+    if slots is None:
+        for key in _REPLAY_KEYS:
+            if trainer_config.get(key) is not None:
+                raise ValueError(f"{key} needs replay_slots_per_env")
+        return None
+    if int(slots) != slots or slots < batch_slots + n_step:
+        raise ValueError(f"replay_slots_per_env must be an integer >= train_batch_size / "
+                         f"num_envs + n_step = {batch_slots + n_step}, got {slots}")
+    rows = trainer_config.get("replay_batch_rows")
+    if rows is not None and (int(rows) != rows or not 1 <= rows < 2 ** 31):
+        raise ValueError(f"replay_batch_rows must be an integer in [1, 2^31), got {rows}")
+    updates = trainer_config.get("updates_per_iteration", 1)
+    if int(updates) != updates or updates < 1:
+        raise ValueError(f"updates_per_iteration must be an integer >= 1, got {updates}")
+    warmup = trainer_config.get("replay_warmup_slots", batch_slots + n_step)
+    if int(warmup) != warmup or not n_step + 1 <= warmup <= slots:
+        raise ValueError(f"replay_warmup_slots must be an integer in [n_step + 1, "
+                         f"replay_slots_per_env] = [{n_step + 1}, {slots}], got {warmup}")
+    return {"slots": int(slots), "batch_rows": None if rows is None else int(rows),
+            "updates": int(updates), "warmup": int(warmup)}
 
 
 class RingRolloutEngine(RolloutEngine):
@@ -135,7 +173,12 @@ class TrainerDDPG(Trainer):
         ahead."""
         self.n_step = int(trainer_config.get("n_step", 1))
         assert self.n_step >= 1
-        self.ring_capacity = self.training_batch_size_per_env + self.n_step - 1
+        self.replay = replay_settings(trainer_config, self.training_batch_size_per_env,
+                                      self.n_step)
+        if self.replay is not None:
+            self.ring_capacity = self.replay["slots"]
+        else:
+            self.ring_capacity = self.training_batch_size_per_env + self.n_step - 1
         return self.ring_capacity
 
     def _create_network_dicts(self):
@@ -144,6 +187,7 @@ class TrainerDDPG(Trainer):
         self.actor_optimizers, self.critic_optimizers = {}, {}
         self.actor_lr_schedules, self.critic_lr_schedules = {}, {}
         self.tau, self.fused_updates = {}, {}
+        self.replay_windows, self.replay_draws = {}, 0
         # `models`: the networks the rollout runs
         self.models = self.actor_models
 
@@ -201,10 +245,35 @@ class TrainerDDPG(Trainer):
         n_agents = len(self.policy_tag_to_agent_id_map[policy])
         args = (self.num_envs, n_agents, self.ring_capacity, self.n_step)
         actor, critic = self.actor_models[policy], self.critic_models[policy]
-        if fused_ddpg_supported(self.trainers[policy], actor, critic, *args):
+        rows = self._init_replay(policy)
+        if fused_ddpg_supported(self.trainers[policy], actor, critic, *args, replay_rows=rows):
             self.fused_updates[policy] = FusedDDPGUpdate(
                 actor, critic, self.target_actor_models[policy],
-                self.target_critic_models[policy], *args, gamma=c["gamma"])
+                self.target_critic_models[policy], *args, gamma=c["gamma"], replay_rows=rows)
+
+    def _init_replay(self, policy):
+        """With a replay buffer: the policy's window buffer (int32 [B, 2]) and the log line
+        of the store's size.  Returns B, the loss rows per update (None without a buffer)."""
+        if self.replay is None:
+            return None
+        n_agents = len(self.policy_tag_to_agent_id_map[policy])
+        rows = self.replay["batch_rows"]
+        if rows is None:
+            rows = self.training_batch_size_per_env * self.num_envs * n_agents
+        dev = next(self.actor_models[policy].parameters()).device
+        self.replay_windows[policy] = torch.zeros((rows, 2), dtype=torch.int32, device=dev)
+        dm = self.cuda_envs.cuda_data_manager
+        names = [f"{_PROCESSED_OBSERVATIONS}_batch_{policy}", f"{_ACTIONS}_batch_{policy}",
+                 f"{_REWARDS}_batch_{policy}", f"{_DONE_FLAGS}_batch"]
+        nbytes = sum(t.numel() * t.element_size()
+                     for t in map(dm.data_on_device_via_torch, names))
+        if self.verbose:
+            print(f"[Device {self.device_id}]: replay buffer of policy '{policy}': "
+                  f"{self.ring_capacity} slots x {self.num_envs} envs x {n_agents} agents = "
+                  f"{self.ring_capacity * self.num_envs * n_agents} transitions, {nbytes} "
+                  f"bytes on the device; {rows} rows per update, {self.replay['updates']} "
+                  f"updates per iteration")
+        return rows
 
     def _make_engine(self, use_cuda_graph):
         engine = RingRolloutEngine(
@@ -216,24 +285,115 @@ class TrainerDDPG(Trainer):
 
     # ------------------------------------------------------------------ update
     def _update_model_params(self, iteration):
+        """After a rollout: nothing while the ring fills; then one update over every window of
+        the ring, or -- with a replay buffer -- `updates_per_iteration` updates over freshly
+        sampled windows.  Only the last update of a logging iteration collects metrics."""
         logging_flag = self._is_logging_iteration(iteration)
         loss_metrics = {}
-        if self.engine.isfull():       # until then the rollouts only fill the replay ring
+        step_info = {policy: ({}, {}) for policy in self.policies_to_train}
+        if self._ready_to_update():
             for policy in self.policies_to_train:
                 self._advance_timestep(policy)
-                fused = self.fused_updates.get(policy)
-                if fused is not None and self.trainers[policy].use_fused_update:
-                    loss_metrics[policy] = self._fused_gradients(policy, fused, logging_flag)
-                else:
-                    loss_metrics[policy] = self._torch_gradients(policy, logging_flag)
-        metrics_dict = self._step_optimizers(loss_metrics, logging_flag)
+            updates = 1 if self.replay is None else self.replay["updates"]
+            for k in range(updates):
+                loss_metrics = self._one_update(logging_flag and k == updates - 1, step_info)
+        metrics_dict = self._finish_update(loss_metrics, step_info, logging_flag)
+        if self.replay is not None:
+            for metrics in metrics_dict.values():
+                metrics["Replay buffer fill"] = self.engine.ring_filled / self.ring_capacity
+        self._add_test_metrics(metrics_dict, logging_flag)
+        return metrics_dict
+
+    def _ready_to_update(self):
+        """Until then the rollouts only fill the ring."""
+        if self.replay is None:
+            return self.engine.isfull()
+        return self.engine.ring_filled >= self.replay["warmup"]
+
+    def _one_update(self, logging_flag, step_info):
+        """Gradients, optimizer steps and target tracking of every trained policy; returns
+        their loss metrics (filled when logging_flag)."""
+        loss_metrics = {}
+        for policy in self.policies_to_train:
+            self._sample_replay_windows(policy)
+            fused = self.fused_updates.get(policy)
+            if fused is not None and self.trainers[policy].use_fused_update:
+                loss_metrics[policy] = self._fused_gradients(policy, fused, logging_flag)
+            elif self.replay is not None:
+                loss_metrics[policy] = self._torch_replay_gradients(policy, logging_flag)
+            else:
+                loss_metrics[policy] = self._torch_gradients(policy, logging_flag)
+        step_info.update(self._optimizer_step(loss_metrics, logging_flag))
         for policy in loss_metrics:
             soft_update(self.target_actor_models[policy], self.actor_models[policy],
                         self.tau[policy])
             soft_update(self.target_critic_models[policy], self.critic_models[policy],
                         self.tau[policy])
-        self._add_test_metrics(metrics_dict, logging_flag)
-        return metrics_dict
+        return loss_metrics
+
+    # ------------------------------------------------------------------ replay buffer
+    def _sample_replay_windows(self, policy):
+        """With a replay buffer: draws this update's windows of `policy` on the device into
+        replay_windows[policy] (one launch, no host wait).  The draw is a function of the
+        trainer seed (rank-dependent) and the running draw count."""
+        if self.replay is None:
+            return
+        eng, windows = self.engine, self.replay_windows[policy]
+        self.replay_draws += 1
+        oldest = eng.ring_cursor if eng.ring_filled == eng.ring_capacity else 0
+        n_agents = len(self.policy_tag_to_agent_id_map[policy])
+        _lib.check(_lib.load().wdb_replay_sample_windows(
+            _lib.stream_ptr(), _lib.ptr(windows), int(windows.shape[0]), self.seed,
+            self.replay_draws, oldest, eng.ring_filled, eng.ring_capacity, self.n_step,
+            self.num_envs * n_agents), "replay_sample_windows")
+
+    def _gather_windows(self, policy):
+        """The sampled windows of `policy` gathered by index from the physical ring (never
+        unrolled: that would copy all of it): obs [B, F], actions [B, A], rewards [n_step, B],
+        done [n_step, B] (float), bootstrap obs [B, F]."""
+        eng, C = self.engine, self.ring_capacity
+        windows = self.replay_windows[policy].long()
+        start, row = windows[:, 0], windows[:, 1]
+        steps = (start[None, :] + torch.arange(self.n_step + 1, device=start.device)[:, None]) % C
+        obs = eng._tensor(f"{_PROCESSED_OBSERVATIONS}_batch_{policy}")
+        actions = eng._tensor(f"{_ACTIONS}_batch_{policy}")
+        rewards = eng._tensor(f"{_REWARDS}_batch_{policy}")
+        done = eng._tensor(f"{_DONE_FLAGS}_batch")
+        n_agents = rewards.shape[2]
+        obs = obs.reshape(C, -1, obs.shape[-1])
+        return (obs[start, row], actions.reshape(C, -1, actions.shape[-1])[start, row],
+                rewards.reshape(C, -1)[steps[:-1], row],
+                done[steps[:-1], row // n_agents].to(rewards.dtype), obs[steps[-1], row])
+
+    @staticmethod
+    def _batch_metrics(metrics):
+        """Metrics of a sampled batch (laid out as one timestep of B envs): the spreads over
+        agents and over time do not exist for it and are dropped."""
+        return {k: v for k, v in metrics.items() if not (isinstance(v, float) and math.isnan(v))}
+
+    def _torch_replay_gradients(self, policy, logging_flag):
+        """_torch_gradients over the sampled windows: the losses of wdb_ddpg_update_sampled by
+        torch autograd on the gathered batch."""
+        algo = self.trainers[policy]
+        obs, actions, rewards, done, boot_obs = self._gather_windows(policy)
+        actor, critic = self.actor_models[policy], self.critic_models[policy]
+        with torch.no_grad():
+            boot = self.target_critic_models[policy](
+                obs=boot_obs, action=self.target_actor_models[policy](obs=boot_obs))
+            returns = algo.sampled_returns(rewards, done, boot)
+        values = critic(obs=obs, action=actions)
+        j_values = critic(obs=obs, action=actor(obs=obs))
+        actor_loss, critic_loss = -j_values.mean(), torch.nn.functional.mse_loss(values, returns)
+        self.actor_optimizers[policy].zero_grad()
+        self.critic_optimizers[policy].zero_grad()
+        actor_loss.backward()
+        critic_loss.backward()
+        if not logging_flag:
+            return {}
+        return self._batch_metrics(algo.loss_metrics(
+            actor_loss.item(), critic_loss.item(), rewards[0][None, :, None],
+            actions[None, :, None], values.detach()[None, :, None],
+            j_values.detach()[None, :, None], returns[None, :, None]))
 
     # the sampler arguments of the evaluator's noise-free test episodes
     _test_sample_params = {"scale": 0}
@@ -280,17 +440,24 @@ class TrainerDDPG(Trainer):
         eng = self.engine
         rewards = eng._tensor(f"{_REWARDS}_batch_{policy}")
         actions = eng._tensor(f"{_ACTIONS}_batch_{policy}")
+        windows = self.replay_windows.get(policy)
         outputs = None
         if logging_flag:
-            shape = (fused.valid,) + tuple(rewards.shape[1:])
+            shape = (fused.valid,) + tuple(rewards.shape[1:]) if windows is None else (
+                1, fused.rows, 1)
             outputs = tuple(torch.empty(shape, device=rewards.device) for _ in range(3))
         sums = fused.launch(eng._tensor(f"{_PROCESSED_OBSERVATIONS}_batch_{policy}"), actions,
                             rewards, eng._tensor(f"{_DONE_FLAGS}_batch"), eng.ring_cursor,
-                            outputs)
+                            outputs, windows=windows)
         if not logging_flag:
             return {}
         s = sums.tolist()
         values, j_values, returns = outputs
+        if windows is not None:       # the metrics of the sampled rows' first step
+            _, actions, rewards, _, _ = self._gather_windows(policy)
+            return self._batch_metrics(self.trainers[policy].loss_metrics(
+                -s[1] / fused.rows, s[0] / fused.rows, rewards[0][None, :, None],
+                actions[None, :, None], values, j_values, returns))
         # the ring in slot order: the metrics are means / extremes / spreads over all of it
         return self.trainers[policy].loss_metrics(
             -s[1] / fused.rows, s[0] / fused.rows, rewards, actions, values, j_values, returns)

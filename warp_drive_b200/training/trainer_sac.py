@@ -20,7 +20,8 @@ Per policy and update:
 The critic's eps' and the actor's eps are drawn per update from a CUDA generator seeded from
 the trainer seed into two preallocated [valid, E, Np, A] buffers, indexed by logical window; the
 fused and the torch update read the same buffers.  On one GPU the host waits only on logging
-iterations.
+iterations.  With a replay buffer (trainer_ddpg.py) every iteration runs `updates_per_iteration`
+such updates, each over its own sampled windows, and the noise buffers are [B, A].
 """
 import math
 import os
@@ -29,7 +30,8 @@ import torch
 from torch import nn
 
 from warp_drive_b200.training.algorithms.fused_sac import FusedSACUpdate, fused_sac_supported
-from warp_drive_b200.training.algorithms.sac import SAC, torch_actor_loss, torch_critic_loss
+from warp_drive_b200.training.algorithms.sac import (SAC, torch_actor_loss, torch_critic_loss,
+                                                     torch_sampled_critic_loss)
 from warp_drive_b200.training.trainer_ddpg import hard_update, soft_update
 from warp_drive_b200.training.trainer_td3 import TrainerTD3
 from warp_drive_b200.training.utils.param_scheduler import ParamScheduler
@@ -120,7 +122,8 @@ class TrainerSAC(TrainerTD3):
         n_agents = len(self.policy_tag_to_agent_id_map[policy])
         dev = next(actor.parameters()).device
         valid = self.ring_capacity - self.n_step + 1
-        shape = (valid, self.num_envs, n_agents, A)
+        rows = self._init_replay(policy)
+        shape = self._noise_shape(rows, valid, n_agents, A)
         self.critic_noise[policy] = torch.zeros(shape, device=dev)
         self.actor_noise[policy] = torch.zeros(shape, device=dev)
         self.bootstrap_index[policy] = torch.tensor(algo.bootstrap_slots(self.ring_capacity),
@@ -131,23 +134,21 @@ class TrainerSAC(TrainerTD3):
             self._noise_generator.manual_seed(self.seed)
         args = (self.num_envs, n_agents, self.ring_capacity, self.n_step)
         critic, critic2 = self.critic_models[policy], self.critic2_models[policy]
-        if fused_sac_supported(algo, actor, critic, critic2, *args):
+        if fused_sac_supported(algo, actor, critic, critic2, *args, replay_rows=rows):
             self.fused_updates[policy] = FusedSACUpdate(
                 actor, critic, critic2, self.target_critic_models[policy],
                 self.target_critic2_models[policy], self.temperatures[policy].log_alpha, *args,
-                gamma=c["gamma"])
+                gamma=c["gamma"], replay_rows=rows)
 
     # ------------------------------------------------------------------ update
-    def _update_model_params(self, iteration):
-        logging_flag = self._is_logging_iteration(iteration)
-        loss_metrics, step_info = {}, {}
-        if self.engine.isfull():       # until then the rollouts only fill the replay ring
-            for policy in self.policies_to_train:
-                self._advance_timestep(policy)
-                self.update_count[policy] += 1
-                self.critic_noise[policy].normal_(generator=self._noise_generator)
-                self.actor_noise[policy].normal_(generator=self._noise_generator)
-                loss_metrics[policy] = self._critic_gradients(policy, logging_flag)
+    def _one_update(self, logging_flag, step_info):
+        loss_metrics = {}
+        for policy in self.policies_to_train:
+            self.update_count[policy] += 1
+            self._sample_replay_windows(policy)
+            self.critic_noise[policy].normal_(generator=self._noise_generator)
+            self.actor_noise[policy].normal_(generator=self._noise_generator)
+            loss_metrics[policy] = self._critic_gradients(policy, logging_flag)
         self._step(loss_metrics, 1, logging_flag, step_info)
         stepped = list(loss_metrics)
         for policy in stepped:
@@ -160,32 +161,48 @@ class TrainerSAC(TrainerTD3):
             for target, source in ((self.target_critic_models, self.critic_models),
                                    (self.target_critic2_models, self.critic2_models)):
                 soft_update(target[policy], source[policy], self.tau[policy])
-        metrics_dict = self._finish_update(loss_metrics, step_info, logging_flag)
-        self._add_test_metrics(metrics_dict, logging_flag)
-        return metrics_dict
+        return loss_metrics
 
     def _critic_gradients(self, policy, logging_flag):
         """Both critics' gradients into the arena's .grad views; the critic metrics of a
         logging iteration."""
         eng, algo, fused = self.engine, self.trainers[policy], self._fused(policy)
         log_alpha = self.temperatures[policy].log_alpha
+        windows = self.replay_windows.get(policy)
         if fused is not None:
             rewards = eng._tensor(f"{_REWARDS}_batch_{policy}")
             actions = eng._tensor(f"{_ACTIONS}_batch_{policy}")
             outputs = None
             if logging_flag:
-                shape = (fused.valid,) + tuple(rewards.shape[1:])
+                shape = (fused.valid,) + tuple(rewards.shape[1:]) if windows is None else (
+                    1, fused.rows, 1)
                 outputs = tuple(torch.empty(shape, device=rewards.device) for _ in range(3))
             sums = fused.critic_launch(
                 eng._tensor(f"{_PROCESSED_OBSERVATIONS}_batch_{policy}"), actions, rewards,
                 eng._tensor(f"{_DONE_FLAGS}_batch"), eng.ring_cursor, self.critic_noise[policy],
-                outputs)
+                outputs, windows=windows)
             if not logging_flag:
                 return {}
             s = sums.tolist()
             q1, _, returns = outputs
+            if windows is not None:
+                return self._replay_critic_metrics(policy, s[0] / fused.rows, s[1] / fused.rows,
+                                                   q1, returns)
             return algo.loss_metrics(s[0] / fused.rows, s[1] / fused.rows, rewards, actions, q1,
                                      returns)
+        if windows is not None:
+            l1, l2, q1, _, returns = torch_sampled_critic_loss(
+                algo, self.actor_models[policy], self.target_critic_models[policy],
+                self.target_critic2_models[policy], self.critic_models[policy],
+                self.critic2_models[policy], log_alpha, *self._gather_windows(policy),
+                self.critic_noise[policy])
+            self.critic_optimizers[policy].zero_grad()
+            (l1 + l2).backward()
+            if not logging_flag:
+                return {}
+            return self._replay_critic_metrics(policy, l1.item(), l2.item(),
+                                               q1.detach()[None, :, None],
+                                               returns[None, :, None])
         rewards = eng.unroll(f"{_REWARDS}_batch_{policy}")
         actions = eng.unroll(f"{_ACTIONS}_batch_{policy}")
         l1, l2, q1, _, returns = torch_critic_loss(
@@ -208,20 +225,24 @@ class TrainerSAC(TrainerTD3):
         eng, algo, fused = self.engine, self.trainers[policy], self._fused(policy)
         obs_name = f"{_PROCESSED_OBSERVATIONS}_batch_{policy}"
         log_alpha = self.temperatures[policy].log_alpha
+        windows = self.replay_windows.get(policy)
         if fused is not None:
             sums = fused.actor_launch(eng._tensor(obs_name), eng.ring_cursor,
-                                      self.actor_noise[policy])
+                                      self.actor_noise[policy], windows=windows)
             rows = fused.rows
             sum_q, sum_log_pi = sums[2], sums[3]
             alpha = log_alpha.detach().exp()
             actor_loss = None
         else:
             actor = self.actor_models[policy]
-            valid = self.actor_noise[policy].shape[0]
+            if windows is not None:
+                obs_rows = self._gather_windows(policy)[0]
+            else:
+                obs_rows = eng.unroll(obs_name)[:self.actor_noise[policy].shape[0]]
             self.actor_optimizers[policy].zero_grad()
             loss, q, log_pi = torch_actor_loss(
                 algo, actor, self.critic_models[policy], self.critic2_models[policy], log_alpha,
-                eng.unroll(obs_name)[:valid], self.actor_noise[policy])
+                obs_rows, self.actor_noise[policy])
             loss.backward(inputs=list(actor.parameters()))
             rows = log_pi.numel()
             sum_log_pi = log_pi.detach().double().sum()

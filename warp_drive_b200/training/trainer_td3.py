@@ -14,6 +14,9 @@ policy (k = 1, 2, ...):
 The target-policy noise is one draw of a CUDA generator seeded from the trainer seed per update
 into a preallocated [valid, E, Np, A] buffer, indexed by logical window; the fused and the
 torch update read the same buffer.  On one GPU the host waits only on logging iterations.
+With a replay buffer (trainer_ddpg.py) k counts the `updates_per_iteration` updates of every
+iteration, each over its own sampled windows, and the noise buffer is [B, A], one row per
+sampled window.
 """
 import os
 
@@ -21,7 +24,8 @@ import torch
 from torch import nn
 
 from warp_drive_b200.training.algorithms.fused_td3 import FusedTD3Update, fused_td3_supported
-from warp_drive_b200.training.algorithms.td3 import TD3, torch_actor_loss, torch_critic_loss
+from warp_drive_b200.training.algorithms.td3 import (TD3, torch_actor_loss, torch_critic_loss,
+                                                     torch_sampled_critic_loss)
 from warp_drive_b200.training.trainer_ddpg import TrainerDDPG, hard_update, soft_update
 from warp_drive_b200.utils.constants import Constants
 
@@ -80,8 +84,9 @@ class TrainerTD3(TrainerDDPG):
         actor = self.actor_models[policy]
         dev = next(actor.parameters()).device
         valid = self.ring_capacity - self.n_step + 1
+        rows = self._init_replay(policy)
         self.target_noise[policy] = torch.zeros(
-            (valid, self.num_envs, n_agents, int(actor.output_dims[0])), device=dev)
+            self._noise_shape(rows, valid, n_agents, int(actor.output_dims[0])), device=dev)
         self.bootstrap_index[policy] = torch.tensor(algo.bootstrap_slots(self.ring_capacity),
                                                     device=dev)
         self.update_count[policy] = 0
@@ -90,22 +95,26 @@ class TrainerTD3(TrainerDDPG):
             self._noise_generator.manual_seed(self.seed)
         args = (self.num_envs, n_agents, self.ring_capacity, self.n_step)
         critic, critic2 = self.critic_models[policy], self.critic2_models[policy]
-        if fused_td3_supported(algo, actor, critic, critic2, *args):
+        if fused_td3_supported(algo, actor, critic, critic2, *args, replay_rows=rows):
             self.fused_updates[policy] = FusedTD3Update(
                 algo, actor, critic, critic2, self.target_actor_models[policy],
                 self.target_critic_models[policy], self.target_critic2_models[policy], *args,
-                gamma=c["gamma"])
+                gamma=c["gamma"], replay_rows=rows)
+
+    def _noise_shape(self, replay_rows, valid, n_agents, action_dim):
+        """One row of noise per loss row: per window of the ring, or per sampled window."""
+        if replay_rows is None:
+            return (valid, self.num_envs, n_agents, action_dim)
+        return (replay_rows, action_dim)
 
     # ------------------------------------------------------------------ update
-    def _update_model_params(self, iteration):
-        logging_flag = self._is_logging_iteration(iteration)
-        loss_metrics, step_info = {}, {}
-        if self.engine.isfull():       # until then the rollouts only fill the replay ring
-            for policy in self.policies_to_train:
-                self._advance_timestep(policy)
-                self.update_count[policy] += 1
-                self.target_noise[policy].normal_(generator=self._noise_generator)
-                loss_metrics[policy] = self._critic_gradients(policy, logging_flag)
+    def _one_update(self, logging_flag, step_info):
+        loss_metrics = {}
+        for policy in self.policies_to_train:
+            self.update_count[policy] += 1
+            self._sample_replay_windows(policy)
+            self.target_noise[policy].normal_(generator=self._noise_generator)
+            loss_metrics[policy] = self._critic_gradients(policy, logging_flag)
         self._step(loss_metrics, 1, logging_flag, step_info)
         actors = [p for p in loss_metrics
                   if self.update_count[p] % self.trainers[p].policy_delay == 0]
@@ -119,9 +128,7 @@ class TrainerTD3(TrainerDDPG):
                     (self.target_critic_models, self.critic_models),
                     (self.target_critic2_models, self.critic2_models)):
                 soft_update(target[policy], source[policy], self.tau[policy])
-        metrics_dict = self._finish_update(loss_metrics, step_info, logging_flag)
-        self._add_test_metrics(metrics_dict, logging_flag)
-        return metrics_dict
+        return loss_metrics
 
     def _step(self, stepped, which, logging_flag, step_info):
         """One all-reduce of the gradient arena, then clipping + Adam of network `which` (0:
@@ -149,23 +156,41 @@ class TrainerTD3(TrainerDDPG):
         """Both critics' gradients into the arena's .grad views; the critic metrics of a
         logging iteration."""
         eng, algo, fused = self.engine, self.trainers[policy], self._fused(policy)
+        windows = self.replay_windows.get(policy)
         if fused is not None:
             rewards = eng._tensor(f"{_REWARDS}_batch_{policy}")
             actions = eng._tensor(f"{_ACTIONS}_batch_{policy}")
             outputs = None
             if logging_flag:
-                shape = (fused.valid,) + tuple(rewards.shape[1:])
+                shape = (fused.valid,) + tuple(rewards.shape[1:]) if windows is None else (
+                    1, fused.rows, 1)
                 outputs = tuple(torch.empty(shape, device=rewards.device) for _ in range(3))
             sums = fused.critic_launch(
                 eng._tensor(f"{_PROCESSED_OBSERVATIONS}_batch_{policy}"), actions, rewards,
                 eng._tensor(f"{_DONE_FLAGS}_batch"), eng.ring_cursor, self.target_noise[policy],
-                outputs)
+                outputs, windows=windows)
             if not logging_flag:
                 return {}
             s = sums.tolist()
             q1, _, returns = outputs
+            if windows is not None:
+                return self._replay_critic_metrics(policy, s[0] / fused.rows, s[1] / fused.rows,
+                                                   q1, returns)
             return algo.loss_metrics(s[0] / fused.rows, s[1] / fused.rows, rewards, actions, q1,
                                      returns)
+        if windows is not None:
+            l1, l2, q1, _, returns = torch_sampled_critic_loss(
+                algo, self.target_actor_models[policy], self.target_critic_models[policy],
+                self.target_critic2_models[policy], self.critic_models[policy],
+                self.critic2_models[policy], *self._gather_windows(policy),
+                self.target_noise[policy])
+            self.critic_optimizers[policy].zero_grad()
+            (l1 + l2).backward()
+            if not logging_flag:
+                return {}
+            return self._replay_critic_metrics(policy, l1.item(), l2.item(),
+                                               q1.detach()[None, :, None],
+                                               returns[None, :, None])
         rewards = eng.unroll(f"{_REWARDS}_batch_{policy}")
         actions = eng.unroll(f"{_ACTIONS}_batch_{policy}")
         l1, l2, q1, _, returns = torch_critic_loss(
@@ -180,18 +205,28 @@ class TrainerTD3(TrainerDDPG):
             return {}
         return algo.loss_metrics(l1.item(), l2.item(), rewards, actions, q1.detach(), returns)
 
+    def _replay_critic_metrics(self, policy, loss1, loss2, q1, returns):
+        """The critic metrics of an update over sampled windows: q1 and returns [1, B, 1], the
+        rewards and actions of the windows' first step."""
+        _, actions, rewards, _, _ = self._gather_windows(policy)
+        return self._batch_metrics(self.trainers[policy].loss_metrics(
+            loss1, loss2, rewards[0][None, :, None], actions[None, :, None], q1, returns))
+
     def _actor_gradients(self, policy, logging_flag):
         """The actor's gradient (through Q1 as the critic step left it) into its .grad views
         only; the actor metrics of a logging iteration."""
         eng, algo, fused = self.engine, self.trainers[policy], self._fused(policy)
         obs_name = f"{_PROCESSED_OBSERVATIONS}_batch_{policy}"
+        windows = self.replay_windows.get(policy)
         if fused is not None:
-            sums = fused.actor_launch(eng._tensor(obs_name), eng.ring_cursor)
+            sums = fused.actor_launch(eng._tensor(obs_name), eng.ring_cursor, windows=windows)
             return algo.actor_metrics(-float(sums[2]) / fused.rows) if logging_flag else {}
         actor = self.actor_models[policy]
-        valid = self.target_noise[policy].shape[0]
-        loss, _ = torch_actor_loss(algo, actor, self.critic_models[policy],
-                                   eng.unroll(obs_name)[:valid])
+        if windows is not None:
+            obs_rows = self._gather_windows(policy)[0]
+        else:
+            obs_rows = eng.unroll(obs_name)[:self.target_noise[policy].shape[0]]
+        loss, _ = torch_actor_loss(algo, actor, self.critic_models[policy], obs_rows)
         self.actor_optimizers[policy].zero_grad()
         loss.backward(inputs=list(actor.parameters()))
         return algo.actor_metrics(loss.item()) if logging_flag else {}
