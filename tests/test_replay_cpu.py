@@ -152,12 +152,14 @@ def test_sampled_supported_takes_the_ring_shapes_and_checks_the_windows():
 
 
 @pytest.mark.skipif(shutil.which("nvcc") is None, reason="needs nvcc")
-def test_sampled_kernels_compile_without_spills(tmp_path):
+def test_sampled_pass_instantiations_compile_without_spills(tmp_path):
     flags = ["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17",
              "-Xptxas", "-v", "-cubin"]
-    want = {"wdb_ddpg_update.cu": ["ddpg_update_sampled", "td3_critic_sampled",
-                                   "td3_actor_sampled", "sac_critic_sampled",
-                                   "sac_actor_sampled"],
+    from test_td3_cpu import SAMPLED
+
+    want = {"wdb_ddpg_update.cu": [k + SAMPLED for k in ("ddpg_update_kernel", "td3_critic_kernel",
+                                                         "td3_actor_kernel", "sac_critic_kernel",
+                                                         "sac_actor_kernel")],
             "wdb_core.cu": ["replay_sample_windows_kernel"]}
     for src, kernels in want.items():
         err = subprocess.run(flags + [os.path.join(CSRC, src), "-o", str(tmp_path / "k.cubin")],

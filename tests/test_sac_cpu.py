@@ -23,6 +23,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from sac_update_reference import sac_actor_update, sac_critic_update  # noqa: E402
 from test_abi_layout_cpu import _c_fields  # noqa: E402
 from test_ddpg_update_reference_cpu import _Env, layers, make_ring, rel  # noqa: E402
+from test_td3_cpu import RING  # noqa: E402
 
 NVCC_SM90A = ["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC"]
@@ -419,6 +420,7 @@ def _sass_hashes(cubin, keys):
             name = m.group(1)
             cur = next((k for k in keys if k in name and "squashed" not in name), None)
             if cur is not None:
+                assert cur not in funcs, (cur, name)
                 funcs[cur] = []
         elif cur is not None:
             funcs[cur].append(re.sub(r"/\*[0-9a-f]{4}\*/", "", line).rstrip())
@@ -429,10 +431,13 @@ def _sass_hashes(cubin, keys):
 # the parent commit with nvcc 12.9.
 _KEPT_SASS_SHA256 = {
     "wdb_ddpg_update.cu": {
-        "ddpg_update_kernel": "43727eb73fb299e5ca72c15d364be91aa0dc4bb253d8bcd24a5d3ef3d3cdd04f",
+        "ddpg_update_kernel" + RING:
+            "43727eb73fb299e5ca72c15d364be91aa0dc4bb253d8bcd24a5d3ef3d3cdd04f",
         "ddpg_reduce_kernel": "4ad80efbdf62dead0279d0872ad06dadfc625476fb41c2e1bf18b8292e280def",
-        "td3_critic_kernel": "9ea51c60bf071869f36de6c0668b280a7dc51dc454cd5abd4af04307c46f3ac4",
-        "td3_actor_kernel": "baa1f44c5fde6671d02a45f1973dd31e95d8d52b2cd29ad6f81c106bc5a9b612",
+        "td3_critic_kernel" + RING:
+            "9ea51c60bf071869f36de6c0668b280a7dc51dc454cd5abd4af04307c46f3ac4",
+        "td3_actor_kernel" + RING:
+            "baa1f44c5fde6671d02a45f1973dd31e95d8d52b2cd29ad6f81c106bc5a9b612",
     },
     "wdb_core.cu": {
         "sample_gaussian_kernel":
@@ -447,9 +452,9 @@ _KEPT_SASS_SHA256 = {
 
 
 @pytest.mark.skipif(shutil.which("nvcc") is None, reason="needs nvcc")
-def test_sac_kernels_compile_without_spills_and_existing_kernels_keep_their_code(tmp_path):
+def test_sac_ring_passes_compile_without_spills_and_existing_kernels_keep_their_code(tmp_path):
     stats, _ = _cubin(os.path.join(CSRC, "wdb_ddpg_update.cu"), tmp_path)
-    for k in ("sac_critic_kernel", "sac_actor_kernel"):
+    for k in ("sac_critic_kernel" + RING, "sac_actor_kernel" + RING):
         hits = [v for n, v in stats.items() if k in n]
         assert len(hits) == 1, (k, list(stats))
         assert hits[0]["spill"] == (0, 0), (k, hits[0])

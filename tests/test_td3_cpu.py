@@ -1,8 +1,8 @@
 """CPU tests of TD3: the float64 restatement of both update passes (tests/td3_update_reference.py)
 pinned to what TrainerTD3's torch update computes by autograd -- the real TD3 class and actor /
 critic modules, in float64; the ctypes layout of the new ABI struct; the support envelope; the
-run config and the refusals; what ptxas makes of the new kernels, and the fused DDPG update's
-kernels keeping their code."""
+run config and the refusals; what ptxas makes of the new kernels, and every kernel of the
+fused update file keeping its code."""
 import ctypes
 import hashlib
 import os
@@ -288,18 +288,44 @@ def _cubin(tmp_path):
     return stats, str(tmp_path / "k.cubin")
 
 
-# The normalised SASS (addresses and the kernel's own name dropped) of the fused DDPG update's
-# two kernels before the TD3 kernels joined their file, with nvcc 12.9.
+# Each update pass kernel is a template over its row source; these mangled-name fragments
+# select its instantiation over every window of the ring and over sampled windows.
+RING = "INS_9NoWindowsE"
+SAMPLED = "IPK4int2E"
+
+# The normalised SASS (addresses and the kernel's own name dropped) of every kernel of
+# wdb_ddpg_update.cu with nvcc 12.9: both instantiations of each pass, the reduction and DQN's
+# pass.
 _DDPG_SASS_SHA256 = {
-    "ddpg_update_kernel": "43727eb73fb299e5ca72c15d364be91aa0dc4bb253d8bcd24a5d3ef3d3cdd04f",
+    "ddpg_update_kernel" + RING:
+        "43727eb73fb299e5ca72c15d364be91aa0dc4bb253d8bcd24a5d3ef3d3cdd04f",
+    "td3_critic_kernel" + RING:
+        "9ea51c60bf071869f36de6c0668b280a7dc51dc454cd5abd4af04307c46f3ac4",
+    "td3_actor_kernel" + RING:
+        "baa1f44c5fde6671d02a45f1973dd31e95d8d52b2cd29ad6f81c106bc5a9b612",
+    "sac_critic_kernel" + RING:
+        "e963a0aa5bfe088ed0ac0b725bf126499d2386a18edfda269dd6c9078dbb4266",
+    "sac_actor_kernel" + RING:
+        "5e3dddfb3ee486667e1c9cc52d3fe31e7c70a2445be11b4e0f8cf8ecd3766537",
+    "ddpg_update_kernel" + SAMPLED:
+        "3c1bc0aad87b8df9296a4e1b260f6561df0e407bc08c6a97ac4f681cd717437e",
+    "td3_critic_kernel" + SAMPLED:
+        "bdb79e4a2a1926b5d2a56d689ceae355645d294d6a67bbf9c564d66a1b5a73bb",
+    "td3_actor_kernel" + SAMPLED:
+        "785909197a2abef31f4c2f8fdaf922101bf73d455fe421dbc2377bea8ab4a388",
+    "sac_critic_kernel" + SAMPLED:
+        "cc8270109477b67b20fd7165e43fee4063342aa9dc811c221db428abad943258",
+    "sac_actor_kernel" + SAMPLED:
+        "86bea485eed4957d8e592ffcd6888de1976c8e612d9d2266a7242acea2184237",
     "ddpg_reduce_kernel": "4ad80efbdf62dead0279d0872ad06dadfc625476fb41c2e1bf18b8292e280def",
+    "dqn_pass_kernel": "6ddc90ace4fb4f4e215234478611c5493c6e854d826da4ab2c899380da37d283",
 }
 
 
 @pytest.mark.skipif(shutil.which("nvcc") is None, reason="needs nvcc")
-def test_td3_kernels_compile_without_spills_and_ddpg_keeps_its_code(tmp_path):
+def test_td3_ring_passes_compile_without_spills_and_every_update_kernel_keeps_its_code(tmp_path):
     stats, cubin = _cubin(tmp_path)
-    for k in ("td3_critic_kernel", "td3_actor_kernel"):
+    for k in ("td3_critic_kernel" + RING, "td3_actor_kernel" + RING):
         hits = [v for n, v in stats.items() if k in n]
         assert len(hits) == 1, (k, list(stats))
         assert hits[0]["spill"] == (0, 0), (k, hits[0])
@@ -314,6 +340,7 @@ def test_td3_kernels_compile_without_spills_and_ddpg_keeps_its_code(tmp_path):
         if m:
             cur = next((k for k in _DDPG_SASS_SHA256 if k in m.group(1)), None)
             if cur is not None:
+                assert cur not in funcs, (cur, m.group(1))
                 funcs[cur] = []
         elif cur is not None:
             funcs[cur].append(re.sub(r"/\*[0-9a-f]{4}\*/", "", line).rstrip())

@@ -34,9 +34,11 @@
 //     through Q1 to its action inputs only (no critic weight gradient), the tanh head and the
 //     actor.
 //
-// Replay buffer (wdb_*_update_sampled): each of the five passes also exists over B sampled
-// windows of a long ring, row g = windows[g] instead of (g / EN, g % EN) -- the *_sampled
-// kernels after the ring kernels.
+// Replay buffer (wdb_*_update_sampled): each of the five passes also runs over B sampled
+// windows of a long ring, row g = windows[g] instead of (g / EN, g % EN) -- the same kernel
+// template instantiated for the other row source ("loss rows" below).
+#include <type_traits>
+
 #include "wdb_common.cuh"
 
 using namespace wdb;
@@ -288,9 +290,66 @@ __device__ void load_net(float *dst, const wdb_ddpg_net &net, const Plan &P, int
   }
 }
 
+// ---------------------------------------------------------------------------- loss rows
+// Every pass kernel is a template over its row source, Windows:
+//   NoWindows      every window of the ring: row g is logical window i = g / EN (slots from
+//                  `cursor`) of agent row n = g % EN, and the last window bootstraps from slot
+//                  C - 1 undiscounted (ddpg.py:62-79);
+//   const int2 *   B sampled windows (wdb_replay_windows): row g = windows[g], M = B, and every
+//                  window bootstraps discounted.
+// The two differ only in where a row's step-0 and bootstrap slots are and in the n-step
+// return; a kernel picks them with `if constexpr (kSampled)`.  The ring branches keep their
+// statements in the order the pinned machine code (tests/test_td3_cpu.py) was compiled from:
+// nvcc 12.9 allocates registers differently when they are reordered, so a value the code after
+// a branch uses is declared before it and assigned inside, and nothing is hoisted out of it.
+struct NoWindows {};
+
+// A sampled loss row: the n-step window of agent row n (env * Np + agent) whose step 0 is at
+// physical ring slot s.
+struct Row {
+  int s;
+  long long n;
+};
+
+// The sampled row source: row g = windows[g] = {s, n}, any n_step + 1 consecutive slots (mod C)
+// of the ring, in any order, duplicates allowed.  slot(w, j) is the physical slot of the
+// window's step j; step n_step holds the bootstrap observation.
+struct SampledRows {
+  const int2 *windows;
+  int C;
+  __device__ __forceinline__ Row at(long long g) const {
+    const int2 w = windows[g];
+    return {w.x, w.y};
+  }
+  __device__ __forceinline__ int slot(const Row &w, int j) const {
+    const int s = w.s + j;
+    return s >= C ? s - C : s;
+  }
+};
+
+// The n-step return of sampled window w from its bootstrap value qt: the recursion of a
+// regular window of the ring in the same float32 operations, for all three algorithms'
+// argument structs.
+template <class Args>
+__device__ __forceinline__ float sampled_return(const Args &U, const Plan &P,
+                                                const SampledRows &rows, const Row &w, float qt) {
+  const int ns = U.n_step;
+  const long long EN = P.EN, E = U.n_envs, n = w.n, env = n / U.n_agents;
+  float ret = qt;
+  for (int j = ns - 1; j >= 0; j--) {
+    const int pk = rows.slot(w, j);
+    const float dk = (float)U.done[(long long)pk * E + env];
+    const float rk = U.rewards[(long long)pk * EN + n];
+    ret = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(1.0f, dk), U.gamma), ret), rk);
+  }
+  return ret;
+}
+
+template <class Windows>
 __global__ void __launch_bounds__(kThreads, 1)
 ddpg_update_kernel(const __grid_constant__ wdb_ddpg_update_args U, const __grid_constant__ Plan Pg,
-                   float *partials, double *psums) {
+                   float *partials, double *psums, Windows windows) {
+  constexpr bool kSampled = !std::is_same<Windows, NoWindows>::value;
   extern __shared__ __align__(16) float smem[];
   __shared__ Plan P;                           // dynamic indexing of the kernel parameter goes
   __shared__ double s_err[kRows], s_j[kRows];  // through local memory: copy it once
@@ -334,14 +393,26 @@ ddpg_update_kernel(const __grid_constant__ wdb_ddpg_update_args U, const __grid_
       const long long g = g0 + r;
       float xq = 0.0f, xt = 0.0f;
       if (g < M) {
-        const int i = (int)(g / EN);
-        const long long n = g - (long long)i * EN;
-        const long long row = (long long)phys(i) * EN + n;
-        if (c < F) {
-          xq = U.obs[row * F + c];
-          xt = U.obs[((long long)phys(target_slot(i)) * EN + n) * F + c];
+        if constexpr (kSampled) {
+          const SampledRows rows = {windows, C};
+          const Row w = rows.at(g);
+          const long long row = (long long)rows.slot(w, 0) * EN + w.n;
+          if (c < F) {
+            xq = U.obs[row * F + c];
+            xt = U.obs[((long long)rows.slot(w, ns) * EN + w.n) * F + c];
+          } else {
+            xq = U.actions[row * A + (c - F)];
+          }
         } else {
-          xq = U.actions[row * A + (c - F)];
+          const int i = (int)(g / EN);
+          const long long n = g - (long long)i * EN;
+          const long long row = (long long)phys(i) * EN + n;
+          if (c < F) {
+            xq = U.obs[row * F + c];
+            xt = U.obs[((long long)phys(target_slot(i)) * EN + n) * F + c];
+          } else {
+            xq = U.actions[row * A + (c - F)];
+          }
         }
       }
       XQ[r * kPitch + c] = xq;
@@ -378,20 +449,31 @@ ddpg_update_kernel(const __grid_constant__ wdb_ddpg_update_args U, const __grid_
       const long long g = g0 + r;
       float dq = 0.0f, dj = 0.0f;
       if (g < M) {
-        const int i = (int)(g / EN);
-        const long long n = g - (long long)i * EN, env = n / Np;
-        const float qt = V[r * kPitch], q = V[r * kPitch + 1], jv = V[r * kPitch + 2];
-        const int pl = phys(i + ns - 1);
-        const float rl = U.rewards[(long long)pl * EN + n];
-        const float dl = (float)U.done[(long long)pl * E + env];
-        const float om = __fsub_rn(1.0f, dl);
-        float ret = i < valid - 1 ? __fadd_rn(rl, __fmul_rn(__fmul_rn(om, gamma), qt))
-                                  : __fadd_rn(__fmul_rn(dl, rl), __fmul_rn(om, qt));
-        for (int j = 1; j < ns; j++) {
-          const int pk = phys(ns - 1 - j + i);
-          const float dk = (float)U.done[(long long)pk * E + env];
-          ret = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(1.0f, dk), gamma), ret),
-                          U.rewards[(long long)pk * EN + n]);
+        float q, jv, ret;
+        if constexpr (kSampled) {
+          const SampledRows rows = {windows, C};
+          const float qt = V[r * kPitch];
+          q = V[r * kPitch + 1];
+          jv = V[r * kPitch + 2];
+          ret = sampled_return(U, P, rows, rows.at(g), qt);
+        } else {
+          const int i = (int)(g / EN);
+          const long long n = g - (long long)i * EN, env = n / Np;
+          const float qt = V[r * kPitch];
+          q = V[r * kPitch + 1];
+          jv = V[r * kPitch + 2];
+          const int pl = phys(i + ns - 1);
+          const float rl = U.rewards[(long long)pl * EN + n];
+          const float dl = (float)U.done[(long long)pl * E + env];
+          const float om = __fsub_rn(1.0f, dl);
+          ret = i < valid - 1 ? __fadd_rn(rl, __fmul_rn(__fmul_rn(om, gamma), qt))
+                              : __fadd_rn(__fmul_rn(dl, rl), __fmul_rn(om, qt));
+          for (int j = 1; j < ns; j++) {
+            const int pk = phys(ns - 1 - j + i);
+            const float dk = (float)U.done[(long long)pk * E + env];
+            ret = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(1.0f, dk), gamma), ret),
+                            U.rewards[(long long)pk * EN + n]);
+          }
         }
         const float diff = __fsub_rn(q, ret);
         dq = __fmul_rn(diff, norm_q);
@@ -497,9 +579,11 @@ __device__ __forceinline__ float td3_return(const Args &U, const Plan &P, int i,
 }
 
 // Critic pass: the gradients of mse(Q1, R) + mse(Q2, R) into per-CTA partials [G1 | G2].
+template <class Windows>
 __global__ void __launch_bounds__(kThreads, 1)
 td3_critic_kernel(const __grid_constant__ wdb_td3_update_args U, const __grid_constant__ Plan Pg,
-                  float *partials, double *psums) {
+                  float *partials, double *psums, Windows windows) {
+  constexpr bool kSampled = !std::is_same<Windows, NoWindows>::value;
   extern __shared__ __align__(16) float smem[];
   __shared__ Plan P;
   __shared__ double s_e1[kRows], s_e2[kRows];
@@ -545,14 +629,26 @@ td3_critic_kernel(const __grid_constant__ wdb_td3_update_args U, const __grid_co
       const long long g = g0 + r;
       float xq = 0.0f, xt = 0.0f;
       if (g < M) {
-        const int i = (int)(g / EN);
-        const long long n = g - (long long)i * EN;
-        const long long row = (long long)phys(i) * EN + n;
-        if (c < F) {
-          xq = U.obs[row * F + c];
-          xt = U.obs[((long long)phys(target_slot(i)) * EN + n) * F + c];
+        if constexpr (kSampled) {
+          const SampledRows rows = {windows, C};
+          const Row w = rows.at(g);
+          const long long row = (long long)rows.slot(w, 0) * EN + w.n;
+          if (c < F) {
+            xq = U.obs[row * F + c];
+            xt = U.obs[((long long)rows.slot(w, ns) * EN + w.n) * F + c];
+          } else {
+            xq = U.actions[row * A + (c - F)];
+          }
         } else {
-          xq = U.actions[row * A + (c - F)];
+          const int i = (int)(g / EN);
+          const long long n = g - (long long)i * EN;
+          const long long row = (long long)phys(i) * EN + n;
+          if (c < F) {
+            xq = U.obs[row * F + c];
+            xt = U.obs[((long long)phys(target_slot(i)) * EN + n) * F + c];
+          } else {
+            xq = U.actions[row * A + (c - F)];
+          }
         }
       }
       XQ[r * kPitch + c] = xq;
@@ -586,11 +682,21 @@ td3_critic_kernel(const __grid_constant__ wdb_td3_update_args U, const __grid_co
       const long long g = g0 + r;
       float d1 = 0.0f, d2 = 0.0f;
       if (g < M) {
-        const int i = (int)(g / EN);
-        const long long n = g - (long long)i * EN;
-        const float qt = fminf(V[r * kPitch], V[r * kPitch + 1]);
-        const float q1 = V[r * kPitch + 2], q2 = V[r * kPitch + 3];
-        const float ret = td3_return(U, P, i, n, qt);
+        float q1, q2, ret;
+        if constexpr (kSampled) {
+          const SampledRows rows = {windows, C};
+          const float qt = fminf(V[r * kPitch], V[r * kPitch + 1]);
+          q1 = V[r * kPitch + 2];
+          q2 = V[r * kPitch + 3];
+          ret = sampled_return(U, P, rows, rows.at(g), qt);
+        } else {
+          const int i = (int)(g / EN);
+          const long long n = g - (long long)i * EN;
+          const float qt = fminf(V[r * kPitch], V[r * kPitch + 1]);
+          q1 = V[r * kPitch + 2];
+          q2 = V[r * kPitch + 3];
+          ret = td3_return(U, P, i, n, qt);
+        }
         const float e1 = __fsub_rn(q1, ret), e2 = __fsub_rn(q2, ret);
         d1 = __fmul_rn(e1, norm_q);
         d2 = __fmul_rn(e2, norm_q);
@@ -631,9 +737,11 @@ td3_critic_kernel(const __grid_constant__ wdb_td3_update_args U, const __grid_co
 
 // Actor pass: the gradient of -mean Q1(obs, actor(obs)) into per-CTA actor partials; the
 // critic's weights only carry the gradient to its action inputs.
+template <class Windows>
 __global__ void __launch_bounds__(kThreads, 1)
 td3_actor_kernel(const __grid_constant__ wdb_td3_update_args U, const __grid_constant__ Plan Pg,
-                 float *partials, double *psums) {
+                 float *partials, double *psums, Windows windows) {
+  constexpr bool kSampled = !std::is_same<Windows, NoWindows>::value;
   extern __shared__ __align__(16) float smem[];
   __shared__ Plan P;
   __shared__ double s_j[kRows];
@@ -670,9 +778,15 @@ td3_actor_kernel(const __grid_constant__ wdb_td3_update_args U, const __grid_con
       const long long g = g0 + r;
       float x = 0.0f;
       if (g < M) {
-        const int i = (int)(g / EN);
-        const long long n = g - (long long)i * EN;
-        x = U.obs[((long long)phys(i) * EN + n) * F + c];
+        if constexpr (kSampled) {
+          const SampledRows rows = {windows, C};
+          const Row w = rows.at(g);
+          x = U.obs[((long long)rows.slot(w, 0) * EN + w.n) * F + c];
+        } else {
+          const int i = (int)(g / EN);
+          const long long n = g - (long long)i * EN;
+          x = U.obs[((long long)phys(i) * EN + n) * F + c];
+        }
       }
       XJ[r * kPitch + c] = x;
     }
@@ -754,9 +868,11 @@ __device__ __forceinline__ SquashedDim squashed_dim(const float *z, int A, int c
 
 // Critic pass: the gradients of mse(Q1, R) + mse(Q2, R) into per-CTA partials [G1 | G2], R
 // bootstrapped with min(Q1', Q2')(obs', a') - alpha log pi(a' | obs'), a' from the actor.
+template <class Windows>
 __global__ void __launch_bounds__(kThreads, 1)
 sac_critic_kernel(const __grid_constant__ wdb_sac_update_args U, const __grid_constant__ Plan Pg,
-                  float *partials, double *psums) {
+                  float *partials, double *psums, Windows windows) {
+  constexpr bool kSampled = !std::is_same<Windows, NoWindows>::value;
   extern __shared__ __align__(16) float smem[];
   __shared__ Plan P;
   __shared__ double s_e1[kRows], s_e2[kRows];
@@ -802,14 +918,26 @@ sac_critic_kernel(const __grid_constant__ wdb_sac_update_args U, const __grid_co
       const long long g = g0 + r;
       float xq = 0.0f, xt = 0.0f;
       if (g < M) {
-        const int i = (int)(g / EN);
-        const long long n = g - (long long)i * EN;
-        const long long row = (long long)phys(i) * EN + n;
-        if (c < F) {
-          xq = U.obs[row * F + c];
-          xt = U.obs[((long long)phys(target_slot(i)) * EN + n) * F + c];
+        if constexpr (kSampled) {
+          const SampledRows rows = {windows, C};
+          const Row w = rows.at(g);
+          const long long row = (long long)rows.slot(w, 0) * EN + w.n;
+          if (c < F) {
+            xq = U.obs[row * F + c];
+            xt = U.obs[((long long)rows.slot(w, ns) * EN + w.n) * F + c];
+          } else {
+            xq = U.actions[row * A + (c - F)];
+          }
         } else {
-          xq = U.actions[row * A + (c - F)];
+          const int i = (int)(g / EN);
+          const long long n = g - (long long)i * EN;
+          const long long row = (long long)phys(i) * EN + n;
+          if (c < F) {
+            xq = U.obs[row * F + c];
+            xt = U.obs[((long long)phys(target_slot(i)) * EN + n) * F + c];
+          } else {
+            xq = U.actions[row * A + (c - F)];
+          }
         }
       }
       XQ[r * kPitch + c] = xq;
@@ -843,13 +971,25 @@ sac_critic_kernel(const __grid_constant__ wdb_sac_update_args U, const __grid_co
       const long long g = g0 + r;
       float d1 = 0.0f, d2 = 0.0f;
       if (g < M) {
-        const int i = (int)(g / EN);
-        const long long n = g - (long long)i * EN;
-        float lp = 0.0f;
-        for (int c = 0; c < A; c++) lp += Z[r * kPitch + c];
-        const float qt = __fsub_rn(fminf(V[r * kPitch], V[r * kPitch + 1]), __fmul_rn(alpha, lp));
-        const float q1 = V[r * kPitch + 2], q2 = V[r * kPitch + 3];
-        const float ret = td3_return(U, P, i, n, qt);
+        float q1, q2, ret;
+        if constexpr (kSampled) {
+          const SampledRows rows = {windows, C};
+          float lp = 0.0f;
+          for (int c = 0; c < A; c++) lp += Z[r * kPitch + c];
+          const float qt = __fsub_rn(fminf(V[r * kPitch], V[r * kPitch + 1]), __fmul_rn(alpha, lp));
+          q1 = V[r * kPitch + 2];
+          q2 = V[r * kPitch + 3];
+          ret = sampled_return(U, P, rows, rows.at(g), qt);
+        } else {
+          const int i = (int)(g / EN);
+          const long long n = g - (long long)i * EN;
+          float lp = 0.0f;
+          for (int c = 0; c < A; c++) lp += Z[r * kPitch + c];
+          const float qt = __fsub_rn(fminf(V[r * kPitch], V[r * kPitch + 1]), __fmul_rn(alpha, lp));
+          q1 = V[r * kPitch + 2];
+          q2 = V[r * kPitch + 3];
+          ret = td3_return(U, P, i, n, qt);
+        }
         const float e1 = __fsub_rn(q1, ret), e2 = __fsub_rn(q2, ret);
         d1 = __fmul_rn(e1, norm_q);
         d2 = __fmul_rn(e2, norm_q);
@@ -892,9 +1032,11 @@ sac_critic_kernel(const __grid_constant__ wdb_sac_update_args U, const __grid_co
 // actor partials.  Both critics run forward; the one the minimum picks (ties: Q1) carries the
 // row's gradient to its action inputs (the other's row delta is 0), then through the tanh,
 // the reparameterisation and the clamp into mu and the log-std.
+template <class Windows>
 __global__ void __launch_bounds__(kThreads, 1)
 sac_actor_kernel(const __grid_constant__ wdb_sac_update_args U, const __grid_constant__ Plan Pg,
-                 float *partials, double *psums) {
+                 float *partials, double *psums, Windows windows) {
+  constexpr bool kSampled = !std::is_same<Windows, NoWindows>::value;
   extern __shared__ __align__(16) float smem[];
   __shared__ Plan P;
   __shared__ double s_q[kRows], s_lp[kRows];
@@ -937,685 +1079,15 @@ sac_actor_kernel(const __grid_constant__ wdb_sac_update_args U, const __grid_con
       const long long g = g0 + r;
       float x = 0.0f;
       if (g < M) {
-        const int i = (int)(g / EN);
-        const long long n = g - (long long)i * EN;
-        x = U.obs[((long long)phys(i) * EN + n) * F + c];
-      }
-      XJ[r * kPitch + c] = x;
-    }
-    __syncthreads();
-    // ---- actor -> a into XJ's action columns (log-prob terms into DA); Q1, Q2 on (obs, a)
-    net_forward(Wa, P, 0, XJ, [&](int l) { return l == P.L[0] - 1 ? Z : HA + l * kTile; });
-    for (int e = tid; e < kRows * A; e += kThreads) {
-      const int r = e / A, c = e - r * A;
-      const long long g = g0 + r;
-      const float eps = g < M ? U.actor_noise[g * A + c] : 0.0f;
-      const SquashedDim s = squashed_dim(Z + r * kPitch, A, c, eps, lo, hi);
-      XJ[r * kPitch + F + c] = __fadd_rn(__fmul_rn(scale, s.y), bias);
-      DA[r * kPitch + c] = s.term;
-    }
-    __syncthreads();
-    net_forward(Wc1, P, 1, XJ, [&](int l) { return l == P.L[1] - 1 ? V : H1 + l * kTile; });
-    net_forward(Wc2, P, 1, XJ, [&](int l) { return l == P.L[1] - 1 ? V + 1 : H2 + l * kTile; });
-    if (tid < kRows) {
-      const int r = tid;
-      const long long g = g0 + r;
-      float d1 = 0.0f, d2 = 0.0f;
-      if (g < M) {
-        const float q1 = V[r * kPitch], q2 = V[r * kPitch + 1];
-        const bool first = q1 <= q2;
-        float lp = 0.0f;
-        for (int c = 0; c < A; c++) lp += DA[r * kPitch + c];
-        d1 = first ? d_q : 0.0f;
-        d2 = first ? 0.0f : d_q;
-        q_acc += (double)(first ? q1 : q2);
-        lp_acc += (double)lp;
-        if (U.log_probs) U.log_probs[g] = lp;
-      }
-      V[r * kPitch + 8] = d1;
-      V[r * kPitch + 12] = d2;
-    }
-    __syncthreads();
-    // ---- backward: Q1 to its action inputs (kept in DA), Q2 likewise
-    const float *da1 = net_backward<false>(
-        Wc1, P, 1, nullptr, V + 8, [&](int l) { return l == 0 ? XJ : H1 + (l - 1) * kTile; },
-        D0, D1, F);
-    for (int e = tid; e < kRows * A; e += kThreads) {
-      const int r = e / A, c = e - r * A;
-      DA[r * kPitch + c] = da1[r * kPitch + F + c];
-    }
-    __syncthreads();
-    const float *da2 = net_backward<false>(
-        Wc2, P, 1, nullptr, V + 12, [&](int l) { return l == 0 ? XJ : H2 + (l - 1) * kTile; },
-        D0, D1, F);
-    // ---- the tanh, the reparameterisation, the log-prob's own terms and the clamp
-    float *dz = da2 == D0 ? D1 : D0;
-    for (int e = tid; e < kRows * A; e += kThreads) {
-      const int r = e / A, c = e - r * A;
-      const long long g = g0 + r;
-      float dmu = 0.0f, dls = 0.0f;
-      if (g < M) {
-        const float eps = U.actor_noise[g * A + c];
-        const SquashedDim s = squashed_dim(Z + r * kPitch, A, c, eps, lo, hi);
-        const float da = __fadd_rn(DA[r * kPitch + c], da2[r * kPitch + F + c]);
-        const float du = fmaf(__fmul_rn(da, scale), __fsub_rn(1.0f, __fmul_rn(s.y, s.y)),
-                              __fmul_rn(d_lp, 2.0f * s.y));
-        dmu = du;
-        dls = s.in_range ? fmaf(__fmul_rn(du, s.sigma), eps, -d_lp) : 0.0f;
-      }
-      dz[r * kPitch + c] = dmu;
-      dz[r * kPitch + A + c] = dls;
-    }
-    __syncthreads();
-    net_backward(Wa, P, 0, Ga, dz, [&](int l) { return l == 0 ? XJ : HA + (l - 1) * kTile; },
-                 D0, D1, -1);
-  }
-
-  float *part = partials + (long long)blockIdx.x * g_total;
-  for (int e = tid; e < g_total; e += kThreads) part[e] = Ga[e];
-  if (tid < kRows) {
-    s_q[tid] = q_acc;
-    s_lp[tid] = lp_acc;
-  }
-  __syncthreads();
-  if (tid == 0) {
-    double a = 0.0, b = 0.0;
-    for (int r = 0; r < kRows; r++) {
-      a += s_q[r];
-      b += s_lp[r];
-    }
-    psums[2 * blockIdx.x] = a;
-    psums[2 * blockIdx.x + 1] = b;
-  }
-}
-
-// ---------------------------------------------------------------------------- sampled rows
-// The five passes over B sampled windows (wdb_replay_windows) instead of every window of the
-// ring: the kernels above with a different row source, M = B and no last-window rule, on the
-// same tile primitives, Plan layout and reduction.  They are separate kernels because the ring
-// kernels' machine code is pinned (tests/test_td3_cpu.py) and does not survive being
-// instantiated from a shared template.
-
-// A sampled loss row: the n-step window of agent row n (env * Np + agent) whose step 0 is at
-// physical ring slot s.
-struct Row {
-  int s;
-  long long n;
-};
-
-// The row source of the *_sampled kernels: row g = windows[g] = {s, n}, any n_step + 1
-// consecutive slots (mod C) of the ring, in any order, duplicates allowed.  slot(w, j) is the
-// physical slot of the window's step j; step n_step holds the bootstrap observation.  Unlike the
-// ring kernels' last window, every window bootstraps discounted.
-struct SampledRows {
-  const int2 *windows;
-  int C;
-  __device__ __forceinline__ Row at(long long g) const {
-    const int2 w = windows[g];
-    return {w.x, w.y};
-  }
-  __device__ __forceinline__ int slot(const Row &w, int j) const {
-    const int s = w.s + j;
-    return s >= C ? s - C : s;
-  }
-};
-
-// The n-step return of sampled window w from its bootstrap value qt: the recursion of a
-// regular window of the ring kernels in the same float32 operations, for all three algorithms'
-// argument structs.
-template <class Args>
-__device__ __forceinline__ float sampled_return(const Args &U, const Plan &P,
-                                                const SampledRows &rows, const Row &w, float qt) {
-  const int ns = U.n_step;
-  const long long EN = P.EN, E = U.n_envs, n = w.n, env = n / U.n_agents;
-  float ret = qt;
-  for (int j = ns - 1; j >= 0; j--) {
-    const int pk = rows.slot(w, j);
-    const float dk = (float)U.done[(long long)pk * E + env];
-    const float rk = U.rewards[(long long)pk * EN + n];
-    ret = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(1.0f, dk), U.gamma), ret), rk);
-  }
-  return ret;
-}
-
-// ddpg_update_kernel over sampled windows.
-__global__ void __launch_bounds__(kThreads, 1)
-ddpg_update_sampled(const __grid_constant__ wdb_ddpg_update_args U, const __grid_constant__ Plan Pg,
-                    float *partials, double *psums, const int2 *windows) {
-  extern __shared__ __align__(16) float smem[];
-  __shared__ Plan P;                           // dynamic indexing of the kernel parameter goes
-  __shared__ double s_err[kRows], s_j[kRows];  // through local memory: copy it once
-  if (threadIdx.x == 0) P = Pg;
-  __syncthreads();
-  const int tid = threadIdx.x;
-  float *Wa = smem, *Wc = Wa + P.wfloats[0], *Wta = Wc + P.wfloats[1], *Wtc = Wta + P.wfloats[0];
-  float *Ga = Wtc + P.wfloats[1], *Gc = Ga + P.gfloats[0];
-  const int g_total = P.gfloats[0] + P.gfloats[1];
-  float *XQ = Ga + ((g_total + 3) / 4) * 4;      // obs ++ actions
-  float *XJ = XQ + kTile;                      // obs ++ pi (target path: scratch)
-  float *V = XJ + kTile;                       // columns: 0 target Q, 1 Q, 2 J, 4 dQ, 8 dJ
-  float *Z = V + kTile;                        // actor head pre-activation
-  float *D0 = Z + kTile, *D1 = D0 + kTile;     // deltas (target path: obs' and scratch)
-  float *HQ = D1 + kTile;                      // critic hidden outputs, (obs, actions) path
-  float *HJ = HQ + (P.L[1] - 1) * kTile;       // critic hidden outputs, (obs, pi) path
-  float *HA = HJ + (P.L[1] - 1) * kTile;       // actor hidden outputs
-
-  load_net(Wa, U.actor, P, 0);
-  load_net(Wc, U.critic, P, 1);
-  load_net(Wta, U.target_actor, P, 0);
-  load_net(Wtc, U.target_critic, P, 1);
-  for (int e = tid; e < g_total; e += kThreads) Ga[e] = 0.0f;
-  for (int e = tid; e < P.n_buf * kTile; e += kThreads) XQ[e] = 0.0f;
-  __syncthreads();
-
-  const int F = U.obs_dim, A = U.action_dim, FA = F + A;
-  const SampledRows rows = {windows, U.capacity};
-  const long long EN = P.EN, M = P.M;
-  const float scale = U.action_scale, bias = U.action_bias;
-  const float norm_q = (float)(2.0 / (double)M);         // mse_loss backward: 2 / numel
-  const float d_j = -1.0f / (float)M;                    // -mean backward
-  double err_acc = 0.0, j_acc = 0.0;
-
-  for (long long g0 = (long long)blockIdx.x * kRows; g0 < M; g0 += (long long)gridDim.x * kRows) {
-    // ---- inputs: XQ = obs ++ actions at slot i, D0 = obs at the bootstrap slot
-    for (int e = tid; e < kRows * FA; e += kThreads) {
-      const int r = e / FA, c = e - r * FA;
-      const long long g = g0 + r;
-      float xq = 0.0f, xt = 0.0f;
-      if (g < M) {
-        const Row w = rows.at(g);
-        const long long row = (long long)rows.slot(w, 0) * EN + w.n;
-        if (c < F) {
-          xq = U.obs[row * F + c];
-          xt = U.obs[((long long)rows.slot(w, U.n_step) * EN + w.n) * F + c];
+        if constexpr (kSampled) {
+          const SampledRows rows = {windows, C};
+          const Row w = rows.at(g);
+          x = U.obs[((long long)rows.slot(w, 0) * EN + w.n) * F + c];
         } else {
-          xq = U.actions[row * A + (c - F)];
+          const int i = (int)(g / EN);
+          const long long n = g - (long long)i * EN;
+          x = U.obs[((long long)phys(i) * EN + n) * F + c];
         }
-      }
-      XQ[r * kPitch + c] = xq;
-      if (c < F) D0[r * kPitch + c] = xt;
-    }
-    __syncthreads();
-    // ---- target actor -> a' = scale * tanh(z) + bias into D0's action columns
-    net_forward(Wta, P, 0, D0,
-                [&](int l) { return l == P.L[0] - 1 ? Z : (l % 2 == 0 ? D1 : XJ); });
-    for (int e = tid; e < kRows * A; e += kThreads) {
-      const int r = e / A, c = e - r * A;
-      D0[r * kPitch + F + c] = __fadd_rn(__fmul_rn(scale, tanhf(Z[r * kPitch + c])), bias);
-    }
-    __syncthreads();
-    // ---- target critic -> V[., 0]; critic on (obs, actions) -> V[., 1]; actor -> Z
-    net_forward(Wtc, P, 1, D0,
-                [&](int l) { return l == P.L[1] - 1 ? V : (l % 2 == 0 ? D1 : XJ); });
-    net_forward(Wc, P, 1, XQ,
-                [&](int l) { return l == P.L[1] - 1 ? V + 1 : HQ + l * kTile; });
-    net_forward(Wa, P, 0, XQ,
-                [&](int l) { return l == P.L[0] - 1 ? Z : HA + l * kTile; });
-    // ---- critic on (obs, pi) -> V[., 2]
-    for (int e = tid; e < kRows * FA; e += kThreads) {
-      const int r = e / FA, c = e - r * FA;
-      XJ[r * kPitch + c] = c < F ? XQ[r * kPitch + c]
-                                 : __fadd_rn(__fmul_rn(scale, tanhf(Z[r * kPitch + c - F])), bias);
-    }
-    __syncthreads();
-    net_forward(Wc, P, 1, XJ,
-                [&](int l) { return l == P.L[1] - 1 ? V + 2 : HJ + l * kTile; });
-    // ---- n-step return (ddpg.py:62-79, same float32 operations) and the loss gradients
-    if (tid < kRows) {
-      const int r = tid;
-      const long long g = g0 + r;
-      float dq = 0.0f, dj = 0.0f;
-      if (g < M) {
-        const float qt = V[r * kPitch], q = V[r * kPitch + 1], jv = V[r * kPitch + 2];
-        const float ret = sampled_return(U, P, rows, rows.at(g), qt);
-        const float diff = __fsub_rn(q, ret);
-        dq = __fmul_rn(diff, norm_q);
-        dj = d_j;
-        err_acc += (double)diff * (double)diff;
-        j_acc += (double)jv;
-        if (U.values) U.values[g] = q;
-        if (U.j_values) U.j_values[g] = jv;
-        if (U.returns) U.returns[g] = ret;
-      }
-      V[r * kPitch + 4] = dq;
-      V[r * kPitch + 8] = dj;
-    }
-    __syncthreads();
-    // ---- backward: critic on both paths, then the tanh head and the actor
-    net_backward(Wc, P, 1, Gc, V + 4,
-                 [&](int l) { return l == 0 ? XQ : HQ + (l - 1) * kTile; }, D0, D1, -1);
-    const float *dpi = net_backward(
-        Wc, P, 1, Gc, V + 8, [&](int l) { return l == 0 ? XJ : HJ + (l - 1) * kTile; }, D0, D1, F);
-    float *dz = dpi == D0 ? D1 : D0;
-    for (int e = tid; e < kRows * A; e += kThreads) {
-      const int r = e / A, c = e - r * A;
-      const float y = tanhf(Z[r * kPitch + c]);
-      dz[r * kPitch + c] = __fmul_rn(__fmul_rn(dpi[r * kPitch + F + c], scale),
-                                     __fsub_rn(1.0f, __fmul_rn(y, y)));
-    }
-    __syncthreads();
-    net_backward(Wa, P, 0, Ga, dz, [&](int l) { return l == 0 ? XQ : HA + (l - 1) * kTile; },
-                 D0, D1, -1);
-  }
-
-  // ---- this CTA's partials
-  float *part = partials + (long long)blockIdx.x * g_total;
-  for (int e = tid; e < g_total; e += kThreads) part[e] = Ga[e];
-  if (tid < kRows) {
-    s_err[tid] = err_acc;
-    s_j[tid] = j_acc;
-  }
-  __syncthreads();
-  if (tid == 0) {
-    double a = 0.0, b = 0.0;
-    for (int r = 0; r < kRows; r++) {
-      a += s_err[r];
-      b += s_j[r];
-    }
-    psums[2 * blockIdx.x] = a;
-    psums[2 * blockIdx.x + 1] = b;
-  }
-}
-
-// td3_critic_kernel over sampled windows.
-__global__ void __launch_bounds__(kThreads, 1)
-td3_critic_sampled(const __grid_constant__ wdb_td3_update_args U, const __grid_constant__ Plan Pg,
-                   float *partials, double *psums, const int2 *windows) {
-  extern __shared__ __align__(16) float smem[];
-  __shared__ Plan P;
-  __shared__ double s_e1[kRows], s_e2[kRows];
-  if (threadIdx.x == 0) P = Pg;
-  __syncthreads();
-  const int tid = threadIdx.x;
-  float *Wta = smem, *Wc1 = Wta + P.wfloats[0], *Wc2 = Wc1 + P.wfloats[1];
-  float *Wt1 = Wc2 + P.wfloats[1], *Wt2 = Wt1 + P.wfloats[1];
-  float *G1 = Wt2 + P.wfloats[1], *G2 = G1 + P.gfloats[1];
-  const int g_total = 2 * P.gfloats[1];
-  float *XQ = G1 + ((g_total + 3) / 4) * 4;      // obs ++ actions
-  float *XS = XQ + kTile;                      // scratch of the target forwards
-  float *V = XS + kTile;                       // columns: 0 Q1', 1 Q2', 2 Q1, 3 Q2, 4 dQ1, 8 dQ2
-  float *Z = V + kTile;                        // target actor head pre-activation
-  float *D0 = Z + kTile, *D1 = D0 + kTile;     // deltas (target path: obs' ++ a' and scratch)
-  float *H1 = D1 + kTile;                      // Q1 hidden outputs
-  float *H2 = H1 + (P.L[1] - 1) * kTile;       // Q2 hidden outputs
-
-  load_net(Wta, U.target_actor, P, 0);
-  load_net(Wc1, U.critic, P, 1);
-  load_net(Wc2, U.critic2, P, 1);
-  load_net(Wt1, U.target_critic, P, 1);
-  load_net(Wt2, U.target_critic2, P, 1);
-  for (int e = tid; e < g_total; e += kThreads) G1[e] = 0.0f;
-  for (int e = tid; e < P.n_buf * kTile; e += kThreads) XQ[e] = 0.0f;
-  __syncthreads();
-
-  const int F = U.obs_dim, A = U.action_dim, FA = F + A;
-  const SampledRows rows = {windows, U.capacity};
-  const long long EN = P.EN, M = P.M;
-  const float scale = U.action_scale, bias = U.action_bias;
-  const float sd = __fmul_rn(U.target_noise, scale), clip = __fmul_rn(U.target_noise_clip, scale);
-  const float lo = __fsub_rn(bias, scale), hi = __fadd_rn(bias, scale);
-  const float norm_q = (float)(2.0 / (double)M);
-  double e1_acc = 0.0, e2_acc = 0.0;
-
-  for (long long g0 = (long long)blockIdx.x * kRows; g0 < M; g0 += (long long)gridDim.x * kRows) {
-    // ---- inputs: XQ = obs ++ actions at slot i, D0 = obs at the bootstrap slot
-    for (int e = tid; e < kRows * FA; e += kThreads) {
-      const int r = e / FA, c = e - r * FA;
-      const long long g = g0 + r;
-      float xq = 0.0f, xt = 0.0f;
-      if (g < M) {
-        const Row w = rows.at(g);
-        const long long row = (long long)rows.slot(w, 0) * EN + w.n;
-        if (c < F) {
-          xq = U.obs[row * F + c];
-          xt = U.obs[((long long)rows.slot(w, U.n_step) * EN + w.n) * F + c];
-        } else {
-          xq = U.actions[row * A + (c - F)];
-        }
-      }
-      XQ[r * kPitch + c] = xq;
-      if (c < F) D0[r * kPitch + c] = xt;
-    }
-    __syncthreads();
-    // ---- target actor + clipped noise -> a' into D0's action columns
-    net_forward(Wta, P, 0, D0,
-                [&](int l) { return l == P.L[0] - 1 ? Z : (l % 2 == 0 ? D1 : XS); });
-    for (int e = tid; e < kRows * A; e += kThreads) {
-      const int r = e / A, c = e - r * A;
-      const long long g = g0 + r;
-      const float pi = __fadd_rn(__fmul_rn(scale, tanhf(Z[r * kPitch + c])), bias);
-      const float eps = g < M ? U.noise[g * A + c] : 0.0f;
-      const float nz = fminf(fmaxf(__fmul_rn(eps, sd), -clip), clip);
-      D0[r * kPitch + F + c] = fminf(fmaxf(__fadd_rn(pi, nz), lo), hi);
-    }
-    __syncthreads();
-    // ---- target critics -> V[., 0], V[., 1]; critics on (obs, actions) -> V[., 2], V[., 3]
-    net_forward(Wt1, P, 1, D0,
-                [&](int l) { return l == P.L[1] - 1 ? V : (l % 2 == 0 ? D1 : XS); });
-    net_forward(Wt2, P, 1, D0,
-                [&](int l) { return l == P.L[1] - 1 ? V + 1 : (l % 2 == 0 ? D1 : XS); });
-    net_forward(Wc1, P, 1, XQ,
-                [&](int l) { return l == P.L[1] - 1 ? V + 2 : H1 + l * kTile; });
-    net_forward(Wc2, P, 1, XQ,
-                [&](int l) { return l == P.L[1] - 1 ? V + 3 : H2 + l * kTile; });
-    // ---- the n-step return from min(Q1', Q2') and the loss gradients
-    if (tid < kRows) {
-      const int r = tid;
-      const long long g = g0 + r;
-      float d1 = 0.0f, d2 = 0.0f;
-      if (g < M) {
-        const float qt = fminf(V[r * kPitch], V[r * kPitch + 1]);
-        const float q1 = V[r * kPitch + 2], q2 = V[r * kPitch + 3];
-        const float ret = sampled_return(U, P, rows, rows.at(g), qt);
-        const float e1 = __fsub_rn(q1, ret), e2 = __fsub_rn(q2, ret);
-        d1 = __fmul_rn(e1, norm_q);
-        d2 = __fmul_rn(e2, norm_q);
-        e1_acc += (double)e1 * (double)e1;
-        e2_acc += (double)e2 * (double)e2;
-        if (U.q1_values) U.q1_values[g] = q1;
-        if (U.q2_values) U.q2_values[g] = q2;
-        if (U.returns) U.returns[g] = ret;
-      }
-      V[r * kPitch + 4] = d1;
-      V[r * kPitch + 8] = d2;
-    }
-    __syncthreads();
-    // ---- backward: each critic on (obs, actions) into its own gradient block
-    net_backward(Wc1, P, 1, G1, V + 4,
-                 [&](int l) { return l == 0 ? XQ : H1 + (l - 1) * kTile; }, D0, D1, -1);
-    net_backward(Wc2, P, 1, G2, V + 8,
-                 [&](int l) { return l == 0 ? XQ : H2 + (l - 1) * kTile; }, D0, D1, -1);
-  }
-
-  float *part = partials + (long long)blockIdx.x * g_total;
-  for (int e = tid; e < g_total; e += kThreads) part[e] = G1[e];
-  if (tid < kRows) {
-    s_e1[tid] = e1_acc;
-    s_e2[tid] = e2_acc;
-  }
-  __syncthreads();
-  if (tid == 0) {
-    double a = 0.0, b = 0.0;
-    for (int r = 0; r < kRows; r++) {
-      a += s_e1[r];
-      b += s_e2[r];
-    }
-    psums[2 * blockIdx.x] = a;
-    psums[2 * blockIdx.x + 1] = b;
-  }
-}
-
-// td3_actor_kernel over sampled windows.
-__global__ void __launch_bounds__(kThreads, 1)
-td3_actor_sampled(const __grid_constant__ wdb_td3_update_args U, const __grid_constant__ Plan Pg,
-                  float *partials, double *psums, const int2 *windows) {
-  extern __shared__ __align__(16) float smem[];
-  __shared__ Plan P;
-  __shared__ double s_j[kRows];
-  if (threadIdx.x == 0) P = Pg;
-  __syncthreads();
-  const int tid = threadIdx.x;
-  float *Wa = smem, *Wc = Wa + P.wfloats[0];
-  float *Ga = Wc + P.wfloats[1];
-  const int g_total = P.gfloats[0];
-  float *XJ = Ga + ((g_total + 3) / 4) * 4;      // obs ++ pi
-  float *V = XJ + kTile;                       // columns: 0 J, 8 dJ
-  float *Z = V + kTile;                        // actor head pre-activation
-  float *D0 = Z + kTile, *D1 = D0 + kTile;     // deltas
-  float *HJ = D1 + kTile;                      // Q1 hidden outputs on (obs, pi)
-  float *HA = HJ + (P.L[1] - 1) * kTile;       // actor hidden outputs
-
-  load_net(Wa, U.actor, P, 0);
-  load_net(Wc, U.critic, P, 1);
-  for (int e = tid; e < g_total; e += kThreads) Ga[e] = 0.0f;
-  for (int e = tid; e < P.n_buf * kTile; e += kThreads) XJ[e] = 0.0f;
-  __syncthreads();
-
-  const int F = U.obs_dim, A = U.action_dim;
-  const SampledRows rows = {windows, U.capacity};
-  const long long EN = P.EN, M = P.M;
-  const float scale = U.action_scale, bias = U.action_bias;
-  const float d_j = -1.0f / (float)M;
-  double j_acc = 0.0;
-
-  for (long long g0 = (long long)blockIdx.x * kRows; g0 < M; g0 += (long long)gridDim.x * kRows) {
-    for (int e = tid; e < kRows * F; e += kThreads) {
-      const int r = e / F, c = e - r * F;
-      const long long g = g0 + r;
-      float x = 0.0f;
-      if (g < M) {
-        const Row w = rows.at(g);
-        x = U.obs[((long long)rows.slot(w, 0) * EN + w.n) * F + c];
-      }
-      XJ[r * kPitch + c] = x;
-    }
-    __syncthreads();
-    // ---- actor -> pi into XJ's action columns; Q1 on (obs, pi) -> V[., 0]
-    net_forward(Wa, P, 0, XJ, [&](int l) { return l == P.L[0] - 1 ? Z : HA + l * kTile; });
-    for (int e = tid; e < kRows * A; e += kThreads) {
-      const int r = e / A, c = e - r * A;
-      XJ[r * kPitch + F + c] = __fadd_rn(__fmul_rn(scale, tanhf(Z[r * kPitch + c])), bias);
-    }
-    __syncthreads();
-    net_forward(Wc, P, 1, XJ, [&](int l) { return l == P.L[1] - 1 ? V : HJ + l * kTile; });
-    if (tid < kRows) {
-      const int r = tid;
-      const long long g = g0 + r;
-      float dj = 0.0f;
-      if (g < M) {
-        const float jv = V[r * kPitch];
-        dj = d_j;
-        j_acc += (double)jv;
-        if (U.j_values) U.j_values[g] = jv;
-      }
-      V[r * kPitch + 8] = dj;
-    }
-    __syncthreads();
-    // ---- backward: Q1 to its action inputs, the tanh head, the actor
-    const float *dpi = net_backward<false>(
-        Wc, P, 1, nullptr, V + 8, [&](int l) { return l == 0 ? XJ : HJ + (l - 1) * kTile; },
-        D0, D1, F);
-    float *dz = dpi == D0 ? D1 : D0;
-    for (int e = tid; e < kRows * A; e += kThreads) {
-      const int r = e / A, c = e - r * A;
-      const float y = tanhf(Z[r * kPitch + c]);
-      dz[r * kPitch + c] = __fmul_rn(__fmul_rn(dpi[r * kPitch + F + c], scale),
-                                     __fsub_rn(1.0f, __fmul_rn(y, y)));
-    }
-    __syncthreads();
-    net_backward(Wa, P, 0, Ga, dz, [&](int l) { return l == 0 ? XJ : HA + (l - 1) * kTile; },
-                 D0, D1, -1);
-  }
-
-  float *part = partials + (long long)blockIdx.x * g_total;
-  for (int e = tid; e < g_total; e += kThreads) part[e] = Ga[e];
-  if (tid < kRows) s_j[tid] = j_acc;
-  __syncthreads();
-  if (tid == 0) {
-    double a = 0.0;
-    for (int r = 0; r < kRows; r++) a += s_j[r];
-    psums[2 * blockIdx.x] = a;
-    psums[2 * blockIdx.x + 1] = 0.0;
-  }
-}
-
-// sac_critic_kernel over sampled windows.
-__global__ void __launch_bounds__(kThreads, 1)
-sac_critic_sampled(const __grid_constant__ wdb_sac_update_args U, const __grid_constant__ Plan Pg,
-                   float *partials, double *psums, const int2 *windows) {
-  extern __shared__ __align__(16) float smem[];
-  __shared__ Plan P;
-  __shared__ double s_e1[kRows], s_e2[kRows];
-  if (threadIdx.x == 0) P = Pg;
-  __syncthreads();
-  const int tid = threadIdx.x;
-  float *Wa = smem, *Wc1 = Wa + P.wfloats[0], *Wc2 = Wc1 + P.wfloats[1];
-  float *Wt1 = Wc2 + P.wfloats[1], *Wt2 = Wt1 + P.wfloats[1];
-  float *G1 = Wt2 + P.wfloats[1], *G2 = G1 + P.gfloats[1];
-  const int g_total = 2 * P.gfloats[1];
-  float *XQ = G1 + ((g_total + 3) / 4) * 4;      // obs ++ actions
-  float *XS = XQ + kTile;                      // scratch of the bootstrap forwards
-  float *V = XS + kTile;                       // columns: 0 Q1', 1 Q2', 2 Q1, 3 Q2, 4 dQ1, 8 dQ2
-  float *Z = V + kTile;                        // actor head on obs'; then [0, A): log-prob terms
-  float *D0 = Z + kTile, *D1 = D0 + kTile;     // deltas (bootstrap path: obs' ++ a' and scratch)
-  float *H1 = D1 + kTile;                      // Q1 hidden outputs
-  float *H2 = H1 + (P.L[1] - 1) * kTile;       // Q2 hidden outputs
-
-  load_net(Wa, U.actor, P, 0);
-  load_net(Wc1, U.critic, P, 1);
-  load_net(Wc2, U.critic2, P, 1);
-  load_net(Wt1, U.target_critic, P, 1);
-  load_net(Wt2, U.target_critic2, P, 1);
-  for (int e = tid; e < g_total; e += kThreads) G1[e] = 0.0f;
-  for (int e = tid; e < P.n_buf * kTile; e += kThreads) XQ[e] = 0.0f;
-  __syncthreads();
-
-  const int F = U.obs_dim, A = U.action_dim, FA = F + A;
-  const SampledRows rows = {windows, U.capacity};
-  const long long EN = P.EN, M = P.M;
-  const float scale = U.action_scale, bias = U.action_bias;
-  const float lo = U.log_std_min, hi = U.log_std_max;
-  const float alpha = expf(*U.log_alpha);
-  const float norm_q = (float)(2.0 / (double)M);
-  double e1_acc = 0.0, e2_acc = 0.0;
-
-  for (long long g0 = (long long)blockIdx.x * kRows; g0 < M; g0 += (long long)gridDim.x * kRows) {
-    // ---- inputs: XQ = obs ++ actions at slot i, D0 = obs at the bootstrap slot
-    for (int e = tid; e < kRows * FA; e += kThreads) {
-      const int r = e / FA, c = e - r * FA;
-      const long long g = g0 + r;
-      float xq = 0.0f, xt = 0.0f;
-      if (g < M) {
-        const Row w = rows.at(g);
-        const long long row = (long long)rows.slot(w, 0) * EN + w.n;
-        if (c < F) {
-          xq = U.obs[row * F + c];
-          xt = U.obs[((long long)rows.slot(w, U.n_step) * EN + w.n) * F + c];
-        } else {
-          xq = U.actions[row * A + (c - F)];
-        }
-      }
-      XQ[r * kPitch + c] = xq;
-      if (c < F) D0[r * kPitch + c] = xt;
-    }
-    __syncthreads();
-    // ---- actor on obs' -> a' ~ pi(. | obs') into D0's action columns, log-prob terms into Z
-    net_forward(Wa, P, 0, D0,
-                [&](int l) { return l == P.L[0] - 1 ? Z : (l % 2 == 0 ? D1 : XS); });
-    for (int e = tid; e < kRows * A; e += kThreads) {
-      const int r = e / A, c = e - r * A;
-      const long long g = g0 + r;
-      const float eps = g < M ? U.critic_noise[g * A + c] : 0.0f;
-      const SquashedDim s = squashed_dim(Z + r * kPitch, A, c, eps, lo, hi);
-      D0[r * kPitch + F + c] = __fadd_rn(__fmul_rn(scale, s.y), bias);
-      Z[r * kPitch + c] = s.term;
-    }
-    __syncthreads();
-    // ---- target critics -> V[., 0], V[., 1]; critics on (obs, actions) -> V[., 2], V[., 3]
-    net_forward(Wt1, P, 1, D0,
-                [&](int l) { return l == P.L[1] - 1 ? V : (l % 2 == 0 ? D1 : XS); });
-    net_forward(Wt2, P, 1, D0,
-                [&](int l) { return l == P.L[1] - 1 ? V + 1 : (l % 2 == 0 ? D1 : XS); });
-    net_forward(Wc1, P, 1, XQ,
-                [&](int l) { return l == P.L[1] - 1 ? V + 2 : H1 + l * kTile; });
-    net_forward(Wc2, P, 1, XQ,
-                [&](int l) { return l == P.L[1] - 1 ? V + 3 : H2 + l * kTile; });
-    // ---- the n-step return from min(Q1', Q2') - alpha log pi' and the loss gradients
-    if (tid < kRows) {
-      const int r = tid;
-      const long long g = g0 + r;
-      float d1 = 0.0f, d2 = 0.0f;
-      if (g < M) {
-        float lp = 0.0f;
-        for (int c = 0; c < A; c++) lp += Z[r * kPitch + c];
-        const float qt = __fsub_rn(fminf(V[r * kPitch], V[r * kPitch + 1]), __fmul_rn(alpha, lp));
-        const float q1 = V[r * kPitch + 2], q2 = V[r * kPitch + 3];
-        const float ret = sampled_return(U, P, rows, rows.at(g), qt);
-        const float e1 = __fsub_rn(q1, ret), e2 = __fsub_rn(q2, ret);
-        d1 = __fmul_rn(e1, norm_q);
-        d2 = __fmul_rn(e2, norm_q);
-        e1_acc += (double)e1 * (double)e1;
-        e2_acc += (double)e2 * (double)e2;
-        if (U.q1_values) U.q1_values[g] = q1;
-        if (U.q2_values) U.q2_values[g] = q2;
-        if (U.returns) U.returns[g] = ret;
-      }
-      V[r * kPitch + 4] = d1;
-      V[r * kPitch + 8] = d2;
-    }
-    __syncthreads();
-    // ---- backward: each critic on (obs, actions) into its own gradient block
-    net_backward(Wc1, P, 1, G1, V + 4,
-                 [&](int l) { return l == 0 ? XQ : H1 + (l - 1) * kTile; }, D0, D1, -1);
-    net_backward(Wc2, P, 1, G2, V + 8,
-                 [&](int l) { return l == 0 ? XQ : H2 + (l - 1) * kTile; }, D0, D1, -1);
-  }
-
-  float *part = partials + (long long)blockIdx.x * g_total;
-  for (int e = tid; e < g_total; e += kThreads) part[e] = G1[e];
-  if (tid < kRows) {
-    s_e1[tid] = e1_acc;
-    s_e2[tid] = e2_acc;
-  }
-  __syncthreads();
-  if (tid == 0) {
-    double a = 0.0, b = 0.0;
-    for (int r = 0; r < kRows; r++) {
-      a += s_e1[r];
-      b += s_e2[r];
-    }
-    psums[2 * blockIdx.x] = a;
-    psums[2 * blockIdx.x + 1] = b;
-  }
-}
-
-// sac_actor_kernel over sampled windows.
-__global__ void __launch_bounds__(kThreads, 1)
-sac_actor_sampled(const __grid_constant__ wdb_sac_update_args U, const __grid_constant__ Plan Pg,
-                  float *partials, double *psums, const int2 *windows) {
-  extern __shared__ __align__(16) float smem[];
-  __shared__ Plan P;
-  __shared__ double s_q[kRows], s_lp[kRows];
-  if (threadIdx.x == 0) P = Pg;
-  __syncthreads();
-  const int tid = threadIdx.x;
-  float *Wa = smem, *Wc1 = Wa + P.wfloats[0], *Wc2 = Wc1 + P.wfloats[1];
-  float *Ga = Wc2 + P.wfloats[1];
-  const int g_total = P.gfloats[0];
-  float *XJ = Ga + ((g_total + 3) / 4) * 4;      // obs ++ a
-  float *V = XJ + kTile;                       // columns: 0 Q1, 1 Q2, 8 dQ1, 12 dQ2
-  float *Z = V + kTile;                        // actor head: mu ++ raw log-std
-  float *D0 = Z + kTile, *D1 = D0 + kTile;     // deltas
-  float *DA = D1 + kTile;                      // log-prob terms, then Q1's action gradient
-  float *H1 = DA + kTile;                      // Q1 hidden outputs on (obs, a)
-  float *H2 = H1 + (P.L[1] - 1) * kTile;       // Q2 hidden outputs on (obs, a)
-  float *HA = H2 + (P.L[1] - 1) * kTile;       // actor hidden outputs
-
-  load_net(Wa, U.actor, P, 0);
-  load_net(Wc1, U.critic, P, 1);
-  load_net(Wc2, U.critic2, P, 1);
-  for (int e = tid; e < g_total; e += kThreads) Ga[e] = 0.0f;
-  for (int e = tid; e < P.n_buf * kTile; e += kThreads) XJ[e] = 0.0f;
-  __syncthreads();
-
-  const int F = U.obs_dim, A = U.action_dim;
-  const SampledRows rows = {windows, U.capacity};
-  const long long EN = P.EN, M = P.M;
-  const float scale = U.action_scale, bias = U.action_bias;
-  const float lo = U.log_std_min, hi = U.log_std_max;
-  const float alpha = expf(*U.log_alpha);
-  const float d_q = -1.0f / (float)M;                    // d loss / d min(Q1, Q2)
-  const float d_lp = alpha / (float)M;                   // d loss / d log pi
-  double q_acc = 0.0, lp_acc = 0.0;
-
-  for (long long g0 = (long long)blockIdx.x * kRows; g0 < M; g0 += (long long)gridDim.x * kRows) {
-    for (int e = tid; e < kRows * F; e += kThreads) {
-      const int r = e / F, c = e - r * F;
-      const long long g = g0 + r;
-      float x = 0.0f;
-      if (g < M) {
-        const Row w = rows.at(g);
-        x = U.obs[((long long)rows.slot(w, 0) * EN + w.n) * F + c];
       }
       XJ[r * kPitch + c] = x;
     }
@@ -1938,11 +1410,12 @@ bool sac_plan(const wdb_sac_update_args *u, const wdb_replay_windows *w, bool ac
 }
 
 
-// Launches one pass (`ring` over every window of the ring, or `sampled` over w's windows) and
-// the reduction R of its per-CTA partials into the gradient arena and `sums`.
+// Launches one pass kernel (its NoWindows instantiation over every window of the ring, or its
+// const int2 * one over w's windows) and the reduction R of its per-CTA partials into the
+// gradient arena and `sums`.
 template <class Args>
 int launch_pass(void *stream, const Args *u, const Plan &P, const wdb_replay_windows *w,
-                void (*ring)(const Args, const Plan, float *, double *),
+                void (*ring)(const Args, const Plan, float *, double *, NoWindows),
                 void (*sampled)(const Args, const Plan, float *, double *, const int2 *),
                 size_t *configured, Reduce *R, int widest, double *sums) {
   if (!u->workspace || (w && !w->windows)) return (int)cudaErrorInvalidValue;
@@ -1956,7 +1429,7 @@ int launch_pass(void *stream, const Args *u, const Plan &P, const wdb_replay_win
     sampled<<<P.grid, kThreads, smem, as_stream(stream)>>>(
         *u, P, partials, psums, reinterpret_cast<const int2 *>(w->windows));
   else
-    ring<<<P.grid, kThreads, smem, as_stream(stream)>>>(*u, P, partials, psums);
+    ring<<<P.grid, kThreads, smem, as_stream(stream)>>>(*u, P, partials, psums, NoWindows{});
   rc = finish_launch();
   if (rc != cudaSuccess) return rc;
   R->grid = P.grid;
@@ -1973,8 +1446,8 @@ int ddpg_update(void *stream, const wdb_ddpg_update_args *u, const wdb_replay_wi
   add_segments(&R, P, 0, 0, u->actor, &widest);
   add_segments(&R, P, 1, P.gfloats[0], u->critic, &widest);
   static size_t configured[2] = {0, 0};
-  return launch_pass(stream, u, P, w, ddpg_update_kernel, ddpg_update_sampled, configured, &R,
-                     widest, u->sums);
+  return launch_pass(stream, u, P, w, ddpg_update_kernel<NoWindows>,
+                     ddpg_update_kernel<const int2 *>, configured, &R, widest, u->sums);
 }
 
 int td3_critic_update(void *stream, const wdb_td3_update_args *u, const wdb_replay_windows *w) {
@@ -1992,8 +1465,8 @@ int td3_critic_update(void *stream, const wdb_td3_update_args *u, const wdb_repl
   add_segments(&R, P, 1, 0, u->critic, &widest);
   add_segments(&R, P, 1, P.gfloats[1], u->critic2, &widest);
   static size_t configured[2] = {0, 0};
-  return launch_pass(stream, u, P, w, td3_critic_kernel, td3_critic_sampled, configured, &R,
-                     widest, u->sums);
+  return launch_pass(stream, u, P, w, td3_critic_kernel<NoWindows>,
+                     td3_critic_kernel<const int2 *>, configured, &R, widest, u->sums);
 }
 
 int td3_actor_update(void *stream, const wdb_td3_update_args *u, const wdb_replay_windows *w) {
@@ -2007,8 +1480,9 @@ int td3_actor_update(void *stream, const wdb_td3_update_args *u, const wdb_repla
   int widest = 1;
   add_segments(&R, P, 0, 0, u->actor, &widest);
   static size_t configured[2] = {0, 0};
-  return launch_pass(stream, u, P, w, td3_actor_kernel, td3_actor_sampled, configured, &R,
-                     widest, u->sums ? u->sums + 2 : nullptr);
+  return launch_pass(stream, u, P, w, td3_actor_kernel<NoWindows>,
+                     td3_actor_kernel<const int2 *>, configured, &R, widest,
+                     u->sums ? u->sums + 2 : nullptr);
 }
 
 int sac_critic_update(void *stream, const wdb_sac_update_args *u, const wdb_replay_windows *w) {
@@ -2026,8 +1500,8 @@ int sac_critic_update(void *stream, const wdb_sac_update_args *u, const wdb_repl
   add_segments(&R, P, 1, 0, u->critic, &widest);
   add_segments(&R, P, 1, P.gfloats[1], u->critic2, &widest);
   static size_t configured[2] = {0, 0};
-  return launch_pass(stream, u, P, w, sac_critic_kernel, sac_critic_sampled, configured, &R,
-                     widest, u->sums);
+  return launch_pass(stream, u, P, w, sac_critic_kernel<NoWindows>,
+                     sac_critic_kernel<const int2 *>, configured, &R, widest, u->sums);
 }
 
 int sac_actor_update(void *stream, const wdb_sac_update_args *u, const wdb_replay_windows *w) {
@@ -2042,8 +1516,9 @@ int sac_actor_update(void *stream, const wdb_sac_update_args *u, const wdb_repla
   int widest = 1;
   add_segments(&R, P, 0, 0, u->actor, &widest);
   static size_t configured[2] = {0, 0};
-  return launch_pass(stream, u, P, w, sac_actor_kernel, sac_actor_sampled, configured, &R,
-                     widest, u->sums ? u->sums + 2 : nullptr);
+  return launch_pass(stream, u, P, w, sac_actor_kernel<NoWindows>,
+                     sac_actor_kernel<const int2 *>, configured, &R, widest,
+                     u->sums ? u->sums + 2 : nullptr);
 }
 
 // DQN's plan: the online and target Q networks in the actor-shaped slot (input F, head = A).
