@@ -999,6 +999,74 @@ long long wdb_dqn_update_sampled_workspace_bytes(const wdb_dqn_update_args *upda
 int wdb_dqn_update_sampled(void *stream, const wdb_dqn_update_args *update,
                            const wdb_replay_windows *windows);
 
+/* wdb_dqn_update_sampled with importance-sampling weights w [B] (wdb_per_sample_windows):
+ *   loss = (1/B) sum_g w_g huber(Q_g - R_g, delta), head gradient w_g clamp(Q - R, -delta,
+ *   delta) / B in column a, sums[0] = sum_g w_g huber(Q_g - R_g), sums[1] = sum Q(obs, a).
+ * The weight multiplies the clamped difference before the 1 / B and the Huber value before the
+ * sum, so all weights 1 reproduce wdb_dqn_update_sampled bit for bit.  Same shapes, workspace,
+ * reduction and launch count (two). */
+int wdb_dqn_update_prioritized_supported(const wdb_dqn_update_args *update, int n_windows);
+long long wdb_dqn_update_prioritized_workspace_bytes(const wdb_dqn_update_args *update,
+                                                     int n_windows);
+/* cudaErrorInvalidValue without launching if unsupported or a required pointer (weights
+ * included) is NULL. */
+int wdb_dqn_update_prioritized(void *stream, const wdb_dqn_update_args *update,
+                               const wdb_replay_windows *windows, const float *weights);
+
+/* Prioritized replay (Schaul et al. 2016, proportional) over the replay ring's n-step windows.
+ * One float32 leaf per (physical slot s, agent row n), leaf s * n_rows + n: p^alpha of the
+ * window that starts at slot s for agent row n (windows[g] = {s, n} as above), and 0 exactly
+ * when that window is not valid -- its logical start k (slots after the oldest) is not in
+ * [0, filled - n_step - 1].  Over the leaves a sum tree of fan-out 32 with float64 nodes, level
+ * by level from the leaves' parents up to the root; a node is its (up to 32, zero-padded)
+ * children summed pairwise, v[i] += v[i + h] for h = 16, 8, 4, 2, 1.  Every write repairs the
+ * paths above the leaves it touched, one launch per tree level, by recomputing each node from
+ * its children, so the tree is always a pure function of the leaves (bit for bit what a fresh
+ * build gives).  p_max is the running maximum of the priorities (|delta| + epsilon) written,
+ * 1 at the start; new windows enter at p_max^alpha.  The leaf count capacity * n_rows must be
+ * below 2^31. */
+typedef struct wdb_per_store {
+  int capacity, n_rows, n_step;      /* ring slots C (>= n_step + 1), E * Np, n-step horizon */
+  float alpha, epsilon;              /* alpha in [0, 1], epsilon > 0 */
+  float *leaves;                     /* device [C * n_rows], zeros at the start */
+  double *nodes;                     /* device [wdb_per_nodes(C * n_rows)], zeros at the start */
+  float *p_max;                      /* device [1], 1 at the start */
+} wdb_per_store;
+/* The float64 nodes / the levels of the tree over n_leaves leaves; -1 unless 1 <= n_leaves <
+ * 2^31.  No CUDA call. */
+long long wdb_per_nodes(long long n_leaves);
+int wdb_per_levels(long long n_leaves);
+/* After each rollout of T slots, given the ring's cursor and fill level before and after it
+ * (T = cursor_after - cursor_before mod C): the leaves of the starts that have just become
+ * valid get p_max^alpha, those of the newest n_step slots (the slots the rollout overwrote among
+ * them) get 0, then the touched paths are repaired.  Needs 1 <= T, T + n_step <= C and
+ * filled_after = min(C, filled_before + T).  1 + levels launches. */
+int wdb_per_admit(void *stream, const wdb_per_store *store, int cursor_before, int filled_before,
+                  int cursor_after, int filled_after);
+/* B windows by stratified proportional sampling: row g draws u in [g S / B, (g + 1) S / B) (S:
+ * the root, read on the device) as lo + U (hi - lo), U = (a >> 5 * 2^26 + b >> 6) / 2^53 from
+ * the words a, b of Philox4x32-10 with key `seed` at counter (counter, g), and descends: the
+ * children of a node are scanned in order with a running float64 prefix, the first with
+ * positive mass whose prefix end exceeds u is entered and u drops by the prefix before it; if
+ * rounding puts u at or past the node's total, the last child with positive mass is entered
+ * (a zero-sum child never is).  Writes windows[g] = {s, n}, priorities[g] = the leaf p^alpha,
+ * and, from a second one-CTA launch, weights[g] = (priorities[g] / min_g priorities)^-beta with
+ * beta read from the device (the weights normalised by the batch's largest, as Dopamine and
+ * Rainbow do).  The store must hold a valid window.  Two launches, no host wait. */
+int wdb_per_sample_windows(void *stream, const wdb_per_store *store,
+                           int *windows /* out [B][2] */, float *priorities /* out [B] */,
+                           float *weights /* out [B] */, int n_windows,
+                           unsigned long long seed, unsigned long long counter,
+                           const float *beta /* device [1] */);
+/* Writes (|q_values[g] - returns[g]| + epsilon)^alpha to the leaf of each window that is a
+ * valid start of the ring (`oldest`, `filled` as wdb_replay_sample_windows; other rows are
+ * skipped), raises p_max, and repairs the touched paths.  A window given twice keeps its larger
+ * priority whatever the order.  A non-finite priority is taken as the largest float.
+ * 2 + levels launches. */
+int wdb_per_set_priorities(void *stream, const wdb_per_store *store, const int *windows,
+                           int n_windows, const float *q_values, const float *returns,
+                           int oldest, int filled);
+
 #ifdef __cplusplus
 }
 #endif

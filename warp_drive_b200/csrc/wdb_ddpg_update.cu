@@ -1183,9 +1183,12 @@ sac_actor_kernel(const __grid_constant__ wdb_sac_update_args U, const __grid_con
 // kept for the backward), target Q'(obs') and, with double_q, online Q(obs'); per row the
 // bootstrap, the n-step return and the Huber gradient in the action's column; then back
 // through the online network.  A separate kernel, so the pinned ones above keep their code.
-__global__ void __launch_bounds__(kThreads, 1)
-dqn_pass_kernel(const __grid_constant__ wdb_dqn_update_args U, const __grid_constant__ Plan Pg,
-                float *partials, double *psums, const int2 *windows) {
+// kWeighted (wdb_dqn_update_prioritized): row g's Huber value and clamped difference are scaled
+// by weights[g] -- the clamped difference before the 1 / B, so a weight of 1 changes no bit.
+template <bool kWeighted>
+__device__ __forceinline__ void dqn_tile_pass(const wdb_dqn_update_args &U, const Plan &Pg,
+                                              float *partials, double *psums,
+                                              const int2 *windows, const float *weights) {
   extern __shared__ __align__(16) float smem[];
   __shared__ Plan P;
   __shared__ double s_h[kRows], s_q[kRows];
@@ -1271,10 +1274,18 @@ dqn_pass_kernel(const __grid_constant__ wdb_dqn_update_args U, const __grid_cons
         if (a >= 0 && a < A) {
           const float q = QS[r * kPitch + a];
           const float diff = __fsub_rn(q, ret);
-          dq[a] = __fmul_rn(fminf(fmaxf(diff, -delta), delta), norm);
           const double ad = fabs((double)diff);
-          h_acc += ad < (double)delta ? 0.5 * ad * ad
-                                      : (double)delta * (ad - 0.5 * (double)delta);
+          if constexpr (kWeighted) {
+            const float w = weights[g];
+            const double wd = (double)w;
+            dq[a] = __fmul_rn(__fmul_rn(fminf(fmaxf(diff, -delta), delta), w), norm);
+            h_acc += ad < (double)delta ? (0.5 * wd) * ad * ad
+                                        : (wd * (double)delta) * (ad - 0.5 * (double)delta);
+          } else {
+            dq[a] = __fmul_rn(fminf(fmaxf(diff, -delta), delta), norm);
+            h_acc += ad < (double)delta ? 0.5 * ad * ad
+                                        : (double)delta * (ad - 0.5 * (double)delta);
+          }
           q_acc += (double)q;
           if (U.q_values) U.q_values[g] = q;
         }
@@ -1303,6 +1314,18 @@ dqn_pass_kernel(const __grid_constant__ wdb_dqn_update_args U, const __grid_cons
     psums[2 * blockIdx.x] = a;
     psums[2 * blockIdx.x + 1] = b;
   }
+}
+
+__global__ void __launch_bounds__(kThreads, 1)
+dqn_pass_kernel(const __grid_constant__ wdb_dqn_update_args U, const __grid_constant__ Plan Pg,
+                float *partials, double *psums, const int2 *windows) {
+  dqn_tile_pass<false>(U, Pg, partials, psums, windows, nullptr);
+}
+
+__global__ void __launch_bounds__(kThreads, 1)
+dqn_weighted_kernel(const __grid_constant__ wdb_dqn_update_args U, const __grid_constant__ Plan Pg,
+                    float *partials, double *psums, const int2 *windows, const float *weights) {
+  dqn_tile_pass<true>(U, Pg, partials, psums, windows, weights);
 }
 
 // ---------------------------------------------------------------------------- host side
@@ -1538,7 +1561,9 @@ bool dqn_plan(const wdb_dqn_update_args *u, const wdb_replay_windows *w, Plan *p
 
 long long dqn_workspace_bytes(const Plan &P) { return 16ll * P.grid + 4ll * P.grid * P.gfloats[0]; }
 
-int dqn_update_sampled(void *stream, const wdb_dqn_update_args *u, const wdb_replay_windows *w) {
+// weights NULL: wdb_dqn_update_sampled; else wdb_dqn_update_prioritized.
+int dqn_update_sampled(void *stream, const wdb_dqn_update_args *u, const wdb_replay_windows *w,
+                       const float *weights) {
   Plan P;
   if (!dqn_plan(u, w, &P) || !w->windows) return (int)cudaErrorInvalidValue;
   if (!net_ok(u->q, P.L[0], true) || !net_ok(u->target_q, P.L[0], false))
@@ -1549,14 +1574,20 @@ int dqn_update_sampled(void *stream, const wdb_dqn_update_args *u, const wdb_rep
   R.g_total = P.gfloats[0];
   int widest = 1;
   add_segments(&R, P, 0, 0, u->q, &widest);
-  static size_t configured = 0;
+  static size_t configured[2] = {0, 0};
   const size_t smem = (size_t)P.smem_floats * sizeof(float);
-  int rc = allow_smem((const void *)dqn_pass_kernel, smem, &configured);
+  const void *kernel = weights ? (const void *)dqn_weighted_kernel : (const void *)dqn_pass_kernel;
+  int rc = allow_smem(kernel, smem, &configured[weights ? 1 : 0]);
   if (rc != cudaSuccess) return rc;
   double *psums = static_cast<double *>(u->workspace);
   float *partials = reinterpret_cast<float *>(psums + 2 * P.grid);
-  dqn_pass_kernel<<<P.grid, kThreads, smem, as_stream(stream)>>>(
-      *u, P, partials, psums, reinterpret_cast<const int2 *>(w->windows));
+  const int2 *windows = reinterpret_cast<const int2 *>(w->windows);
+  if (weights)
+    dqn_weighted_kernel<<<P.grid, kThreads, smem, as_stream(stream)>>>(*u, P, partials, psums,
+                                                                       windows, weights);
+  else
+    dqn_pass_kernel<<<P.grid, kThreads, smem, as_stream(stream)>>>(*u, P, partials, psums,
+                                                                   windows);
   rc = finish_launch();
   if (rc != cudaSuccess) return rc;
   R.grid = P.grid;
@@ -1629,5 +1660,18 @@ WDB_API long long wdb_dqn_update_sampled_workspace_bytes(const wdb_dqn_update_ar
 }
 WDB_API int wdb_dqn_update_sampled(void *stream, const wdb_dqn_update_args *u,
                                    const wdb_replay_windows *w) {
-  return dqn_update_sampled(stream, u, w);
+  return dqn_update_sampled(stream, u, w, nullptr);
+}
+
+// The importance-weighted pass has the unweighted one's shapes and workspace
+WDB_API int wdb_dqn_update_prioritized_supported(const wdb_dqn_update_args *u, int n_windows) {
+  return wdb_dqn_update_sampled_supported(u, n_windows);
+}
+WDB_API long long wdb_dqn_update_prioritized_workspace_bytes(const wdb_dqn_update_args *u,
+                                                             int n_windows) {
+  return wdb_dqn_update_sampled_workspace_bytes(u, n_windows);
+}
+WDB_API int wdb_dqn_update_prioritized(void *stream, const wdb_dqn_update_args *u,
+                                       const wdb_replay_windows *w, const float *weights) {
+  return weights ? dqn_update_sampled(stream, u, w, weights) : (int)cudaErrorInvalidValue;
 }

@@ -307,6 +307,15 @@ class DqnUpdate(ctypes.Structure):
     ]
 
 
+class PerStore(ctypes.Structure):
+    """struct wdb_per_store (include/wdb200.h)."""
+
+    _fields_ = [
+        ("capacity", _i), ("n_rows", _i), ("n_step", _i), ("alpha", _f), ("epsilon", _f),
+        ("leaves", _fp), ("nodes", _fp), ("p_max", _fp),
+    ]
+
+
 _SIGNATURES = {
     "wdb_abi_version": (_i, []),
     "wdb_error_string": (ctypes.c_char_p, [_i]),
@@ -415,7 +424,18 @@ _SIGNATURES = {
     "wdb_dqn_update_sampled_workspace_bytes": (_ll, [ctypes.POINTER(DqnUpdate), _i]),
     "wdb_dqn_update_sampled": (
         _i, [_vp, ctypes.POINTER(DqnUpdate), ctypes.POINTER(ReplayWindows)]),
+    "wdb_dqn_update_prioritized_supported": (_i, [ctypes.POINTER(DqnUpdate), _i]),
+    "wdb_dqn_update_prioritized_workspace_bytes": (_ll, [ctypes.POINTER(DqnUpdate), _i]),
+    "wdb_dqn_update_prioritized": (
+        _i, [_vp, ctypes.POINTER(DqnUpdate), ctypes.POINTER(ReplayWindows), _vp]),
     "wdb_replay_sample_windows": (_i, [_vp, _vp, _i, _ull, _ull, _i, _i, _i, _i, _i]),
+    "wdb_per_nodes": (_ll, [_ll]),
+    "wdb_per_levels": (_i, [_ll]),
+    "wdb_per_admit": (_i, [_vp, ctypes.POINTER(PerStore), _i, _i, _i, _i]),
+    "wdb_per_sample_windows": (
+        _i, [_vp, ctypes.POINTER(PerStore), _vp, _vp, _vp, _i, _ull, _ull, _vp]),
+    "wdb_per_set_priorities": (
+        _i, [_vp, ctypes.POINTER(PerStore), _vp, _i, _vp, _vp, _i, _i]),
     "wdb_single_agent_rollout_supported": (_i, [_i, ctypes.POINTER(_i)]),
     "wdb_single_agent_rollout": (_i, [_vp, ctypes.POINTER(SaRollout)]),
     "wdb_mountain_car_step": (

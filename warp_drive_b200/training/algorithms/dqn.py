@@ -47,14 +47,20 @@ class DQN:
                 return q_target.gather(-1, best)[..., 0]
             return q_target.max(dim=-1).values
 
-    def loss(self, q_net, target_net, obs, actions, rewards, done, boot_obs):
+    def loss(self, q_net, target_net, obs, actions, rewards, done, boot_obs, weights=None):
         """(Huber loss, Q(obs, a) [B], R [B]) of B sampled windows: obs [B, F], actions [B, 1]
-        (int), rewards / done [n_step, B], boot_obs [B, F]."""
+        (int), rewards / done [n_step, B], boot_obs [B, F].  weights [B]: prioritized replay's
+        importance-sampling weights, the loss (1/B) sum w_g huber(Q_g - R_g) of
+        wdb_dqn_update_prioritized."""
         with torch.no_grad():
             returns = self.sampled_returns(rewards, done, self.bootstrap(q_net, target_net,
                                                                          boot_obs))
         q = q_net.q_values(obs).gather(-1, actions.long().reshape(-1, 1))[..., 0]
-        loss = func.huber_loss(q, returns, delta=self.huber_delta)
+        if weights is None:
+            loss = func.huber_loss(q, returns, delta=self.huber_delta)
+        else:
+            loss = (weights * func.huber_loss(q, returns, reduction="none",
+                                              delta=self.huber_delta)).mean()
         return loss, q, returns
 
     @staticmethod

@@ -55,11 +55,12 @@ class FusedDQNUpdate:
         self.workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         self.sums = torch.zeros(2, dtype=torch.float64, device=dev)
 
-    def launch(self, obs, actions, rewards, done, windows, outputs=None):
+    def launch(self, obs, actions, rewards, done, windows, outputs=None, weights=None):
         """The Q network's gradient into its `.grad`.  obs [C, E, Np, F], actions [C, E, Np, 1]
         (int32), rewards [C, E, Np], done [C, E] are the ring in physical slot order; windows
         int32 [rows, 2] the sampled windows.  outputs: optional (q_values, returns) float32
-        tensors [rows] for the metrics."""
+        tensors [rows] for the metrics.  weights: float32 [rows] importance-sampling weights
+        (prioritized replay): wdb_dqn_update_prioritized instead of wdb_dqn_update_sampled."""
         u = self.u
         q_net, target_net = self.models
         # parameters may have been re-allocated (load_state_dict keeps storage; .to() does not)
@@ -72,7 +73,13 @@ class FusedDQNUpdate:
         u.sums = _lib.ptr(self.sums)
         u.workspace = _lib.ptr(self.workspace)
         assert windows.shape[0] == self.rows
-        _lib.check(self.lib.wdb_dqn_update_sampled(
-            _lib.stream_ptr(), ctypes.byref(u), ctypes.byref(replay_windows(windows))),
-            "dqn_update_sampled")
+        if weights is None:
+            _lib.check(self.lib.wdb_dqn_update_sampled(
+                _lib.stream_ptr(), ctypes.byref(u), ctypes.byref(replay_windows(windows))),
+                "dqn_update_sampled")
+        else:
+            assert weights.shape == (self.rows,) and weights.dtype == torch.float32
+            _lib.check(self.lib.wdb_dqn_update_prioritized(
+                _lib.stream_ptr(), ctypes.byref(u), ctypes.byref(replay_windows(windows)),
+                _lib.ptr(weights)), "dqn_update_prioritized")
         return self.sums

@@ -95,6 +95,45 @@ def replay_settings(trainer_config, batch_slots, n_step):
             "updates": int(updates), "warmup": int(warmup)}
 
 
+_PRIORITY_KEYS = ("priority_alpha", "priority_beta", "priority_epsilon")
+
+
+def _unit_number(v):
+    return isinstance(v, (int, float)) and not isinstance(v, bool) and 0 <= v <= 1
+
+
+def prioritized_settings(trainer_config, replay):
+    """The validated prioritized-replay keys of a trainer config, or None without
+    `prioritized_replay`.  `replay`: replay_settings' result.  Returns {"alpha", "beta" (a
+    ParamScheduler over the policy timestep), "epsilon"}."""
+    if not trainer_config.get("prioritized_replay"):
+        for key in _PRIORITY_KEYS:
+            if trainer_config.get(key) is not None:
+                raise ValueError(f"{key} needs prioritized_replay")
+        return None
+    if trainer_config["prioritized_replay"] is not True:
+        raise ValueError(f"prioritized_replay is True or False, got "
+                         f"{trainer_config['prioritized_replay']!r}")
+    if replay is None:
+        raise ValueError("prioritized_replay needs replay_slots_per_env")
+    alpha = trainer_config.get("priority_alpha", 0.6)
+    if not _unit_number(alpha):
+        raise ValueError(f"priority_alpha must lie in [0, 1], got {alpha}")
+    beta = trainer_config.get("priority_beta", 0.5)
+    knots = beta if isinstance(beta, list) else [[0, beta]]
+    if not knots or not all(isinstance(k, (list, tuple)) and len(k) == 2 and _unit_number(k[1])
+                            for k in knots):
+        raise ValueError(f"priority_beta must be a number or [[t, v], ...] with v in [0, 1], "
+                         f"got {beta}")
+    if [k[0] for k in knots] != sorted(k[0] for k in knots):
+        raise ValueError(f"priority_beta's timesteps must be increasing, got {beta}")
+    eps = trainer_config.get("priority_epsilon", 1e-6)
+    if not (isinstance(eps, (int, float)) and not isinstance(eps, bool) and 0 < eps
+            and math.isfinite(eps)):
+        raise ValueError(f"priority_epsilon must be a finite number > 0, got {eps}")
+    return {"alpha": float(alpha), "beta": ParamScheduler(beta), "epsilon": float(eps)}
+
+
 class RingRolloutEngine(RolloutEngine):
     """RolloutEngine whose batch index wraps: timestep t of a rollout lands in slot
     (cursor + t) mod capacity of every `*_batch*` array."""
@@ -157,6 +196,9 @@ class TrainerDDPG(Trainer):
                          obs_dim_corresponding_to_num_agents, num_devices, device_id,
                          results_dir, verbose, use_cuda_graph=False)
 
+    # the trainer key prioritized_replay (TrainerDQN); the actor-critic passes have no weights
+    _takes_prioritized_replay = False
+
     # ------------------------------------------------------------------ setup
     @staticmethod
     def _check_obs_dim(obs_dim_corresponding_to_num_agents):
@@ -175,6 +217,10 @@ class TrainerDDPG(Trainer):
         assert self.n_step >= 1
         self.replay = replay_settings(trainer_config, self.training_batch_size_per_env,
                                       self.n_step)
+        self.prioritized = prioritized_settings(trainer_config, self.replay)
+        if self.prioritized is not None and not self._takes_prioritized_replay:
+            raise ValueError(f"prioritized_replay is DQN's: {type(self).__name__} samples its "
+                             f"replay windows uniformly")
         if self.replay is not None:
             self.ring_capacity = self.replay["slots"]
         else:

@@ -17,6 +17,14 @@ differs is one Q network (`fully_connected_q`) and its target per policy:
 
 Policy keys: `double_q` (True), `huber_delta` (1.0), `tau` (1.0), `target_update_period` (1),
 and Trainer's `lr`, `model`, `gamma`, `clip_grad_norm`, `max_grad_norm`; trainer key `n_step`.
+
+Prioritized replay (trainer key `prioritized_replay`, see trainer_ddpg.prioritized_settings):
+each policy's windows carry priorities in a device sum tree (utils/prioritized_replay.py).  Every
+rollout admits its windows at the running maximum priority (wdb_per_admit), each update draws
+its windows by stratified proportional sampling with importance-sampling weights
+(wdb_per_sample_windows, beta from `priority_beta` over the policy timestep), takes the weighted
+gradient (wdb_dqn_update_prioritized, or the weighted torch loss) and writes the windows' new
+priorities (wdb_per_set_priorities) before the optimizer step.
 """
 import os
 
@@ -27,6 +35,7 @@ from warp_drive_b200.training.algorithms.fused_dqn import FusedDQNUpdate, fused_
 from warp_drive_b200.training.trainer_ddpg import (
     RingRolloutEngine, TrainerDDPG, hard_update, soft_update)
 from warp_drive_b200.training.utils.param_scheduler import ParamScheduler
+from warp_drive_b200.training.utils.prioritized_replay import PrioritizedReplay
 from warp_drive_b200.utils.constants import Constants
 
 _ACTIONS = Constants.ACTIONS
@@ -74,6 +83,7 @@ class TrainerDQN(TrainerDDPG):
 
     # the evaluator plays greedily
     _test_sample_params = {"epsilon": 0}
+    _takes_prioritized_replay = True
 
     def __init__(self, env_wrapper=None, config=None, policy_tag_to_agent_id_map=None,
                  create_separate_placeholders_for_each_policy=False,
@@ -100,6 +110,7 @@ class TrainerDQN(TrainerDDPG):
         self.optimizers, self.lr_schedules = {}, {}
         self.tau, self.target_update_period, self.update_count = {}, {}, {}
         self.fused_updates, self.replay_windows, self.replay_draws = {}, {}, 0
+        self.priority_stores = {}
         self.last_epsilon = None
         # the networks the rollout runs (TrainerDDPG's replay helpers know them as actors)
         self.models = self.actor_models = self.q_models
@@ -145,6 +156,15 @@ class TrainerDQN(TrainerDDPG):
         n_agents = len(self.policy_tag_to_agent_id_map[policy])
         rows = self._init_replay(policy)
         q_net = self.q_models[policy]
+        if self.prioritized is not None:
+            store = self.priority_stores[policy] = PrioritizedReplay(
+                self.ring_capacity, self.num_envs * n_agents, self.n_step, rows,
+                self.prioritized["alpha"], self.prioritized["epsilon"],
+                next(q_net.parameters()).device)
+            if self.verbose:
+                print(f"[Device {self.device_id}]: priority store of policy '{policy}': "
+                      f"{store.leaves.numel()} windows, a sum tree of {store.levels} levels, "
+                      f"{store.nbytes()} bytes on the device")
         if fused_dqn_supported(algo, q_net, self.num_envs, n_agents, self.ring_capacity, rows):
             self.fused_updates[policy] = FusedDQNUpdate(
                 algo, q_net, self.target_q_models[policy], self.num_envs, n_agents,
@@ -157,9 +177,15 @@ class TrainerDQN(TrainerDDPG):
             ring_capacity=self.ring_capacity)
 
     # ------------------------------------------------------------------ update
+    def _ring_state(self):
+        return self.engine.ring_cursor, self.engine.ring_filled
+
     def _generate_rollout_batch(self):
+        before = self._ring_state()
         params = super()._generate_rollout_batch()
         self.last_epsilon = params["epsilon"]
+        for store in self.priority_stores.values():     # warm-up rollouts included
+            store.admit(before, self._ring_state())
         return params
 
     def _update_model_params(self, iteration):
@@ -167,7 +193,23 @@ class TrainerDQN(TrainerDDPG):
         if self.last_epsilon is not None:      # the rollout's exploration rate
             for metrics in metrics_dict.values():
                 metrics["Epsilon"] = float(self.last_epsilon)
+        for policy, metrics in metrics_dict.items():
+            store = self.priority_stores.get(policy)
+            if store is not None and "Q loss" in metrics:   # the last update's sample
+                metrics["Priority beta"] = float(store.beta)
+                metrics["Mean IS weight"] = float(store.weights.double().mean())
+                metrics["Max priority"] = float(store.p_max)
         return metrics_dict
+
+    def _sample_replay_windows(self, policy):
+        """Uniform windows (TrainerDDPG), or with prioritized replay stratified proportional
+        ones and their importance-sampling weights (two launches, no host wait)."""
+        store = self.priority_stores.get(policy)
+        if store is None:
+            return super()._sample_replay_windows(policy)
+        self.replay_draws += 1
+        store.set_beta(self.prioritized["beta"].get_param_value(self.current_timestep[policy]))
+        store.sample(self.replay_windows[policy], self.seed, self.replay_draws)
 
     def _one_update(self, logging_flag, step_info):
         """The Q gradient of every trained policy, one optimizer step, and the targets' tracking
@@ -182,6 +224,12 @@ class TrainerDQN(TrainerDDPG):
                 loss_metrics[policy] = self._fused_q_gradients(policy, fused, logging_flag)
             else:
                 loss_metrics[policy] = self._torch_q_gradients(policy, logging_flag)
+            store = self.priority_stores.get(policy)
+            if store is not None:
+                eng = self.engine
+                oldest = eng.ring_cursor if eng.ring_filled == eng.ring_capacity else 0
+                store.set_priorities(self.replay_windows[policy], store.q_values, store.returns,
+                                     oldest, eng.ring_filled)
         step_info.update(self._optimizer_step(loss_metrics, logging_flag))
         for policy in loss_metrics:
             if self.update_count[policy] % self.target_update_period[policy] == 0:
@@ -193,8 +241,13 @@ class TrainerDQN(TrainerDDPG):
         """The Q gradient by torch autograd on the gathered windows (the loss of
         wdb_dqn_update_sampled), accumulated into the arena's .grad views."""
         algo = self.trainers[policy]
+        store = self.priority_stores.get(policy)
         loss, q, returns = algo.loss(self.q_models[policy], self.target_q_models[policy],
-                                     *self._gather_windows(policy))
+                                     *self._gather_windows(policy),
+                                     weights=None if store is None else store.weights)
+        if store is not None:                  # the inputs of the new priorities
+            store.q_values.copy_(q.detach())
+            store.returns.copy_(returns)
         self.optimizers[policy].zero_grad()
         loss.backward()
         if not logging_flag:
@@ -205,15 +258,18 @@ class TrainerDQN(TrainerDDPG):
         """The same gradient from wdb_dqn_update_sampled, written straight into the arena's
         .grad views; the host waits only on logging iterations (metrics)."""
         eng = self.engine
-        outputs = None
-        if logging_flag:
+        outputs, weights = None, None
+        store = self.priority_stores.get(policy)
+        if store is not None:                  # the weighted pass; Q and R feed the priorities
+            outputs, weights = (store.q_values, store.returns), store.weights
+        elif logging_flag:
             dev = fused.sums.device
             outputs = (torch.empty(fused.rows, device=dev), torch.empty(fused.rows, device=dev))
         sums = fused.launch(eng._tensor(f"{_PROCESSED_OBSERVATIONS}_batch_{policy}"),
                             eng._tensor(f"{_ACTIONS}_batch_{policy}"),
                             eng._tensor(f"{_REWARDS}_batch_{policy}"),
                             eng._tensor(f"{_DONE_FLAGS}_batch"), self.replay_windows[policy],
-                            outputs)
+                            outputs, weights)
         if not logging_flag:
             return {}
         s = sums.tolist()
