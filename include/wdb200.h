@@ -1013,6 +1013,33 @@ long long wdb_dqn_update_prioritized_workspace_bytes(const wdb_dqn_update_args *
 int wdb_dqn_update_prioritized(void *stream, const wdb_dqn_update_args *update,
                                const wdb_replay_windows *windows, const float *weights);
 
+/* One quantile-regression DQN update (Dabney et al. 2018) over B sampled windows, read as
+ * wdb_dqn_update_sampled reads them.  The networks' head has A * N outputs (n_actions = A,
+ * n_quantiles = N); column a * N + i is quantile i of action a.  Per loss row g with action a:
+ *   theta_i = online(obs)[a, i],  tau_i = (2 i + 1) / (2 N),
+ *   a*      = the first argmax over actions of sum_j online(obs')[., j] (double_q) or of
+ *             sum_j target(obs')[., j],
+ *   T_j     = DQN's n-step recursion (float32, every non-zero done terminal) on
+ *             target(obs')[a*, j],
+ *   loss_g  = (1/N) sum_i sum_j |tau_i - 1{u_ij < 0}| huber(u_ij, kappa) / kappa,
+ *             u_ij = T_j - theta_i, kappa = huber_delta,
+ *   loss    = (1/B) sum_g w_g loss_g,  w_g = weights[g], or 1 when weights is NULL,
+ * and its gradient, -w_g / (kappa N B) sum_j |tau_i - 1{u_ij < 0}| clamp(u_ij, -kappa, kappa)
+ * in column a * N + i (the sum over j in order), back through the online network into q.gw /
+ * gb.  sums[0] = sum_g w_g loss_g, sums[1] = sum_g mean_i theta_i; the optional outputs [B] are
+ * q_values = mean_i theta_i and returns = mean_j T_j.  The weight multiplies a row's gradient
+ * and loss once each, so unit weights reproduce the unweighted pass bit for bit.  Per-CTA
+ * partials summed in a fixed order by a second launch: bit-reproducible.  Two launches.
+ * Supported: the shapes of wdb_dqn_update_sampled_supported with n_quantiles >= 1 and the head
+ * A * N <= 64.  No CUDA call. */
+int wdb_qr_dqn_update_sampled_supported(const wdb_dqn_update_args *update, int n_quantiles,
+                                        int n_windows);
+long long wdb_qr_dqn_update_sampled_workspace_bytes(const wdb_dqn_update_args *update,
+                                                    int n_quantiles, int n_windows);
+/* cudaErrorInvalidValue without launching if unsupported or a required pointer is NULL. */
+int wdb_qr_dqn_update_sampled(void *stream, const wdb_dqn_update_args *update, int n_quantiles,
+                              const wdb_replay_windows *windows, const float *weights);
+
 /* Prioritized replay (Schaul et al. 2016, proportional) over the replay ring's n-step windows.
  * One float32 leaf per (physical slot s, agent row n), leaf s * n_rows + n: p^alpha of the
  * window that starts at slot s for agent row n (windows[g] = {s, n} as above), and 0 exactly

@@ -1328,6 +1328,179 @@ dqn_weighted_kernel(const __grid_constant__ wdb_dqn_update_args U, const __grid_
   dqn_tile_pass<true>(U, Pg, partials, psums, windows, weights);
 }
 
+// ---------------------------------------------------------------------------- QR-DQN
+// wdb_qr_dqn_update_sampled's tile kernel: DQN's networks and forwards with a head of A * N
+// quantiles (column a * N + i: quantile i of action a).  Per row: a* the first argmax of the
+// quantile sums of online(obs') (double_q) or target(obs'), the N targets T_j (DQN's n-step
+// recursion on each target(obs')[a*, j]), and the quantile Huber gradient of each theta_i =
+// online(obs)[a, i] in column a * N + i.  The row's 16 threads share its N x N pairs: thread k
+// owns the quantiles i = k, k + 16, ... and sums over j in order, so no atomics and an update
+// is bit-reproducible.  kWeighted: row g's gradient and loss are scaled by weights[g] with one
+// multiply each, so unit weights change no bit.
+template <bool kWeighted>
+__device__ __forceinline__ void qr_dqn_tile_pass(const wdb_dqn_update_args &U, const Plan &Pg,
+                                                 int nq, float *partials, double *psums,
+                                                 const int2 *windows, const float *weights) {
+  constexpr int kLanes = kThreads / kRows;     // threads per row
+  extern __shared__ __align__(16) float smem[];
+  __shared__ Plan P;
+  __shared__ double s_h[kRows], s_q[kRows];
+  if (threadIdx.x == 0) P = Pg;
+  __syncthreads();
+  const int tid = threadIdx.x;
+  float *Wq = smem, *Wt = Wq + P.wfloats[0];
+  float *G = Wt + P.wfloats[0];
+  const int g_total = P.gfloats[0];
+  float *X = G + ((g_total + 3) / 4) * 4;      // obs at slot(0)
+  float *XB = X + kTile;                       // bootstrap obs at slot(n_step), then T_j
+  float *QS = XB + kTile;                      // online quantiles at obs
+  float *QT = QS + kTile;                      // target quantiles at obs'
+  float *QD = QT + kTile;                      // online quantiles at obs' (double_q)
+  float *DQ = QD + kTile;                      // head delta
+  float *D0 = DQ + kTile, *D1 = D0 + kTile;    // deltas (the obs' forwards: scratch)
+  float *H = D1 + kTile;                       // online hidden outputs on obs
+
+  load_net(Wq, U.q, P, 0);
+  load_net(Wt, U.target_q, P, 0);
+  for (int e = tid; e < g_total; e += kThreads) G[e] = 0.0f;
+  for (int e = tid; e < P.n_buf * kTile; e += kThreads) X[e] = 0.0f;
+  __syncthreads();
+
+  const int F = U.obs_dim, A = U.n_actions, N = nq, L = P.L[0], ns = U.n_step;
+  const SampledRows rows = {windows, U.capacity};
+  const long long EN = P.EN, M = P.M, E = U.n_envs, Np = U.n_agents;
+  const float gamma = U.gamma, kappa = U.huber_delta;
+  // d loss / d theta_i = -(1 / (kappa N B)) sum_j |tau_i - 1{u_ij < 0}| clamp(u_ij, -kappa, kappa)
+  const float norm = (float)(1.0 / ((double)kappa * (double)N * (double)M));
+  const int r = tid / kLanes, k = tid - r * kLanes;
+  double h_acc = 0.0, q_acc = 0.0;
+
+  for (long long g0 = (long long)blockIdx.x * kRows; g0 < M; g0 += (long long)gridDim.x * kRows) {
+    // ---- inputs: X = obs at slot(0), XB = obs at slot(n_step)
+    for (int e = tid; e < kRows * F; e += kThreads) {
+      const int rr = e / F, c = e - rr * F;
+      const long long g = g0 + rr;
+      float x = 0.0f, xb = 0.0f;
+      if (g < M) {
+        const Row w = rows.at(g);
+        x = U.obs[((long long)rows.slot(w, 0) * EN + w.n) * F + c];
+        xb = U.obs[((long long)rows.slot(w, ns) * EN + w.n) * F + c];
+      }
+      X[rr * kPitch + c] = x;
+      XB[rr * kPitch + c] = xb;
+    }
+    __syncthreads();
+    net_forward(Wq, P, 0, X, [&](int l) { return l == L - 1 ? QS : H + l * kTile; });
+    net_forward(Wt, P, 0, XB, [&](int l) { return l == L - 1 ? QT : (l % 2 == 0 ? D0 : D1); });
+    if (U.double_q)
+      net_forward(Wq, P, 0, XB, [&](int l) { return l == L - 1 ? QD : (l % 2 == 0 ? D0 : D1); });
+    // ---- per row (its kLanes threads): a*, the targets T_j into XB, a zeroed head delta
+    const long long g = g0 + r;
+    float *dq = DQ + r * kPitch, *T = XB + r * kPitch;
+    for (int c = k; c < A * N; c += kLanes) dq[c] = 0.0f;
+    Row w = {0, 0};
+    int a = -1;
+    if (g < M) {
+      w = rows.at(g);
+      a = U.actions[(long long)rows.slot(w, 0) * EN + w.n];
+      const float *qa = U.double_q ? QD + r * kPitch : QT + r * kPitch;
+      int best = 0;                            // the first maximum of the quantile sums
+      float best_sum = 0.0f;
+      for (int c = 0; c < A; c++) {
+        float s = 0.0f;
+        for (int j = 0; j < N; j++) s = __fadd_rn(s, qa[c * N + j]);
+        if (c == 0 || best_sum < s) { best_sum = s; best = c; }
+      }
+      const float *boot = QT + r * kPitch + best * N;
+      const long long env = w.n / Np;
+      for (int j = k; j < N; j += kLanes) {
+        float ret = boot[j];
+        for (int t = ns - 1; t >= 0; t--) {
+          const int pk = rows.slot(w, t);
+          const float om = U.done[(long long)pk * E + env] != 0 ? 0.0f : 1.0f;
+          ret = __fadd_rn(__fmul_rn(__fmul_rn(om, gamma), ret),
+                          U.rewards[(long long)pk * EN + w.n]);
+        }
+        T[j] = ret;
+      }
+    }
+    __syncthreads();
+    // ---- the pairs: thread k, quantiles i = k, k + kLanes, ...; T_j in order
+    // (an action outside [0, A) -- never written by the samplers -- contributes nothing)
+    if (g < M && a >= 0 && a < A) {
+      const float *theta = QS + r * kPitch + a * N;
+      const float wg = kWeighted ? weights[g] : 1.0f;
+      double h_row = 0.0;
+      for (int i = k; i < N; i += kLanes) {
+        const float th = theta[i];
+        const float tau = (float)(2 * i + 1) / (float)(2 * N);
+        float acc = 0.0f;
+        for (int j = 0; j < N; j++) {
+          const float u = __fsub_rn(T[j], th);
+          const float m = u < 0.0f ? __fsub_rn(1.0f, tau) : tau;     // |tau - 1{u < 0}|
+          acc = fmaf(m, fminf(fmaxf(u, -kappa), kappa), acc);
+          const double au = fabs((double)u);
+          h_row += (double)m * (au < (double)kappa ? 0.5 * au * au
+                                                   : (double)kappa * (au - 0.5 * (double)kappa));
+        }
+        if constexpr (kWeighted) acc = __fmul_rn(acc, wg);
+        dq[a * N + i] = __fmul_rn(-acc, norm);
+      }
+      if constexpr (kWeighted) h_row *= (double)wg;
+      h_acc += h_row;
+    }
+    if (k == 0 && g < M) {                     // the row's mean quantile and mean target
+      double rbar = 0.0;
+      for (int j = 0; j < N; j++) rbar += (double)T[j];
+      rbar /= (double)N;
+      if (U.returns) U.returns[g] = (float)rbar;
+      if (a >= 0 && a < A) {
+        double qbar = 0.0;
+        for (int i = 0; i < N; i++) qbar += (double)QS[r * kPitch + a * N + i];
+        qbar /= (double)N;
+        q_acc += qbar;
+        if (U.q_values) U.q_values[g] = (float)qbar;
+      }
+    }
+    __syncthreads();
+    net_backward(Wq, P, 0, G, DQ, [&](int l) { return l == 0 ? X : H + (l - 1) * kTile; }, D0,
+                 D1, -1);
+  }
+
+  // ---- this CTA's partials: sums[0] = sum_g w_g loss_g, sums[1] = sum_g mean_i theta_i
+  float *part = partials + (long long)blockIdx.x * g_total;
+  for (int e = tid; e < g_total; e += kThreads) part[e] = G[e];
+  for (int off = kLanes / 2; off > 0; off /= 2)   // the row's lanes, in a fixed order
+    h_acc += __shfl_xor_sync(0xffffffffu, h_acc, off, kLanes);
+  if (k == 0) {
+    s_h[r] = h_acc;
+    s_q[r] = q_acc;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    double a = 0.0, b = 0.0;
+    for (int t = 0; t < kRows; t++) {
+      a += s_h[t];
+      b += s_q[t];
+    }
+    psums[2 * blockIdx.x] = a / ((double)kappa * (double)N);
+    psums[2 * blockIdx.x + 1] = b;
+  }
+}
+
+__global__ void __launch_bounds__(kThreads, 1)
+qr_dqn_kernel(const __grid_constant__ wdb_dqn_update_args U, const __grid_constant__ Plan Pg,
+              int nq, float *partials, double *psums, const int2 *windows) {
+  qr_dqn_tile_pass<false>(U, Pg, nq, partials, psums, windows, nullptr);
+}
+
+__global__ void __launch_bounds__(kThreads, 1)
+qr_dqn_prioritized_kernel(const __grid_constant__ wdb_dqn_update_args U,
+                          const __grid_constant__ Plan Pg, int nq, float *partials,
+                          double *psums, const int2 *windows, const float *weights) {
+  qr_dqn_tile_pass<true>(U, Pg, nq, partials, psums, windows, weights);
+}
+
 // ---------------------------------------------------------------------------- host side
 long long workspace_bytes(const Plan &P) {
   return 16ll * P.grid + 4ll * P.grid * (P.gfloats[0] + P.gfloats[1]);
@@ -1594,6 +1767,53 @@ int dqn_update_sampled(void *stream, const wdb_dqn_update_args *u, const wdb_rep
   return launch_reduce(stream, R, widest, partials, psums, u->sums);
 }
 
+// QR-DQN's plan: DQN's with a head of A * N quantiles (<= 64).
+bool qr_dqn_plan(const wdb_dqn_update_args *u, int nq, const wdb_replay_windows *w, Plan *p) {
+  if (!u || !w || !(u->huber_delta > 0.0f)) return false;
+  if (nq < 1 || nq > kMaxWidth || u->n_actions < 1 || u->n_actions > kMaxWidth) return false;
+  const wdb_ddpg_net *qs[2] = {&u->q, &u->target_q};
+  const wdb_ddpg_net *const *nets[2] = {qs, qs};
+  const int count[2] = {2, 2};
+  if (!plan_layout(u->n_envs, u->n_agents, u->obs_dim, 1, u->n_actions * nq, u->capacity, 0,
+                   u->n_step, w, nets, count, p))
+    return false;
+  return plan_smem(p, 8 + (p->L[0] - 1), 2ll * p->wfloats[0], p->gfloats[0]);
+}
+
+// weights NULL: the uniform-replay kernel; else the importance-weighted one.
+int qr_dqn_update_sampled(void *stream, const wdb_dqn_update_args *u, int nq,
+                          const wdb_replay_windows *w, const float *weights) {
+  Plan P;
+  if (!qr_dqn_plan(u, nq, w, &P) || !w->windows) return (int)cudaErrorInvalidValue;
+  if (!net_ok(u->q, P.L[0], true) || !net_ok(u->target_q, P.L[0], false))
+    return (int)cudaErrorInvalidValue;
+  if (!u->obs || !u->actions || !u->rewards || !u->done || !u->workspace)
+    return (int)cudaErrorInvalidValue;
+  Reduce R = {};
+  R.g_total = P.gfloats[0];
+  int widest = 1;
+  add_segments(&R, P, 0, 0, u->q, &widest);
+  static size_t configured[2] = {0, 0};
+  const size_t smem = (size_t)P.smem_floats * sizeof(float);
+  const void *kernel =
+      weights ? (const void *)qr_dqn_prioritized_kernel : (const void *)qr_dqn_kernel;
+  int rc = allow_smem(kernel, smem, &configured[weights ? 1 : 0]);
+  if (rc != cudaSuccess) return rc;
+  double *psums = static_cast<double *>(u->workspace);
+  float *partials = reinterpret_cast<float *>(psums + 2 * P.grid);
+  const int2 *windows = reinterpret_cast<const int2 *>(w->windows);
+  if (weights)
+    qr_dqn_prioritized_kernel<<<P.grid, kThreads, smem, as_stream(stream)>>>(
+        *u, P, nq, partials, psums, windows, weights);
+  else
+    qr_dqn_kernel<<<P.grid, kThreads, smem, as_stream(stream)>>>(*u, P, nq, partials,
+                                                                      psums, windows);
+  rc = finish_launch();
+  if (rc != cudaSuccess) return rc;
+  R.grid = P.grid;
+  return launch_reduce(stream, R, widest, partials, psums, u->sums);
+}
+
 }  // namespace
 
 // ---------------------------------------------------------------------------- entry points
@@ -1674,4 +1894,23 @@ WDB_API long long wdb_dqn_update_prioritized_workspace_bytes(const wdb_dqn_updat
 WDB_API int wdb_dqn_update_prioritized(void *stream, const wdb_dqn_update_args *u,
                                        const wdb_replay_windows *w, const float *weights) {
   return weights ? dqn_update_sampled(stream, u, w, weights) : (int)cudaErrorInvalidValue;
+}
+
+// QR-DQN: DQN's argument struct, plus the number of quantiles per action
+WDB_API int wdb_qr_dqn_update_sampled_supported(const wdb_dqn_update_args *u, int n_quantiles,
+                                                int n_windows) {
+  const wdb_replay_windows w = {nullptr, n_windows};
+  Plan P;
+  return qr_dqn_plan(u, n_quantiles, &w, &P) ? 1 : 0;
+}
+WDB_API long long wdb_qr_dqn_update_sampled_workspace_bytes(const wdb_dqn_update_args *u,
+                                                            int n_quantiles, int n_windows) {
+  const wdb_replay_windows w = {nullptr, n_windows};
+  Plan P;
+  return qr_dqn_plan(u, n_quantiles, &w, &P) ? dqn_workspace_bytes(P) : -1;
+}
+WDB_API int wdb_qr_dqn_update_sampled(void *stream, const wdb_dqn_update_args *u,
+                                      int n_quantiles, const wdb_replay_windows *w,
+                                      const float *weights) {
+  return qr_dqn_update_sampled(stream, u, n_quantiles, w, weights);
 }

@@ -428,6 +428,10 @@ _SIGNATURES = {
     "wdb_dqn_update_prioritized_workspace_bytes": (_ll, [ctypes.POINTER(DqnUpdate), _i]),
     "wdb_dqn_update_prioritized": (
         _i, [_vp, ctypes.POINTER(DqnUpdate), ctypes.POINTER(ReplayWindows), _vp]),
+    "wdb_qr_dqn_update_sampled_supported": (_i, [ctypes.POINTER(DqnUpdate), _i, _i]),
+    "wdb_qr_dqn_update_sampled_workspace_bytes": (_ll, [ctypes.POINTER(DqnUpdate), _i, _i]),
+    "wdb_qr_dqn_update_sampled": (
+        _i, [_vp, ctypes.POINTER(DqnUpdate), _i, ctypes.POINTER(ReplayWindows), _vp]),
     "wdb_replay_sample_windows": (_i, [_vp, _vp, _i, _ull, _ull, _i, _i, _i, _i, _i]),
     "wdb_per_nodes": (_ll, [_ll]),
     "wdb_per_levels": (_i, [_ll]),

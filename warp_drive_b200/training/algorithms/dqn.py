@@ -3,7 +3,8 @@ returns and a Huber loss (Mnih et al. 2015).
 
 The torch statement of wdb_dqn_update_sampled (include/wdb200.h): TrainerDQN runs it for the
 shapes the native pass does not take, and tests/dqn_update_reference.py restates it in float64
-NumPy."""
+NumPy.  QuantileDQN is quantile-regression DQN on the same windows (wdb_qr_dqn_update_sampled,
+tests/qr_dqn_reference.py)."""
 import torch
 from torch.nn import functional as func
 
@@ -69,3 +70,42 @@ class DQN:
         of the returns [B]."""
         return {"Q loss": float(loss), "Mean Q value": float(mean_q),
                 "Mean return": float(returns.double().mean())}
+
+
+class QuantileDQN(DQN):
+    """Quantile-regression DQN (Dabney et al. 2018) on DQN's windows, n-step recursion and
+    bootstrap rule: the torch statement of wdb_qr_dqn_update_sampled (include/wdb200.h) for a
+    FullyConnectedQuantileQ, restated in float64 NumPy by tests/qr_dqn_reference.py.
+    `huber_delta` is the quantile Huber loss's kappa."""
+
+    def bootstrap_quantiles(self, q_net, target_net, boot_obs):
+        """target(obs')[a*] [B, N] (no gradient), a* the first argmax of the mean quantile of
+        online(obs') with double_q, else of target(obs')."""
+        with torch.no_grad():
+            boot = target_net.quantiles(boot_obs)
+            chooser = q_net.quantiles(boot_obs) if self.double_q else boot
+            best = chooser.mean(dim=-1).argmax(dim=-1)
+            return boot[torch.arange(boot.shape[0], device=boot.device), best]
+
+    def loss(self, q_net, target_net, obs, actions, rewards, done, boot_obs, weights=None):
+        """(quantile Huber loss, Q-bar [B], R-bar [B]) of B sampled windows, the arguments of
+        DQN.loss.  theta_i = quantiles(obs)[a, i] at tau_i = (2i + 1) / (2N), T_j the n-step
+        recursion on each bootstrap quantile, u_ij = T_j - theta_i, and the row loss
+        (1/N) sum_i sum_j |tau_i - 1{u_ij < 0}| huber(u_ij, kappa) / kappa; the loss is the mean
+        over rows of w_g times it (w = 1 without weights).  Q-bar = mean_i theta_i and
+        R-bar = mean_j T_j feed the metrics and the priorities."""
+        with torch.no_grad():
+            boot = self.bootstrap_quantiles(q_net, target_net, boot_obs)
+            targets = self.sampled_returns(rewards[..., None], done[..., None], boot)
+        quantiles = q_net.quantiles(obs)
+        n = quantiles.shape[-1]
+        theta = quantiles[torch.arange(quantiles.shape[0], device=quantiles.device),
+                          actions.long().reshape(-1)]
+        tau = (2 * torch.arange(n, device=theta.device, dtype=theta.dtype) + 1) / (2 * n)
+        u = targets[:, None, :] - theta[:, :, None]             # [B, i, j]
+        below = (u.detach() < 0).to(theta.dtype)
+        rho = (tau[:, None] - below).abs() * func.huber_loss(
+            u, torch.zeros_like(u), reduction="none", delta=self.huber_delta) / self.huber_delta
+        rows = rho.sum(dim=1).mean(dim=-1)
+        loss = rows.mean() if weights is None else (weights * rows).mean()
+        return loss, theta.mean(dim=-1), targets.mean(dim=-1)

@@ -98,6 +98,14 @@ class FusedSingleAgentRollout:
         r.rewards = _p(dm.device_data(_REWARDS))
         r.sampled_actions = _p(dm.device_data(_ACTIONS))
         layers = _layers(model)
+        # QR-DQN's quantile network: the kernel runs epsilon-greedy over the mean quantile, the
+        # head collapsed to A rows (collapsed_head), kept in buffers of its own and recomputed
+        # from the live head at every launch
+        self._quantile = model if getattr(_unwrap(model), "is_quantile_q", False) else None
+        if self._quantile is not None:
+            with torch.no_grad():
+                w, b = _unwrap(model).collapsed_head()
+            layers[-1] = self._collapsed = (w.contiguous(), b.contiguous())
         r.n_hidden = len(layers) - 1
         dims = [int(_unwrap(model).flattened_obs_size)] + [int(w.shape[0]) for w, _ in layers]
         for i, d in enumerate(dims):
@@ -171,6 +179,10 @@ class FusedSingleAgentRollout:
         samples epsilon-greedily as CUDASampler.sample_epsilon_greedy with `epsilon` (default 0;
         use_argmax: 0), one draw per step; `probs_out` [n_steps, E, A] records the Q values."""
         dm, r, p = self.dm, self.r, self.policy
+        if self._quantile is not None:
+            with torch.no_grad():
+                for buf, v in zip(self._collapsed, _unwrap(self._quantile).collapsed_head()):
+                    buf.copy_(v)
         # parameters may have been re-allocated (load_state_dict keeps storage; .to() does not)
         for i, (w, b) in enumerate(self._params):
             r.w[i], r.b[i] = _p(w.data), _p(b.data)

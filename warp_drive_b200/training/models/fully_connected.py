@@ -203,6 +203,12 @@ class ModelFactory:
             from warp_drive_b200.training.models.fully_connected_q import FullyConnectedQ
 
             cls._registry[model_name] = FullyConnectedQ
+        if model_name == "fully_connected_quantile_q" and model_name not in cls._registry:
+            # QR-DQN's distributional Q network, imported on first use
+            from warp_drive_b200.training.models.fully_connected_q import (
+                FullyConnectedQuantileQ)
+
+            cls._registry[model_name] = FullyConnectedQuantileQ
         if model_name not in cls._registry and model_name in (
                 "fully_connected_actor", "fully_connected_action_value_critic",
                 "fully_connected_sac_actor"):

@@ -7,6 +7,7 @@ head.  `q_values(obs)` is what the update uses; `forward(obs)` keeps the rollout
 by `is_q_network` and samples its actions epsilon-greedily (CUDASampler.sample_epsilon_greedy).
 """
 from torch import nn
+from torch.nn import functional as func
 
 from warp_drive_b200.training.utils.data_loader import (
     action_head_sizes, dict_observation_keys, get_flattened_obs_size)
@@ -52,3 +53,49 @@ class FullyConnectedQ(nn.Module):
 
     def forward(self, obs=None, action=None, action_mask=None):
         return [self.q_values(obs)], None
+
+
+class FullyConnectedQuantileQ(FullyConnectedQ):
+    """The distributional Q network of quantile-regression DQN (algorithms/dqn.py QuantileDQN,
+    Dabney et al. 2018): FullyConnectedQ's trunk and one raw `policy_head = Linear(H, A * N)`,
+    N = `num_quantiles` (an integer in [2, 256]); column a * N + i is quantile i of action a.
+    `quantiles(obs)` is what the update uses; `q_values(obs)` -- and so `forward` and the
+    rollout's epsilon-greedy actions -- is the mean over the quantiles, computed through the
+    collapsed head (`collapsed_head()`: W and b averaged over each action's N rows)."""
+    name = "torch_fully_connected_quantile_q"
+    is_quantile_q = True
+
+    def __init__(self, env, model_config, policy, policy_tag_to_agent_id_map,
+                 create_separate_placeholders_for_each_policy=False,
+                 obs_dim_corresponding_to_num_agents="first"):
+        n = model_config.get("num_quantiles")
+        if isinstance(n, bool) or not isinstance(n, int) or not 2 <= n <= 256:
+            raise ValueError("fully_connected_quantile_q needs model.num_quantiles, an integer in "
+                             f"[2, 256], got {n!r}")
+        super().__init__(env, model_config, policy, policy_tag_to_agent_id_map,
+                         create_separate_placeholders_for_each_policy,
+                         obs_dim_corresponding_to_num_agents)
+        self.num_quantiles = n
+        self.policy_head = nn.Linear(self.policy_head.in_features, self.output_dims[0] * n)
+
+    def trunk(self, obs):
+        x = obs
+        for i in range(len(self.fc)):
+            x = self.fc[str(i)](x)
+        return x
+
+    def quantiles(self, obs):
+        """The N quantiles of every action: [..., A, N]."""
+        y = self.policy_head(self.trunk(obs))
+        return y.reshape(*y.shape[:-1], self.output_dims[0], self.num_quantiles)
+
+    def collapsed_head(self):
+        """(W.view(A, N, H).mean(1), b.view(A, N).mean(1)): the head of the mean quantile."""
+        A, n = self.output_dims[0], self.num_quantiles
+        w, b = self.policy_head.weight, self.policy_head.bias
+        return w.view(A, n, w.shape[1]).mean(1), b.view(A, n).mean(1)
+
+    def q_values(self, obs):
+        """The mean quantile of every action: [..., A]."""
+        w, b = self.collapsed_head()
+        return func.linear(self.trunk(obs), w, b)

@@ -25,13 +25,20 @@ its windows by stratified proportional sampling with importance-sampling weights
 (wdb_per_sample_windows, beta from `priority_beta` over the policy timestep), takes the weighted
 gradient (wdb_dqn_update_prioritized, or the weighted torch loss) and writes the windows' new
 priorities (wdb_per_set_priorities) before the optimizer step.
+
+Quantile-regression DQN: a `fully_connected_quantile_q` model (`num_quantiles` N) trains with
+QuantileDQN's quantile Huber loss (wdb_qr_dqn_update_sampled, 2 launches, or torch autograd)
+on the same windows, targets and schedule.  Its `Mean Q value` and `Mean return` are the means
+of Q-bar = mean_i theta_i and R-bar = mean_j T_j, and with prioritized replay the priorities are
+(|Q-bar - R-bar| + epsilon)^alpha.
 """
 import os
 
 import torch
 
-from warp_drive_b200.training.algorithms.dqn import DQN
-from warp_drive_b200.training.algorithms.fused_dqn import FusedDQNUpdate, fused_dqn_supported
+from warp_drive_b200.training.algorithms.dqn import DQN, QuantileDQN
+from warp_drive_b200.training.algorithms.fused_dqn import (
+    FusedDQNUpdate, FusedQRDQNUpdate, fused_dqn_supported, fused_qr_dqn_supported)
 from warp_drive_b200.training.trainer_ddpg import (
     RingRolloutEngine, TrainerDDPG, hard_update, soft_update)
 from warp_drive_b200.training.utils.param_scheduler import ParamScheduler
@@ -123,7 +130,8 @@ class TrainerDQN(TrainerDDPG):
         model_cfg = c["model"]
         self.q_models[policy] = self._build_model(policy, model_cfg)
         if not getattr(self.q_models[policy], "is_q_network", False):
-            raise ValueError(f"DQN's model is a `fully_connected_q`, got '{model_cfg.get('type')}'")
+            raise ValueError("DQN's model is a `fully_connected_q` or a "
+                             f"`fully_connected_quantile_q`, got '{model_cfg.get('type')}'")
         self.target_q_models[policy] = self._build_model(policy, model_cfg)
         hard_update(self.target_q_models[policy], self.q_models[policy])
 
@@ -150,12 +158,13 @@ class TrainerDQN(TrainerDDPG):
             self.max_grad_norm[policy] = c["max_grad_norm"]
         self.tau[policy], self.target_update_period[policy] = tau, period
         self.update_count[policy] = 0
-        algo = self.trainers[policy] = DQN(
+        q_net = self.q_models[policy]
+        quantile = getattr(q_net, "is_quantile_q", False)
+        algo = self.trainers[policy] = (QuantileDQN if quantile else DQN)(
             discount_factor_gamma=c["gamma"], n_step=self.n_step, double_q=double_q,
             huber_delta=delta)
         n_agents = len(self.policy_tag_to_agent_id_map[policy])
         rows = self._init_replay(policy)
-        q_net = self.q_models[policy]
         if self.prioritized is not None:
             store = self.priority_stores[policy] = PrioritizedReplay(
                 self.ring_capacity, self.num_envs * n_agents, self.n_step, rows,
@@ -165,8 +174,10 @@ class TrainerDQN(TrainerDDPG):
                 print(f"[Device {self.device_id}]: priority store of policy '{policy}': "
                       f"{store.leaves.numel()} windows, a sum tree of {store.levels} levels, "
                       f"{store.nbytes()} bytes on the device")
-        if fused_dqn_supported(algo, q_net, self.num_envs, n_agents, self.ring_capacity, rows):
-            self.fused_updates[policy] = FusedDQNUpdate(
+        supported, fused = ((fused_qr_dqn_supported, FusedQRDQNUpdate) if quantile
+                            else (fused_dqn_supported, FusedDQNUpdate))
+        if supported(algo, q_net, self.num_envs, n_agents, self.ring_capacity, rows):
+            self.fused_updates[policy] = fused(
                 algo, q_net, self.target_q_models[policy], self.num_envs, n_agents,
                 self.ring_capacity, rows)
 
@@ -239,7 +250,8 @@ class TrainerDQN(TrainerDDPG):
 
     def _torch_q_gradients(self, policy, logging_flag):
         """The Q gradient by torch autograd on the gathered windows (the loss of
-        wdb_dqn_update_sampled), accumulated into the arena's .grad views."""
+        wdb_dqn_update_sampled, or of wdb_qr_dqn_update_sampled for a quantile network),
+        accumulated into the arena's .grad views."""
         algo = self.trainers[policy]
         store = self.priority_stores.get(policy)
         loss, q, returns = algo.loss(self.q_models[policy], self.target_q_models[policy],
@@ -255,8 +267,9 @@ class TrainerDQN(TrainerDDPG):
         return algo.loss_metrics(loss.item(), q.detach().double().mean(), returns)
 
     def _fused_q_gradients(self, policy, fused, logging_flag):
-        """The same gradient from wdb_dqn_update_sampled, written straight into the arena's
-        .grad views; the host waits only on logging iterations (metrics)."""
+        """The same gradient from the native pass (FusedDQNUpdate or FusedQRDQNUpdate),
+        written straight into the arena's .grad views; the host waits only on logging
+        iterations (metrics)."""
         eng = self.engine
         outputs, weights = None, None
         store = self.priority_stores.get(policy)
