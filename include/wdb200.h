@@ -1040,6 +1040,47 @@ long long wdb_qr_dqn_update_sampled_workspace_bytes(const wdb_dqn_update_args *u
 int wdb_qr_dqn_update_sampled(void *stream, const wdb_dqn_update_args *update, int n_quantiles,
                               const wdb_replay_windows *windows, const float *weights);
 
+/* One implicit quantile network update (IQN; Dabney, Ostrovski, Silver & Munos 2018) over B
+ * sampled windows, read as wdb_dqn_update_sampled reads them.  q / target_q are the trunk psi
+ * (their hidden Linear + ReLU layers, at least one, width H) and a raw head Linear(H, A); the
+ * tau embedding of each is phi(tau) = ReLU(E f(tau) + e), E [H, n_cos], with the cosine
+ * features f_c(tau) = cos(float(pi * c) * tau), c = 0 .. n_cos - 1 (float32 multiply, cosf).
+ * Z_tau(x, .) = head(psi(x) * phi(tau)).  Per loss row g with action a, levels tau_i = taus[g][i]
+ * (i < N) and tau'_j = taus[g][N + j] (j < N'):
+ *   c-bar   = mean_k phi(tau~_k) over the K midpoints tau~_k = (2k + 1) / (2K), of the online
+ *             embedding (double_q) or the target one; Q-bar(x, .) = head(psi(x) * c-bar),
+ *   a*      = the first argmax of Q-bar of online(obs') (double_q) or of target(obs'),
+ *   theta_i = Z_tau_i(obs)[a] (online),  T_j = DQN's n-step recursion (float32, every non-zero
+ *             done terminal) on the target's Z_tau'_j(obs')[a*],
+ *   loss_g  = (1/N') sum_i sum_j |tau_i - 1{u_ij < 0}| huber(u_ij, kappa) / kappa,
+ *             u_ij = T_j - theta_i, kappa = huber_delta,
+ *   loss    = (1/B) sum_g w_g loss_g,  w_g = weights[g], or 1 when weights is NULL,
+ * and its gradient, d loss / d theta_i = -w_g / (kappa N' B) sum_j |tau_i - 1{u_ij < 0}|
+ * clamp(u_ij, -kappa, kappa) (the sum over j in order), back through the head (summed over the
+ * row's pairs), the merge (d psi summed over i in order) and the embedding (through its ReLU,
+ * the cosine features recomputed) into q.gw / gb and embed_gw / gb.  sums[0] = sum_g w_g
+ * loss_g, sums[1] = sum_g mean_i theta_i; the optional outputs [B] are q_values = mean_i
+ * theta_i and returns = mean_j T_j.  The weight multiplies a row's gradient and loss once each,
+ * so unit weights reproduce the unweighted pass bit for bit.  Per-CTA partials summed in a fixed
+ * order by a second launch: bit-reproducible.  Two launches. */
+typedef struct wdb_iqn_args {
+  int n_cos, n_tau, n_tau_prime, n_quantile_samples;   /* n_cos, N, N', K */
+  const float *taus;                 /* [B, N + N']: each row's tau_i, then its tau'_j */
+  wdb_ddpg_net embed, target_embed;  /* the tau embeddings, n_hidden = 0: w[0] = E [H, n_cos],
+                                        b[0] = e [H]; gw[0] / gb[0] the online one's gradients */
+} wdb_iqn_args;
+/* Supported: the shapes of wdb_dqn_update_sampled_supported with at least one hidden layer,
+ * 1 <= n_cos, N, N' <= 64, 1 <= K <= 256, and both Q networks, both embeddings, both gradient
+ * blocks and the row tiles in one CTA's shared memory.  No CUDA call. */
+int wdb_iqn_update_sampled_supported(const wdb_dqn_update_args *update, const wdb_iqn_args *iqn,
+                                     int n_windows);
+long long wdb_iqn_update_sampled_workspace_bytes(const wdb_dqn_update_args *update,
+                                                 const wdb_iqn_args *iqn, int n_windows);
+/* cudaErrorInvalidValue without launching if unsupported or a required pointer is NULL. */
+int wdb_iqn_update_sampled(void *stream, const wdb_dqn_update_args *update,
+                           const wdb_iqn_args *iqn, const wdb_replay_windows *windows,
+                           const float *weights);
+
 /* Prioritized replay (Schaul et al. 2016, proportional) over the replay ring's n-step windows.
  * One float32 leaf per (physical slot s, agent row n), leaf s * n_rows + n: p^alpha of the
  * window that starts at slot s for agent row n (windows[g] = {s, n} as above), and 0 exactly

@@ -307,6 +307,15 @@ class DqnUpdate(ctypes.Structure):
     ]
 
 
+class IqnArgs(ctypes.Structure):
+    """struct wdb_iqn_args (include/wdb200.h)."""
+
+    _fields_ = [
+        ("n_cos", _i), ("n_tau", _i), ("n_tau_prime", _i), ("n_quantile_samples", _i),
+        ("taus", _fp), ("embed", DdpgNet), ("target_embed", DdpgNet),
+    ]
+
+
 class PerStore(ctypes.Structure):
     """struct wdb_per_store (include/wdb200.h)."""
 
@@ -432,6 +441,13 @@ _SIGNATURES = {
     "wdb_qr_dqn_update_sampled_workspace_bytes": (_ll, [ctypes.POINTER(DqnUpdate), _i, _i]),
     "wdb_qr_dqn_update_sampled": (
         _i, [_vp, ctypes.POINTER(DqnUpdate), _i, ctypes.POINTER(ReplayWindows), _vp]),
+    "wdb_iqn_update_sampled_supported": (
+        _i, [ctypes.POINTER(DqnUpdate), ctypes.POINTER(IqnArgs), _i]),
+    "wdb_iqn_update_sampled_workspace_bytes": (
+        _ll, [ctypes.POINTER(DqnUpdate), ctypes.POINTER(IqnArgs), _i]),
+    "wdb_iqn_update_sampled": (
+        _i, [_vp, ctypes.POINTER(DqnUpdate), ctypes.POINTER(IqnArgs),
+             ctypes.POINTER(ReplayWindows), _vp]),
     "wdb_replay_sample_windows": (_i, [_vp, _vp, _i, _ull, _ull, _i, _i, _i, _i, _i]),
     "wdb_per_nodes": (_ll, [_ll]),
     "wdb_per_levels": (_i, [_ll]),

@@ -4,7 +4,8 @@ returns and a Huber loss (Mnih et al. 2015).
 The torch statement of wdb_dqn_update_sampled (include/wdb200.h): TrainerDQN runs it for the
 shapes the native pass does not take, and tests/dqn_update_reference.py restates it in float64
 NumPy.  QuantileDQN is quantile-regression DQN on the same windows (wdb_qr_dqn_update_sampled,
-tests/qr_dqn_reference.py)."""
+tests/qr_dqn_reference.py), ImplicitQuantileDQN implicit quantile networks
+(wdb_iqn_update_sampled, tests/iqn_reference.py)."""
 import torch
 from torch.nn import functional as func
 
@@ -105,6 +106,47 @@ class QuantileDQN(DQN):
         u = targets[:, None, :] - theta[:, :, None]             # [B, i, j]
         below = (u.detach() < 0).to(theta.dtype)
         rho = (tau[:, None] - below).abs() * func.huber_loss(
+            u, torch.zeros_like(u), reduction="none", delta=self.huber_delta) / self.huber_delta
+        rows = rho.sum(dim=1).mean(dim=-1)
+        loss = rows.mean() if weights is None else (weights * rows).mean()
+        return loss, theta.mean(dim=-1), targets.mean(dim=-1)
+
+
+class ImplicitQuantileDQN(DQN):
+    """Implicit quantile networks (IQN; Dabney, Ostrovski, Silver & Munos 2018) on DQN's
+    windows, n-step recursion and bootstrap rule: the torch statement of wdb_iqn_update_sampled
+    (include/wdb200.h) for a FullyConnectedIQN, restated in float64 NumPy by
+    tests/iqn_reference.py.  The levels come in: `taus` [B, N + N'] holds each loss row's N
+    online levels tau_i, then its N' target levels tau'_j.  `huber_delta` is kappa."""
+
+    def bootstrap_quantiles(self, q_net, target_net, boot_obs, taus_prime):
+        """The target's Z at tau'_j of a* [B, N'] (no gradient), a* the first argmax of the
+        collapsed Q of online(obs') with double_q, else of target(obs')."""
+        with torch.no_grad():
+            best = (q_net if self.double_q else target_net).q_values(boot_obs).argmax(dim=-1)
+            z = target_net.quantiles_at(boot_obs, taus_prime)           # [B, N', A]
+            return z.gather(-1, best[:, None, None].expand(-1, z.shape[1], 1))[..., 0]
+
+    def loss(self, q_net, target_net, obs, actions, rewards, done, boot_obs, weights=None,
+             taus=None):
+        """(quantile Huber loss, Q-bar [B], R-bar [B]) of B sampled windows, the arguments of
+        DQN.loss and the levels `taus`.  theta_i = Z_tau_i(obs)[a], T_j the n-step recursion on
+        the target's Z_tau'_j(obs')[a*], u_ij = T_j - theta_i, and the row loss
+        (1/N') sum_i sum_j |tau_i - 1{u_ij < 0}| huber(u_ij, kappa) / kappa; the loss is the mean
+        over rows of w_g times it (w = 1 without weights).  Q-bar = mean_i theta_i and
+        R-bar = mean_j T_j feed the metrics and the priorities."""
+        n = q_net.num_tau_samples
+        assert taus is not None and taus.shape == (obs.shape[0], n + q_net.num_tau_prime_samples)
+        tau, tau_prime = taus[:, :n].to(obs.dtype), taus[:, n:].to(obs.dtype)
+        with torch.no_grad():
+            boot = self.bootstrap_quantiles(q_net, target_net, boot_obs, tau_prime)
+            targets = self.sampled_returns(rewards[..., None], done[..., None], boot)
+        z = q_net.quantiles_at(obs, tau)                                 # [B, N, A]
+        a = actions.long().reshape(-1)
+        theta = z.gather(-1, a[:, None, None].expand(-1, n, 1))[..., 0]  # [B, N]
+        u = targets[:, None, :] - theta[:, :, None]                      # [B, i, j]
+        below = (u.detach() < 0).to(theta.dtype)
+        rho = (tau[:, :, None] - below).abs() * func.huber_loss(
             u, torch.zeros_like(u), reduction="none", delta=self.huber_delta) / self.huber_delta
         rows = rho.sum(dim=1).mean(dim=-1)
         loss = rows.mean() if weights is None else (weights * rows).mean()

@@ -3,8 +3,9 @@ network's gradient of one TrainerDQN update over the sampled windows of the repl
 place -- the online and target forwards, the double-Q bootstrap, the n-step returns, the Huber
 loss and the backward pass -- and writes it straight into the `.grad` views of the gradient
 arena.  `wdb_qr_dqn_update_sampled` does the same for quantile-regression DQN
-(FusedQRDQNUpdate).  The torch autograd updates (algorithms/dqn.py) stay for the shapes these do
-not take."""
+(FusedQRDQNUpdate) and `wdb_iqn_update_sampled` (csrc/wdb_iqn_update.cu) for implicit quantile
+networks (FusedIQNUpdate).  The torch autograd updates (algorithms/dqn.py) stay for the shapes
+these do not take."""
 import ctypes
 
 import torch
@@ -140,4 +141,81 @@ class FusedQRDQNUpdate:
         _lib.check(self.lib.wdb_qr_dqn_update_sampled(
             _lib.stream_ptr(), ctypes.byref(u), self.n_quantiles,
             ctypes.byref(replay_windows(windows)), _lib.ptr(weights)), "qr_dqn_update_sampled")
+        return self.sums
+
+
+def _iqn_struct(q_net, target_net=None):
+    """struct wdb_iqn_args of an IQN pair: the counts, and the embeddings' pointers when the
+    networks are given."""
+    a = _lib.IqnArgs()
+    a.n_cos, a.n_tau = int(q_net.num_cosines), int(q_net.num_tau_samples)
+    a.n_tau_prime = int(q_net.num_tau_prime_samples)
+    a.n_quantile_samples = int(q_net.num_quantile_samples)
+    if target_net is not None:
+        for net, model, grads in ((a.embed, q_net, True), (a.target_embed, target_net, False)):
+            e = model.tau_embedding
+            net.w[0], net.b[0] = _lib.ptr(e.weight.data), _lib.ptr(e.bias.data)
+            if grads:
+                net.gw[0], net.gb[0] = _lib.ptr(e.weight.grad), _lib.ptr(e.bias.grad)
+    return a
+
+
+def fused_iqn_supported(algo, q_net, n_envs, n_agents, capacity, replay_rows):
+    """True if `wdb_iqn_update_sampled` takes this policy: a FullyConnectedIQN over a Box
+    observation with 1..3 hidden layers of width <= 64, F <= 63, A <= 64, n_cos, N and N' <= 64,
+    everything in one CTA's shared memory, and replay_rows sampled windows per update."""
+    from warp_drive_b200.training.models.fully_connected_q import FullyConnectedIQN
+
+    if type(q_net) is not FullyConnectedIQN or not isinstance(q_net.observation_space, Box):
+        return False
+    if len(q_net.fc_dims) > 3:
+        return False
+    u = _shape_struct(algo, q_net, n_envs, n_agents, capacity)
+    return bool(_lib.load().wdb_iqn_update_sampled_supported(
+        ctypes.byref(u), ctypes.byref(_iqn_struct(q_net)), int(replay_rows)))
+
+
+class FusedIQNUpdate:
+    """One policy's `wdb_iqn_update_sampled` launch: DQN's argument struct and the IQN one
+    beside it; the sums are sum w_g loss_g and sum Q-bar, the outputs Q-bar and R-bar."""
+
+    def __init__(self, algo, q_net, target_net, n_envs, n_agents, capacity, replay_rows):
+        self.models = (q_net, target_net)
+        self.u = _shape_struct(algo, q_net, n_envs, n_agents, capacity)
+        self.iqn = _iqn_struct(q_net)
+        self.lib = _lib.load()
+        self.rows = int(replay_rows)
+        nbytes = int(self.lib.wdb_iqn_update_sampled_workspace_bytes(
+            ctypes.byref(self.u), ctypes.byref(self.iqn), self.rows))
+        assert nbytes > 0, "shapes not supported by wdb_iqn_update_sampled"
+        dev = next(q_net.parameters()).device
+        self.workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        self.sums = torch.zeros(2, dtype=torch.float64, device=dev)
+
+    def launch(self, obs, actions, rewards, done, windows, outputs=None, weights=None,
+               taus=None):
+        """The network's gradient (trunk, head and tau embedding) into its `.grad`; the
+        arguments of FusedDQNUpdate.launch and the levels `taus`, float32 [rows, N + N']
+        (outputs: Q-bar and R-bar)."""
+        u = self.u
+        q_net, target_net = self.models
+        _set_pointers(u.q, q_net, True)
+        _set_pointers(u.target_q, target_net, False)
+        iqn = self.iqn = _iqn_struct(q_net, target_net)
+        n = iqn.n_tau + iqn.n_tau_prime
+        assert taus is not None and taus.shape == (self.rows, n) and taus.dtype == torch.float32
+        assert taus.is_contiguous()
+        iqn.taus = _lib.ptr(taus)
+        u.obs, u.actions = _lib.ptr(obs), _lib.ptr(actions)
+        u.rewards, u.done = _lib.ptr(rewards), _lib.ptr(done)
+        q_values, returns = outputs if outputs is not None else (None, None)
+        u.q_values, u.returns = _lib.ptr(q_values), _lib.ptr(returns)
+        u.sums = _lib.ptr(self.sums)
+        u.workspace = _lib.ptr(self.workspace)
+        assert windows.shape[0] == self.rows
+        if weights is not None:
+            assert weights.shape == (self.rows,) and weights.dtype == torch.float32
+        _lib.check(self.lib.wdb_iqn_update_sampled(
+            _lib.stream_ptr(), ctypes.byref(u), ctypes.byref(iqn),
+            ctypes.byref(replay_windows(windows)), _lib.ptr(weights)), "iqn_update_sampled")
         return self.sums

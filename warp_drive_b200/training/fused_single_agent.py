@@ -98,10 +98,10 @@ class FusedSingleAgentRollout:
         r.rewards = _p(dm.device_data(_REWARDS))
         r.sampled_actions = _p(dm.device_data(_ACTIONS))
         layers = _layers(model)
-        # QR-DQN's quantile network: the kernel runs epsilon-greedy over the mean quantile, the
-        # head collapsed to A rows (collapsed_head), kept in buffers of its own and recomputed
-        # from the live head at every launch
-        self._quantile = model if getattr(_unwrap(model), "is_quantile_q", False) else None
+        # a distributional Q network (QR-DQN's, IQN's): the kernel runs epsilon-greedy over its
+        # mean, the head collapsed to one Linear(H, A) (collapsed_head), kept in buffers of its
+        # own and recomputed from the live parameters at every launch
+        self._quantile = model if hasattr(_unwrap(model), "collapsed_head") else None
         if self._quantile is not None:
             with torch.no_grad():
                 w, b = _unwrap(model).collapsed_head()

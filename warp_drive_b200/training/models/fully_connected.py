@@ -209,6 +209,11 @@ class ModelFactory:
                 FullyConnectedQuantileQ)
 
             cls._registry[model_name] = FullyConnectedQuantileQ
+        if model_name == "fully_connected_iqn" and model_name not in cls._registry:
+            # IQN's implicit quantile network, imported on first use
+            from warp_drive_b200.training.models.fully_connected_q import FullyConnectedIQN
+
+            cls._registry[model_name] = FullyConnectedIQN
         if model_name not in cls._registry and model_name in (
                 "fully_connected_actor", "fully_connected_action_value_critic",
                 "fully_connected_sac_actor"):

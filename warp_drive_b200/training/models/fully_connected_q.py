@@ -6,6 +6,9 @@ head.  `q_values(obs)` is what the update uses; `forward(obs)` keeps the rollout
 `(outputs per head, values)` contract as `([Q], None)`, and the engine recognises the network
 by `is_q_network` and samples its actions epsilon-greedily (CUDASampler.sample_epsilon_greedy).
 """
+import math
+
+import torch
 from torch import nn
 from torch.nn import functional as func
 
@@ -97,5 +100,96 @@ class FullyConnectedQuantileQ(FullyConnectedQ):
 
     def q_values(self, obs):
         """The mean quantile of every action: [..., A]."""
+        w, b = self.collapsed_head()
+        return func.linear(self.trunk(obs), w, b)
+
+
+class FullyConnectedIQN(FullyConnectedQ):
+    """The implicit quantile network of IQN (algorithms/dqn.py ImplicitQuantileDQN; Dabney,
+    Ostrovski, Silver & Munos 2018): the return distribution as a function of the level tau.
+
+    Trunk psi(x): FullyConnectedQ's `fc_dims` layers (at least one), width H.  Embedding
+    phi(tau) = ReLU(`tau_embedding`(cos(pi i tau) for i = 0 .. n_cos - 1)), `tau_embedding` =
+    Linear(n_cos, H) (i = 0 is the constant 1, as in the paper).  Value at level tau:
+    Z_tau(x, .) = `policy_head`(psi(x) * phi(tau)), `policy_head` one raw Linear(H, A).  The paper
+    puts one more hidden layer after the merge; here the head is one raw Linear, as QR-DQN's, so
+    that acting collapses exactly into one Linear (below).
+
+    Model keys (Dopamine's names; Dopamine calls n_cos `quantile_embedding_dim`):
+    `num_cosines` n_cos (64, in [1, 64]), `num_tau_samples` N (32, in [1, 64]) and
+    `num_tau_prime_samples` N' (32, in [1, 64]), the online and target levels per loss row, and
+    `num_quantile_samples` K (32, in [1, 256]), the levels averaged for acting and for the
+    bootstrap action.
+
+    Acting averages Z over the fixed midpoints tau~_k = (2k + 1) / (2K) rather than over K fresh
+    samples per step as the paper does -- a deliberate divergence that keeps it deterministic:
+    Q(x, a) = mean_k Z_tau~k(x, a) = `policy_head`(psi(x) * c-bar), c-bar = mean_k phi(tau~_k),
+    so `collapsed_head()` = (W diag(c-bar), b) is exact.  `q_values`, and through it `forward`,
+    the per-step epsilon-greedy path, the one-launch rollout and the evaluator, go through it.
+    `quantiles_at(x, taus)` is what the update uses."""
+    name = "torch_fully_connected_iqn"
+    is_implicit_quantile_q = True
+
+    # (key, default, largest value); each is an integer of at least 1
+    KEYS = (("num_cosines", 64, 64), ("num_tau_samples", 32, 64),
+            ("num_tau_prime_samples", 32, 64), ("num_quantile_samples", 32, 256))
+
+    def __init__(self, env, model_config, policy, policy_tag_to_agent_id_map,
+                 create_separate_placeholders_for_each_policy=False,
+                 obs_dim_corresponding_to_num_agents="first"):
+        dims = model_config.get("fc_dims")
+        if not dims:
+            raise ValueError("fully_connected_iqn needs model.fc_dims with at least one hidden "
+                             f"layer (the trunk the tau embedding multiplies), got {dims!r}")
+        counts = {}
+        for key, default, top in self.KEYS:
+            v = model_config.get(key, default)
+            if isinstance(v, bool) or not isinstance(v, int) or not 1 <= v <= top:
+                raise ValueError(f"fully_connected_iqn's model.{key} is an integer in [1, {top}], "
+                                 f"got {v!r}")
+            counts[key] = v
+        super().__init__(env, model_config, policy, policy_tag_to_agent_id_map,
+                         create_separate_placeholders_for_each_policy,
+                         obs_dim_corresponding_to_num_agents)
+        for key, v in counts.items():
+            setattr(self, key, v)
+        self.tau_embedding = nn.Linear(self.num_cosines, self.policy_head.in_features)
+
+    def trunk(self, obs):
+        """psi(obs): [..., H]."""
+        x = obs
+        for i in range(len(self.fc)):
+            x = self.fc[str(i)](x)
+        return x
+
+    def cos_features(self, taus):
+        """cos(pi i tau) for i = 0 .. n_cos - 1: [..., n_cos].  pi i is rounded once to the
+        levels' dtype, then multiplied by tau: the float32 operations of the native pass."""
+        freq = math.pi * torch.arange(self.num_cosines, dtype=torch.float64, device=taus.device)
+        return torch.cos(taus[..., None] * freq.to(taus.dtype))
+
+    def embedding(self, taus):
+        """phi(tau): [..., H]."""
+        return func.relu(self.tau_embedding(self.cos_features(taus)))
+
+    def quantiles_at(self, obs, taus):
+        """Z at the given levels: obs [B, F], taus [B, T] (each row its own levels) or [T]
+        (shared) -> [B, T, A]."""
+        return self.policy_head(self.trunk(obs)[..., None, :] * self.embedding(taus))
+
+    def acting_levels(self):
+        """The K midpoints tau~_k = (2k + 1) / (2K) that acting and a* average over."""
+        w = self.policy_head.weight
+        k = self.num_quantile_samples
+        return (2 * torch.arange(k, dtype=w.dtype, device=w.device) + 1) / (2 * k)
+
+    def collapsed_head(self):
+        """(W diag(c-bar), b), c-bar = mean_k phi(tau~_k): the head of the mean over the K
+        midpoints."""
+        cbar = self.embedding(self.acting_levels()).mean(0)
+        return self.policy_head.weight * cbar, self.policy_head.bias
+
+    def q_values(self, obs):
+        """The mean of Z over the K midpoints, for every action: [..., A]."""
         w, b = self.collapsed_head()
         return func.linear(self.trunk(obs), w, b)

@@ -31,14 +31,22 @@ QuantileDQN's quantile Huber loss (wdb_qr_dqn_update_sampled, 2 launches, or tor
 on the same windows, targets and schedule.  Its `Mean Q value` and `Mean return` are the means
 of Q-bar = mean_i theta_i and R-bar = mean_j T_j, and with prioritized replay the priorities are
 (|Q-bar - R-bar| + epsilon)^alpha.
+
+Implicit quantile networks: a `fully_connected_iqn` model trains with ImplicitQuantileDQN's
+quantile Huber loss over sampled levels (wdb_iqn_update_sampled, 2 launches, or torch autograd)
+on the same windows, targets and schedule.  Each update draws its levels -- N online and N'
+target ones per loss row, uniform on [0, 1) -- into one [B, N + N'] buffer with a CUDA
+generator seeded from the trainer seed (1 launch); the native and the torch path read the same
+buffer.  Metrics and priorities are QR-DQN's.
 """
 import os
 
 import torch
 
-from warp_drive_b200.training.algorithms.dqn import DQN, QuantileDQN
+from warp_drive_b200.training.algorithms.dqn import DQN, ImplicitQuantileDQN, QuantileDQN
 from warp_drive_b200.training.algorithms.fused_dqn import (
-    FusedDQNUpdate, FusedQRDQNUpdate, fused_dqn_supported, fused_qr_dqn_supported)
+    FusedDQNUpdate, FusedIQNUpdate, FusedQRDQNUpdate, fused_dqn_supported, fused_iqn_supported,
+    fused_qr_dqn_supported)
 from warp_drive_b200.training.trainer_ddpg import (
     RingRolloutEngine, TrainerDDPG, hard_update, soft_update)
 from warp_drive_b200.training.utils.param_scheduler import ParamScheduler
@@ -118,6 +126,8 @@ class TrainerDQN(TrainerDDPG):
         self.tau, self.target_update_period, self.update_count = {}, {}, {}
         self.fused_updates, self.replay_windows, self.replay_draws = {}, {}, 0
         self.priority_stores = {}
+        # IQN: each policy's levels of one update [B, N + N'] and the generator that draws them
+        self.iqn_taus, self._tau_generator = {}, None
         self.last_epsilon = None
         # the networks the rollout runs (TrainerDDPG's replay helpers know them as actors)
         self.models = self.actor_models = self.q_models
@@ -130,8 +140,8 @@ class TrainerDQN(TrainerDDPG):
         model_cfg = c["model"]
         self.q_models[policy] = self._build_model(policy, model_cfg)
         if not getattr(self.q_models[policy], "is_q_network", False):
-            raise ValueError("DQN's model is a `fully_connected_q` or a "
-                             f"`fully_connected_quantile_q`, got '{model_cfg.get('type')}'")
+            raise ValueError("DQN's model is a `fully_connected_q`, a `fully_connected_quantile_q` "
+                             f"or a `fully_connected_iqn`, got '{model_cfg.get('type')}'")
         self.target_q_models[policy] = self._build_model(policy, model_cfg)
         hard_update(self.target_q_models[policy], self.q_models[policy])
 
@@ -160,7 +170,9 @@ class TrainerDQN(TrainerDDPG):
         self.update_count[policy] = 0
         q_net = self.q_models[policy]
         quantile = getattr(q_net, "is_quantile_q", False)
-        algo = self.trainers[policy] = (QuantileDQN if quantile else DQN)(
+        implicit = getattr(q_net, "is_implicit_quantile_q", False)
+        algo = self.trainers[policy] = (
+            ImplicitQuantileDQN if implicit else QuantileDQN if quantile else DQN)(
             discount_factor_gamma=c["gamma"], n_step=self.n_step, double_q=double_q,
             huber_delta=delta)
         n_agents = len(self.policy_tag_to_agent_id_map[policy])
@@ -174,7 +186,15 @@ class TrainerDQN(TrainerDDPG):
                 print(f"[Device {self.device_id}]: priority store of policy '{policy}': "
                       f"{store.leaves.numel()} windows, a sum tree of {store.levels} levels, "
                       f"{store.nbytes()} bytes on the device")
-        supported, fused = ((fused_qr_dqn_supported, FusedQRDQNUpdate) if quantile
+        if implicit:
+            dev = next(q_net.parameters()).device
+            self.iqn_taus[policy] = torch.zeros(
+                rows, q_net.num_tau_samples + q_net.num_tau_prime_samples, device=dev)
+            if self._tau_generator is None:
+                self._tau_generator = torch.Generator(device=dev)
+                self._tau_generator.manual_seed(self.seed)
+        supported, fused = ((fused_iqn_supported, FusedIQNUpdate) if implicit
+                            else (fused_qr_dqn_supported, FusedQRDQNUpdate) if quantile
                             else (fused_dqn_supported, FusedDQNUpdate))
         if supported(algo, q_net, self.num_envs, n_agents, self.ring_capacity, rows):
             self.fused_updates[policy] = fused(
@@ -230,6 +250,8 @@ class TrainerDQN(TrainerDDPG):
         for policy in self.policies_to_train:
             self.update_count[policy] += 1
             self._sample_replay_windows(policy)
+            if policy in self.iqn_taus:
+                self.iqn_taus[policy].uniform_(generator=self._tau_generator)
             fused = self.fused_updates.get(policy)
             if fused is not None and self.trainers[policy].use_fused_update:
                 loss_metrics[policy] = self._fused_q_gradients(policy, fused, logging_flag)
@@ -250,13 +272,14 @@ class TrainerDQN(TrainerDDPG):
 
     def _torch_q_gradients(self, policy, logging_flag):
         """The Q gradient by torch autograd on the gathered windows (the loss of
-        wdb_dqn_update_sampled, or of wdb_qr_dqn_update_sampled for a quantile network),
-        accumulated into the arena's .grad views."""
+        wdb_dqn_update_sampled, or of wdb_qr_dqn_update_sampled / wdb_iqn_update_sampled for a
+        quantile network), accumulated into the arena's .grad views."""
         algo = self.trainers[policy]
         store = self.priority_stores.get(policy)
         loss, q, returns = algo.loss(self.q_models[policy], self.target_q_models[policy],
                                      *self._gather_windows(policy),
-                                     weights=None if store is None else store.weights)
+                                     weights=None if store is None else store.weights,
+                                     **self._levels(policy))
         if store is not None:                  # the inputs of the new priorities
             store.q_values.copy_(q.detach())
             store.returns.copy_(returns)
@@ -267,9 +290,9 @@ class TrainerDQN(TrainerDDPG):
         return algo.loss_metrics(loss.item(), q.detach().double().mean(), returns)
 
     def _fused_q_gradients(self, policy, fused, logging_flag):
-        """The same gradient from the native pass (FusedDQNUpdate or FusedQRDQNUpdate),
-        written straight into the arena's .grad views; the host waits only on logging
-        iterations (metrics)."""
+        """The same gradient from the native pass (FusedDQNUpdate, FusedQRDQNUpdate or
+        FusedIQNUpdate), written straight into the arena's .grad views; the host waits only on
+        logging iterations (metrics)."""
         eng = self.engine
         outputs, weights = None, None
         store = self.priority_stores.get(policy)
@@ -282,12 +305,18 @@ class TrainerDQN(TrainerDDPG):
                             eng._tensor(f"{_ACTIONS}_batch_{policy}"),
                             eng._tensor(f"{_REWARDS}_batch_{policy}"),
                             eng._tensor(f"{_DONE_FLAGS}_batch"), self.replay_windows[policy],
-                            outputs, weights)
+                            outputs, weights, **self._levels(policy))
         if not logging_flag:
             return {}
         s = sums.tolist()
         return self.trainers[policy].loss_metrics(s[0] / fused.rows, s[1] / fused.rows,
                                                   outputs[1])
+
+    def _levels(self, policy):
+        """IQN's levels of this update, as the `taus` argument of its loss and its native pass
+        (nothing for the other Q networks)."""
+        taus = self.iqn_taus.get(policy)
+        return {} if taus is None else {"taus": taus}
 
     # ------------------------------------------------------------------ checkpoints
     def _checkpointed_networks(self):
