@@ -401,10 +401,20 @@ typedef struct wdb_sa_rollout {
    * are Q values, written to probs_batch when given, and the action is sampled as
    * wdb_sample_epsilon_greedy (stream = env, one draw per step) with epsilon = log_std[0], a
    * device float in [0, 1] (use_argmax: epsilon = 0).  Needs log_std and rng_state; `uniforms`
-   * must be NULL.  (The struct keeps its layout.) */
+   * must be NULL.  (The struct keeps its layout.)
+   * Discrete kinds, categorical Q head (gaussian_head = 4; C51's FullyConnectedCategoricalQ):
+   * the head is A blocks of N atom logits, dims[n_hidden + 1] = A * N with A the kind's action
+   * count.  Each block is reduced to Q[a] = sum_j z_j softmax_j over the env's 8 lanes (lane k:
+   * j = k, k + 8, ... in order, then an xor butterfly; e_j = expf(y_j - max y), Q = (sum z_j
+   * e_j) / (sum e_j)); Q is written to probs_batch when given and sampled as the Q head is.
+   * log_std = [epsilon, z_0, ..., z_{N-1}] on the device. */
 } wdb_sa_rollout;
 
 int wdb_single_agent_rollout_supported(int n_hidden, const int *dims);
+/* 1 if a categorical Q head of dims[n_hidden + 1] = A * N outputs runs in one launch: the
+ * hidden widths and F as wdb_single_agent_rollout_supported takes them, 2 <= N <= 64, N
+ * dividing the head, and the same cap on the network's floats. */
+int wdb_single_agent_rollout_categorical_supported(int n_hidden, const int *dims, int n_atoms);
 int wdb_single_agent_rollout(void *stream, const wdb_sa_rollout *rollout);
 
 /* -------------------------------------------------- rollout of ANY env: data movement ---- */
@@ -1080,6 +1090,42 @@ long long wdb_iqn_update_sampled_workspace_bytes(const wdb_dqn_update_args *upda
 int wdb_iqn_update_sampled(void *stream, const wdb_dqn_update_args *update,
                            const wdb_iqn_args *iqn, const wdb_replay_windows *windows,
                            const float *weights);
+
+/* One categorical DQN update (C51; Bellemare, Dabney & Munos 2017) over B sampled windows, read
+ * as wdb_dqn_update_sampled reads them.  The networks' head has A * N outputs (n_actions = A,
+ * n_atoms = N); column a * N + j is the logit of atom j of action a.  support [N] (device) holds
+ * the atoms z_0 < ... < z_{N-1}, delta_z > 0 their spacing.  Per loss row g with action a, in
+ * float32 (sums "over the row": lane k of the row's 16 threads takes j = k, k + 16, ... in
+ * order, then the 16 lanes are combined by an xor butterfly; every lane gets the same bits):
+ *   Q(x, c)  = q / s over the row, e_j = expf(y_j - max_j y_j), s = sum e_j, q = sum fmaf(z_j,
+ *              e_j, .), y = the logits of action c at x,
+ *   a*       = the first argmax over c of Q(obs', c) of online (double_q) or target,
+ *   p'_j     = e_j / s of target(obs')[a*],
+ *   Tz_j     = DQN's n-step recursion (float32, every non-zero done terminal) on z_j, then
+ *              fminf(fmaxf(., z_0), z_{N-1}),
+ *   m_i      = sum_j (j in order) fmaf(clip(1 - |Tz_j - z_i| / delta_z, 0, 1), p'_j, .),
+ *   p_i      = expf(l_i - max l) / s of the online logits l = online(obs)[a],
+ *   loss_g   = -sum_i m_i log_softmax(l)_i (in float64),
+ *   loss     = (1/B) sum_g w_g loss_g,  w_g = weights[g], or 1 when weights is NULL,
+ * and its gradient d loss / d l_i = ((p_i * sum_k m_k - m_i) * w_g) * (1/B) (sum_k m_k over the
+ * row; not assumed to be 1) in column a * N + i, back through the online network into q.gw /
+ * gb.  sums[0] = sum_g w_g loss_g, sums[1] = sum_g Q-bar_g; the optional outputs [B] are
+ * q_values = Q-bar = sum_i z_i p_i and returns = R-bar = sum_i z_i m_i (float64 sums, stored
+ * as float32).  huber_delta is not read.  The weight multiplies a row's gradient and loss once
+ * each, so unit weights reproduce the unweighted pass bit for bit.  Per-CTA partials summed in
+ * a fixed order by a second launch: bit-reproducible.  Two launches.
+ * Supported: the shapes of wdb_dqn_update_sampled_supported (the head A * N may exceed 64) with
+ * 2 <= N <= 64, and both networks, the gradient block and the row tiles in one CTA's shared
+ * memory.  No CUDA call. */
+int wdb_c51_update_sampled_supported(const wdb_dqn_update_args *update, int n_atoms,
+                                     int n_windows);
+long long wdb_c51_update_sampled_workspace_bytes(const wdb_dqn_update_args *update,
+                                                 int n_atoms, int n_windows);
+/* cudaErrorInvalidValue without launching if unsupported, a required pointer is NULL or
+ * delta_z <= 0. */
+int wdb_c51_update_sampled(void *stream, const wdb_dqn_update_args *update, int n_atoms,
+                           const float *support, float delta_z,
+                           const wdb_replay_windows *windows, const float *weights);
 
 /* Prioritized replay (Schaul et al. 2016, proportional) over the replay ring's n-step windows.
  * One float32 leaf per (physical slot s, agent row n), leaf s * n_rows + n: p^alpha of the

@@ -30,20 +30,6 @@ namespace {
 
 constexpr int kMaxQuantileSamples = 256;   // K
 
-// The trunk (layers 0 .. L - 2 of net k, Linear + ReLU) on the tile; outbuf(l) is where hidden
-// layer l writes.
-template <class OutBuf>
-__device__ __forceinline__ void trunk_forward(const float *W, const Plan &P, int k, const float *X,
-                                              OutBuf outbuf) {
-  const float *x = X;
-  for (int l = 0; l < P.L[k] - 1; l++) {
-    float *y = outbuf(l);
-    layer_forward(W + P.woff[k][l], P.pw[k][l], P.in[k][l], P.out[k][l], x, y, true);
-    __syncthreads();
-    x = y;
-  }
-}
-
 // The cosine features of one tile of levels: CF[r][c] = cos(freq[c] * tau(r)) for c < n_cos,
 // freq[c] = float(pi * c) -- the float32 operations of FullyConnectedIQN.cos_features.
 template <class Tau>

@@ -1,8 +1,9 @@
 // wdb_update_tiles.cuh -- the tile primitives of the replay-update passes: the shared-memory
 // Plan of a pass's networks, the row-tile layer forward / input-gradient / weight-gradient steps,
 // the sampled row source and the fixed-order reduction of the per-CTA partials into the
-// gradient arena.  wdb_ddpg_update.cu (DDPG, TD3, SAC, DQN, QR-DQN) and wdb_iqn_update.cu (IQN)
-// build their passes on them; each translation unit gets its own copy (anonymous namespace).
+// gradient arena.  wdb_ddpg_update.cu (DDPG, TD3, SAC, DQN, QR-DQN), wdb_iqn_update.cu (IQN) and
+// wdb_c51_update.cu (C51) build their passes on them; each translation unit gets its own copy
+// (anonymous namespace).
 #pragma once
 
 #include "wdb_common.cuh"
@@ -200,6 +201,20 @@ __device__ __forceinline__ void net_forward(const float *W, const Plan &P, int k
   for (int l = 0; l < P.L[k]; l++) {
     float *y = outbuf(l);
     layer_forward(W + P.woff[k][l], P.pw[k][l], P.in[k][l], P.out[k][l], x, y, l < P.L[k] - 1);
+    __syncthreads();
+    x = y;
+  }
+}
+
+// The trunk (layers 0 .. L - 2 of net k, Linear + ReLU) on the tile; outbuf(l) is where hidden
+// layer l writes.
+template <class OutBuf>
+__device__ __forceinline__ void trunk_forward(const float *W, const Plan &P, int k, const float *X,
+                                              OutBuf outbuf) {
+  const float *x = X;
+  for (int l = 0; l < P.L[k] - 1; l++) {
+    float *y = outbuf(l);
+    layer_forward(W + P.woff[k][l], P.pw[k][l], P.in[k][l], P.out[k][l], x, y, true);
     __syncthreads();
     x = y;
   }

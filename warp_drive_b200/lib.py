@@ -448,6 +448,10 @@ _SIGNATURES = {
     "wdb_iqn_update_sampled": (
         _i, [_vp, ctypes.POINTER(DqnUpdate), ctypes.POINTER(IqnArgs),
              ctypes.POINTER(ReplayWindows), _vp]),
+    "wdb_c51_update_sampled_supported": (_i, [ctypes.POINTER(DqnUpdate), _i, _i]),
+    "wdb_c51_update_sampled_workspace_bytes": (_ll, [ctypes.POINTER(DqnUpdate), _i, _i]),
+    "wdb_c51_update_sampled": (
+        _i, [_vp, ctypes.POINTER(DqnUpdate), _i, _vp, _f, ctypes.POINTER(ReplayWindows), _vp]),
     "wdb_replay_sample_windows": (_i, [_vp, _vp, _i, _ull, _ull, _i, _i, _i, _i, _i]),
     "wdb_per_nodes": (_ll, [_ll]),
     "wdb_per_levels": (_i, [_ll]),
@@ -457,6 +461,7 @@ _SIGNATURES = {
     "wdb_per_set_priorities": (
         _i, [_vp, ctypes.POINTER(PerStore), _vp, _i, _vp, _vp, _i, _i]),
     "wdb_single_agent_rollout_supported": (_i, [_i, ctypes.POINTER(_i)]),
+    "wdb_single_agent_rollout_categorical_supported": (_i, [_i, ctypes.POINTER(_i), _i]),
     "wdb_single_agent_rollout": (_i, [_vp, ctypes.POINTER(SaRollout)]),
     "wdb_mountain_car_step": (
         _i, [_vp, _i, _vp, _vp, _vp, _vp, _vp] + [_f] * 7 + [_vp, _i]),

@@ -5,7 +5,8 @@ The torch statement of wdb_dqn_update_sampled (include/wdb200.h): TrainerDQN run
 shapes the native pass does not take, and tests/dqn_update_reference.py restates it in float64
 NumPy.  QuantileDQN is quantile-regression DQN on the same windows (wdb_qr_dqn_update_sampled,
 tests/qr_dqn_reference.py), ImplicitQuantileDQN implicit quantile networks
-(wdb_iqn_update_sampled, tests/iqn_reference.py)."""
+(wdb_iqn_update_sampled, tests/iqn_reference.py), CategoricalDQN categorical DQN
+(wdb_c51_update_sampled, tests/c51_reference.py)."""
 import torch
 from torch.nn import functional as func
 
@@ -151,3 +152,46 @@ class ImplicitQuantileDQN(DQN):
         rows = rho.sum(dim=1).mean(dim=-1)
         loss = rows.mean() if weights is None else (weights * rows).mean()
         return loss, theta.mean(dim=-1), targets.mean(dim=-1)
+
+
+class CategoricalDQN(DQN):
+    """Categorical DQN (C51; Bellemare, Dabney & Munos 2017) on DQN's windows, n-step recursion
+    and bootstrap rule: the torch statement of wdb_c51_update_sampled (include/wdb200.h) for a
+    FullyConnectedCategoricalQ, restated in float64 NumPy by tests/c51_reference.py.  C51 has no
+    Huber loss: `huber_delta` is not used (TrainerDQN refuses it in a categorical policy's
+    config).
+
+    Priorities: prioritized replay writes (|Q-bar - R-bar| + epsilon)^alpha, as for QR-DQN and
+    IQN, so the store is shared by every Q network; Rainbow uses the row's cross-entropy
+    instead -- a deliberate divergence."""
+
+    def bootstrap_distribution(self, q_net, target_net, boot_obs):
+        """p' = softmax(target.logits(obs')[a*]) [B, N] (no gradient), a* the first argmax of
+        the expectation of online(obs') with double_q, else of target(obs')."""
+        with torch.no_grad():
+            best = (q_net if self.double_q else target_net).q_values(boot_obs).argmax(dim=-1)
+            p = target_net.probabilities(boot_obs)
+            return p[torch.arange(p.shape[0], device=p.device), best]
+
+    def loss(self, q_net, target_net, obs, actions, rewards, done, boot_obs, weights=None):
+        """(cross-entropy loss, Q-bar [B], R-bar [B]) of B sampled windows, the arguments of
+        DQN.loss.  Tz_j is the n-step recursion on each atom z_j, clamped to [z_0, z_{N-1}];
+        the projection m_i = sum_j clip(1 - |Tz_j - z_i| / dz, 0, 1) p'_j (Dopamine's dense
+        form); the row loss -sum_i m_i log_softmax(l)_i over the online logits l of the row's
+        action, and the loss the mean over rows of w_g times it (w = 1 without weights).
+        Q-bar = sum_i z_i p_i and R-bar = sum_i z_i m_i feed the metrics and the priorities."""
+        z = q_net.support.to(obs.dtype)
+        with torch.no_grad():
+            p_boot = self.bootstrap_distribution(q_net, target_net, boot_obs)
+            tz = self.sampled_returns(rewards[..., None], done[..., None],
+                                      z.expand(obs.shape[0], -1))
+            tz = tz.clamp(z[0], z[-1])
+            pair = (1 - (tz[:, None, :] - z[None, :, None]).abs() / q_net.delta_z).clamp(0, 1)
+            m = (pair * p_boot[:, None, :]).sum(dim=-1)                 # [B, i]
+        logits = q_net.logits(obs)
+        logits = logits[torch.arange(logits.shape[0], device=logits.device),
+                        actions.long().reshape(-1)]                      # [B, N]
+        rows = -(m * func.log_softmax(logits, dim=-1)).sum(dim=-1)
+        loss = rows.mean() if weights is None else (weights * rows).mean()
+        qbar = (torch.softmax(logits.detach(), dim=-1) * z).sum(dim=-1)
+        return loss, qbar, (m * z).sum(dim=-1)

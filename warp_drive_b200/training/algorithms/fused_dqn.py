@@ -4,7 +4,8 @@ place -- the online and target forwards, the double-Q bootstrap, the n-step retu
 loss and the backward pass -- and writes it straight into the `.grad` views of the gradient
 arena.  `wdb_qr_dqn_update_sampled` does the same for quantile-regression DQN
 (FusedQRDQNUpdate) and `wdb_iqn_update_sampled` (csrc/wdb_iqn_update.cu) for implicit quantile
-networks (FusedIQNUpdate).  The torch autograd updates (algorithms/dqn.py) stay for the shapes
+networks (FusedIQNUpdate), and `wdb_c51_update_sampled` (csrc/wdb_c51_update.cu) for categorical
+DQN (FusedC51Update).  The torch autograd updates (algorithms/dqn.py) stay for the shapes
 these do not take."""
 import ctypes
 
@@ -218,4 +219,63 @@ class FusedIQNUpdate:
         _lib.check(self.lib.wdb_iqn_update_sampled(
             _lib.stream_ptr(), ctypes.byref(u), ctypes.byref(iqn),
             ctypes.byref(replay_windows(windows)), _lib.ptr(weights)), "iqn_update_sampled")
+        return self.sums
+
+
+def fused_c51_supported(algo, q_net, n_envs, n_agents, capacity, replay_rows):
+    """True if `wdb_c51_update_sampled` takes this policy: a FullyConnectedCategoricalQ over a
+    Box observation with 0..3 hidden layers of width <= 64, F <= 63, A <= 64 and 2 <= N <= 64
+    atoms, everything in one CTA's shared memory, and replay_rows sampled windows per update."""
+    from warp_drive_b200.training.models.fully_connected_q import FullyConnectedCategoricalQ
+
+    if type(q_net) is not FullyConnectedCategoricalQ or not isinstance(q_net.observation_space,
+                                                                       Box):
+        return False
+    if len(q_net.fc_dims) > 3:
+        return False
+    u = _shape_struct(algo, q_net, n_envs, n_agents, capacity)
+    return bool(_lib.load().wdb_c51_update_sampled_supported(
+        ctypes.byref(u), int(q_net.num_atoms), int(replay_rows)))
+
+
+class FusedC51Update:
+    """One policy's `wdb_c51_update_sampled` launch: DQN's argument struct with the number of
+    atoms, the model's support (float32, on the device) and its spacing beside it; the sums are
+    sum w_g loss_g and sum Q-bar, the outputs Q-bar and R-bar."""
+
+    def __init__(self, algo, q_net, target_net, n_envs, n_agents, capacity, replay_rows):
+        self.models = (q_net, target_net)
+        self.u = _shape_struct(algo, q_net, n_envs, n_agents, capacity)
+        self.n_atoms = int(q_net.num_atoms)
+        self.lib = _lib.load()
+        self.rows = int(replay_rows)
+        nbytes = int(self.lib.wdb_c51_update_sampled_workspace_bytes(
+            ctypes.byref(self.u), self.n_atoms, self.rows))
+        assert nbytes > 0, "shapes not supported by wdb_c51_update_sampled"
+        dev = next(q_net.parameters()).device
+        self.workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        self.sums = torch.zeros(2, dtype=torch.float64, device=dev)
+        self.support = q_net.support.to(device=dev, dtype=torch.float32).contiguous()
+        self.delta_z = float(q_net.delta_z)
+
+    def launch(self, obs, actions, rewards, done, windows, outputs=None, weights=None):
+        """The categorical network's gradient into its `.grad`; the arguments of
+        FusedDQNUpdate.launch (outputs: Q-bar and R-bar)."""
+        u = self.u
+        q_net, target_net = self.models
+        _set_pointers(u.q, q_net, True)
+        _set_pointers(u.target_q, target_net, False)
+        u.obs, u.actions = _lib.ptr(obs), _lib.ptr(actions)
+        u.rewards, u.done = _lib.ptr(rewards), _lib.ptr(done)
+        q_values, returns = outputs if outputs is not None else (None, None)
+        u.q_values, u.returns = _lib.ptr(q_values), _lib.ptr(returns)
+        u.sums = _lib.ptr(self.sums)
+        u.workspace = _lib.ptr(self.workspace)
+        assert windows.shape[0] == self.rows
+        if weights is not None:
+            assert weights.shape == (self.rows,) and weights.dtype == torch.float32
+        _lib.check(self.lib.wdb_c51_update_sampled(
+            _lib.stream_ptr(), ctypes.byref(u), self.n_atoms, _lib.ptr(self.support),
+            self.delta_z, ctypes.byref(replay_windows(windows)), _lib.ptr(weights)),
+            "c51_update_sampled")
         return self.sums

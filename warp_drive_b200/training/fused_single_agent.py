@@ -71,8 +71,14 @@ class FusedSingleAgentRollout:
             if not 0 <= len(model.fc) <= 3:
                 return False
             head = int(model.policy_head.out_features if continuous else model.output_dims[0])
+            categorical = getattr(model, "is_categorical_q", False)
+            if categorical:                    # C51: A blocks of N atom logits
+                head = int(model.policy_head.out_features)
             dims = [int(model.flattened_obs_size)] + [int(d) for d in model.fc_dims] + [head]
             arr = (ctypes.c_int * 5)(*(dims + [0] * (5 - len(dims))))
+            if categorical:
+                return bool(_lib.load().wdb_single_agent_rollout_categorical_supported(
+                    len(model.fc), arr, int(model.num_atoms)))
             return bool(_lib.load().wdb_single_agent_rollout_supported(len(model.fc), arr))
         except Exception:  # noqa: BLE001
             return False
@@ -122,10 +128,17 @@ class FusedSingleAgentRollout:
         self.squashed = bool(getattr(_unwrap(model), "is_squashed_gaussian", False))
         # DQN's Q network: epsilon-greedy over the raw head (sampler param `epsilon`)
         self.q_network = bool(getattr(_unwrap(model), "is_q_network", False))
+        # C51's categorical Q network: the kernel reduces each action's atoms to their
+        # expectation, and reads [epsilon, z_0 .. z_{N-1}] from the device (refreshed at every
+        # launch); the categorical head is 4
+        self.categorical = bool(getattr(_unwrap(model), "is_categorical_q", False))
+        if self.categorical:
+            self.A = int(_unwrap(model).output_dims[0])
         if self.q_network:
             # the kernel reads epsilon from the device (the log_std field; the Q head is 3)
-            r.gaussian_head = 3
-            self._epsilon = torch.zeros(1, dtype=torch.float32, device=dm.device)
+            r.gaussian_head = 4 if self.categorical else 3
+            n = 1 + (int(_unwrap(model).num_atoms) if self.categorical else 0)
+            self._epsilon = torch.zeros(n, dtype=torch.float32, device=dm.device)
             r.log_std = _p(self._epsilon)
         if self.squashed:
             actor = _unwrap(model)
@@ -177,7 +190,8 @@ class FusedSingleAgentRollout:
         (use_argmax: scale * tanh(mu) + bias) (`normals` [n_steps, E] replaces the RNG draw,
         `probs_out` [n_steps, E] records the mean, raw mu for the squashed head).  A Q network
         samples epsilon-greedily as CUDASampler.sample_epsilon_greedy with `epsilon` (default 0;
-        use_argmax: 0), one draw per step; `probs_out` [n_steps, E, A] records the Q values."""
+        use_argmax: 0), one draw per step; `probs_out` [n_steps, E, A] records the Q values (a
+        categorical Q network's expectations)."""
         dm, r, p = self.dm, self.r, self.policy
         if self._quantile is not None:
             with torch.no_grad():
@@ -200,7 +214,9 @@ class FusedSingleAgentRollout:
             eps = float(0.0 if epsilon is None else epsilon)
             if not 0.0 <= eps <= 1.0:
                 raise ValueError(f"epsilon must be in [0, 1], got {epsilon}")
-            self._epsilon.fill_(eps)
+            self._epsilon[0] = eps
+            if self.categorical:
+                self._epsilon[1:].copy_(_unwrap(self.model).support)
         if record:
             obs_b = dm.data_on_device_via_torch(f"{_PROCESSED_OBSERVATIONS}_batch_{p}")
             assert t0 + n_steps <= obs_b.shape[0]

@@ -214,6 +214,12 @@ class ModelFactory:
             from warp_drive_b200.training.models.fully_connected_q import FullyConnectedIQN
 
             cls._registry[model_name] = FullyConnectedIQN
+        if model_name == "fully_connected_categorical_q" and model_name not in cls._registry:
+            # C51's categorical Q network, imported on first use
+            from warp_drive_b200.training.models.fully_connected_q import (
+                FullyConnectedCategoricalQ)
+
+            cls._registry[model_name] = FullyConnectedCategoricalQ
         if model_name not in cls._registry and model_name in (
                 "fully_connected_actor", "fully_connected_action_value_critic",
                 "fully_connected_sac_actor"):

@@ -193,3 +193,70 @@ class FullyConnectedIQN(FullyConnectedQ):
         """The mean of Z over the K midpoints, for every action: [..., A]."""
         w, b = self.collapsed_head()
         return func.linear(self.trunk(obs), w, b)
+
+
+class FullyConnectedCategoricalQ(FullyConnectedQ):
+    """The categorical Q network of C51 (algorithms/dqn.py CategoricalDQN; Bellemare, Dabney &
+    Munos 2017): a softmax over N fixed atoms of the return per action.
+
+    FullyConnectedQ's trunk and one raw `policy_head = Linear(H, A * N)`; column a * N + j is the
+    logit of atom j of action a (QR-DQN's layout).  Model keys: `num_atoms` N (51, an integer in
+    [2, 64]) and the required finite `v_min` < `v_max`.  The support z_j = v_min + j dz,
+    dz = (v_max - v_min) / (N - 1), is computed in float64 and rounded once to float32; it is a
+    non-persistent buffer (checkpoints hold the parameters only) and `delta_z` is dz rounded the
+    same way, so the torch path and both native paths read the same values.
+
+    `logits(obs)` [..., A, N] and `probabilities(obs)` (their softmax over the atoms) are what
+    the update uses; `q_values(obs)` = sum_j z_j p_j [..., A] -- and so `forward`, the per-step
+    epsilon-greedy path and the evaluator -- is the expectation.  The expectation is not linear
+    in the head, so there is no collapsed_head()."""
+    name = "torch_fully_connected_categorical_q"
+    is_categorical_q = True
+
+    def __init__(self, env, model_config, policy, policy_tag_to_agent_id_map,
+                 create_separate_placeholders_for_each_policy=False,
+                 obs_dim_corresponding_to_num_agents="first"):
+        n = model_config.get("num_atoms", 51)
+        if isinstance(n, bool) or not isinstance(n, int) or not 2 <= n <= 64:
+            raise ValueError("fully_connected_categorical_q's model.num_atoms is an integer in "
+                             f"[2, 64], got {n!r}")
+        bounds = {}
+        for key in ("v_min", "v_max"):
+            v = model_config.get(key)
+            if isinstance(v, bool) or not isinstance(v, (int, float)) or not math.isfinite(v):
+                raise ValueError(f"fully_connected_categorical_q needs model.{key}, a finite "
+                                 f"number, got {v!r}")
+            bounds[key] = float(v)
+        if not bounds["v_min"] < bounds["v_max"]:
+            raise ValueError("fully_connected_categorical_q needs model.v_min < model.v_max, got "
+                             f"v_min {bounds['v_min']!r} and v_max {bounds['v_max']!r}")
+        super().__init__(env, model_config, policy, policy_tag_to_agent_id_map,
+                         create_separate_placeholders_for_each_policy,
+                         obs_dim_corresponding_to_num_agents)
+        self.num_atoms = n
+        self.v_min, self.v_max = bounds["v_min"], bounds["v_max"]
+        dz = (self.v_max - self.v_min) / (n - 1)
+        support = self.v_min + dz * torch.arange(n, dtype=torch.float64)
+        self.delta_z = float(torch.tensor(dz, dtype=torch.float64).float())
+        self.register_buffer("support", support.float(), persistent=False)
+        self.policy_head = nn.Linear(self.policy_head.in_features, self.output_dims[0] * n)
+
+    def trunk(self, obs):
+        x = obs
+        for i in range(len(self.fc)):
+            x = self.fc[str(i)](x)
+        return x
+
+    def logits(self, obs):
+        """The atom logits of every action: [..., A, N]."""
+        y = self.policy_head(self.trunk(obs))
+        return y.reshape(*y.shape[:-1], self.output_dims[0], self.num_atoms)
+
+    def probabilities(self, obs):
+        """The softmax over the atoms of every action: [..., A, N]."""
+        return torch.softmax(self.logits(obs), dim=-1)
+
+    def q_values(self, obs):
+        """The expectation sum_j z_j p_j of every action: [..., A]."""
+        p = self.probabilities(obs)
+        return (p * self.support.to(p.dtype)).sum(dim=-1)

@@ -38,15 +38,24 @@ on the same windows, targets and schedule.  Each update draws its levels -- N on
 target ones per loss row, uniform on [0, 1) -- into one [B, N + N'] buffer with a CUDA
 generator seeded from the trainer seed (1 launch); the native and the torch path read the same
 buffer.  Metrics and priorities are QR-DQN's.
+
+Categorical DQN (C51): a `fully_connected_categorical_q` model (`num_atoms` N, `v_min`, `v_max`)
+trains with CategoricalDQN's projected cross-entropy (wdb_c51_update_sampled, 2 launches, or
+torch autograd) on the same windows, targets and schedule.  C51 has no Huber loss, so a
+categorical policy config that sets `huber_delta` is refused.  Its `Mean Q value` and `Mean
+return` are the means of Q-bar = sum_i z_i p_i and R-bar = sum_i z_i m_i, and with prioritized
+replay the priorities are (|Q-bar - R-bar| + epsilon)^alpha, as for QR-DQN and IQN (Rainbow
+uses the cross-entropy).
 """
 import os
 
 import torch
 
-from warp_drive_b200.training.algorithms.dqn import DQN, ImplicitQuantileDQN, QuantileDQN
+from warp_drive_b200.training.algorithms.dqn import (
+    DQN, CategoricalDQN, ImplicitQuantileDQN, QuantileDQN)
 from warp_drive_b200.training.algorithms.fused_dqn import (
-    FusedDQNUpdate, FusedIQNUpdate, FusedQRDQNUpdate, fused_dqn_supported, fused_iqn_supported,
-    fused_qr_dqn_supported)
+    FusedC51Update, FusedDQNUpdate, FusedIQNUpdate, FusedQRDQNUpdate, fused_c51_supported,
+    fused_dqn_supported, fused_iqn_supported, fused_qr_dqn_supported)
 from warp_drive_b200.training.trainer_ddpg import (
     RingRolloutEngine, TrainerDDPG, hard_update, soft_update)
 from warp_drive_b200.training.utils.param_scheduler import ParamScheduler
@@ -90,6 +99,15 @@ def dqn_policy_settings(policy_config):
     if int(period) != period or period < 1:
         raise ValueError(f"target_update_period must be an integer >= 1, got {period}")
     return bool(c.get("double_q", True)), float(delta), float(tau), int(period)
+
+
+def categorical_policy_settings(policy_config):
+    """dqn_policy_settings of a policy with a categorical (C51) Q network, which has no Huber
+    loss: a `huber_delta` set in its config is refused rather than ignored."""
+    if "huber_delta" in policy_config:
+        raise ValueError("a fully_connected_categorical_q policy has no Huber loss: remove "
+                         f"huber_delta (got {policy_config['huber_delta']!r})")
+    return dqn_policy_settings(policy_config)
 
 
 class TrainerDQN(TrainerDDPG):
@@ -140,8 +158,9 @@ class TrainerDQN(TrainerDDPG):
         model_cfg = c["model"]
         self.q_models[policy] = self._build_model(policy, model_cfg)
         if not getattr(self.q_models[policy], "is_q_network", False):
-            raise ValueError("DQN's model is a `fully_connected_q`, a `fully_connected_quantile_q` "
-                             f"or a `fully_connected_iqn`, got '{model_cfg.get('type')}'")
+            raise ValueError("DQN's model is a `fully_connected_q`, a `fully_connected_quantile_q`, "
+                             "a `fully_connected_iqn` or a `fully_connected_categorical_q`, got "
+                             f"'{model_cfg.get('type')}'")
         self.target_q_models[policy] = self._build_model(policy, model_cfg)
         hard_update(self.target_q_models[policy], self.q_models[policy])
 
@@ -162,17 +181,20 @@ class TrainerDQN(TrainerDDPG):
 
     def _initialize_policy_algorithm(self, policy):
         c = self._get_config(["policy", policy])
-        double_q, delta, tau, period = dqn_policy_settings(c)
+        q_net = self.q_models[policy]
+        categorical = getattr(q_net, "is_categorical_q", False)
+        double_q, delta, tau, period = (
+            categorical_policy_settings if categorical else dqn_policy_settings)(c)
         self.clip_grad_norm[policy] = c["clip_grad_norm"]
         if c["clip_grad_norm"]:
             self.max_grad_norm[policy] = c["max_grad_norm"]
         self.tau[policy], self.target_update_period[policy] = tau, period
         self.update_count[policy] = 0
-        q_net = self.q_models[policy]
         quantile = getattr(q_net, "is_quantile_q", False)
         implicit = getattr(q_net, "is_implicit_quantile_q", False)
         algo = self.trainers[policy] = (
-            ImplicitQuantileDQN if implicit else QuantileDQN if quantile else DQN)(
+            CategoricalDQN if categorical else ImplicitQuantileDQN if implicit
+            else QuantileDQN if quantile else DQN)(
             discount_factor_gamma=c["gamma"], n_step=self.n_step, double_q=double_q,
             huber_delta=delta)
         n_agents = len(self.policy_tag_to_agent_id_map[policy])
@@ -193,7 +215,8 @@ class TrainerDQN(TrainerDDPG):
             if self._tau_generator is None:
                 self._tau_generator = torch.Generator(device=dev)
                 self._tau_generator.manual_seed(self.seed)
-        supported, fused = ((fused_iqn_supported, FusedIQNUpdate) if implicit
+        supported, fused = ((fused_c51_supported, FusedC51Update) if categorical
+                            else (fused_iqn_supported, FusedIQNUpdate) if implicit
                             else (fused_qr_dqn_supported, FusedQRDQNUpdate) if quantile
                             else (fused_dqn_supported, FusedDQNUpdate))
         if supported(algo, q_net, self.num_envs, n_agents, self.ring_capacity, rows):
@@ -272,8 +295,8 @@ class TrainerDQN(TrainerDDPG):
 
     def _torch_q_gradients(self, policy, logging_flag):
         """The Q gradient by torch autograd on the gathered windows (the loss of
-        wdb_dqn_update_sampled, or of wdb_qr_dqn_update_sampled / wdb_iqn_update_sampled for a
-        quantile network), accumulated into the arena's .grad views."""
+        wdb_dqn_update_sampled, or of wdb_qr_dqn_update_sampled / wdb_iqn_update_sampled /
+        wdb_c51_update_sampled for a distributional network), accumulated into the arena's .grad views."""
         algo = self.trainers[policy]
         store = self.priority_stores.get(policy)
         loss, q, returns = algo.loss(self.q_models[policy], self.target_q_models[policy],
@@ -290,8 +313,8 @@ class TrainerDQN(TrainerDDPG):
         return algo.loss_metrics(loss.item(), q.detach().double().mean(), returns)
 
     def _fused_q_gradients(self, policy, fused, logging_flag):
-        """The same gradient from the native pass (FusedDQNUpdate, FusedQRDQNUpdate or
-        FusedIQNUpdate), written straight into the arena's .grad views; the host waits only on
+        """The same gradient from the native pass (FusedDQNUpdate, FusedQRDQNUpdate,
+        FusedIQNUpdate or FusedC51Update), written straight into the arena's .grad views; the host waits only on
         logging iterations (metrics)."""
         eng = self.engine
         outputs, weights = None, None
