@@ -1127,6 +1127,50 @@ int wdb_c51_update_sampled(void *stream, const wdb_dqn_update_args *update, int 
                            const float *support, float delta_z,
                            const wdb_replay_windows *windows, const float *weights);
 
+/* Dueling head (Wang et al. 2016, the mean combine) of a DQN or C51 network, and its fold into
+ * the plain MLP head the passes above run.  The head reads the trunk output h (width H) through
+ * two streams, each with one hidden Linear(H, S) + ReLU when S > 0 and none when S = 0 (the
+ * output layer then reads h):
+ *   V = value(h) [N],  Adv = advantage(h) [A N],
+ *   out[a N + j] = V_j + Adv[a N + j] - (1/A) sum_c Adv[c N + j]   (N = 1: DQN, N atoms: C51).
+ * The combine is linear in the output layers, so the head is exactly this folded network:
+ *   hidden (S > 0): w = [value_hw; adv_hw] [2S, H], b = [value_hb; adv_hb] [2S],
+ *   output, K = 2S: ow[a N + j] = [value_ow[j] | adv_ow[a N + j] - m_j], m_j = (1/A) sum_c
+ *                   adv_ow[c N + j] ([A N, 2S]),
+ *           K = H (S = 0): ow[a N + j] = value_ow[j] + (adv_ow[a N + j] - m_j) ([A N, H]),
+ *   ob[a N + j] = value_ob[j] + (adv_ob[a N + j] - m'_j), m'_j the same mean of adv_ob.
+ * Means are float32 sums over c = 0 .. A - 1 in order, divided by A, so a fold or an unfold is
+ * bit-reproducible.  Row-major nn.Linear layouts throughout ([out, in] weights). */
+typedef struct wdb_dueling_head {
+  int n_actions, n_atoms, in_dim, stream_dim;   /* A, N, H, S (0: no stream hidden layer) */
+  const float *value_hw, *value_hb;  /* value stream hidden Linear(H, S) (S > 0; else unread) */
+  const float *value_ow, *value_ob;  /* value stream output Linear(S or H, N) */
+  const float *adv_hw, *adv_hb;      /* advantage stream hidden Linear(H, S) (S > 0) */
+  const float *adv_ow, *adv_ob;      /* advantage stream output Linear(S or H, A N) */
+  float *value_ghw, *value_ghb, *value_gow, *value_gob;   /* stream gradients, the shapes above */
+  float *adv_ghw, *adv_ghb, *adv_gow, *adv_gob;           /* (written by the unfold) */
+  float *hw, *hb, *ow, *ob;          /* folded layers (written by the fold; hw, hb when S > 0) */
+  const float *ghw, *ghb, *gow, *gob;  /* their gradients (read by the unfold; ghw, ghb: S > 0) */
+} wdb_dueling_head;
+/* 1 if the fold / unfold take the shape: A, N, H >= 1, S >= 0, and every folded layer below
+ * 2^31 elements.  No CUDA call. */
+int wdb_dueling_fold_supported(const wdb_dueling_head *head);
+int wdb_dueling_unfold_grads_supported(const wdb_dueling_head *head);
+/* Writes head's folded layers from its stream parameters and, when target is not NULL, the
+ * target's from its own (same shape; its gradient pointers are not read).  One launch.
+ * cudaErrorInvalidValue without launching if unsupported, the shapes differ or a required
+ * pointer is NULL. */
+int wdb_dueling_fold(void *stream, const wdb_dueling_head *head, const wdb_dueling_head *target);
+/* Writes the stream parameters' gradients from the folded layers' gradients, through the
+ * transpose of the fold:
+ *   hidden: value_ghw / ghb = rows 0 .. S - 1 of ghw / ghb, adv_ghw / ghb = rows S .. 2S - 1,
+ *   value_gow[j][k] = sum_a gow[a N + j][k]   (k < S; all of row k when S = 0), value_gob alike,
+ *   adv_gow[a N + j][k] = g[a N + j][k] - (1/A) sum_c g[c N + j][k], g = gow's columns S .. 2S-1
+ *                         (S > 0) or all of gow (S = 0), adv_gob alike from gob.
+ * Sums over a and c in order.  One launch.  cudaErrorInvalidValue without launching if
+ * unsupported or a required pointer is NULL. */
+int wdb_dueling_unfold_grads(void *stream, const wdb_dueling_head *head);
+
 /* Prioritized replay (Schaul et al. 2016, proportional) over the replay ring's n-step windows.
  * One float32 leaf per (physical slot s, agent row n), leaf s * n_rows + n: p^alpha of the
  * window that starts at slot s for agent row n (windows[g] = {s, n} as above), and 0 exactly

@@ -316,6 +316,20 @@ class IqnArgs(ctypes.Structure):
     ]
 
 
+class DuelingHead(ctypes.Structure):
+    """struct wdb_dueling_head (include/wdb200.h)."""
+
+    _fields_ = [
+        ("n_actions", _i), ("n_atoms", _i), ("in_dim", _i), ("stream_dim", _i),
+        ("value_hw", _fp), ("value_hb", _fp), ("value_ow", _fp), ("value_ob", _fp),
+        ("adv_hw", _fp), ("adv_hb", _fp), ("adv_ow", _fp), ("adv_ob", _fp),
+        ("value_ghw", _fp), ("value_ghb", _fp), ("value_gow", _fp), ("value_gob", _fp),
+        ("adv_ghw", _fp), ("adv_ghb", _fp), ("adv_gow", _fp), ("adv_gob", _fp),
+        ("hw", _fp), ("hb", _fp), ("ow", _fp), ("ob", _fp),
+        ("ghw", _fp), ("ghb", _fp), ("gow", _fp), ("gob", _fp),
+    ]
+
+
 class PerStore(ctypes.Structure):
     """struct wdb_per_store (include/wdb200.h)."""
 
@@ -452,6 +466,11 @@ _SIGNATURES = {
     "wdb_c51_update_sampled_workspace_bytes": (_ll, [ctypes.POINTER(DqnUpdate), _i, _i]),
     "wdb_c51_update_sampled": (
         _i, [_vp, ctypes.POINTER(DqnUpdate), _i, _vp, _f, ctypes.POINTER(ReplayWindows), _vp]),
+    "wdb_dueling_fold_supported": (_i, [ctypes.POINTER(DuelingHead)]),
+    "wdb_dueling_unfold_grads_supported": (_i, [ctypes.POINTER(DuelingHead)]),
+    "wdb_dueling_fold": (
+        _i, [_vp, ctypes.POINTER(DuelingHead), ctypes.POINTER(DuelingHead)]),
+    "wdb_dueling_unfold_grads": (_i, [_vp, ctypes.POINTER(DuelingHead)]),
     "wdb_replay_sample_windows": (_i, [_vp, _vp, _i, _ull, _ull, _i, _i, _i, _i, _i]),
     "wdb_per_nodes": (_ll, [_ll]),
     "wdb_per_levels": (_i, [_ll]),

@@ -15,6 +15,9 @@ def _layers(model):
     """[(weight, bias)] of the hidden Linear layers, then the head (actor: policy_head,
     critic: vf_head)."""
     head = model.policy_head if hasattr(model, "policy_head") else model.vf_head
+    if getattr(head, "is_dueling", False):
+        raise TypeError("a dueling head has no one output layer: the native passes run its "
+                        "folded layers (fused_dqn.FusedDuelingUpdate)")
     return [(model.fc[str(i)][0].weight, model.fc[str(i)][0].bias)
             for i in range(len(model.fc))] + [(head.weight, head.bias)]
 

@@ -5,8 +5,10 @@ loss and the backward pass -- and writes it straight into the `.grad` views of t
 arena.  `wdb_qr_dqn_update_sampled` does the same for quantile-regression DQN
 (FusedQRDQNUpdate) and `wdb_iqn_update_sampled` (csrc/wdb_iqn_update.cu) for implicit quantile
 networks (FusedIQNUpdate), and `wdb_c51_update_sampled` (csrc/wdb_c51_update.cu) for categorical
-DQN (FusedC51Update).  The torch autograd updates (algorithms/dqn.py) stay for the shapes
-these do not take."""
+DQN (FusedC51Update).  A dueling DQN or C51 network runs the same passes on its folded network
+(FusedDuelingUpdate; csrc/wdb_dueling.cu folds the head before the pass and unfolds its gradients
+after it).  The torch autograd updates (algorithms/dqn.py) stay for the shapes these do not
+take."""
 import ctypes
 
 import torch
@@ -37,7 +39,7 @@ def fused_dqn_supported(algo, q_net, n_envs, n_agents, capacity, replay_rows):
 
     if type(q_net) is not FullyConnectedQ or not isinstance(q_net.observation_space, Box):
         return False
-    if len(q_net.fc_dims) > 3:
+    if q_net.dueling or len(q_net.fc_dims) > 3:      # dueling: fused_dueling_supported
         return False
     u = _shape_struct(algo, q_net, n_envs, n_agents, capacity)
     return bool(_lib.load().wdb_dqn_update_sampled_supported(ctypes.byref(u), int(replay_rows)))
@@ -231,7 +233,7 @@ def fused_c51_supported(algo, q_net, n_envs, n_agents, capacity, replay_rows):
     if type(q_net) is not FullyConnectedCategoricalQ or not isinstance(q_net.observation_space,
                                                                        Box):
         return False
-    if len(q_net.fc_dims) > 3:
+    if q_net.dueling or len(q_net.fc_dims) > 3:      # dueling: fused_dueling_supported
         return False
     u = _shape_struct(algo, q_net, n_envs, n_agents, capacity)
     return bool(_lib.load().wdb_c51_update_sampled_supported(
@@ -278,4 +280,174 @@ class FusedC51Update:
             _lib.stream_ptr(), ctypes.byref(u), self.n_atoms, _lib.ptr(self.support),
             self.delta_z, ctypes.byref(replay_windows(windows)), _lib.ptr(weights)),
             "c51_update_sampled")
+        return self.sums
+
+
+def folded_widths(q_net):
+    """The hidden widths of a dueling network's folded form: the trunk's, then the stacked
+    stream hidden layer 2S when S > 0 (DuelingHead.folded)."""
+    s = q_net.policy_head.stream_dim
+    return [int(w) for w in q_net.fc_dims] + ([2 * s] if s else [])
+
+
+def dueling_shape(head):
+    """struct wdb_dueling_head of a DuelingHead with its shape only (no pointers)."""
+    d = _lib.DuelingHead()
+    d.n_actions, d.n_atoms = int(head.n_actions), int(head.n_outputs)
+    d.in_dim, d.stream_dim = int(head.in_features), int(head.stream_dim)
+    return d
+
+
+class DuelingFold:
+    """A DuelingHead's folded layers in buffers of their own (and, with grads, buffers for their
+    gradients), and the struct wdb_dueling_head that ties them to the live stream parameters."""
+
+    def __init__(self, model, grads=False):
+        self.model = model
+        head = model.policy_head
+        s, h, out = head.stream_dim, head.in_features, head.out_features
+        shapes = ([(2 * s, h), (2 * s,)] if s else []) + [(out, 2 * s if s else h), (out,)]
+        dev = next(model.parameters()).device
+
+        def buffers():
+            t = [torch.zeros(shape, dtype=torch.float32, device=dev) for shape in shapes]
+            return list(zip(t[0::2], t[1::2]))
+        self.layers = buffers()                  # [(weight, bias)]: [hidden,] output
+        self.grads = buffers() if grads else None
+
+    def struct(self):
+        head = self.model.policy_head
+        d = dueling_shape(head)
+        (vh, vo), (ah, ao) = head.streams()
+        for prefix, hidden, out in (("value_", vh, vo), ("adv_", ah, ao)):
+            for name, layer in (("h", hidden), ("o", out)):
+                if layer is None:
+                    continue
+                setattr(d, prefix + name + "w", _lib.ptr(layer.weight.data))
+                setattr(d, prefix + name + "b", _lib.ptr(layer.bias.data))
+                if self.grads is not None:
+                    setattr(d, prefix + "g" + name + "w", _lib.ptr(layer.weight.grad))
+                    setattr(d, prefix + "g" + name + "b", _lib.ptr(layer.bias.grad))
+        names = (["h"] if head.stream_dim else []) + ["o"]
+        for name, (w, b) in zip(names, self.layers):
+            setattr(d, name + "w", _lib.ptr(w))
+            setattr(d, name + "b", _lib.ptr(b))
+        for name, (w, b) in zip(names, self.grads or []):
+            setattr(d, "g" + name + "w", _lib.ptr(w))
+            setattr(d, "g" + name + "b", _lib.ptr(b))
+        return d
+
+
+def fold(online, target=None):
+    """wdb_dueling_fold of one or two DuelingFolds: one launch."""
+    t = None if target is None else ctypes.byref(target.struct())
+    _lib.check(_lib.load().wdb_dueling_fold(_lib.stream_ptr(), ctypes.byref(online.struct()), t),
+               "dueling_fold")
+
+
+def _dueling_shape_struct(algo, q_net, n_envs, n_agents, capacity):
+    """_shape_struct with the folded network's hidden widths."""
+    u = _shape_struct(algo, q_net, n_envs, n_agents, capacity)
+    widths = folded_widths(q_net)
+    for net in (u.q, u.target_q):
+        net.n_hidden = len(widths)
+        for i, w in enumerate(widths):
+            net.widths[i] = w
+    return u
+
+
+def fused_dueling_supported(algo, q_net, n_envs, n_agents, capacity, replay_rows):
+    """True if the folded network of a dueling FullyConnectedQ (wdb_dqn_update_sampled) or
+    FullyConnectedCategoricalQ (wdb_c51_update_sampled) is in that pass's envelope: at most 3
+    hidden layers in all (a one-layer stream allows a trunk of at most 2), each, 2S included,
+    of width <= 64, F <= 63, and C51's shared-memory cap."""
+    from warp_drive_b200.training.models.fully_connected_q import (
+        FullyConnectedCategoricalQ, FullyConnectedQ)
+
+    if type(q_net) not in (FullyConnectedQ, FullyConnectedCategoricalQ) or not q_net.dueling:
+        return False
+    if not isinstance(q_net.observation_space, Box) or len(folded_widths(q_net)) > 3:
+        return False
+    L = _lib.load()
+    if not L.wdb_dueling_fold_supported(ctypes.byref(dueling_shape(q_net.policy_head))):
+        return False
+    u = _dueling_shape_struct(algo, q_net, n_envs, n_agents, capacity)
+    if getattr(q_net, "is_categorical_q", False):
+        return bool(L.wdb_c51_update_sampled_supported(
+            ctypes.byref(u), int(q_net.num_atoms), int(replay_rows)))
+    return bool(L.wdb_dqn_update_sampled_supported(ctypes.byref(u), int(replay_rows)))
+
+
+class FusedDuelingUpdate:
+    """One update of a dueling DQN or C51 policy: wdb_dueling_fold of the online and the target
+    head (1 launch), the plain pass -- wdb_dqn_update_sampled / _prioritized, or
+    wdb_c51_update_sampled -- on networks made of the live trunk layers and the folded layers (2
+    launches), then wdb_dueling_unfold_grads (1 launch).  The pass writes the trunk's gradients
+    straight into the arena's `.grad` views and the folded layers' into scratch, which the
+    unfold maps onto the stream parameters' `.grad` views.  Sums and outputs are the plain
+    pass's."""
+
+    def __init__(self, algo, q_net, target_net, n_envs, n_agents, capacity, replay_rows):
+        self.models = (q_net, target_net)
+        self.categorical = bool(getattr(q_net, "is_categorical_q", False))
+        self.u = _dueling_shape_struct(algo, q_net, n_envs, n_agents, capacity)
+        self.lib = _lib.load()
+        self.rows = int(replay_rows)
+        if self.categorical:
+            self.n_atoms = int(q_net.num_atoms)
+            nbytes = self.lib.wdb_c51_update_sampled_workspace_bytes(
+                ctypes.byref(self.u), self.n_atoms, self.rows)
+        else:
+            nbytes = self.lib.wdb_dqn_update_sampled_workspace_bytes(ctypes.byref(self.u),
+                                                                     self.rows)
+        assert nbytes > 0, "folded shapes not supported by the pass"
+        dev = next(q_net.parameters()).device
+        self.workspace = torch.empty(int(nbytes), dtype=torch.uint8, device=dev)
+        self.sums = torch.zeros(2, dtype=torch.float64, device=dev)
+        if self.categorical:
+            self.support = q_net.support.to(device=dev, dtype=torch.float32).contiguous()
+            self.delta_z = float(q_net.delta_z)
+        self.online, self.target = DuelingFold(q_net, grads=True), DuelingFold(target_net)
+
+    @staticmethod
+    def _point(net, model, folded, grads):
+        trunk = [(model.fc[str(i)][0].weight, model.fc[str(i)][0].bias)
+                 for i in range(len(model.fc))]
+        for i, (w, b) in enumerate(trunk + folded.layers):
+            net.w[i], net.b[i] = _lib.ptr(w.data), _lib.ptr(b.data)
+        if grads:
+            for i, (w, b) in enumerate([(w.grad, b.grad) for w, b in trunk] + folded.grads):
+                net.gw[i], net.gb[i] = _lib.ptr(w), _lib.ptr(b)
+
+    def launch(self, obs, actions, rewards, done, windows, outputs=None, weights=None):
+        """The network's gradient (trunk and both streams) into its `.grad`; the arguments of
+        FusedDQNUpdate.launch."""
+        u = self.u
+        q_net, target_net = self.models
+        fold(self.online, self.target)
+        self._point(u.q, q_net, self.online, True)
+        self._point(u.target_q, target_net, self.target, False)
+        u.obs, u.actions = _lib.ptr(obs), _lib.ptr(actions)
+        u.rewards, u.done = _lib.ptr(rewards), _lib.ptr(done)
+        q_values, returns = outputs if outputs is not None else (None, None)
+        u.q_values, u.returns = _lib.ptr(q_values), _lib.ptr(returns)
+        u.sums = _lib.ptr(self.sums)
+        u.workspace = _lib.ptr(self.workspace)
+        assert windows.shape[0] == self.rows
+        if weights is not None:
+            assert weights.shape == (self.rows,) and weights.dtype == torch.float32
+        win = ctypes.byref(replay_windows(windows))
+        if self.categorical:
+            _lib.check(self.lib.wdb_c51_update_sampled(
+                _lib.stream_ptr(), ctypes.byref(u), self.n_atoms, _lib.ptr(self.support),
+                self.delta_z, win, _lib.ptr(weights)), "c51_update_sampled")
+        elif weights is None:
+            _lib.check(self.lib.wdb_dqn_update_sampled(_lib.stream_ptr(), ctypes.byref(u), win),
+                       "dqn_update_sampled")
+        else:
+            _lib.check(self.lib.wdb_dqn_update_prioritized(
+                _lib.stream_ptr(), ctypes.byref(u), win, _lib.ptr(weights)),
+                "dqn_update_prioritized")
+        _lib.check(self.lib.wdb_dueling_unfold_grads(
+            _lib.stream_ptr(), ctypes.byref(self.online.struct())), "dueling_unfold_grads")
         return self.sums

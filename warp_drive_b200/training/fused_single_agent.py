@@ -37,9 +37,12 @@ def _unwrap(model):
 
 
 def _layers(model):
-    """[(weight, bias)] of the hidden layers followed by the (single) action head."""
+    """[(weight, bias)] of the hidden layers followed by the (single) action head.  A dueling head
+    has no one output layer: its rollout runs the folded layers of a DuelingFold instead."""
     model = _unwrap(model)
     out = [(model.fc[str(i)][0].weight, model.fc[str(i)][0].bias) for i in range(len(model.fc))]
+    if getattr(model, "dueling", False):
+        raise TypeError("a dueling head runs as its folded layers (DuelingFold)")
     # the discrete heads are an nn.ModuleList, the deterministic (tanh) head and a Q network's
     # head one nn.Linear
     single = model.is_deterministic or getattr(model, "is_q_network", False)
@@ -68,18 +71,24 @@ class FusedSingleAgentRollout:
                 return False
             if getattr(model, "action_mask", None) is not None:
                 return False
-            if not 0 <= len(model.fc) <= 3:
+            # a dueling head runs as its folded layers: the stacked 2S stream layer, if any,
+            # then the A * N outputs
+            widths = [int(d) for d in model.fc_dims]
+            if getattr(model, "dueling", False):
+                from warp_drive_b200.training.algorithms.fused_dqn import folded_widths
+                widths = folded_widths(model)
+            if not 0 <= len(widths) <= 3:
                 return False
             head = int(model.policy_head.out_features if continuous else model.output_dims[0])
             categorical = getattr(model, "is_categorical_q", False)
             if categorical:                    # C51: A blocks of N atom logits
                 head = int(model.policy_head.out_features)
-            dims = [int(model.flattened_obs_size)] + [int(d) for d in model.fc_dims] + [head]
+            dims = [int(model.flattened_obs_size)] + widths + [head]
             arr = (ctypes.c_int * 5)(*(dims + [0] * (5 - len(dims))))
             if categorical:
                 return bool(_lib.load().wdb_single_agent_rollout_categorical_supported(
-                    len(model.fc), arr, int(model.num_atoms)))
-            return bool(_lib.load().wdb_single_agent_rollout_supported(len(model.fc), arr))
+                    len(widths), arr, int(model.num_atoms)))
+            return bool(_lib.load().wdb_single_agent_rollout_supported(len(widths), arr))
         except Exception:  # noqa: BLE001
             return False
 
@@ -103,7 +112,17 @@ class FusedSingleAgentRollout:
         r.env_timestep = _p(dm.device_data("_timestep_"))
         r.rewards = _p(dm.device_data(_REWARDS))
         r.sampled_actions = _p(dm.device_data(_ACTIONS))
-        layers = _layers(model)
+        # a dueling Q network: the kernel runs its folded layers, kept in buffers of their own
+        # and refreshed from the live parameters by one wdb_dueling_fold launch per rollout
+        self._dueling = None
+        if getattr(_unwrap(model), "dueling", False):
+            from warp_drive_b200.training.algorithms.fused_dqn import DuelingFold
+            m = _unwrap(model)
+            self._dueling = DuelingFold(m)
+            layers = [(m.fc[str(i)][0].weight, m.fc[str(i)][0].bias)
+                      for i in range(len(m.fc))] + self._dueling.layers
+        else:
+            layers = _layers(model)
         # a distributional Q network (QR-DQN's, IQN's): the kernel runs epsilon-greedy over its
         # mean, the head collapsed to one Linear(H, A) (collapsed_head), kept in buffers of its
         # own and recomputed from the live parameters at every launch
@@ -193,6 +212,9 @@ class FusedSingleAgentRollout:
         use_argmax: 0), one draw per step; `probs_out` [n_steps, E, A] records the Q values (a
         categorical Q network's expectations)."""
         dm, r, p = self.dm, self.r, self.policy
+        if self._dueling is not None:
+            from warp_drive_b200.training.algorithms.fused_dqn import fold
+            fold(self._dueling)
         if self._quantile is not None:
             with torch.no_grad():
                 for buf, v in zip(self._collapsed, _unwrap(self._quantile).collapsed_head()):

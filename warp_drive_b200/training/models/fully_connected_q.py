@@ -5,6 +5,11 @@ raw `policy_head = Linear(fc_dims[-1], A)`: Q(obs, .) for every action, no softm
 head.  `q_values(obs)` is what the update uses; `forward(obs)` keeps the rollout engine's
 `(outputs per head, values)` contract as `([Q], None)`, and the engine recognises the network
 by `is_q_network` and samples its actions epsilon-greedily (CUDASampler.sample_epsilon_greedy).
+
+Dueling (Wang et al. 2016): with the model key `dueling: true` the head is a DuelingHead (value
+and advantage streams combined by the mean rule) with `stream_fc_dims` ([] or [S]) hidden
+layers per stream, for fully_connected_q and fully_connected_categorical_q.  Its forward has the
+plain head's column layout, so everything that reads the head's outputs works unchanged.
 """
 import math
 
@@ -15,6 +20,84 @@ from torch.nn import functional as func
 from warp_drive_b200.training.utils.data_loader import (
     action_head_sizes, dict_observation_keys, get_flattened_obs_size)
 from warp_drive_b200.utils.spaces import Discrete
+
+
+def dueling_settings(model_config, model_type):
+    """(dueling, stream_fc_dims) of a Q model config, validated; `model_type` names the model in
+    the messages."""
+    dueling = model_config.get("dueling", False)
+    if not isinstance(dueling, bool):
+        raise ValueError(f"{model_type}'s model.dueling is true or false, got {dueling!r}")
+    if "stream_fc_dims" not in model_config:
+        return dueling, []
+    dims = model_config["stream_fc_dims"]
+    if not dueling:
+        raise ValueError(f"{model_type}'s model.stream_fc_dims needs model.dueling: true, got "
+                         f"stream_fc_dims {dims!r} without it")
+    if not isinstance(dims, list) or len(dims) > 1 or not all(
+            isinstance(d, int) and not isinstance(d, bool) and d > 0 for d in dims):
+        raise ValueError(f"{model_type}'s model.stream_fc_dims is a list of at most one positive "
+                         f"integer, got {dims!r}")
+    return dueling, list(dims)
+
+
+class DuelingHead(nn.Module):
+    """The dueling head (Wang et al. 2016) over a trunk output h of width H, for A actions of N
+    outputs each (N = 1: Q values; N atoms: C51's logits).  Each stream has one hidden Linear(H,
+    S) + ReLU when `stream_dim` S > 0, and reads h directly when S = 0:
+        V = value(h) [..., N],  Adv = advantage(h) [..., A * N],
+        out[a * N + j] = V_j + Adv[a * N + j] - (1/A) sum_c Adv[c * N + j]
+    (the mean form of the paper's eq. 9), in the plain head's column layout [..., A * N].
+    Parameters: `value.*` and `advantage.*` (Sequential(Linear, ReLU, Linear) or one Linear)."""
+    is_dueling = True
+
+    def __init__(self, in_features, n_actions, n_outputs, stream_dim):
+        super().__init__()
+        self.in_features, self.n_actions, self.n_outputs = in_features, n_actions, n_outputs
+        self.stream_dim = stream_dim
+        self.out_features = n_actions * n_outputs
+
+        def stream(width):
+            if stream_dim == 0:
+                return nn.Linear(in_features, width)
+            return nn.Sequential(nn.Linear(in_features, stream_dim), nn.ReLU(),
+                                 nn.Linear(stream_dim, width))
+        self.value = stream(n_outputs)
+        self.advantage = stream(n_actions * n_outputs)
+
+    def streams(self):
+        """[(hidden, output)] Linear layers of the value and the advantage stream (hidden: None
+        when S = 0)."""
+        if self.stream_dim == 0:
+            return [(None, self.value), (None, self.advantage)]
+        return [(self.value[0], self.value[2]), (self.advantage[0], self.advantage[2])]
+
+    def forward(self, h):
+        A, N = self.n_actions, self.n_outputs
+        v = self.value(h)
+        adv = self.advantage(h)
+        adv = adv.reshape(*adv.shape[:-1], A, N)
+        out = v[..., None, :] + (adv - adv.mean(dim=-2, keepdim=True))
+        return out.reshape(*out.shape[:-2], A * N)
+
+    def folded(self):
+        """[(weight, bias)] of the plain layers this head equals: the stacked stream hidden
+        layer ([2S, H], S > 0) and the output layer [A * N, 2S or H] -- the reference statement of
+        the fold (wdb_dueling_fold).  Differentiable in the stream parameters."""
+        A, N = self.n_actions, self.n_outputs
+        (vh, vo), (ah, ao) = self.streams()
+
+        def centred(x):                    # rows a * N + j minus the mean over a
+            y = x.reshape(A, N, *x.shape[1:])
+            return (y - y.mean(dim=0, keepdim=True)).reshape(x.shape)
+        if self.stream_dim == 0:
+            w = vo.weight.repeat(A, 1) + centred(ao.weight)
+            b = vo.bias.repeat(A) + centred(ao.bias)
+            return [(w, b)]
+        hidden = (torch.cat([vh.weight, ah.weight]), torch.cat([vh.bias, ah.bias]))
+        w = torch.cat([vo.weight.repeat(A, 1), centred(ao.weight)], dim=1)
+        b = vo.bias.repeat(A) + centred(ao.bias)
+        return [hidden, (w, b)]
 
 
 class FullyConnectedQ(nn.Module):
@@ -42,10 +125,19 @@ class FullyConnectedQ(nn.Module):
         self.flattened_obs_size = get_flattened_obs_size(self.observation_space)
         self.output_dims = [int(heads[0])]
         dims = [self.flattened_obs_size] + self.fc_dims
+        self.dueling, self.stream_fc_dims = dueling_settings(
+            model_config, model_config.get("type", "fully_connected_q"))
         self.fc = nn.ModuleDict({
             str(i): nn.Sequential(nn.Linear(dims[i], dims[i + 1]), nn.ReLU())
             for i in range(len(self.fc_dims))})
-        self.policy_head = nn.Linear(dims[-1], self.output_dims[0])
+        self.policy_head = self._head(dims[-1], 1)
+
+    def _head(self, in_features, n_outputs):
+        """The head of A * n_outputs raw outputs: one Linear, or a DuelingHead."""
+        A = self.output_dims[0]
+        if self.dueling:
+            return DuelingHead(in_features, A, n_outputs, sum(self.stream_fc_dims))
+        return nn.Linear(in_features, A * n_outputs)
 
     def q_values(self, obs):
         """Q(obs, a) for every action: [..., A]."""
@@ -56,6 +148,15 @@ class FullyConnectedQ(nn.Module):
 
     def forward(self, obs=None, action=None, action_mask=None):
         return [self.q_values(obs)], None
+
+
+def _refuse_dueling(model_config, model_type):
+    """QR-DQN's collapsed head and IQN's post-merge head would each need a fold of their own."""
+    for key in ("dueling", "stream_fc_dims"):
+        if key in model_config and model_config[key] not in (False, None):
+            raise ValueError(f"{model_type} does not take model.{key} (dueling heads are "
+                             f"fully_connected_q's and fully_connected_categorical_q's), got "
+                             f"{model_config[key]!r}")
 
 
 class FullyConnectedQuantileQ(FullyConnectedQ):
@@ -71,6 +172,7 @@ class FullyConnectedQuantileQ(FullyConnectedQ):
     def __init__(self, env, model_config, policy, policy_tag_to_agent_id_map,
                  create_separate_placeholders_for_each_policy=False,
                  obs_dim_corresponding_to_num_agents="first"):
+        _refuse_dueling(model_config, "fully_connected_quantile_q")
         n = model_config.get("num_quantiles")
         if isinstance(n, bool) or not isinstance(n, int) or not 2 <= n <= 256:
             raise ValueError("fully_connected_quantile_q needs model.num_quantiles, an integer in "
@@ -137,6 +239,7 @@ class FullyConnectedIQN(FullyConnectedQ):
     def __init__(self, env, model_config, policy, policy_tag_to_agent_id_map,
                  create_separate_placeholders_for_each_policy=False,
                  obs_dim_corresponding_to_num_agents="first"):
+        _refuse_dueling(model_config, "fully_connected_iqn")
         dims = model_config.get("fc_dims")
         if not dims:
             raise ValueError("fully_connected_iqn needs model.fc_dims with at least one hidden "
@@ -239,7 +342,7 @@ class FullyConnectedCategoricalQ(FullyConnectedQ):
         support = self.v_min + dz * torch.arange(n, dtype=torch.float64)
         self.delta_z = float(torch.tensor(dz, dtype=torch.float64).float())
         self.register_buffer("support", support.float(), persistent=False)
-        self.policy_head = nn.Linear(self.policy_head.in_features, self.output_dims[0] * n)
+        self.policy_head = self._head(self.policy_head.in_features, n)
 
     def trunk(self, obs):
         x = obs

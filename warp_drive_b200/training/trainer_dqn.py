@@ -46,6 +46,13 @@ categorical policy config that sets `huber_delta` is refused.  Its `Mean Q value
 return` are the means of Q-bar = sum_i z_i p_i and R-bar = sum_i z_i m_i, and with prioritized
 replay the priorities are (|Q-bar - R-bar| + epsilon)^alpha, as for QR-DQN and IQN (Rainbow
 uses the cross-entropy).
+
+Dueling: a `fully_connected_q` or `fully_connected_categorical_q` model with `dueling: true`
+(and `stream_fc_dims` [] or [S]) trains with the same losses, windows, targets and schedule.
+Per update the native path folds the online and target heads (wdb_dueling_fold, 1 launch), runs
+the plain pass on the folded network (2 launches) and unfolds its head gradients onto the two
+streams (wdb_dueling_unfold_grads, 1 launch); shapes outside the pass's envelope train through
+torch autograd on the DuelingHead.
 """
 import os
 
@@ -54,8 +61,9 @@ import torch
 from warp_drive_b200.training.algorithms.dqn import (
     DQN, CategoricalDQN, ImplicitQuantileDQN, QuantileDQN)
 from warp_drive_b200.training.algorithms.fused_dqn import (
-    FusedC51Update, FusedDQNUpdate, FusedIQNUpdate, FusedQRDQNUpdate, fused_c51_supported,
-    fused_dqn_supported, fused_iqn_supported, fused_qr_dqn_supported)
+    FusedC51Update, FusedDQNUpdate, FusedDuelingUpdate, FusedIQNUpdate, FusedQRDQNUpdate,
+    fused_c51_supported, fused_dqn_supported, fused_dueling_supported, fused_iqn_supported,
+    fused_qr_dqn_supported)
 from warp_drive_b200.training.trainer_ddpg import (
     RingRolloutEngine, TrainerDDPG, hard_update, soft_update)
 from warp_drive_b200.training.utils.param_scheduler import ParamScheduler
@@ -215,7 +223,8 @@ class TrainerDQN(TrainerDDPG):
             if self._tau_generator is None:
                 self._tau_generator = torch.Generator(device=dev)
                 self._tau_generator.manual_seed(self.seed)
-        supported, fused = ((fused_c51_supported, FusedC51Update) if categorical
+        supported, fused = ((fused_dueling_supported, FusedDuelingUpdate) if q_net.dueling
+                            else (fused_c51_supported, FusedC51Update) if categorical
                             else (fused_iqn_supported, FusedIQNUpdate) if implicit
                             else (fused_qr_dqn_supported, FusedQRDQNUpdate) if quantile
                             else (fused_dqn_supported, FusedDQNUpdate))
@@ -314,7 +323,7 @@ class TrainerDQN(TrainerDDPG):
 
     def _fused_q_gradients(self, policy, fused, logging_flag):
         """The same gradient from the native pass (FusedDQNUpdate, FusedQRDQNUpdate,
-        FusedIQNUpdate or FusedC51Update), written straight into the arena's .grad views; the host waits only on
+        FusedIQNUpdate, FusedC51Update or FusedDuelingUpdate), written straight into the arena's .grad views; the host waits only on
         logging iterations (metrics)."""
         eng = self.engine
         outputs, weights = None, None
