@@ -411,34 +411,10 @@ bool c51_plan(const wdb_dqn_update_args *u, int N, const wdb_replay_windows *w, 
 int c51_update_sampled(void *stream, const wdb_dqn_update_args *u, int N, const float *support,
                        float dz, const wdb_replay_windows *w, const float *weights) {
   Plan P;
-  if (!c51_plan(u, N, w, &P) || !w->windows || !support || !(dz > 0.0f))
-    return (int)cudaErrorInvalidValue;
-  if (!net_ok(u->q, P.L[0], true) || !net_ok(u->target_q, P.L[0], false))
-    return (int)cudaErrorInvalidValue;
-  if (!u->obs || !u->actions || !u->rewards || !u->done || !u->workspace)
-    return (int)cudaErrorInvalidValue;
-  Reduce R = {};
-  R.g_total = P.gfloats[0];
-  int widest = 1;
-  add_segments(&R, P, 0, 0, u->q, &widest);
+  if (!c51_plan(u, N, w, &P) || !support || !(dz > 0.0f)) return (int)cudaErrorInvalidValue;
   static size_t configured[2] = {0, 0};
-  const size_t smem = (size_t)P.smem_floats * sizeof(float);
-  const void *kernel = weights ? (const void *)c51_prioritized_kernel : (const void *)c51_kernel;
-  int rc = allow_smem(kernel, smem, &configured[weights ? 1 : 0]);
-  if (rc != cudaSuccess) return rc;
-  double *psums = static_cast<double *>(u->workspace);
-  float *partials = reinterpret_cast<float *>(psums + 2 * P.grid);
-  const int2 *windows = reinterpret_cast<const int2 *>(w->windows);
-  if (weights)
-    c51_prioritized_kernel<<<P.grid, kThreads, smem, as_stream(stream)>>>(
-        *u, P, N, support, dz, partials, psums, windows, weights);
-  else
-    c51_kernel<<<P.grid, kThreads, smem, as_stream(stream)>>>(*u, P, N, support, dz, partials,
-                                                              psums, windows);
-  rc = finish_launch();
-  if (rc != cudaSuccess) return rc;
-  R.grid = P.grid;
-  return launch_reduce(stream, R, widest, partials, psums, u->sums);
+  return launch_q_pass(stream, u, P, w, weights, configured, nullptr, c51_kernel,
+                       c51_prioritized_kernel, *u, P, N, support, dz);
 }
 
 }  // namespace

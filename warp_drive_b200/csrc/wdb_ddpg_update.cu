@@ -1389,57 +1389,11 @@ int sac_actor_update(void *stream, const wdb_sac_update_args *u, const wdb_repla
                      u->sums ? u->sums + 2 : nullptr);
 }
 
-// DQN's plan: the online and target Q networks in the actor-shaped slot (input F, head = A).
-// plan_layout also lays out a critic-shaped slot, which DQN does not use: it is given an action
-// width of 1, so its input F + 1 only asks F <= 63 of the Q network (F + A is no limit).  The
-// kernel holds both networks, their gradient block and 8 + (hidden layers) row tiles.
-bool dqn_plan(const wdb_dqn_update_args *u, const wdb_replay_windows *w, Plan *p) {
-  if (!u || !w || !(u->huber_delta > 0.0f)) return false;
-  const wdb_ddpg_net *qs[2] = {&u->q, &u->target_q};
-  const wdb_ddpg_net *const *nets[2] = {qs, qs};
-  const int count[2] = {2, 2};
-  if (u->n_actions < 1 || !plan_layout(u->n_envs, u->n_agents, u->obs_dim, 1, u->n_actions,
-                                       u->capacity, 0, u->n_step, w, nets, count, p))
-    return false;
-  return plan_smem(p, 8 + (p->L[0] - 1), 2ll * p->wfloats[0], p->gfloats[0]);
-}
-
-long long dqn_workspace_bytes(const Plan &P) { return 16ll * P.grid + 4ll * P.grid * P.gfloats[0]; }
-
-// weights NULL: wdb_dqn_update_sampled; else wdb_dqn_update_prioritized.
-int dqn_update_sampled(void *stream, const wdb_dqn_update_args *u, const wdb_replay_windows *w,
-                       const float *weights) {
-  Plan P;
-  if (!dqn_plan(u, w, &P) || !w->windows) return (int)cudaErrorInvalidValue;
-  if (!net_ok(u->q, P.L[0], true) || !net_ok(u->target_q, P.L[0], false))
-    return (int)cudaErrorInvalidValue;
-  if (!u->obs || !u->actions || !u->rewards || !u->done || !u->workspace)
-    return (int)cudaErrorInvalidValue;
-  Reduce R = {};
-  R.g_total = P.gfloats[0];
-  int widest = 1;
-  add_segments(&R, P, 0, 0, u->q, &widest);
-  static size_t configured[2] = {0, 0};
-  const size_t smem = (size_t)P.smem_floats * sizeof(float);
-  const void *kernel = weights ? (const void *)dqn_weighted_kernel : (const void *)dqn_pass_kernel;
-  int rc = allow_smem(kernel, smem, &configured[weights ? 1 : 0]);
-  if (rc != cudaSuccess) return rc;
-  double *psums = static_cast<double *>(u->workspace);
-  float *partials = reinterpret_cast<float *>(psums + 2 * P.grid);
-  const int2 *windows = reinterpret_cast<const int2 *>(w->windows);
-  if (weights)
-    dqn_weighted_kernel<<<P.grid, kThreads, smem, as_stream(stream)>>>(*u, P, partials, psums,
-                                                                       windows, weights);
-  else
-    dqn_pass_kernel<<<P.grid, kThreads, smem, as_stream(stream)>>>(*u, P, partials, psums,
-                                                                   windows);
-  rc = finish_launch();
-  if (rc != cudaSuccess) return rc;
-  R.grid = P.grid;
-  return launch_reduce(stream, R, widest, partials, psums, u->sums);
-}
-
-// QR-DQN's plan: DQN's with a head of A * N quantiles (<= 64).
+// QR-DQN's plan, and DQN's at N = 1: the online and target Q networks in the actor-shaped slot
+// (input F, head A * N <= 64).  plan_layout also lays out a critic-shaped slot, which the Q
+// passes do not use: it is given an action width of 1, so its input F + 1 only asks F <= 63 of
+// the Q network (F + A is no limit).  The kernel holds both networks, their gradient block and
+// 8 + (hidden layers) row tiles.
 bool qr_dqn_plan(const wdb_dqn_update_args *u, int nq, const wdb_replay_windows *w, Plan *p) {
   if (!u || !w || !(u->huber_delta > 0.0f)) return false;
   if (nq < 1 || nq > kMaxWidth || u->n_actions < 1 || u->n_actions > kMaxWidth) return false;
@@ -1452,38 +1406,26 @@ bool qr_dqn_plan(const wdb_dqn_update_args *u, int nq, const wdb_replay_windows 
   return plan_smem(p, 8 + (p->L[0] - 1), 2ll * p->wfloats[0], p->gfloats[0]);
 }
 
+long long dqn_workspace_bytes(const Plan &P) { return 16ll * P.grid + 4ll * P.grid * P.gfloats[0]; }
+
+// weights NULL: wdb_dqn_update_sampled; else wdb_dqn_update_prioritized.
+int dqn_update_sampled(void *stream, const wdb_dqn_update_args *u, const wdb_replay_windows *w,
+                       const float *weights) {
+  Plan P;
+  if (!qr_dqn_plan(u, 1, w, &P)) return (int)cudaErrorInvalidValue;
+  static size_t configured[2] = {0, 0};
+  return launch_q_pass(stream, u, P, w, weights, configured, nullptr, dqn_pass_kernel,
+                       dqn_weighted_kernel, *u, P);
+}
+
 // weights NULL: the uniform-replay kernel; else the importance-weighted one.
 int qr_dqn_update_sampled(void *stream, const wdb_dqn_update_args *u, int nq,
                           const wdb_replay_windows *w, const float *weights) {
   Plan P;
-  if (!qr_dqn_plan(u, nq, w, &P) || !w->windows) return (int)cudaErrorInvalidValue;
-  if (!net_ok(u->q, P.L[0], true) || !net_ok(u->target_q, P.L[0], false))
-    return (int)cudaErrorInvalidValue;
-  if (!u->obs || !u->actions || !u->rewards || !u->done || !u->workspace)
-    return (int)cudaErrorInvalidValue;
-  Reduce R = {};
-  R.g_total = P.gfloats[0];
-  int widest = 1;
-  add_segments(&R, P, 0, 0, u->q, &widest);
+  if (!qr_dqn_plan(u, nq, w, &P)) return (int)cudaErrorInvalidValue;
   static size_t configured[2] = {0, 0};
-  const size_t smem = (size_t)P.smem_floats * sizeof(float);
-  const void *kernel =
-      weights ? (const void *)qr_dqn_prioritized_kernel : (const void *)qr_dqn_kernel;
-  int rc = allow_smem(kernel, smem, &configured[weights ? 1 : 0]);
-  if (rc != cudaSuccess) return rc;
-  double *psums = static_cast<double *>(u->workspace);
-  float *partials = reinterpret_cast<float *>(psums + 2 * P.grid);
-  const int2 *windows = reinterpret_cast<const int2 *>(w->windows);
-  if (weights)
-    qr_dqn_prioritized_kernel<<<P.grid, kThreads, smem, as_stream(stream)>>>(
-        *u, P, nq, partials, psums, windows, weights);
-  else
-    qr_dqn_kernel<<<P.grid, kThreads, smem, as_stream(stream)>>>(*u, P, nq, partials,
-                                                                      psums, windows);
-  rc = finish_launch();
-  if (rc != cudaSuccess) return rc;
-  R.grid = P.grid;
-  return launch_reduce(stream, R, widest, partials, psums, u->sums);
+  return launch_q_pass(stream, u, P, w, weights, configured, nullptr, qr_dqn_kernel,
+                       qr_dqn_prioritized_kernel, *u, P, nq);
 }
 
 }  // namespace
@@ -1542,13 +1484,13 @@ WDB_PASS_API(sac_actor_update, wdb_sac_update_args, sac_actor_plan, actor_bytes)
 WDB_API int wdb_dqn_update_sampled_supported(const wdb_dqn_update_args *u, int n_windows) {
   const wdb_replay_windows w = {nullptr, n_windows};
   Plan P;
-  return dqn_plan(u, &w, &P) ? 1 : 0;
+  return qr_dqn_plan(u, 1, &w, &P) ? 1 : 0;
 }
 WDB_API long long wdb_dqn_update_sampled_workspace_bytes(const wdb_dqn_update_args *u,
                                                          int n_windows) {
   const wdb_replay_windows w = {nullptr, n_windows};
   Plan P;
-  return dqn_plan(u, &w, &P) ? dqn_workspace_bytes(P) : -1;
+  return qr_dqn_plan(u, 1, &w, &P) ? dqn_workspace_bytes(P) : -1;
 }
 WDB_API int wdb_dqn_update_sampled(void *stream, const wdb_dqn_update_args *u,
                                    const wdb_replay_windows *w) {

@@ -379,36 +379,12 @@ bool iqn_plan(const wdb_dqn_update_args *u, const wdb_iqn_args *q, const wdb_rep
 int iqn_update_sampled(void *stream, const wdb_dqn_update_args *u, const wdb_iqn_args *q,
                        const wdb_replay_windows *w, const float *weights) {
   Plan P;
-  if (!iqn_plan(u, q, w, &P) || !w->windows) return (int)cudaErrorInvalidValue;
-  if (!net_ok(u->q, P.L[0], true) || !net_ok(u->target_q, P.L[0], false))
-    return (int)cudaErrorInvalidValue;
+  if (!iqn_plan(u, q, w, &P)) return (int)cudaErrorInvalidValue;
   if (!q->taus || !net_ok(q->embed, 1, true) || !net_ok(q->target_embed, 1, false))
     return (int)cudaErrorInvalidValue;
-  if (!u->obs || !u->actions || !u->rewards || !u->done || !u->workspace)
-    return (int)cudaErrorInvalidValue;
-  Reduce R = {};
-  R.g_total = P.gfloats[0] + P.gfloats[1];
-  int widest = 1;
-  add_segments(&R, P, 0, 0, u->q, &widest);
-  add_segments(&R, P, 1, P.gfloats[0], q->embed, &widest);
   static size_t configured[2] = {0, 0};
-  const size_t smem = (size_t)P.smem_floats * sizeof(float);
-  const void *kernel = weights ? (const void *)iqn_prioritized_kernel : (const void *)iqn_kernel;
-  int rc = allow_smem(kernel, smem, &configured[weights ? 1 : 0]);
-  if (rc != cudaSuccess) return rc;
-  double *psums = static_cast<double *>(u->workspace);
-  float *partials = reinterpret_cast<float *>(psums + 2 * P.grid);
-  const int2 *windows = reinterpret_cast<const int2 *>(w->windows);
-  if (weights)
-    iqn_prioritized_kernel<<<P.grid, kThreads, smem, as_stream(stream)>>>(
-        *u, *q, P, partials, psums, windows, weights);
-  else
-    iqn_kernel<<<P.grid, kThreads, smem, as_stream(stream)>>>(*u, *q, P, partials, psums,
-                                                              windows);
-  rc = finish_launch();
-  if (rc != cudaSuccess) return rc;
-  R.grid = P.grid;
-  return launch_reduce(stream, R, widest, partials, psums, u->sums);
+  return launch_q_pass(stream, u, P, w, weights, configured, &q->embed, iqn_kernel,
+                       iqn_prioritized_kernel, *u, *q, P);
 }
 
 }  // namespace

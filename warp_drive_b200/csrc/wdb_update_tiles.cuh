@@ -1,9 +1,9 @@
 // wdb_update_tiles.cuh -- the tile primitives of the replay-update passes: the shared-memory
 // Plan of a pass's networks, the row-tile layer forward / input-gradient / weight-gradient steps,
 // the sampled row source and the fixed-order reduction of the per-CTA partials into the
-// gradient arena.  wdb_ddpg_update.cu (DDPG, TD3, SAC, DQN, QR-DQN), wdb_iqn_update.cu (IQN) and
-// wdb_c51_update.cu (C51) build their passes on them; each translation unit gets its own copy
-// (anonymous namespace).
+// gradient arena, and the host launcher of the Q passes.  wdb_ddpg_update.cu (DDPG, TD3, SAC,
+// DQN, QR-DQN), wdb_iqn_update.cu (IQN) and wdb_c51_update.cu (C51) build their passes on them;
+// each translation unit gets its own copy (anonymous namespace).
 #pragma once
 
 #include "wdb_common.cuh"
@@ -354,6 +354,44 @@ bool net_ok(const wdb_ddpg_net &net, int layers, bool grads) {
     if (grads && (!net.gw[l] || !net.gb[l])) return false;
   }
   return true;
+}
+
+// Launches one Q pass over w's sampled windows -- plain(lead..., partials, psums, windows), or
+// with weights weighted(lead..., partials, psums, windows, weights), `lead` the arguments each
+// kernel takes before those -- and the reduction of its per-CTA partials into the online
+// network's gradients and u->sums.  embed (IQN's tau embedding, net slot 1 of P) adds its
+// gradient block after the online network's.  configured: the two kernels' shared-memory
+// settings (allow_smem).
+template <class Plain, class Weighted, class... Lead>
+int launch_q_pass(void *stream, const wdb_dqn_update_args *u, const Plan &P,
+                  const wdb_replay_windows *w, const float *weights, size_t configured[2],
+                  const wdb_ddpg_net *embed, Plain plain, Weighted weighted,
+                  const Lead &...lead) {
+  if (!w->windows || !net_ok(u->q, P.L[0], true) || !net_ok(u->target_q, P.L[0], false))
+    return (int)cudaErrorInvalidValue;
+  if (!u->obs || !u->actions || !u->rewards || !u->done || !u->workspace)
+    return (int)cudaErrorInvalidValue;
+  Reduce R = {};
+  R.g_total = P.gfloats[0] + (embed ? P.gfloats[1] : 0);
+  int widest = 1;
+  add_segments(&R, P, 0, 0, u->q, &widest);
+  if (embed) add_segments(&R, P, 1, P.gfloats[0], *embed, &widest);
+  const size_t smem = (size_t)P.smem_floats * sizeof(float);
+  int rc = allow_smem(weights ? (const void *)weighted : (const void *)plain, smem,
+                      &configured[weights ? 1 : 0]);
+  if (rc != cudaSuccess) return rc;
+  double *psums = static_cast<double *>(u->workspace);
+  float *partials = reinterpret_cast<float *>(psums + 2 * P.grid);
+  const int2 *windows = reinterpret_cast<const int2 *>(w->windows);
+  if (weights)
+    weighted<<<P.grid, kThreads, smem, as_stream(stream)>>>(lead..., partials, psums, windows,
+                                                            weights);
+  else
+    plain<<<P.grid, kThreads, smem, as_stream(stream)>>>(lead..., partials, psums, windows);
+  rc = finish_launch();
+  if (rc != cudaSuccess) return rc;
+  R.grid = P.grid;
+  return launch_reduce(stream, R, widest, partials, psums, u->sums);
 }
 
 }  // namespace

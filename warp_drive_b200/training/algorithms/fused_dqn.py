@@ -16,6 +16,8 @@ import torch
 from warp_drive_b200 import lib as _lib
 from warp_drive_b200.training.algorithms.fused_ddpg import (
     _set_pointers, _set_shape, replay_windows)
+from warp_drive_b200.training.models.fully_connected_q import (
+    FullyConnectedCategoricalQ, FullyConnectedIQN, FullyConnectedQ, FullyConnectedQuantileQ)
 from warp_drive_b200.utils.spaces import Box
 
 
@@ -31,107 +33,70 @@ def _shape_struct(algo, q_net, n_envs, n_agents, capacity):
     return u
 
 
-def fused_dqn_supported(algo, q_net, n_envs, n_agents, capacity, replay_rows):
-    """True if `wdb_dqn_update_sampled` takes this policy: a FullyConnectedQ over a Box
-    observation with 0..3 hidden layers of width <= 64, A <= 64 and F <= 63, and replay_rows
-    sampled windows per update."""
-    from warp_drive_b200.training.models.fully_connected_q import FullyConnectedQ
+class FusedQUpdate:
+    """One policy's launch of a Q network's replay pass `wdb_<entry>`: DQN's argument struct,
+    the pass's workspace and the loss sums (device double[2]).  A pass names the model type it
+    takes and its entry point, and states the arguments the entry takes between the struct and
+    the windows (`shape_args` for `_supported` / `_workspace_bytes`, `launch_args` for the
+    launch)."""
+    model = None
+    entry = None
 
-    if type(q_net) is not FullyConnectedQ or not isinstance(q_net.observation_space, Box):
-        return False
-    if q_net.dueling or len(q_net.fc_dims) > 3:      # dueling: fused_dueling_supported
-        return False
-    u = _shape_struct(algo, q_net, n_envs, n_agents, capacity)
-    return bool(_lib.load().wdb_dqn_update_sampled_supported(ctypes.byref(u), int(replay_rows)))
+    @staticmethod
+    def shape_args(q_net):
+        return ()
 
+    @classmethod
+    def supported(cls, algo, q_net, n_envs, n_agents, capacity, replay_rows):
+        """True if `wdb_<entry>` takes this policy: a `model` over a Box observation with at most
+        3 hidden layers and no dueling head (FusedDuelingUpdate), in the pass's envelope for
+        replay_rows sampled windows per update."""
+        if type(q_net) is not cls.model or not isinstance(q_net.observation_space, Box):
+            return False
+        if q_net.dueling or len(q_net.fc_dims) > 3:
+            return False
+        return cls.fits(_shape_struct(algo, q_net, n_envs, n_agents, capacity), q_net,
+                        replay_rows)
 
-class FusedDQNUpdate:
-    """One policy's `wdb_dqn_update_sampled` launch: the argument struct, its workspace and the
-    loss sums (device double[2]: sum huber(Q - R), sum Q(obs, a))."""
+    @classmethod
+    def fits(cls, u, q_net, replay_rows):
+        """`wdb_<entry>_supported` of the shape struct u."""
+        return bool(getattr(_lib.load(), f"wdb_{cls.entry}_supported")(
+            ctypes.byref(u), *cls.shape_args(q_net), int(replay_rows)))
 
-    def __init__(self, algo, q_net, target_net, n_envs, n_agents, capacity, replay_rows):
+    def __init__(self, algo, q_net, target_net, n_envs, n_agents, capacity, replay_rows, u=None,
+                 point=None):
+        """u and point stand in for q_net's shape struct and pointer step when the pass runs on
+        another network of its shape (FusedDuelingUpdate: the trunk and the folded head)."""
         self.models = (q_net, target_net)
-        self.u = _shape_struct(algo, q_net, n_envs, n_agents, capacity)
+        self.u = _shape_struct(algo, q_net, n_envs, n_agents, capacity) if u is None else u
+        self.point = self._point if point is None else point
         self.lib = _lib.load()
         self.rows = int(replay_rows)
-        nbytes = int(self.lib.wdb_dqn_update_sampled_workspace_bytes(
-            ctypes.byref(self.u), self.rows))
-        assert nbytes > 0, "shapes not supported by wdb_dqn_update_sampled"
+        nbytes = int(getattr(self.lib, f"wdb_{self.entry}_workspace_bytes")(
+            ctypes.byref(self.u), *self.shape_args(q_net), self.rows))
+        assert nbytes > 0, f"shapes not supported by wdb_{self.entry}"
         dev = next(q_net.parameters()).device
         self.workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         self.sums = torch.zeros(2, dtype=torch.float64, device=dev)
+
+    def _point(self, u):
+        q_net, target_net = self.models
+        _set_pointers(u.q, q_net, True)
+        _set_pointers(u.target_q, target_net, False)
+
+    def launch_args(self):
+        return self.shape_args(self.models[0])
 
     def launch(self, obs, actions, rewards, done, windows, outputs=None, weights=None):
         """The Q network's gradient into its `.grad`.  obs [C, E, Np, F], actions [C, E, Np, 1]
         (int32), rewards [C, E, Np], done [C, E] are the ring in physical slot order; windows
         int32 [rows, 2] the sampled windows.  outputs: optional (q_values, returns) float32
         tensors [rows] for the metrics.  weights: float32 [rows] importance-sampling weights
-        (prioritized replay): wdb_dqn_update_prioritized instead of wdb_dqn_update_sampled."""
+        (prioritized replay)."""
         u = self.u
-        q_net, target_net = self.models
         # parameters may have been re-allocated (load_state_dict keeps storage; .to() does not)
-        _set_pointers(u.q, q_net, True)
-        _set_pointers(u.target_q, target_net, False)
-        u.obs, u.actions = _lib.ptr(obs), _lib.ptr(actions)
-        u.rewards, u.done = _lib.ptr(rewards), _lib.ptr(done)
-        q_values, returns = outputs if outputs is not None else (None, None)
-        u.q_values, u.returns = _lib.ptr(q_values), _lib.ptr(returns)
-        u.sums = _lib.ptr(self.sums)
-        u.workspace = _lib.ptr(self.workspace)
-        assert windows.shape[0] == self.rows
-        if weights is None:
-            _lib.check(self.lib.wdb_dqn_update_sampled(
-                _lib.stream_ptr(), ctypes.byref(u), ctypes.byref(replay_windows(windows))),
-                "dqn_update_sampled")
-        else:
-            assert weights.shape == (self.rows,) and weights.dtype == torch.float32
-            _lib.check(self.lib.wdb_dqn_update_prioritized(
-                _lib.stream_ptr(), ctypes.byref(u), ctypes.byref(replay_windows(windows)),
-                _lib.ptr(weights)), "dqn_update_prioritized")
-        return self.sums
-
-
-def fused_qr_dqn_supported(algo, q_net, n_envs, n_agents, capacity, replay_rows):
-    """True if `wdb_qr_dqn_update_sampled` takes this policy: a FullyConnectedQuantileQ over a
-    Box observation with 0..3 hidden layers of width <= 64, F <= 63 and a head of
-    A * num_quantiles <= 64 outputs, and replay_rows sampled windows per update."""
-    from warp_drive_b200.training.models.fully_connected_q import FullyConnectedQuantileQ
-
-    if type(q_net) is not FullyConnectedQuantileQ or not isinstance(q_net.observation_space,
-                                                                    Box):
-        return False
-    if len(q_net.fc_dims) > 3:
-        return False
-    u = _shape_struct(algo, q_net, n_envs, n_agents, capacity)
-    return bool(_lib.load().wdb_qr_dqn_update_sampled_supported(
-        ctypes.byref(u), int(q_net.num_quantiles), int(replay_rows)))
-
-
-class FusedQRDQNUpdate:
-    """One policy's `wdb_qr_dqn_update_sampled` launch: DQN's argument struct with the number
-    of quantiles beside it; the sums are sum w_g loss_g and sum Q-bar, the outputs Q-bar and
-    R-bar."""
-
-    def __init__(self, algo, q_net, target_net, n_envs, n_agents, capacity, replay_rows):
-        self.models = (q_net, target_net)
-        self.u = _shape_struct(algo, q_net, n_envs, n_agents, capacity)
-        self.n_quantiles = int(q_net.num_quantiles)
-        self.lib = _lib.load()
-        self.rows = int(replay_rows)
-        nbytes = int(self.lib.wdb_qr_dqn_update_sampled_workspace_bytes(
-            ctypes.byref(self.u), self.n_quantiles, self.rows))
-        assert nbytes > 0, "shapes not supported by wdb_qr_dqn_update_sampled"
-        dev = next(q_net.parameters()).device
-        self.workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        self.sums = torch.zeros(2, dtype=torch.float64, device=dev)
-
-    def launch(self, obs, actions, rewards, done, windows, outputs=None, weights=None):
-        """The quantile network's gradient into its `.grad`; the arguments of
-        FusedDQNUpdate.launch (outputs: Q-bar and R-bar)."""
-        u = self.u
-        q_net, target_net = self.models
-        _set_pointers(u.q, q_net, True)
-        _set_pointers(u.target_q, target_net, False)
+        self.point(u)
         u.obs, u.actions = _lib.ptr(obs), _lib.ptr(actions)
         u.rewards, u.done = _lib.ptr(rewards), _lib.ptr(done)
         q_values, returns = outputs if outputs is not None else (None, None)
@@ -141,10 +106,40 @@ class FusedQRDQNUpdate:
         assert windows.shape[0] == self.rows
         if weights is not None:
             assert weights.shape == (self.rows,) and weights.dtype == torch.float32
-        _lib.check(self.lib.wdb_qr_dqn_update_sampled(
-            _lib.stream_ptr(), ctypes.byref(u), self.n_quantiles,
-            ctypes.byref(replay_windows(windows)), _lib.ptr(weights)), "qr_dqn_update_sampled")
+        self._run(ctypes.byref(u), ctypes.byref(replay_windows(windows)), weights)
         return self.sums
+
+    def _run(self, u, windows, weights):
+        _lib.check(getattr(self.lib, f"wdb_{self.entry}")(
+            _lib.stream_ptr(), u, *self.launch_args(), windows, _lib.ptr(weights)), self.entry)
+
+
+class FusedDQNUpdate(FusedQUpdate):
+    """`wdb_dqn_update_sampled` (FullyConnectedQ): 0..3 hidden layers of width <= 64, A <= 64 and
+    F <= 63.  The sums are sum huber(Q - R) and sum Q(obs, a).  With weights the launch is
+    `wdb_dqn_update_prioritized`, which takes the same shapes and workspace."""
+    model = FullyConnectedQ
+    entry = "dqn_update_sampled"
+
+    def _run(self, u, windows, weights):
+        if weights is None:
+            _lib.check(self.lib.wdb_dqn_update_sampled(_lib.stream_ptr(), u, windows),
+                       "dqn_update_sampled")
+        else:
+            _lib.check(self.lib.wdb_dqn_update_prioritized(
+                _lib.stream_ptr(), u, windows, _lib.ptr(weights)), "dqn_update_prioritized")
+
+
+class FusedQRDQNUpdate(FusedQUpdate):
+    """`wdb_qr_dqn_update_sampled` (FullyConnectedQuantileQ): DQN's shapes with a head of
+    A * num_quantiles <= 64 outputs, the number of quantiles beside the struct.  The sums are
+    sum w_g loss_g and sum Q-bar, the outputs Q-bar and R-bar."""
+    model = FullyConnectedQuantileQ
+    entry = "qr_dqn_update_sampled"
+
+    @staticmethod
+    def shape_args(q_net):
+        return (int(q_net.num_quantiles),)
 
 
 def _iqn_struct(q_net, target_net=None):
@@ -163,124 +158,52 @@ def _iqn_struct(q_net, target_net=None):
     return a
 
 
-def fused_iqn_supported(algo, q_net, n_envs, n_agents, capacity, replay_rows):
-    """True if `wdb_iqn_update_sampled` takes this policy: a FullyConnectedIQN over a Box
-    observation with 1..3 hidden layers of width <= 64, F <= 63, A <= 64, n_cos, N and N' <= 64,
-    everything in one CTA's shared memory, and replay_rows sampled windows per update."""
-    from warp_drive_b200.training.models.fully_connected_q import FullyConnectedIQN
+class FusedIQNUpdate(FusedQUpdate):
+    """`wdb_iqn_update_sampled` (FullyConnectedIQN): DQN's shapes with 1..3 hidden layers, n_cos,
+    N and N' <= 64, everything in one CTA's shared memory, and the IQN struct beside DQN's.  The
+    sums are sum w_g loss_g and sum Q-bar, the outputs Q-bar and R-bar."""
+    model = FullyConnectedIQN
+    entry = "iqn_update_sampled"
 
-    if type(q_net) is not FullyConnectedIQN or not isinstance(q_net.observation_space, Box):
-        return False
-    if len(q_net.fc_dims) > 3:
-        return False
-    u = _shape_struct(algo, q_net, n_envs, n_agents, capacity)
-    return bool(_lib.load().wdb_iqn_update_sampled_supported(
-        ctypes.byref(u), ctypes.byref(_iqn_struct(q_net)), int(replay_rows)))
+    @staticmethod
+    def shape_args(q_net):
+        return (ctypes.byref(_iqn_struct(q_net)),)
 
-
-class FusedIQNUpdate:
-    """One policy's `wdb_iqn_update_sampled` launch: DQN's argument struct and the IQN one
-    beside it; the sums are sum w_g loss_g and sum Q-bar, the outputs Q-bar and R-bar."""
-
-    def __init__(self, algo, q_net, target_net, n_envs, n_agents, capacity, replay_rows):
-        self.models = (q_net, target_net)
-        self.u = _shape_struct(algo, q_net, n_envs, n_agents, capacity)
-        self.iqn = _iqn_struct(q_net)
-        self.lib = _lib.load()
-        self.rows = int(replay_rows)
-        nbytes = int(self.lib.wdb_iqn_update_sampled_workspace_bytes(
-            ctypes.byref(self.u), ctypes.byref(self.iqn), self.rows))
-        assert nbytes > 0, "shapes not supported by wdb_iqn_update_sampled"
-        dev = next(q_net.parameters()).device
-        self.workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        self.sums = torch.zeros(2, dtype=torch.float64, device=dev)
+    def launch_args(self):
+        return (ctypes.byref(self.iqn),)
 
     def launch(self, obs, actions, rewards, done, windows, outputs=None, weights=None,
                taus=None):
         """The network's gradient (trunk, head and tau embedding) into its `.grad`; the
-        arguments of FusedDQNUpdate.launch and the levels `taus`, float32 [rows, N + N']
-        (outputs: Q-bar and R-bar)."""
-        u = self.u
-        q_net, target_net = self.models
-        _set_pointers(u.q, q_net, True)
-        _set_pointers(u.target_q, target_net, False)
-        iqn = self.iqn = _iqn_struct(q_net, target_net)
+        arguments of FusedQUpdate.launch and the levels `taus`, float32 [rows, N + N']."""
+        iqn = self.iqn = _iqn_struct(*self.models)
         n = iqn.n_tau + iqn.n_tau_prime
         assert taus is not None and taus.shape == (self.rows, n) and taus.dtype == torch.float32
         assert taus.is_contiguous()
         iqn.taus = _lib.ptr(taus)
-        u.obs, u.actions = _lib.ptr(obs), _lib.ptr(actions)
-        u.rewards, u.done = _lib.ptr(rewards), _lib.ptr(done)
-        q_values, returns = outputs if outputs is not None else (None, None)
-        u.q_values, u.returns = _lib.ptr(q_values), _lib.ptr(returns)
-        u.sums = _lib.ptr(self.sums)
-        u.workspace = _lib.ptr(self.workspace)
-        assert windows.shape[0] == self.rows
-        if weights is not None:
-            assert weights.shape == (self.rows,) and weights.dtype == torch.float32
-        _lib.check(self.lib.wdb_iqn_update_sampled(
-            _lib.stream_ptr(), ctypes.byref(u), ctypes.byref(iqn),
-            ctypes.byref(replay_windows(windows)), _lib.ptr(weights)), "iqn_update_sampled")
-        return self.sums
+        return super().launch(obs, actions, rewards, done, windows, outputs, weights)
 
 
-def fused_c51_supported(algo, q_net, n_envs, n_agents, capacity, replay_rows):
-    """True if `wdb_c51_update_sampled` takes this policy: a FullyConnectedCategoricalQ over a
-    Box observation with 0..3 hidden layers of width <= 64, F <= 63, A <= 64 and 2 <= N <= 64
-    atoms, everything in one CTA's shared memory, and replay_rows sampled windows per update."""
-    from warp_drive_b200.training.models.fully_connected_q import FullyConnectedCategoricalQ
+class FusedC51Update(FusedQUpdate):
+    """`wdb_c51_update_sampled` (FullyConnectedCategoricalQ): DQN's shapes with 2 <= N <= 64
+    atoms and everything in one CTA's shared memory; the number of atoms, the model's support
+    (float32, on the device) and its spacing beside the struct.  The sums are sum w_g loss_g
+    and sum Q-bar, the outputs Q-bar and R-bar."""
+    model = FullyConnectedCategoricalQ
+    entry = "c51_update_sampled"
 
-    if type(q_net) is not FullyConnectedCategoricalQ or not isinstance(q_net.observation_space,
-                                                                       Box):
-        return False
-    if q_net.dueling or len(q_net.fc_dims) > 3:      # dueling: fused_dueling_supported
-        return False
-    u = _shape_struct(algo, q_net, n_envs, n_agents, capacity)
-    return bool(_lib.load().wdb_c51_update_sampled_supported(
-        ctypes.byref(u), int(q_net.num_atoms), int(replay_rows)))
+    @staticmethod
+    def shape_args(q_net):
+        return (int(q_net.num_atoms),)
 
-
-class FusedC51Update:
-    """One policy's `wdb_c51_update_sampled` launch: DQN's argument struct with the number of
-    atoms, the model's support (float32, on the device) and its spacing beside it; the sums are
-    sum w_g loss_g and sum Q-bar, the outputs Q-bar and R-bar."""
-
-    def __init__(self, algo, q_net, target_net, n_envs, n_agents, capacity, replay_rows):
-        self.models = (q_net, target_net)
-        self.u = _shape_struct(algo, q_net, n_envs, n_agents, capacity)
-        self.n_atoms = int(q_net.num_atoms)
-        self.lib = _lib.load()
-        self.rows = int(replay_rows)
-        nbytes = int(self.lib.wdb_c51_update_sampled_workspace_bytes(
-            ctypes.byref(self.u), self.n_atoms, self.rows))
-        assert nbytes > 0, "shapes not supported by wdb_c51_update_sampled"
-        dev = next(q_net.parameters()).device
-        self.workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        self.sums = torch.zeros(2, dtype=torch.float64, device=dev)
-        self.support = q_net.support.to(device=dev, dtype=torch.float32).contiguous()
+    def __init__(self, algo, q_net, *args, **kwargs):
+        super().__init__(algo, q_net, *args, **kwargs)
+        self.support = q_net.support.to(device=self.sums.device,
+                                        dtype=torch.float32).contiguous()
         self.delta_z = float(q_net.delta_z)
 
-    def launch(self, obs, actions, rewards, done, windows, outputs=None, weights=None):
-        """The categorical network's gradient into its `.grad`; the arguments of
-        FusedDQNUpdate.launch (outputs: Q-bar and R-bar)."""
-        u = self.u
-        q_net, target_net = self.models
-        _set_pointers(u.q, q_net, True)
-        _set_pointers(u.target_q, target_net, False)
-        u.obs, u.actions = _lib.ptr(obs), _lib.ptr(actions)
-        u.rewards, u.done = _lib.ptr(rewards), _lib.ptr(done)
-        q_values, returns = outputs if outputs is not None else (None, None)
-        u.q_values, u.returns = _lib.ptr(q_values), _lib.ptr(returns)
-        u.sums = _lib.ptr(self.sums)
-        u.workspace = _lib.ptr(self.workspace)
-        assert windows.shape[0] == self.rows
-        if weights is not None:
-            assert weights.shape == (self.rows,) and weights.dtype == torch.float32
-        _lib.check(self.lib.wdb_c51_update_sampled(
-            _lib.stream_ptr(), ctypes.byref(u), self.n_atoms, _lib.ptr(self.support),
-            self.delta_z, ctypes.byref(replay_windows(windows)), _lib.ptr(weights)),
-            "c51_update_sampled")
-        return self.sums
+    def launch_args(self):
+        return self.shape_args(self.models[0]) + (_lib.ptr(self.support), self.delta_z)
 
 
 def folded_widths(q_net):
@@ -356,98 +279,64 @@ def _dueling_shape_struct(algo, q_net, n_envs, n_agents, capacity):
     return u
 
 
-def fused_dueling_supported(algo, q_net, n_envs, n_agents, capacity, replay_rows):
-    """True if the folded network of a dueling FullyConnectedQ (wdb_dqn_update_sampled) or
-    FullyConnectedCategoricalQ (wdb_c51_update_sampled) is in that pass's envelope: at most 3
-    hidden layers in all (a one-layer stream allows a trunk of at most 2), each, 2S included,
-    of width <= 64, F <= 63, and C51's shared-memory cap."""
-    from warp_drive_b200.training.models.fully_connected_q import (
-        FullyConnectedCategoricalQ, FullyConnectedQ)
-
-    if type(q_net) not in (FullyConnectedQ, FullyConnectedCategoricalQ) or not q_net.dueling:
-        return False
-    if not isinstance(q_net.observation_space, Box) or len(folded_widths(q_net)) > 3:
-        return False
-    L = _lib.load()
-    if not L.wdb_dueling_fold_supported(ctypes.byref(dueling_shape(q_net.policy_head))):
-        return False
-    u = _dueling_shape_struct(algo, q_net, n_envs, n_agents, capacity)
-    if getattr(q_net, "is_categorical_q", False):
-        return bool(L.wdb_c51_update_sampled_supported(
-            ctypes.byref(u), int(q_net.num_atoms), int(replay_rows)))
-    return bool(L.wdb_dqn_update_sampled_supported(ctypes.byref(u), int(replay_rows)))
-
-
 class FusedDuelingUpdate:
     """One update of a dueling DQN or C51 policy: wdb_dueling_fold of the online and the target
-    head (1 launch), the plain pass -- wdb_dqn_update_sampled / _prioritized, or
-    wdb_c51_update_sampled -- on networks made of the live trunk layers and the folded layers (2
-    launches), then wdb_dueling_unfold_grads (1 launch).  The pass writes the trunk's gradients
-    straight into the arena's `.grad` views and the folded layers' into scratch, which the
-    unfold maps onto the stream parameters' `.grad` views.  Sums and outputs are the plain
-    pass's."""
-
-    def __init__(self, algo, q_net, target_net, n_envs, n_agents, capacity, replay_rows):
-        self.models = (q_net, target_net)
-        self.categorical = bool(getattr(q_net, "is_categorical_q", False))
-        self.u = _dueling_shape_struct(algo, q_net, n_envs, n_agents, capacity)
-        self.lib = _lib.load()
-        self.rows = int(replay_rows)
-        if self.categorical:
-            self.n_atoms = int(q_net.num_atoms)
-            nbytes = self.lib.wdb_c51_update_sampled_workspace_bytes(
-                ctypes.byref(self.u), self.n_atoms, self.rows)
-        else:
-            nbytes = self.lib.wdb_dqn_update_sampled_workspace_bytes(ctypes.byref(self.u),
-                                                                     self.rows)
-        assert nbytes > 0, "folded shapes not supported by the pass"
-        dev = next(q_net.parameters()).device
-        self.workspace = torch.empty(int(nbytes), dtype=torch.uint8, device=dev)
-        self.sums = torch.zeros(2, dtype=torch.float64, device=dev)
-        if self.categorical:
-            self.support = q_net.support.to(device=dev, dtype=torch.float32).contiguous()
-            self.delta_z = float(q_net.delta_z)
-        self.online, self.target = DuelingFold(q_net, grads=True), DuelingFold(target_net)
+    head (1 launch), the plain pass -- FusedDQNUpdate or FusedC51Update -- on networks made of the
+    live trunk layers and the folded layers (2 launches), then wdb_dueling_unfold_grads (1
+    launch).  The pass writes the trunk's gradients straight into the arena's `.grad` views and
+    the folded layers' into scratch, which the unfold maps onto the stream parameters' `.grad`
+    views.  Sums and outputs are the plain pass's."""
 
     @staticmethod
-    def _point(net, model, folded, grads):
-        trunk = [(model.fc[str(i)][0].weight, model.fc[str(i)][0].bias)
-                 for i in range(len(model.fc))]
-        for i, (w, b) in enumerate(trunk + folded.layers):
-            net.w[i], net.b[i] = _lib.ptr(w.data), _lib.ptr(b.data)
-        if grads:
-            for i, (w, b) in enumerate([(w.grad, b.grad) for w, b in trunk] + folded.grads):
-                net.gw[i], net.gb[i] = _lib.ptr(w), _lib.ptr(b)
+    def plain_type(q_net):
+        return FusedC51Update if getattr(q_net, "is_categorical_q", False) else FusedDQNUpdate
+
+    @classmethod
+    def supported(cls, algo, q_net, n_envs, n_agents, capacity, replay_rows):
+        """True if the folded network of a dueling FullyConnectedQ or FullyConnectedCategoricalQ
+        is in the plain pass's envelope: at most 3 hidden layers in all (a one-layer stream
+        allows a trunk of at most 2), each, 2S included, of width <= 64, F <= 63, and C51's
+        shared-memory cap."""
+        if type(q_net) not in (FullyConnectedQ, FullyConnectedCategoricalQ) or not q_net.dueling:
+            return False
+        if not isinstance(q_net.observation_space, Box) or len(folded_widths(q_net)) > 3:
+            return False
+        head = ctypes.byref(dueling_shape(q_net.policy_head))
+        if not _lib.load().wdb_dueling_fold_supported(head):
+            return False
+        u = _dueling_shape_struct(algo, q_net, n_envs, n_agents, capacity)
+        return cls.plain_type(q_net).fits(u, q_net, replay_rows)
+
+    def __init__(self, algo, q_net, target_net, n_envs, n_agents, capacity, replay_rows):
+        self.online, self.target = DuelingFold(q_net, grads=True), DuelingFold(target_net)
+        self.plain = self.plain_type(q_net)(
+            algo, q_net, target_net, n_envs, n_agents, capacity, replay_rows,
+            u=_dueling_shape_struct(algo, q_net, n_envs, n_agents, capacity), point=self._point)
+        self.rows, self.sums = self.plain.rows, self.plain.sums
+
+    def _point(self, u):
+        for net, folded, grads in ((u.q, self.online, True), (u.target_q, self.target, False)):
+            fc = folded.model.fc
+            trunk = [(fc[str(i)][0].weight, fc[str(i)][0].bias) for i in range(len(fc))]
+            for i, (w, b) in enumerate(trunk + folded.layers):
+                net.w[i], net.b[i] = _lib.ptr(w.data), _lib.ptr(b.data)
+            if grads:
+                for i, (w, b) in enumerate([(w.grad, b.grad) for w, b in trunk] + folded.grads):
+                    net.gw[i], net.gb[i] = _lib.ptr(w), _lib.ptr(b)
 
     def launch(self, obs, actions, rewards, done, windows, outputs=None, weights=None):
         """The network's gradient (trunk and both streams) into its `.grad`; the arguments of
-        FusedDQNUpdate.launch."""
-        u = self.u
-        q_net, target_net = self.models
+        FusedQUpdate.launch."""
         fold(self.online, self.target)
-        self._point(u.q, q_net, self.online, True)
-        self._point(u.target_q, target_net, self.target, False)
-        u.obs, u.actions = _lib.ptr(obs), _lib.ptr(actions)
-        u.rewards, u.done = _lib.ptr(rewards), _lib.ptr(done)
-        q_values, returns = outputs if outputs is not None else (None, None)
-        u.q_values, u.returns = _lib.ptr(q_values), _lib.ptr(returns)
-        u.sums = _lib.ptr(self.sums)
-        u.workspace = _lib.ptr(self.workspace)
-        assert windows.shape[0] == self.rows
-        if weights is not None:
-            assert weights.shape == (self.rows,) and weights.dtype == torch.float32
-        win = ctypes.byref(replay_windows(windows))
-        if self.categorical:
-            _lib.check(self.lib.wdb_c51_update_sampled(
-                _lib.stream_ptr(), ctypes.byref(u), self.n_atoms, _lib.ptr(self.support),
-                self.delta_z, win, _lib.ptr(weights)), "c51_update_sampled")
-        elif weights is None:
-            _lib.check(self.lib.wdb_dqn_update_sampled(_lib.stream_ptr(), ctypes.byref(u), win),
-                       "dqn_update_sampled")
-        else:
-            _lib.check(self.lib.wdb_dqn_update_prioritized(
-                _lib.stream_ptr(), ctypes.byref(u), win, _lib.ptr(weights)),
-                "dqn_update_prioritized")
-        _lib.check(self.lib.wdb_dueling_unfold_grads(
+        self.plain.launch(obs, actions, rewards, done, windows, outputs, weights)
+        _lib.check(_lib.load().wdb_dueling_unfold_grads(
             _lib.stream_ptr(), ctypes.byref(self.online.struct())), "dueling_unfold_grads")
         return self.sums
+
+
+# The envelope checks by their function names: each is the class's `supported`.
+fused_dqn_supported = FusedDQNUpdate.supported
+fused_qr_dqn_supported = FusedQRDQNUpdate.supported
+fused_iqn_supported = FusedIQNUpdate.supported
+fused_c51_supported = FusedC51Update.supported
+fused_dueling_supported = FusedDuelingUpdate.supported

@@ -61,9 +61,7 @@ import torch
 from warp_drive_b200.training.algorithms.dqn import (
     DQN, CategoricalDQN, ImplicitQuantileDQN, QuantileDQN)
 from warp_drive_b200.training.algorithms.fused_dqn import (
-    FusedC51Update, FusedDQNUpdate, FusedDuelingUpdate, FusedIQNUpdate, FusedQRDQNUpdate,
-    fused_c51_supported, fused_dqn_supported, fused_dueling_supported, fused_iqn_supported,
-    fused_qr_dqn_supported)
+    FusedC51Update, FusedDQNUpdate, FusedDuelingUpdate, FusedIQNUpdate, FusedQRDQNUpdate)
 from warp_drive_b200.training.trainer_ddpg import (
     RingRolloutEngine, TrainerDDPG, hard_update, soft_update)
 from warp_drive_b200.training.utils.param_scheduler import ParamScheduler
@@ -223,12 +221,10 @@ class TrainerDQN(TrainerDDPG):
             if self._tau_generator is None:
                 self._tau_generator = torch.Generator(device=dev)
                 self._tau_generator.manual_seed(self.seed)
-        supported, fused = ((fused_dueling_supported, FusedDuelingUpdate) if q_net.dueling
-                            else (fused_c51_supported, FusedC51Update) if categorical
-                            else (fused_iqn_supported, FusedIQNUpdate) if implicit
-                            else (fused_qr_dqn_supported, FusedQRDQNUpdate) if quantile
-                            else (fused_dqn_supported, FusedDQNUpdate))
-        if supported(algo, q_net, self.num_envs, n_agents, self.ring_capacity, rows):
+        fused = (FusedDuelingUpdate if q_net.dueling else FusedC51Update if categorical
+                 else FusedIQNUpdate if implicit else FusedQRDQNUpdate if quantile
+                 else FusedDQNUpdate)
+        if fused.supported(algo, q_net, self.num_envs, n_agents, self.ring_capacity, rows):
             self.fused_updates[policy] = fused(
                 algo, q_net, self.target_q_models[policy], self.num_envs, n_agents,
                 self.ring_capacity, rows)
