@@ -396,7 +396,8 @@ typedef struct wdb_sa_rollout {
   const float *log_std;              /* required with gaussian_head: [1] the log-std (1), or
                                       * [2] the log-std's clamp bounds min <= max (2) */
   int gaussian_head;                 /* 0: tanh + OU, 1: Gaussian, 2: squashed Gaussian;
-                                      * discrete kinds: 3 = Q head, else softmax */
+                                      * discrete kinds: 3 = Q head, 4 = categorical Q head,
+                                      * 5 = noisy Q head, else softmax */
   /* Discrete kinds, Q head (gaussian_head = 3; DQN's FullyConnectedQ): the head's raw outputs
    * are Q values, written to probs_batch when given, and the action is sampled as
    * wdb_sample_epsilon_greedy (stream = env, one draw per step) with epsilon = log_std[0], a
@@ -407,7 +408,15 @@ typedef struct wdb_sa_rollout {
    * count.  Each block is reduced to Q[a] = sum_j z_j softmax_j over the env's 8 lanes (lane k:
    * j = k, k + 8, ... in order, then an xor butterfly; e_j = expf(y_j - max y), Q = (sum z_j
    * e_j) / (sum e_j)); Q is written to probs_batch when given and sampled as the Q head is.
-   * log_std = [epsilon, z_0, ..., z_{N-1}] on the device. */
+   * log_std = [epsilon, z_0, ..., z_{N-1}] on the device.
+   * Discrete kinds, noisy Q head (gaussian_head = 5; FullyConnectedQ with a noisy output layer):
+   * w / b of the head are mu_W, mu_b.  log_std = [epsilon, key words, sigma_W [A][H], sigma_b
+   * [A]] on the device, the four key words (raw 32-bit: seed low, seed high, step low, step
+   * high) giving the noise of wdb_noisy_* in the acting domain, layer 0, counter row = env, step
+   * = the given step + t at timestep t.  Output j = fmaf(f(eps_out)_j, s_j, m_j): m_j the Q head's
+   * output (bias, then fmaf over the inputs in order), s_j = sigma_b_j then fmaf(sigma_W[j][i],
+   * f(eps_in)_i * h_i, .) over i in order; use_argmax: m_j alone (the mean network) and epsilon
+   * 0.  Then sampled as the Q head is. */
 } wdb_sa_rollout;
 
 int wdb_single_agent_rollout_supported(int n_hidden, const int *dims);
@@ -415,6 +424,9 @@ int wdb_single_agent_rollout_supported(int n_hidden, const int *dims);
  * hidden widths and F as wdb_single_agent_rollout_supported takes them, 2 <= N <= 64, N
  * dividing the head, and the same cap on the network's floats. */
 int wdb_single_agent_rollout_categorical_supported(int n_hidden, const int *dims, int n_atoms);
+/* 1 if a noisy Q head runs in one launch: the shapes of wdb_single_agent_rollout_supported, A
+ * <= 8, and the network's floats plus the head's A * H + A sigma floats within the same cap. */
+int wdb_single_agent_rollout_noisy_supported(int n_hidden, const int *dims);
 int wdb_single_agent_rollout(void *stream, const wdb_sa_rollout *rollout);
 
 /* -------------------------------------------------- rollout of ANY env: data movement ---- */
@@ -1170,6 +1182,58 @@ int wdb_dueling_fold(void *stream, const wdb_dueling_head *head, const wdb_dueli
  * Sums over a and c in order.  One launch.  cudaErrorInvalidValue without launching if
  * unsupported or a required pointer is NULL. */
 int wdb_dueling_unfold_grads(void *stream, const wdb_dueling_head *head);
+
+/* Noisy networks (Fortunato et al. 2018, factorized Gaussian noise) of a DQN or C51 head.  A
+ * noisy layer of in_dim inputs and out_dim outputs has parameters mu_W, sigma_W [out, in] and
+ * mu_b, sigma_b [out]; with the noise vectors fi = f(eps_in) [in], fo = f(eps_out) [out],
+ * f(x) = sgn(x) sqrt(|x|), its effective layer is
+ *   W[j][k] = fmaf(sigma_W[j][k], fo[j] * fi[k], mu_W[j][k]),  b[j] = fmaf(sigma_b[j], fo[j], mu_b[j]).
+ * The noise element: eps = u32x2_to_normal of two words of Philox4x32-10 with key `seed` (the
+ * trainer seed) at the counter
+ *   (count mod 2^32, 0x4E000000 | domain << 16 | (count >> 32) mod 2^16, row,
+ *    layer << 16 | e >> 1),
+ * words (x, y) for an even element e and (z, w) for an odd one.  domain 0 is the update (count:
+ * the update number; row 0 the online network's sample, row 1 the target's), domain 1 acting
+ * (count: the policy's acting step; row: the env row).  e < in_dim is eps_in[e], e >= in_dim
+ * eps_out[e - in_dim]; layer numbers the head's noisy layers in module order.  The counter's
+ * second word is at least 0x4E000000, so no draw of wdb_replay_sample_windows,
+ * wdb_per_sample_windows (counter (n, g): second word n >> 32) or of the sampler's per-env and
+ * reset-pool streams (offset (o, o >> 32, stream, stream >> 32)) coincides with a noise draw
+ * below 2^56 draws. */
+#define WDB_NOISY_MAX_LAYERS 4
+typedef struct wdb_noisy_layer {
+  int in_dim, out_dim;               /* in_dim + out_dim <= 2^17 */
+  const float *weight_mu, *weight_sigma;   /* [out, in] */
+  const float *bias_mu, *bias_sigma;       /* [out] */
+  float *noise_in, *noise_out;       /* f(eps_in) [rows, in], f(eps_out) [rows, out] */
+  float *weight, *bias;              /* the effective W [out, in], b [out] (materialize) */
+  const float *grad_weight, *grad_bias;    /* dW, db (read by the grads) */
+  float *grad_weight_mu, *grad_weight_sigma, *grad_bias_mu, *grad_bias_sigma;   /* (written) */
+} wdb_noisy_layer;
+typedef struct wdb_noisy_net {
+  int n_layers;                      /* 1 .. WDB_NOISY_MAX_LAYERS */
+  wdb_noisy_layer layer[WDB_NOISY_MAX_LAYERS];
+} wdb_noisy_net;
+/* 1 if the noisy kernels take the shape: 1 <= n_layers <= 4, every in_dim, out_dim >= 1,
+ * in_dim + out_dim <= 2^17 and in_dim * out_dim < 2^31.  No CUDA call. */
+int wdb_noisy_supported(const wdb_noisy_net *net);
+/* Writes f(eps) of rows row0 .. row0 + n_rows - 1 of (domain, count): layer l's noise_in[r][k]
+ * and noise_out[r][j], r = 0 .. n_rows - 1 for counter row row0 + r.  Only the noise pointers
+ * are read.  One launch.  cudaErrorInvalidValue without launching if unsupported, n_rows < 1,
+ * domain is not 0 or 1, or a noise pointer is NULL. */
+int wdb_noisy_draw(void *stream, const wdb_noisy_net *net, unsigned long long seed, int domain,
+                   unsigned long long count, int row0, int n_rows);
+/* The update's samples: for the online net (row 0) and, when target is not NULL, the target (row
+ * 1) of update `update`, writes f(eps) into noise_in / noise_out ([1, in], [1, out]) and the
+ * effective layers into weight / bias.  One launch.  cudaErrorInvalidValue without launching if
+ * unsupported, the shapes differ or a pointer it reads or writes is NULL. */
+int wdb_noisy_materialize(void *stream, const wdb_noisy_net *online, const wdb_noisy_net *target,
+                          unsigned long long seed, unsigned long long update);
+/* From the effective layers' gradients dW, db and the noise vectors materialize wrote:
+ *   grad_weight_mu = dW, grad_weight_sigma[j][k] = dW[j][k] * (fo[j] * fi[k]),
+ *   grad_bias_mu = db, grad_bias_sigma[j] = db[j] * fo[j]   (float32 products, no sums).
+ * One launch.  cudaErrorInvalidValue without launching if unsupported or a pointer is NULL. */
+int wdb_noisy_grads(void *stream, const wdb_noisy_net *net);
 
 /* Prioritized replay (Schaul et al. 2016, proportional) over the replay ring's n-step windows.
  * One float32 leaf per (physical slot s, agent row n), leaf s * n_rows + n: p^alpha of the

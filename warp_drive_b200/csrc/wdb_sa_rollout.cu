@@ -57,8 +57,19 @@ WDB_API int wdb_single_agent_rollout_categorical_supported(int n_hidden, const i
   return total <= kSaMaxWeights ? 1 : 0;
 }
 
+WDB_API int wdb_single_agent_rollout_noisy_supported(int n_hidden, const int *dims) {
+  if (!wdb_single_agent_rollout_supported(n_hidden, dims)) return 0;
+  const int H = dims[n_hidden], A = dims[n_hidden + 1];
+  if (A > kSaGroup) return 0;                          // one output per lane
+  long long total = 0;
+  for (int l = 0; l <= n_hidden; l++) total += (long long)dims[l] * dims[l + 1] + dims[l + 1];
+  return total + (long long)A * H + A <= kSaMaxWeights ? 1 : 0;   // mu and sigma of the head
+}
+
 // sa_rollout_kernel<kSaCategoricalQ>'s launch (wdb_sa_rollout_categorical.cu)
 int sa_launch_categorical(void *stream, const wdb_sa_rollout *r, size_t smem);
+// sa_rollout_kernel<kSaNoisyQ>'s launch (wdb_sa_rollout_noisy.cu)
+int sa_launch_noisy(void *stream, const wdb_sa_rollout *r, size_t smem);
 
 WDB_API int wdb_single_agent_rollout(void *stream, const wdb_sa_rollout *r) {
   if (!r) return (int)cudaErrorInvalidValue;
@@ -70,10 +81,12 @@ WDB_API int wdb_single_agent_rollout(void *stream, const wdb_sa_rollout *r) {
   const bool gaussian = continuous && r->gaussian_head == 1;
   const bool eps_greedy = !continuous && r->gaussian_head == 3;
   const bool categorical = !continuous && r->gaussian_head == 4;
+  const bool noisy = !continuous && r->gaussian_head == 5;
   if (r->n_steps <= 0) return (int)cudaErrorInvalidValue;
   // the categorical head: A blocks of N atoms, A = the kind's action count
   const int n_atoms = categorical ? r->dims[r->n_hidden + 1] / kSaNActions[r->env_kind] : 1;
   if (categorical ? !wdb_single_agent_rollout_categorical_supported(r->n_hidden, r->dims, n_atoms)
+      : noisy     ? !wdb_single_agent_rollout_noisy_supported(r->n_hidden, r->dims)
                   : !wdb_single_agent_rollout_supported(r->n_hidden, r->dims))
     return (int)cudaErrorInvalidValue;
   for (int l = 0; l <= r->n_hidden; l++)
@@ -88,7 +101,7 @@ WDB_API int wdb_single_agent_rollout(void *stream, const wdb_sa_rollout *r) {
     // the OU state and a normal source unless the bypass (scale < 1e-8) draws nothing
     if (!(r->ou_scale < 1.0e-8f) && (!r->ou_state || (!r->normals && !r->rng_state)))
       return (int)cudaErrorInvalidValue;
-  } else if (eps_greedy || categorical) {
+  } else if (eps_greedy || categorical || noisy) {
     // epsilon on the device; one Philox draw per step whatever it is; no uniforms hook
     if (!r->log_std || !r->rng_state || r->uniforms) return (int)cudaErrorInvalidValue;
   } else if (!r->use_argmax && !r->uniforms && !r->rng_state) {
@@ -112,6 +125,10 @@ WDB_API int wdb_single_agent_rollout(void *stream, const wdb_sa_rollout *r) {
   if (gaussian) return sa_launch<kSaGaussian>(stream, r, smem);
   if (eps_greedy) return sa_launch<kSaEpsGreedy>(stream, r, smem);
   // (and each env's Q row, and the support)
+  if (noisy) {                         // (and the head's sigma_W, sigma_b)
+    const int H = r->dims[r->n_hidden], A = r->dims[r->n_hidden + 1];
+    return sa_launch_noisy(stream, r, smem + (size_t)(A * H + A) * sizeof(float));
+  }
   if (categorical)
     return sa_launch_categorical(
         stream, r, smem + ((size_t)kSaEnvsPerCta * kSaPitch + kSaMaxWidth) * sizeof(float));

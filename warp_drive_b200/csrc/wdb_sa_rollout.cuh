@@ -8,6 +8,7 @@
 
 #include <type_traits>
 
+#include "wdb_noisy.cuh"
 #include "wdb_sa_physics.cuh"
 
 using namespace wdb;
@@ -80,13 +81,24 @@ static __device__ __noinline__ float sa_expectation(const float *y, const float 
 // discrete kinds with DQN's Q head (raw outputs) and epsilon_greedy_step (int32 actions).
 // kSaCategoricalQ: the discrete kinds with C51's categorical head -- A blocks of N atom logits,
 // each reduced to its expectation over the group's lanes -- and epsilon_greedy_step on those.
+// kSaNoisyQ: the discrete kinds with a noisy DQN head (one NoisyLinear, A <= 3 outputs): output
+// j is fmaf(f(eps_out)_j, sigma_b_j + sum_i sigma_W[j][i] (f(eps_in)_i h_i), mu-part_j), the
+// mu-part computed exactly as the Q kind's head, fresh noise (noisy_f) per env row and step;
+// use_argmax: the mu-part alone.  Then epsilon_greedy_step.
+// noisy_f as a call: the noisy kind's Philox, logf and cosf stay out of the rollout loop's
+// registers (inlined, they push the kernel past its register budget into spills)
+__device__ __noinline__ float sa_noise(unsigned long long seed, unsigned long long step,
+                                       uint32_t env, int e) {
+  return noisy_f(seed, 1, step, env, 0, e);
+}
+
 enum { kSaSoftmax = 0, kSaTanhOu = 1, kSaGaussian = 2, kSaSquashed = 3, kSaEpsGreedy = 4,
-       kSaCategoricalQ = 5 };
+       kSaCategoricalQ = 5, kSaNoisyQ = 6 };
 template <int kKind>
 __global__ void __launch_bounds__(kSaThreads, 9)
 sa_rollout_kernel(const __grid_constant__ wdb_sa_rollout R) {
   constexpr bool kContinuous = kKind != kSaSoftmax && kKind != kSaEpsGreedy &&
-                               kKind != kSaCategoricalQ;
+                               kKind != kSaCategoricalQ && kKind != kSaNoisyQ;
   extern __shared__ float s_w[];               // per layer: [Wt (in x out) | b (out)]
   __shared__ int s_dims[8];                    // layer widths (dynamic indexing of the kernel
   if (threadIdx.x < 5) s_dims[threadIdx.x] = R.dims[threadIdx.x];   // parameter goes through
@@ -114,6 +126,12 @@ sa_rollout_kernel(const __grid_constant__ wdb_sa_rollout R) {
       s_dims[5] = n_q;
       s_dims[6] = n_atoms;
     }
+  }
+  // noisy head: sigma_W [A][H] and sigma_b [A] after the activation rows (log_std[5 ..])
+  if constexpr (kKind == kSaNoisyQ) {
+    const int n_sigma = R.dims[n_layers] * R.dims[n_layers - 1] + R.dims[n_layers];
+    float *s_sig = s_act + kSaEnvsPerCta * 2 * kSaPitch;
+    for (int i = threadIdx.x; i < n_sigma; i += blockDim.x) s_sig[i] = R.log_std[5 + i];
   }
   __syncthreads();
   const int sub = threadIdx.x & (kSaGroup - 1);
@@ -150,7 +168,7 @@ sa_rollout_kernel(const __grid_constant__ wdb_sa_rollout R) {
       ls_lo = R.log_std[0];
       ls_hi = R.log_std[1];
     }
-    if constexpr (kKind == kSaEpsGreedy || kKind == kSaCategoricalQ)
+    if constexpr (kKind == kSaEpsGreedy || kKind == kSaCategoricalQ || kKind == kSaNoisyQ)
       eps = R.use_argmax ? 0.0f : R.log_std[0];
   }
 
@@ -170,7 +188,8 @@ sa_rollout_kernel(const __grid_constant__ wdb_sa_rollout R) {
     float *cur = buf0, *nxt = buf1;
     int off = 0;
     // (the categorical head runs after the loop, block by block)
-    const int n_fwd = kKind == kSaCategoricalQ ? n_layers - 1 : n_layers;
+    // (so does the noisy head)
+    const int n_fwd = kKind == kSaCategoricalQ || kKind == kSaNoisyQ ? n_layers - 1 : n_layers;
     for (int l = 0; l < n_fwd; l++) {
       const int in = s_dims[l], out = s_dims[l + 1];
       const float *Wt = s_w + off, *bl = Wt + in * out;
@@ -230,6 +249,41 @@ sa_rollout_kernel(const __grid_constant__ wdb_sa_rollout R) {
       }
       cur = qrow;
     }
+    if constexpr (kKind == kSaNoisyQ) {
+      // f(eps_in) * h into the spare activation row (lanes split i as the layers above), then
+      // lane j < A computes output j: the Q kind's mu-part, then the sigma part and f(eps_out)_j
+      const int in = s_dims[n_layers - 1], out = s_dims[n_layers];
+      const float *Wt = s_w + off, *bl = Wt + in * out;
+      const float *sw = s_act + kSaEnvsPerCta * 2 * kSaPitch, *sb = sw + out * in;
+      const bool noisy = !R.use_argmax;
+      // the noise key: log_std[1 .. 4] as raw words (seed, then the acting step of t = 0), read
+      // here rather than held across the loop (registers)
+      const uint32_t *kw = reinterpret_cast<const uint32_t *>(R.log_std) + 1;
+      const unsigned long long noise_seed =
+          (unsigned long long)kw[0] | ((unsigned long long)kw[1] << 32);
+      const unsigned long long step =
+          ((unsigned long long)kw[2] | ((unsigned long long)kw[3] << 32)) + (unsigned long long)t;
+      if (noisy) {
+        for (int i = sub; i < in; i += kSaGroup)
+          nxt[i] = sa_noise(noise_seed, step, (uint32_t)env, i) * cur[i];
+        __syncwarp();
+      }
+      float q = 0.0f;
+      if (sub < out) {
+        float a = bl[sub];
+        const float *wr = Wt;
+        for (int i = 0; i < in; i++, wr += out) a = fmaf(wr[sub], cur[i], a);
+        if (noisy) {
+          float sg = sb[sub];
+          for (int i = 0; i < in; i++) sg = fmaf(sw[sub * in + i], nxt[i], sg);
+          a = fmaf(sa_noise(noise_seed, step, (uint32_t)env, in + sub), sg, a);
+        }
+        q = a;
+      }
+      __syncwarp();                                     // every lane has read h
+      if (sub < out) cur[sub] = q;
+      __syncwarp();
+    }
     if (lead) {
       std::conditional_t<kContinuous, float, int> action;
       if constexpr (kKind == kSaSquashed) {
@@ -266,7 +320,8 @@ sa_rollout_kernel(const __grid_constant__ wdb_sa_rollout R) {
         action = o.action;
         static_cast<float *>(R.sampled_actions)[env] = action;
         if (R.actions_batch) static_cast<float *>(R.actions_batch)[(size_t)t * E + env] = action;
-      } else if constexpr (kKind == kSaEpsGreedy || kKind == kSaCategoricalQ) {
+      } else if constexpr (kKind == kSaEpsGreedy || kKind == kSaCategoricalQ ||
+                           kKind == kSaNoisyQ) {
         // Q head: the raw outputs are the Q values (categorical head: the expectations); the
         // stand-alone sampler's own rule, one draw of stream `env` per step (epsilon read once
         // above; use_argmax: 0, greedy)

@@ -330,6 +330,28 @@ class DuelingHead(ctypes.Structure):
     ]
 
 
+NOISY_MAX_LAYERS = 4
+
+
+class NoisyLayer(ctypes.Structure):
+    """struct wdb_noisy_layer (include/wdb200.h)."""
+
+    _fields_ = [
+        ("in_dim", _i), ("out_dim", _i),
+        ("weight_mu", _fp), ("weight_sigma", _fp), ("bias_mu", _fp), ("bias_sigma", _fp),
+        ("noise_in", _fp), ("noise_out", _fp), ("weight", _fp), ("bias", _fp),
+        ("grad_weight", _fp), ("grad_bias", _fp),
+        ("grad_weight_mu", _fp), ("grad_weight_sigma", _fp), ("grad_bias_mu", _fp),
+        ("grad_bias_sigma", _fp),
+    ]
+
+
+class NoisyNet(ctypes.Structure):
+    """struct wdb_noisy_net (include/wdb200.h)."""
+
+    _fields_ = [("n_layers", _i), ("layer", NoisyLayer * NOISY_MAX_LAYERS)]
+
+
 class PerStore(ctypes.Structure):
     """struct wdb_per_store (include/wdb200.h)."""
 
@@ -471,6 +493,11 @@ _SIGNATURES = {
     "wdb_dueling_fold": (
         _i, [_vp, ctypes.POINTER(DuelingHead), ctypes.POINTER(DuelingHead)]),
     "wdb_dueling_unfold_grads": (_i, [_vp, ctypes.POINTER(DuelingHead)]),
+    "wdb_noisy_supported": (_i, [ctypes.POINTER(NoisyNet)]),
+    "wdb_noisy_draw": (_i, [_vp, ctypes.POINTER(NoisyNet), _ull, _i, _ull, _i, _i]),
+    "wdb_noisy_materialize": (
+        _i, [_vp, ctypes.POINTER(NoisyNet), ctypes.POINTER(NoisyNet), _ull, _ull]),
+    "wdb_noisy_grads": (_i, [_vp, ctypes.POINTER(NoisyNet)]),
     "wdb_replay_sample_windows": (_i, [_vp, _vp, _i, _ull, _ull, _i, _i, _i, _i, _i]),
     "wdb_per_nodes": (_ll, [_ll]),
     "wdb_per_levels": (_i, [_ll]),
@@ -481,6 +508,7 @@ _SIGNATURES = {
         _i, [_vp, ctypes.POINTER(PerStore), _vp, _i, _vp, _vp, _i, _i]),
     "wdb_single_agent_rollout_supported": (_i, [_i, ctypes.POINTER(_i)]),
     "wdb_single_agent_rollout_categorical_supported": (_i, [_i, ctypes.POINTER(_i), _i]),
+    "wdb_single_agent_rollout_noisy_supported": (_i, [_i, ctypes.POINTER(_i)]),
     "wdb_single_agent_rollout": (_i, [_vp, ctypes.POINTER(SaRollout)]),
     "wdb_mountain_car_step": (
         _i, [_vp, _i, _vp, _vp, _vp, _vp, _vp] + [_f] * 7 + [_vp, _i]),

@@ -18,6 +18,9 @@ def _layers(model):
     if getattr(head, "is_dueling", False):
         raise TypeError("a dueling head has no one output layer: the native passes run its "
                         "folded layers (fused_dqn.FusedDuelingUpdate)")
+    if getattr(head, "is_noisy", False):
+        raise TypeError("a noisy head has no one weight: the native passes run its "
+                        "materialized layers (fused_dqn.FusedNoisyUpdate)")
     return [(model.fc[str(i)][0].weight, model.fc[str(i)][0].bias)
             for i in range(len(model.fc))] + [(head.weight, head.bias)]
 

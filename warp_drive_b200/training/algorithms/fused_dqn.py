@@ -7,8 +7,10 @@ arena.  `wdb_qr_dqn_update_sampled` does the same for quantile-regression DQN
 networks (FusedIQNUpdate), and `wdb_c51_update_sampled` (csrc/wdb_c51_update.cu) for categorical
 DQN (FusedC51Update).  A dueling DQN or C51 network runs the same passes on its folded network
 (FusedDuelingUpdate; csrc/wdb_dueling.cu folds the head before the pass and unfolds its gradients
-after it).  The torch autograd updates (algorithms/dqn.py) stay for the shapes these do not
-take."""
+after it).  A noisy DQN or C51 network, plain or dueling, runs them on its materialized head
+(FusedNoisyUpdate; csrc/wdb_noisy.cu draws the update's noise and writes the effective layers
+before the pass, and maps their gradients onto mu and sigma after it).  The torch autograd
+updates (algorithms/dqn.py) stay for the shapes these do not take."""
 import ctypes
 
 import torch
@@ -49,11 +51,11 @@ class FusedQUpdate:
     @classmethod
     def supported(cls, algo, q_net, n_envs, n_agents, capacity, replay_rows):
         """True if `wdb_<entry>` takes this policy: a `model` over a Box observation with at most
-        3 hidden layers and no dueling head (FusedDuelingUpdate), in the pass's envelope for
-        replay_rows sampled windows per update."""
+        3 hidden layers, no dueling head (FusedDuelingUpdate) and no noisy head
+        (FusedNoisyUpdate), in the pass's envelope for replay_rows sampled windows per update."""
         if type(q_net) is not cls.model or not isinstance(q_net.observation_space, Box):
             return False
-        if q_net.dueling or len(q_net.fc_dims) > 3:
+        if q_net.dueling or q_net.noisy or len(q_net.fc_dims) > 3:
             return False
         return cls.fits(_shape_struct(algo, q_net, n_envs, n_agents, capacity), q_net,
                         replay_rows)
@@ -221,12 +223,19 @@ def dueling_shape(head):
     return d
 
 
+def _live_stream(layer):
+    """(weight, bias, weight grad, bias grad) of a plain stream Linear."""
+    return layer.weight.data, layer.bias.data, layer.weight.grad, layer.bias.grad
+
+
 class DuelingFold:
     """A DuelingHead's folded layers in buffers of their own (and, with grads, buffers for their
-    gradients), and the struct wdb_dueling_head that ties them to the live stream parameters."""
+    gradients), and the struct wdb_dueling_head that ties them to the live stream parameters --
+    or, given `source` (a stream layer -> its (weight, bias, weight grad, bias grad)), to other
+    tensors of the streams' shapes (FusedNoisyUpdate: the materialized noisy layers)."""
 
-    def __init__(self, model, grads=False):
-        self.model = model
+    def __init__(self, model, grads=False, source=_live_stream):
+        self.model, self.source = model, source
         head = model.policy_head
         s, h, out = head.stream_dim, head.in_features, head.out_features
         shapes = ([(2 * s, h), (2 * s,)] if s else []) + [(out, 2 * s if s else h), (out,)]
@@ -246,11 +255,12 @@ class DuelingFold:
             for name, layer in (("h", hidden), ("o", out)):
                 if layer is None:
                     continue
-                setattr(d, prefix + name + "w", _lib.ptr(layer.weight.data))
-                setattr(d, prefix + name + "b", _lib.ptr(layer.bias.data))
+                w, b, gw, gb = self.source(layer)
+                setattr(d, prefix + name + "w", _lib.ptr(w))
+                setattr(d, prefix + name + "b", _lib.ptr(b))
                 if self.grads is not None:
-                    setattr(d, prefix + "g" + name + "w", _lib.ptr(layer.weight.grad))
-                    setattr(d, prefix + "g" + name + "b", _lib.ptr(layer.bias.grad))
+                    setattr(d, prefix + "g" + name + "w", _lib.ptr(gw))
+                    setattr(d, prefix + "g" + name + "b", _lib.ptr(gb))
         names = (["h"] if head.stream_dim else []) + ["o"]
         for name, (w, b) in zip(names, self.layers):
             setattr(d, name + "w", _lib.ptr(w))
@@ -299,6 +309,8 @@ class FusedDuelingUpdate:
         shared-memory cap."""
         if type(q_net) not in (FullyConnectedQ, FullyConnectedCategoricalQ) or not q_net.dueling:
             return False
+        if q_net.noisy:                        # FusedNoisyUpdate
+            return False
         if not isinstance(q_net.observation_space, Box) or len(folded_widths(q_net)) > 3:
             return False
         head = ctypes.byref(dueling_shape(q_net.policy_head))
@@ -334,9 +346,189 @@ class FusedDuelingUpdate:
         return self.sums
 
 
+NOISY_UPDATE, NOISY_ACTING = 0, 1            # the noise counter's domains (include/wdb200.h)
+
+
+class NoisyHead:
+    """A noisy network's head layers (FullyConnectedQ.noisy_layers()) as the struct
+    wdb_noisy_net, with their effective layers in buffers of their own and, with grads, scratch
+    for the effective layers' gradients."""
+
+    def __init__(self, model, grads=False):
+        self.model = model
+        self.noisy = model.noisy_layers()
+        dev = next(model.parameters()).device
+
+        def buffers():
+            return [(torch.zeros(L.out_features, L.in_features, device=dev),
+                     torch.zeros(L.out_features, device=dev)) for L in self.noisy]
+        self.layers = buffers()                  # [(W, b)], one per noisy layer
+        self.grads = buffers() if grads else None
+        self._index = {id(L): i for i, L in enumerate(self.noisy)}
+
+    @staticmethod
+    def shape(model):
+        n = _lib.NoisyNet()
+        layers = model.noisy_layers()
+        n.n_layers = len(layers)
+        if len(layers) > _lib.NOISY_MAX_LAYERS:
+            return None
+        for s, L in zip(n.layer, layers):
+            s.in_dim, s.out_dim = int(L.in_features), int(L.out_features)
+        return n
+
+    def _pointers(self):
+        tensors = [t for L in self.noisy for t in (L.weight_mu, L.weight_sigma, L.bias_mu,
+                                                    L.bias_sigma, L.noise_in, L.noise_out)]
+        tensors += [t for pair in self.layers + (self.grads or []) for t in pair]
+        if self.grads is not None:
+            tensors += [p.grad for L in self.noisy for p in (L.weight_mu, L.weight_sigma,
+                                                             L.bias_mu, L.bias_sigma)]
+        return tuple(None if t is None else t.data_ptr() for t in tensors)
+
+    def struct(self):
+        """The struct, rebuilt only when a tensor it points to has moved (load_state_dict keeps
+        storage; .to() does not)."""
+        key = self._pointers()
+        if getattr(self, "_cached", None) is None or self._cached[0] != key:
+            self._cached = (key, self._build())
+        return self._cached[1]
+
+    def _build(self):
+        n = self.shape(self.model)
+        for i, (s, L) in enumerate(zip(n.layer, self.noisy)):
+            s.weight_mu, s.weight_sigma = _lib.ptr(L.weight_mu.data), _lib.ptr(L.weight_sigma.data)
+            s.bias_mu, s.bias_sigma = _lib.ptr(L.bias_mu.data), _lib.ptr(L.bias_sigma.data)
+            s.noise_in, s.noise_out = _lib.ptr(L.noise_in), _lib.ptr(L.noise_out)
+            s.weight, s.bias = _lib.ptr(self.layers[i][0]), _lib.ptr(self.layers[i][1])
+            if self.grads is not None:
+                s.grad_weight, s.grad_bias = _lib.ptr(self.grads[i][0]), _lib.ptr(self.grads[i][1])
+                s.grad_weight_mu = _lib.ptr(L.weight_mu.grad)
+                s.grad_weight_sigma = _lib.ptr(L.weight_sigma.grad)
+                s.grad_bias_mu, s.grad_bias_sigma = (_lib.ptr(L.bias_mu.grad),
+                                                     _lib.ptr(L.bias_sigma.grad))
+        return n
+
+    def source(self, layer):
+        """A DuelingFold source: the effective layer (and gradient scratch) of a noisy stream
+        layer."""
+        i = self._index[id(layer)]
+        w, b = self.layers[i]
+        gw, gb = self.grads[i] if self.grads is not None else (None, None)
+        return w, b, gw, gb
+
+
+def draw_noise(model, seed, domain, count, row0=0, rows=None):
+    """wdb_noisy_draw into `rows` ([(noise_in [R, in], noise_out [R, out])] per noisy layer,
+    counter rows row0 .. row0 + R - 1) or, by default, into the layers' own buffers (R = 1):
+    one launch."""
+    layers = model.noisy_layers()
+    rows = rows if rows is not None else [(L.noise_in, L.noise_out) for L in layers]
+    n = NoisyHead.shape(model)
+    for s, (fi, fo) in zip(n.layer, rows):
+        s.noise_in, s.noise_out = _lib.ptr(fi), _lib.ptr(fo)
+    n_rows = rows[0][0].numel() // layers[0].in_features
+    _lib.check(_lib.load().wdb_noisy_draw(_lib.stream_ptr(), ctypes.byref(n), int(seed),
+                                          int(domain), int(count), int(row0), int(n_rows)),
+               "noisy_draw")
+
+
+def materialize(online, target, seed, update):
+    """wdb_noisy_materialize of two NoisyHeads (online: row 0, target: row 1): one launch."""
+    t = None if target is None else ctypes.byref(target.struct())
+    _lib.check(_lib.load().wdb_noisy_materialize(
+        _lib.stream_ptr(), ctypes.byref(online.struct()), t, int(seed), int(update)),
+        "noisy_materialize")
+
+
+def noisy_grads(head):
+    """wdb_noisy_grads of a NoisyHead with grads: one launch."""
+    _lib.check(_lib.load().wdb_noisy_grads(_lib.stream_ptr(), ctypes.byref(head.struct())),
+               "noisy_grads")
+
+
+class FusedNoisyUpdate:
+    """One update of a noisy DQN or C51 policy, plain or dueling: wdb_noisy_materialize of the
+    online and the target head under update `update`'s noise (1 launch), for a dueling head
+    wdb_dueling_fold of the materialized streams (1 launch), the plain pass -- FusedDQNUpdate or
+    FusedC51Update -- on the live trunk layers and the materialized (folded) head (2 launches),
+    wdb_dueling_unfold_grads into the streams' gradient scratch (1 launch, dueling), then
+    wdb_noisy_grads onto mu and sigma (1 launch).  Sums and outputs are the plain pass's."""
+
+    plain_type = staticmethod(FusedDuelingUpdate.plain_type)
+
+    @classmethod
+    def supported(cls, algo, q_net, n_envs, n_agents, capacity, replay_rows):
+        """True if a noisy FullyConnectedQ or FullyConnectedCategoricalQ's materialized network
+        (folded, for a dueling head) is in the plain pass's envelope."""
+        if type(q_net) not in (FullyConnectedQ, FullyConnectedCategoricalQ) or not q_net.noisy:
+            return False
+        if not isinstance(q_net.observation_space, Box):
+            return False
+        shape = NoisyHead.shape(q_net)
+        if shape is None or not _lib.load().wdb_noisy_supported(ctypes.byref(shape)):
+            return False
+        if q_net.dueling:
+            if len(folded_widths(q_net)) > 3:
+                return False
+            if not _lib.load().wdb_dueling_fold_supported(
+                    ctypes.byref(dueling_shape(q_net.policy_head))):
+                return False
+            u = _dueling_shape_struct(algo, q_net, n_envs, n_agents, capacity)
+        else:
+            if len(q_net.fc_dims) > 3:
+                return False
+            u = _shape_struct(algo, q_net, n_envs, n_agents, capacity)
+        return cls.plain_type(q_net).fits(u, q_net, replay_rows)
+
+    def __init__(self, algo, q_net, target_net, n_envs, n_agents, capacity, replay_rows, seed):
+        self.seed = int(seed)
+        self.online, self.target = NoisyHead(q_net, grads=True), NoisyHead(target_net)
+        self.dueling = q_net.dueling
+        if self.dueling:
+            self.fold_online = DuelingFold(q_net, grads=True, source=self.online.source)
+            self.fold_target = DuelingFold(target_net, source=self.target.source)
+            u = _dueling_shape_struct(algo, q_net, n_envs, n_agents, capacity)
+        else:
+            u = _shape_struct(algo, q_net, n_envs, n_agents, capacity)
+        self.plain = self.plain_type(q_net)(
+            algo, q_net, target_net, n_envs, n_agents, capacity, replay_rows, u=u,
+            point=self._point)
+        self.rows, self.sums = self.plain.rows, self.plain.sums
+
+    def _point(self, u):
+        pairs = ((u.q, self.online, getattr(self, "fold_online", None), True),
+                 (u.target_q, self.target, getattr(self, "fold_target", None), False))
+        for net, noisy, folded, grads in pairs:
+            fc = noisy.model.fc
+            trunk = [(fc[str(i)][0].weight, fc[str(i)][0].bias) for i in range(len(fc))]
+            head = folded.layers if folded is not None else noisy.layers
+            for i, (w, b) in enumerate(trunk + head):
+                net.w[i], net.b[i] = _lib.ptr(w.data), _lib.ptr(b.data)
+            if grads:
+                head = folded.grads if folded is not None else noisy.grads
+                for i, (w, b) in enumerate([(w.grad, b.grad) for w, b in trunk] + head):
+                    net.gw[i], net.gb[i] = _lib.ptr(w), _lib.ptr(b)
+
+    def launch(self, obs, actions, rewards, done, windows, outputs=None, weights=None, update=0):
+        """The network's gradient (trunk, mu and sigma) into its `.grad` under update `update`'s
+        noise; the other arguments are FusedQUpdate.launch's."""
+        materialize(self.online, self.target, self.seed, update)
+        if self.dueling:
+            fold(self.fold_online, self.fold_target)
+        self.plain.launch(obs, actions, rewards, done, windows, outputs, weights)
+        if self.dueling:
+            _lib.check(_lib.load().wdb_dueling_unfold_grads(
+                _lib.stream_ptr(), ctypes.byref(self.fold_online.struct())),
+                "dueling_unfold_grads")
+        noisy_grads(self.online)
+        return self.sums
+
+
 # The envelope checks by their function names: each is the class's `supported`.
 fused_dqn_supported = FusedDQNUpdate.supported
 fused_qr_dqn_supported = FusedQRDQNUpdate.supported
 fused_iqn_supported = FusedIQNUpdate.supported
 fused_c51_supported = FusedC51Update.supported
 fused_dueling_supported = FusedDuelingUpdate.supported
+fused_noisy_supported = FusedNoisyUpdate.supported

@@ -43,6 +43,8 @@ def _layers(model):
     out = [(model.fc[str(i)][0].weight, model.fc[str(i)][0].bias) for i in range(len(model.fc))]
     if getattr(model, "dueling", False):
         raise TypeError("a dueling head runs as its folded layers (DuelingFold)")
+    if getattr(model, "noisy", False):
+        raise TypeError("a noisy head has no one weight: it acts through the per-step path")
     # the discrete heads are an nn.ModuleList, the deterministic (tanh) head and a Q network's
     # head one nn.Linear
     single = model.is_deterministic or getattr(model, "is_q_network", False)
@@ -71,6 +73,11 @@ class FusedSingleAgentRollout:
                 return False
             if getattr(model, "action_mask", None) is not None:
                 return False
+            # a noisy head draws fresh noise per env and step: the noisy Q kind takes a plain
+            # head of one NoisyLinear; noisy C51 and noisy dueling heads act per step
+            noisy = getattr(model, "noisy", False)
+            if noisy and (model.dueling or getattr(model, "is_categorical_q", False)):
+                return False
             # a dueling head runs as its folded layers: the stacked 2S stream layer, if any,
             # then the A * N outputs
             widths = [int(d) for d in model.fc_dims]
@@ -88,11 +95,13 @@ class FusedSingleAgentRollout:
             if categorical:
                 return bool(_lib.load().wdb_single_agent_rollout_categorical_supported(
                     len(widths), arr, int(model.num_atoms)))
+            if noisy:
+                return bool(_lib.load().wdb_single_agent_rollout_noisy_supported(len(widths), arr))
             return bool(_lib.load().wdb_single_agent_rollout_supported(len(widths), arr))
         except Exception:  # noqa: BLE001
             return False
 
-    def __init__(self, env_wrapper, model, policy, sampler):
+    def __init__(self, env_wrapper, model, policy, sampler, engine=None):
         self.dm = dm = env_wrapper.cuda_data_manager
         self.env_wrapper = env_wrapper
         self.model = model
@@ -121,6 +130,12 @@ class FusedSingleAgentRollout:
             self._dueling = DuelingFold(m)
             layers = [(m.fc[str(i)][0].weight, m.fc[str(i)][0].bias)
                       for i in range(len(m.fc))] + self._dueling.layers
+        elif getattr(_unwrap(model), "noisy", False):
+            # a noisy Q head: the kernel runs mu as the head's layer and reads sigma from the
+            # device buffer below
+            m = _unwrap(model)
+            layers = [(m.fc[str(i)][0].weight, m.fc[str(i)][0].bias) for i in range(len(m.fc))]
+            layers.append((m.policy_head.weight_mu, m.policy_head.bias_mu))
         else:
             layers = _layers(model)
         # a distributional Q network (QR-DQN's, IQN's): the kernel runs epsilon-greedy over its
@@ -153,10 +168,18 @@ class FusedSingleAgentRollout:
         self.categorical = bool(getattr(_unwrap(model), "is_categorical_q", False))
         if self.categorical:
             self.A = int(_unwrap(model).output_dims[0])
+        # a noisy Q head (5): the kernel reads [epsilon, the noise key's four words, sigma_W,
+        # sigma_b] from the device, refreshed at every launch; the key is the engine's
+        # (`noise_seed`, `acting_steps`), so both rollout paths draw the same noise at the same
+        # acting step
+        self.noisy = bool(getattr(_unwrap(model), "noisy", False))
+        self.engine = engine
         if self.q_network:
             # the kernel reads epsilon from the device (the log_std field; the Q head is 3)
-            r.gaussian_head = 4 if self.categorical else 3
-            n = 1 + (int(_unwrap(model).num_atoms) if self.categorical else 0)
+            r.gaussian_head = 5 if self.noisy else 4 if self.categorical else 3
+            head = _unwrap(model).policy_head
+            n = (1 + (int(_unwrap(model).num_atoms) if self.categorical else 0)
+                 + (4 + head.weight_sigma.numel() + head.bias_sigma.numel() if self.noisy else 0))
             self._epsilon = torch.zeros(n, dtype=torch.float32, device=dm.device)
             r.log_std = _p(self._epsilon)
         if self.squashed:
@@ -197,6 +220,25 @@ class FusedSingleAgentRollout:
                 "reset pools need init_reset_pool(data_manager, seed) first")
         return table, n, resetter._pool_rng
 
+    def _noise_words(self, eps, use_argmax, n_steps):
+        """[epsilon, seed low, seed high, step low, step high] into the device buffer (one copy),
+        sigma_W and sigma_b after them; the policy's acting step advances by n_steps unless the
+        rollout is greedy (the mean network draws no noise)."""
+        import numpy as np
+
+        assert self.engine is not None, "a noisy head's rollout takes its noise key from the engine"
+        seed, step = int(self.engine.noise_seed), int(self.engine.acting_steps[self.policy])
+        words = np.array([0, seed, seed >> 32, step, step >> 32], dtype=np.uint64)
+        words = (words & 0xFFFFFFFF).astype(np.uint32)
+        words[0] = np.float32(eps).view(np.uint32)
+        self._epsilon.view(torch.int32)[:5].copy_(torch.from_numpy(words.view(np.int32)))
+        head = _unwrap(self.model).policy_head
+        n_w = head.weight_sigma.numel()
+        self._epsilon[5:5 + n_w].copy_(head.weight_sigma.detach().reshape(-1))
+        self._epsilon[5 + n_w:].copy_(head.bias_sigma.detach())
+        if not use_argmax:
+            self.engine.acting_steps[self.policy] += int(n_steps)
+
     def launch(self, n_steps, t0=0, record=True, uniforms=None, probs_out=None,
                use_argmax=False, reset_done_envs=True, damping=None, stddev=None, scale=None,
                normals=None, epsilon=None):
@@ -236,7 +278,10 @@ class FusedSingleAgentRollout:
             eps = float(0.0 if epsilon is None else epsilon)
             if not 0.0 <= eps <= 1.0:
                 raise ValueError(f"epsilon must be in [0, 1], got {epsilon}")
-            self._epsilon[0] = eps
+            if self.noisy:
+                self._noise_words(eps, use_argmax, n_steps)
+            else:
+                self._epsilon[0] = eps
             if self.categorical:
                 self._epsilon[1:].copy_(_unwrap(self.model).support)
         if record:

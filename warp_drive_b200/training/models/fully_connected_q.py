@@ -10,6 +10,12 @@ Dueling (Wang et al. 2016): with the model key `dueling: true` the head is a Due
 and advantage streams combined by the mean rule) with `stream_fc_dims` ([] or [S]) hidden
 layers per stream, for fully_connected_q and fully_connected_categorical_q.  Its forward has the
 plain head's column layout, so everything that reads the head's outputs works unchanged.
+
+Noisy networks (Fortunato et al. 2018): with the model key `noisy: true` every Linear layer of the
+head -- the plain head's output layer, or every stream layer of a DuelingHead -- is a NoisyLinear
+with factorized Gaussian noise (`noisy_sigma0`, 0.5 by default); the trunk stays plain.  A layer
+uses noise only while its `noise` is set (the update's sample, or per-row acting noise), and is
+the mean network otherwise, so the evaluator plays the mean network.
 """
 import math
 
@@ -41,6 +47,82 @@ def dueling_settings(model_config, model_type):
     return dueling, list(dims)
 
 
+def noisy_settings(model_config, model_type):
+    """(noisy, sigma0) of a Q model config, validated; `model_type` names the model in the
+    messages."""
+    noisy = model_config.get("noisy", False)
+    if not isinstance(noisy, bool):
+        raise ValueError(f"{model_type}'s model.noisy is true or false, got {noisy!r}")
+    if "noisy_sigma0" not in model_config:
+        return noisy, 0.5
+    s = model_config["noisy_sigma0"]
+    if not noisy:
+        raise ValueError(f"{model_type}'s model.noisy_sigma0 needs model.noisy: true, got "
+                         f"noisy_sigma0 {s!r} without it")
+    if isinstance(s, bool) or not isinstance(s, (int, float)) or not math.isfinite(s) or s <= 0:
+        raise ValueError(f"{model_type}'s model.noisy_sigma0 is a finite number > 0, got {s!r}")
+    return noisy, float(s)
+
+
+class NoisyLinear(nn.Module):
+    """Linear(in, out) with factorized Gaussian noise (Fortunato et al. 2018):
+        W = mu_W + sigma_W * (f(eps_out) f(eps_in)^T),  b = mu_b + sigma_b * f(eps_out),
+    f(x) = sgn(x) sqrt(|x|).  mu ~ U(+-1/sqrt(in)), sigma = sigma0 / sqrt(in).  The f(eps)
+    vectors of the update's sample are the non-persistent buffers `noise_in` [in] and
+    `noise_out` [out] (written by wdb_noisy_materialize or wdb_noisy_draw; checkpoints hold the
+    parameters only).  `noise` selects what forward uses: None (the mean network, mu only), the
+    buffers' sample (W, b as materialized()), or per-row acting noise ([..., in], [..., out]
+    matching the input's rows) in the factored form
+        y = mu_W x + mu_b + f(eps_out) * (sigma_W (f(eps_in) * x) + sigma_b)."""
+    is_noisy = True
+
+    def __init__(self, in_features, out_features, sigma0=0.5):
+        super().__init__()
+        self.in_features, self.out_features = in_features, out_features
+        bound = 1.0 / math.sqrt(in_features)
+        self.weight_mu = nn.Parameter(torch.empty(out_features, in_features).uniform_(-bound, bound))
+        self.weight_sigma = nn.Parameter(torch.full((out_features, in_features), sigma0 * bound))
+        self.bias_mu = nn.Parameter(torch.empty(out_features).uniform_(-bound, bound))
+        self.bias_sigma = nn.Parameter(torch.full((out_features,), sigma0 * bound))
+        self.register_buffer("noise_in", torch.zeros(in_features), persistent=False)
+        self.register_buffer("noise_out", torch.zeros(out_features), persistent=False)
+        self.noise = None
+
+    def materialized(self, noise_in=None, noise_out=None):
+        """(W, b) under the noise vectors (default: the buffers): the reference statement of
+        wdb_noisy_materialize, differentiable in the parameters."""
+        fi = self.noise_in if noise_in is None else noise_in
+        fo = self.noise_out if noise_out is None else noise_out
+        w = self.weight_mu + self.weight_sigma * (fo[:, None] * fi[None, :])
+        b = self.bias_mu + self.bias_sigma * fo
+        return w, b
+
+    def forward(self, x):
+        if self.noise is None:
+            return func.linear(x, self.weight_mu, self.bias_mu)
+        fi, fo = self.noise
+        if fi.dim() == 1:
+            return func.linear(x, *self.materialized(fi, fo))
+        rows = x.shape[:-1]
+        fi, fo = fi.reshape(*rows, -1), fo.reshape(*rows, -1)
+        return (func.linear(x, self.weight_mu, self.bias_mu)
+                + fo * func.linear(fi * x, self.weight_sigma, self.bias_sigma))
+
+
+def linear_layer(in_features, out_features, sigma0=None):
+    """nn.Linear, or a NoisyLinear when sigma0 is given."""
+    if sigma0 is None:
+        return nn.Linear(in_features, out_features)
+    return NoisyLinear(in_features, out_features, sigma0)
+
+
+def layer_params(layer):
+    """(weight, bias) of a Linear, or a NoisyLinear's materialized() under its noise buffers."""
+    if getattr(layer, "is_noisy", False):
+        return layer.materialized()
+    return layer.weight, layer.bias
+
+
 class DuelingHead(nn.Module):
     """The dueling head (Wang et al. 2016) over a trunk output h of width H, for A actions of N
     outputs each (N = 1: Q values; N atoms: C51's logits).  Each stream has one hidden Linear(H,
@@ -51,17 +133,17 @@ class DuelingHead(nn.Module):
     Parameters: `value.*` and `advantage.*` (Sequential(Linear, ReLU, Linear) or one Linear)."""
     is_dueling = True
 
-    def __init__(self, in_features, n_actions, n_outputs, stream_dim):
+    def __init__(self, in_features, n_actions, n_outputs, stream_dim, sigma0=None):
         super().__init__()
         self.in_features, self.n_actions, self.n_outputs = in_features, n_actions, n_outputs
         self.stream_dim = stream_dim
         self.out_features = n_actions * n_outputs
 
-        def stream(width):
+        def stream(width):       # sigma0: every stream layer is a NoisyLinear
             if stream_dim == 0:
-                return nn.Linear(in_features, width)
-            return nn.Sequential(nn.Linear(in_features, stream_dim), nn.ReLU(),
-                                 nn.Linear(stream_dim, width))
+                return linear_layer(in_features, width, sigma0)
+            return nn.Sequential(linear_layer(in_features, stream_dim, sigma0), nn.ReLU(),
+                                 linear_layer(stream_dim, width, sigma0))
         self.value = stream(n_outputs)
         self.advantage = stream(n_actions * n_outputs)
 
@@ -83,20 +165,22 @@ class DuelingHead(nn.Module):
     def folded(self):
         """[(weight, bias)] of the plain layers this head equals: the stacked stream hidden
         layer ([2S, H], S > 0) and the output layer [A * N, 2S or H] -- the reference statement of
-        the fold (wdb_dueling_fold).  Differentiable in the stream parameters."""
+        the fold (wdb_dueling_fold).  Differentiable in the stream parameters.  Noisy streams fold
+        their materialized() layers."""
         A, N = self.n_actions, self.n_outputs
-        (vh, vo), (ah, ao) = self.streams()
+        (vh, vo), (ah, ao) = [tuple(None if x is None else layer_params(x) for x in pair)
+                              for pair in self.streams()]
 
         def centred(x):                    # rows a * N + j minus the mean over a
             y = x.reshape(A, N, *x.shape[1:])
             return (y - y.mean(dim=0, keepdim=True)).reshape(x.shape)
         if self.stream_dim == 0:
-            w = vo.weight.repeat(A, 1) + centred(ao.weight)
-            b = vo.bias.repeat(A) + centred(ao.bias)
+            w = vo[0].repeat(A, 1) + centred(ao[0])
+            b = vo[1].repeat(A) + centred(ao[1])
             return [(w, b)]
-        hidden = (torch.cat([vh.weight, ah.weight]), torch.cat([vh.bias, ah.bias]))
-        w = torch.cat([vo.weight.repeat(A, 1), centred(ao.weight)], dim=1)
-        b = vo.bias.repeat(A) + centred(ao.bias)
+        hidden = (torch.cat([vh[0], ah[0]]), torch.cat([vh[1], ah[1]]))
+        w = torch.cat([vo[0].repeat(A, 1), centred(ao[0])], dim=1)
+        b = vo[1].repeat(A) + centred(ao[1])
         return [hidden, (w, b)]
 
 
@@ -125,19 +209,27 @@ class FullyConnectedQ(nn.Module):
         self.flattened_obs_size = get_flattened_obs_size(self.observation_space)
         self.output_dims = [int(heads[0])]
         dims = [self.flattened_obs_size] + self.fc_dims
-        self.dueling, self.stream_fc_dims = dueling_settings(
-            model_config, model_config.get("type", "fully_connected_q"))
+        model_type = model_config.get("type", "fully_connected_q")
+        self.dueling, self.stream_fc_dims = dueling_settings(model_config, model_type)
+        self.noisy, self.noisy_sigma0 = noisy_settings(model_config, model_type)
         self.fc = nn.ModuleDict({
             str(i): nn.Sequential(nn.Linear(dims[i], dims[i + 1]), nn.ReLU())
             for i in range(len(self.fc_dims))})
         self.policy_head = self._head(dims[-1], 1)
 
     def _head(self, in_features, n_outputs):
-        """The head of A * n_outputs raw outputs: one Linear, or a DuelingHead."""
+        """The head of A * n_outputs raw outputs: one Linear, or a DuelingHead (noisy: of
+        NoisyLinear layers)."""
         A = self.output_dims[0]
+        sigma0 = self.noisy_sigma0 if self.noisy else None
         if self.dueling:
-            return DuelingHead(in_features, A, n_outputs, sum(self.stream_fc_dims))
-        return nn.Linear(in_features, A * n_outputs)
+            return DuelingHead(in_features, A, n_outputs, sum(self.stream_fc_dims), sigma0)
+        return linear_layer(in_features, A * n_outputs, sigma0)
+
+    def noisy_layers(self):
+        """The head's NoisyLinear layers in module order (the `layer` of their noise counter);
+        [] for a plain network."""
+        return [m for m in self.policy_head.modules() if getattr(m, "is_noisy", False)]
 
     def q_values(self, obs):
         """Q(obs, a) for every action: [..., A]."""
@@ -151,10 +243,16 @@ class FullyConnectedQ(nn.Module):
 
 
 def _refuse_dueling(model_config, model_type):
-    """QR-DQN's collapsed head and IQN's post-merge head would each need a fold of their own."""
+    """QR-DQN's collapsed head and IQN's post-merge head would each need a fold of their own, and
+    a noise map of their own."""
     for key in ("dueling", "stream_fc_dims"):
         if key in model_config and model_config[key] not in (False, None):
             raise ValueError(f"{model_type} does not take model.{key} (dueling heads are "
+                             f"fully_connected_q's and fully_connected_categorical_q's), got "
+                             f"{model_config[key]!r}")
+    for key in ("noisy", "noisy_sigma0"):
+        if key in model_config and model_config[key] not in (False, None):
+            raise ValueError(f"{model_type} does not take model.{key} (noisy heads are "
                              f"fully_connected_q's and fully_connected_categorical_q's), got "
                              f"{model_config[key]!r}")
 

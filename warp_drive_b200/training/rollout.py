@@ -95,6 +95,19 @@ class RolloutEngine:
         self.q_network = any(self.q_of.values())
         assert self.separate or len(set(self.q_of.values())) == 1, (
             "policies sharing the step placeholders are all Q networks or none is")
+        # noisy Q networks (FullyConnectedQ with `noisy: true`): before each forward of the
+        # per-step path, one wdb_noisy_draw launch per policy writes fresh factorized noise for
+        # every env row, keyed by `noise_seed` (set by the trainer) and the policy's acting step
+        # `acting_steps[p]`, a host counter.  DQN rollouts always pass sample params, so this path
+        # runs eagerly and is never captured into a CUDA graph (rollout() does not capture a
+        # noisy policy either).  The one-launch rollout's noisy Q kind draws the same noise from
+        # the same key and advances the same counter.  Greedy steps (use_argmax) play the mean
+        # network and draw nothing.
+        self.noisy_of = {p: bool(getattr(models[p], "noisy", False)) for p in self.policies}
+        self.noisy = any(self.noisy_of.values())
+        self.noise_seed = 0
+        self.acting_steps = {p: 0 for p in self.policies}
+        self._acting_noise = {}
         # observations reach the policies through wdb_gather_policy_fields unless they are one
         # shared [E, N, F] Box array (wdb_gather_policy_rows)
         self.gather_fields = (self.separate or self.agents_last
@@ -139,7 +152,8 @@ class RolloutEngine:
             if (self.T >= 1
                     and FusedSingleAgentRollout.eligible(env_wrapper, models, self.policy_map)):
                 p0 = self.policies[0]
-                self.sa = FusedSingleAgentRollout(env_wrapper, models[p0], p0, sampler)
+                self.sa = FusedSingleAgentRollout(env_wrapper, models[p0], p0, sampler,
+                                                  engine=self)
                 self.sa.set_bookkeeping(
                     self.reward_running_sum, self.episodic_reward_sum, self.step_running_sum,
                     self.episodic_step_sum, self.num_completed_episodes)
@@ -713,6 +727,31 @@ class RolloutEngine:
         self.step_running_sum.mul_(1 - done)
         self.num_completed_episodes.add_(done.sum())
 
+    def _set_acting_noise(self):
+        """Fresh per-row noise for every noisy policy's head (one launch each), set on its
+        NoisyLinear layers; returns the layers."""
+        from warp_drive_b200.training.algorithms.fused_dqn import NOISY_ACTING, draw_noise
+
+        layers = []
+        for p in self.policies:
+            if not self.noisy_of[p]:
+                continue
+            model = self.models[p]
+            noisy = model.noisy_layers()
+            if p not in self._acting_noise:
+                rows = self.E * len(self.policy_map[p])
+                dev = self.dm.device
+                self._acting_noise[p] = [
+                    (torch.empty(rows, L.in_features, device=dev),
+                     torch.empty(rows, L.out_features, device=dev)) for L in noisy]
+            draw_noise(model, self.noise_seed, NOISY_ACTING, self.acting_steps[p],
+                       rows=self._acting_noise[p])
+            self.acting_steps[p] += 1
+            for L, pair in zip(noisy, self._acting_noise[p]):
+                L.noise = pair
+            layers += noisy
+        return layers
+
     def step(self, t, **sample_params):
         if self.fused is not None and not sample_params:
             return self.step_fused(t)
@@ -720,8 +759,18 @@ class RolloutEngine:
             with torch.no_grad():
                 self.sa.launch(1, t0=max(self._slot(t), 0), record=t >= 0, **sample_params)
             return None
+        greedy = False
+        if self.q_network:                     # use_argmax: the mean network, epsilon 0
+            greedy = bool(sample_params.pop("use_argmax", False))
+            if greedy:
+                sample_params["epsilon"] = 0.0
         with torch.no_grad():
-            probs = self.evaluate_policies(t)
+            noisy = self._set_acting_noise() if self.noisy and not greedy else []
+            try:
+                probs = self.evaluate_policies(t)
+            finally:
+                for L in noisy:
+                    L.noise = None
             self.sample_actions(probs, t, **sample_params)
             self.env_wrapper.step_all_envs()
             self.bookkeep(t)
@@ -748,7 +797,7 @@ class RolloutEngine:
             with torch.no_grad():
                 self.sa.launch(self.T, t0=0, record=True, **sample_params)
             return
-        if not self.use_cuda_graph or sample_params:
+        if not self.use_cuda_graph or sample_params or self.noisy:
             self._rollout_eager(**sample_params)
             return
         if self._graph is None:

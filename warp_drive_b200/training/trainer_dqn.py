@@ -53,6 +53,18 @@ Per update the native path folds the online and target heads (wdb_dueling_fold, 
 the plain pass on the folded network (2 launches) and unfolds its head gradients onto the two
 streams (wdb_dueling_unfold_grads, 1 launch); shapes outside the pass's envelope train through
 torch autograd on the DuelingHead.
+
+Noisy networks: a `fully_connected_q` or `fully_connected_categorical_q` model with `noisy: true`
+(plain or dueling) explores through factorized Gaussian noise on its head.  Per update the native
+path (FusedNoisyUpdate) draws one sample for the online head and an independent one for the
+target, keyed by the trainer seed and the policy's update count, and writes the effective layers
+(wdb_noisy_materialize, 1 launch), runs the plain or dueling pass on them, and maps their
+gradients onto mu and sigma (wdb_noisy_grads, 1 launch); the online sample serves obs and obs'
+alike, the double-Q argmax included.  The torch path draws the same sample into the layers' noise
+buffers (wdb_noisy_draw) and differentiates through NoisyLinear.materialized().  Acting draws
+fresh noise per env row and step on the rollout engine's per-step path; the evaluator plays the
+mean network.  Logging iterations add `Noisy sigma`, the mean |sigma_W| over the head's noisy
+layers.
 """
 import os
 
@@ -61,7 +73,8 @@ import torch
 from warp_drive_b200.training.algorithms.dqn import (
     DQN, CategoricalDQN, ImplicitQuantileDQN, QuantileDQN)
 from warp_drive_b200.training.algorithms.fused_dqn import (
-    FusedC51Update, FusedDQNUpdate, FusedDuelingUpdate, FusedIQNUpdate, FusedQRDQNUpdate)
+    NOISY_UPDATE, FusedC51Update, FusedDQNUpdate, FusedDuelingUpdate, FusedIQNUpdate,
+    FusedNoisyUpdate, FusedQRDQNUpdate, draw_noise)
 from warp_drive_b200.training.trainer_ddpg import (
     RingRolloutEngine, TrainerDDPG, hard_update, soft_update)
 from warp_drive_b200.training.utils.param_scheduler import ParamScheduler
@@ -221,19 +234,22 @@ class TrainerDQN(TrainerDDPG):
             if self._tau_generator is None:
                 self._tau_generator = torch.Generator(device=dev)
                 self._tau_generator.manual_seed(self.seed)
-        fused = (FusedDuelingUpdate if q_net.dueling else FusedC51Update if categorical
-                 else FusedIQNUpdate if implicit else FusedQRDQNUpdate if quantile
-                 else FusedDQNUpdate)
+        fused = (FusedNoisyUpdate if q_net.noisy else FusedDuelingUpdate if q_net.dueling
+                 else FusedC51Update if categorical else FusedIQNUpdate if implicit
+                 else FusedQRDQNUpdate if quantile else FusedDQNUpdate)
         if fused.supported(algo, q_net, self.num_envs, n_agents, self.ring_capacity, rows):
+            extra = (self.seed,) if q_net.noisy else ()
             self.fused_updates[policy] = fused(
                 algo, q_net, self.target_q_models[policy], self.num_envs, n_agents,
-                self.ring_capacity, rows)
+                self.ring_capacity, rows, *extra)
 
     def _make_engine(self, use_cuda_graph):
-        return RingRolloutEngine(
+        engine = RingRolloutEngine(
             self.cuda_envs, self.q_models, self.policy_tag_to_agent_id_map,
             self.cuda_sample_controller, self.training_batch_size_per_env,
             ring_capacity=self.ring_capacity)
+        engine.noise_seed = self.seed          # acting noise: this rank's seed
+        return engine
 
     # ------------------------------------------------------------------ update
     def _ring_state(self):
@@ -253,6 +269,12 @@ class TrainerDQN(TrainerDDPG):
             for metrics in metrics_dict.values():
                 metrics["Epsilon"] = float(self.last_epsilon)
         for policy, metrics in metrics_dict.items():
+            noisy = self.q_models[policy].noisy_layers()
+            if noisy:                          # how far the head has annealed its noise
+                with torch.no_grad():
+                    total = sum(L.weight_sigma.abs().double().sum() for L in noisy)
+                    count = sum(L.weight_sigma.numel() for L in noisy)
+                metrics["Noisy sigma"] = float(total / count)
             store = self.priority_stores.get(policy)
             if store is not None and "Q loss" in metrics:   # the last update's sample
                 metrics["Priority beta"] = float(store.beta)
@@ -304,10 +326,20 @@ class TrainerDQN(TrainerDDPG):
         wdb_c51_update_sampled for a distributional network), accumulated into the arena's .grad views."""
         algo = self.trainers[policy]
         store = self.priority_stores.get(policy)
-        loss, q, returns = algo.loss(self.q_models[policy], self.target_q_models[policy],
-                                     *self._gather_windows(policy),
-                                     weights=None if store is None else store.weights,
-                                     **self._levels(policy))
+        nets = (self.q_models[policy], self.target_q_models[policy])
+        noisy = [L for net in nets for L in net.noisy_layers()]
+        for row, net in enumerate(nets):       # FusedNoisyUpdate's sample of this update
+            if net.noisy:
+                draw_noise(net, self.seed, NOISY_UPDATE, self.update_count[policy], row0=row)
+        for L in noisy:
+            L.noise = (L.noise_in, L.noise_out)
+        try:
+            loss, q, returns = algo.loss(*nets, *self._gather_windows(policy),
+                                         weights=None if store is None else store.weights,
+                                         **self._levels(policy))
+        finally:
+            for L in noisy:
+                L.noise = None
         if store is not None:                  # the inputs of the new priorities
             store.q_values.copy_(q.detach())
             store.returns.copy_(returns)
@@ -319,8 +351,8 @@ class TrainerDQN(TrainerDDPG):
 
     def _fused_q_gradients(self, policy, fused, logging_flag):
         """The same gradient from the native pass (FusedDQNUpdate, FusedQRDQNUpdate,
-        FusedIQNUpdate, FusedC51Update or FusedDuelingUpdate), written straight into the arena's .grad views; the host waits only on
-        logging iterations (metrics)."""
+        FusedIQNUpdate, FusedC51Update, FusedDuelingUpdate or FusedNoisyUpdate), written straight
+        into the arena's .grad views; the host waits only on logging iterations (metrics)."""
         eng = self.engine
         outputs, weights = None, None
         store = self.priority_stores.get(policy)
@@ -333,7 +365,9 @@ class TrainerDQN(TrainerDDPG):
                             eng._tensor(f"{_ACTIONS}_batch_{policy}"),
                             eng._tensor(f"{_REWARDS}_batch_{policy}"),
                             eng._tensor(f"{_DONE_FLAGS}_batch"), self.replay_windows[policy],
-                            outputs, weights, **self._levels(policy))
+                            outputs, weights, **self._levels(policy),
+                            **({"update": self.update_count[policy]}
+                               if isinstance(fused, FusedNoisyUpdate) else {}))
         if not logging_flag:
             return {}
         s = sums.tolist()
