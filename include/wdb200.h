@@ -129,6 +129,19 @@ int wdb_sample_epsilon_greedy(void *stream, void *rng_state, const float *q_valu
                               int *actions, long long n_rows, int n_actions, float epsilon,
                               const unsigned int *words);
 
+/* wdb_sample_epsilon_greedy over the valid actions of action_mask [n_rows, n_actions] (float32,
+ * non-zero = valid): the same draw (one Philox block per row on stream r, the offset advanced by
+ * 1, or the words hook) and the same u.  With n_valid the row's valid actions, the row explores
+ * iff u <= epsilon, with the k-th valid action in ascending index order, k = high word of
+ * y * n_valid; otherwise it takes the first index of the maximum Q value among the valid
+ * actions.  A row with no valid action takes wdb_sample_epsilon_greedy's action (the device
+ * can neither refuse it nor report it without a host wait).  An all-ones mask gives
+ * wdb_sample_epsilon_greedy's actions and offsets bit for bit.  One launch.
+ * cudaErrorInvalidValue unless 0 <= epsilon <= 1, or if action_mask is NULL. */
+int wdb_sample_epsilon_greedy_masked(void *stream, void *rng_state, const float *q_values,
+                                     const float *action_mask, int *actions, long long n_rows,
+                                     int n_actions, float epsilon, const unsigned int *words);
+
 /* ------------------------------------------------------------------ reset ---- */
 /* Replaces reset_in_{float,int}_when_done_{2d,3d} + undo_done_flag_and_reset_timestep
  * (warp_drive/cuda_includes/core/reset.cu:9-75; one launch per registered array in
@@ -1138,6 +1151,33 @@ long long wdb_c51_update_sampled_workspace_bytes(const wdb_dqn_update_args *upda
 int wdb_c51_update_sampled(void *stream, const wdb_dqn_update_args *update, int n_atoms,
                            const float *support, float delta_z,
                            const wdb_replay_windows *windows, const float *weights);
+
+/* Action masks (DQN and C51).  action_mask [C, E, Np, A] (float32, non-zero = valid) is the
+ * ring's mask array beside obs: the row at a window's slot(n_step) is obs' own mask.  The
+ * bootstrap's a* -- the double-Q argmax of online(obs'), DQN's max_a' target(obs') and C51's
+ * argmax of the expectation -- ranges over the valid actions of that row only; a row with no
+ * valid action takes every action (the unmasked rule: the device can neither refuse it nor
+ * report it without a host wait).  The loss row is unchanged: the action at slot(0) was chosen
+ * under its own mask.  The mask is read by the bootstrap alone, and an all-ones mask gives the
+ * unmasked pass's bits.  weights NULL: the uniform pass; else the importance-weighted one.
+ * Shapes, workspace, sums, outputs and launches (two) are the unmasked pass's. */
+int wdb_dqn_update_masked_supported(const wdb_dqn_update_args *update, int n_windows);
+long long wdb_dqn_update_masked_workspace_bytes(const wdb_dqn_update_args *update,
+                                                int n_windows);
+/* wdb_dqn_update_sampled / _prioritized with the masked bootstrap.  cudaErrorInvalidValue
+ * without launching if unsupported or a required pointer (action_mask included) is NULL. */
+int wdb_dqn_update_masked(void *stream, const wdb_dqn_update_args *update,
+                          const wdb_replay_windows *windows, const float *weights,
+                          const float *action_mask);
+int wdb_c51_update_masked_supported(const wdb_dqn_update_args *update, int n_atoms,
+                                    int n_windows);
+long long wdb_c51_update_masked_workspace_bytes(const wdb_dqn_update_args *update, int n_atoms,
+                                                int n_windows);
+/* wdb_c51_update_sampled with the masked a*.  cudaErrorInvalidValue without launching if
+ * unsupported, a required pointer (action_mask included) is NULL or delta_z <= 0. */
+int wdb_c51_update_masked(void *stream, const wdb_dqn_update_args *update, int n_atoms,
+                          const float *support, float delta_z, const wdb_replay_windows *windows,
+                          const float *weights, const float *action_mask);
 
 /* Dueling head (Wang et al. 2016, the mean combine) of a DQN or C51 network, and its fold into
  * the plain MLP head the passes above run.  The head reads the trunk output h (width H) through

@@ -377,6 +377,7 @@ _SIGNATURES = {
     "wdb_sample_squashed_gaussian": (
         _i, [_vp, _vp, _vp, _vp, _ll, _i, _f, _f, _f, _f, _i, _vp]),
     "wdb_sample_epsilon_greedy": (_i, [_vp, _vp, _vp, _vp, _ll, _i, _f, _vp]),
+    "wdb_sample_epsilon_greedy_masked": (_i, [_vp, _vp, _vp, _vp, _vp, _ll, _i, _f, _vp]),
     "wdb_reset_when_done": (_i, [_vp, _vp, _i, _vp, _vp, _i, _i, _i, _vp]),
     "wdb_reset_log_mask": (_i, [_vp, _vp, _i]),
     "wdb_update_log_mask": (_i, [_vp, _vp, _i, _i]),
@@ -488,6 +489,15 @@ _SIGNATURES = {
     "wdb_c51_update_sampled_workspace_bytes": (_ll, [ctypes.POINTER(DqnUpdate), _i, _i]),
     "wdb_c51_update_sampled": (
         _i, [_vp, ctypes.POINTER(DqnUpdate), _i, _vp, _f, ctypes.POINTER(ReplayWindows), _vp]),
+    "wdb_dqn_update_masked_supported": (_i, [ctypes.POINTER(DqnUpdate), _i]),
+    "wdb_dqn_update_masked_workspace_bytes": (_ll, [ctypes.POINTER(DqnUpdate), _i]),
+    "wdb_dqn_update_masked": (
+        _i, [_vp, ctypes.POINTER(DqnUpdate), ctypes.POINTER(ReplayWindows), _vp, _vp]),
+    "wdb_c51_update_masked_supported": (_i, [ctypes.POINTER(DqnUpdate), _i, _i]),
+    "wdb_c51_update_masked_workspace_bytes": (_ll, [ctypes.POINTER(DqnUpdate), _i, _i]),
+    "wdb_c51_update_masked": (
+        _i, [_vp, ctypes.POINTER(DqnUpdate), _i, _vp, _f, ctypes.POINTER(ReplayWindows), _vp,
+             _vp]),
     "wdb_dueling_fold_supported": (_i, [ctypes.POINTER(DuelingHead)]),
     "wdb_dueling_unfold_grads_supported": (_i, [ctypes.POINTER(DuelingHead)]),
     "wdb_dueling_fold": (

@@ -549,13 +549,17 @@ class CUDASampler:
             "sample_squashed_gaussian")
 
     def sample_epsilon_greedy(self, q_values: torch.Tensor, actions: torch.Tensor,
-                              epsilon: float = 0.0, words=None):
+                              epsilon: float = 0.0, words=None, action_mask=None):
         """Epsilon-greedy over Q values (DQN): q_values [n_envs, n_agents, A] float32 ->
         actions [n_envs, n_agents, 1] int32.  Row r of the [n_envs * n_agents] rows draws one
         Philox block on RNG stream r (its offset advances by 1) and explores iff the uniform of
         its first word is <= epsilon, with the action high(second word * A); otherwise it takes
         the first maximum of its Q values (wdb_sample_epsilon_greedy).  `words` (int32
-        [n_envs, n_agents, 2], the two words of each row) is a test hook replacing the draw."""
+        [n_envs, n_agents, 2], the two words of each row) is a test hook replacing the draw.
+        `action_mask` (float32 [n_envs, n_agents, A], non-zero = valid): the same draw over the
+        row's valid actions only, the k-th valid one when exploring and the first maximum among
+        them otherwise; a row with none valid takes the unmasked action
+        (wdb_sample_epsilon_greedy_masked)."""
         assert self._random_initialized, (
             "sample_epsilon_greedy() requires the random seed initialized first, call "
             "init_random()")
@@ -569,6 +573,14 @@ class CUDASampler:
             assert tuple(words.shape) == tuple(q_values.shape[:-1]) + (2,)
             assert words.dtype == torch.int32 and words.is_contiguous()
         q_values = q_values.detach().float().contiguous()
+        if action_mask is not None:
+            assert tuple(action_mask.shape) == tuple(q_values.shape)
+            assert action_mask.dtype == torch.float32 and action_mask.is_contiguous()
+            _libmod.check(_libmod.load().wdb_sample_epsilon_greedy_masked(
+                _stream(), _P(self.rng_state), _P(q_values), _P(action_mask), _P(actions),
+                int(q_values.shape[0] * q_values.shape[1]), int(q_values.shape[-1]),
+                float(epsilon), _P(words)), "sample_epsilon_greedy_masked")
+            return
         _libmod.check(_libmod.load().wdb_sample_epsilon_greedy(
             _stream(), _P(self.rng_state), _P(q_values), _P(actions),
             int(q_values.shape[0] * q_values.shape[1]), int(q_values.shape[-1]),

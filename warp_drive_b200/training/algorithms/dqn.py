@@ -6,9 +6,24 @@ shapes the native pass does not take, and tests/dqn_update_reference.py restates
 NumPy.  QuantileDQN is quantile-regression DQN on the same windows (wdb_qr_dqn_update_sampled,
 tests/qr_dqn_reference.py), ImplicitQuantileDQN implicit quantile networks
 (wdb_iqn_update_sampled, tests/iqn_reference.py), CategoricalDQN categorical DQN
-(wdb_c51_update_sampled, tests/c51_reference.py)."""
+(wdb_c51_update_sampled, tests/c51_reference.py).
+
+Action masks: every loss takes `boot_mask` [B, A], obs' own action mask; the bootstrap's argmax /
+max then ranges over its valid actions (masked_scores), the rule of wdb_dqn_update_masked and
+wdb_c51_update_masked.  None gives the unmasked ops."""
 import torch
 from torch.nn import functional as func
+
+
+def masked_scores(scores, boot_mask):
+    """scores [B, A] with the actions boot_mask [B, A] marks invalid (zero) at -inf, for the
+    bootstrap's argmax / max over obs' valid actions; a row with no valid action keeps every
+    action (the unmasked rule).  boot_mask None: scores itself."""
+    if boot_mask is None:
+        return scores
+    valid = boot_mask != 0
+    valid = valid | ~valid.any(dim=-1, keepdim=True)
+    return scores.masked_fill(~valid, float("-inf"))
 
 
 class DQN:
@@ -39,25 +54,28 @@ class DQN:
             r = live[j] * self.discount_factor_gamma * r + rewards[j]
         return r
 
-    def bootstrap(self, q_net, target_net, boot_obs):
+    def bootstrap(self, q_net, target_net, boot_obs, boot_mask=None):
         """The bootstrap value [B] at the windows' last observation (no gradient):
         target(obs')[argmax online(obs')] with double_q (the first maximum), else
-        max target(obs')."""
+        max target(obs').  boot_mask [B, A]: obs' own action mask; the argmax / max range over
+        its valid actions (masked_scores)."""
         with torch.no_grad():
             q_target = target_net.q_values(boot_obs)
             if self.double_q:
-                best = q_net.q_values(boot_obs).argmax(dim=-1, keepdim=True)
+                best = masked_scores(q_net.q_values(boot_obs), boot_mask).argmax(
+                    dim=-1, keepdim=True)
                 return q_target.gather(-1, best)[..., 0]
-            return q_target.max(dim=-1).values
+            return masked_scores(q_target, boot_mask).max(dim=-1).values
 
-    def loss(self, q_net, target_net, obs, actions, rewards, done, boot_obs, weights=None):
+    def loss(self, q_net, target_net, obs, actions, rewards, done, boot_obs, weights=None,
+             boot_mask=None):
         """(Huber loss, Q(obs, a) [B], R [B]) of B sampled windows: obs [B, F], actions [B, 1]
         (int), rewards / done [n_step, B], boot_obs [B, F].  weights [B]: prioritized replay's
         importance-sampling weights, the loss (1/B) sum w_g huber(Q_g - R_g) of
-        wdb_dqn_update_prioritized."""
+        wdb_dqn_update_prioritized.  boot_mask [B, A]: obs' action mask (wdb_dqn_update_masked)."""
         with torch.no_grad():
-            returns = self.sampled_returns(rewards, done, self.bootstrap(q_net, target_net,
-                                                                         boot_obs))
+            returns = self.sampled_returns(rewards, done, self.bootstrap(
+                q_net, target_net, boot_obs, boot_mask))
         q = q_net.q_values(obs).gather(-1, actions.long().reshape(-1, 1))[..., 0]
         if weights is None:
             loss = func.huber_loss(q, returns, delta=self.huber_delta)
@@ -80,16 +98,18 @@ class QuantileDQN(DQN):
     FullyConnectedQuantileQ, restated in float64 NumPy by tests/qr_dqn_reference.py.
     `huber_delta` is the quantile Huber loss's kappa."""
 
-    def bootstrap_quantiles(self, q_net, target_net, boot_obs):
+    def bootstrap_quantiles(self, q_net, target_net, boot_obs, boot_mask=None):
         """target(obs')[a*] [B, N] (no gradient), a* the first argmax of the mean quantile of
-        online(obs') with double_q, else of target(obs')."""
+        online(obs') with double_q, else of target(obs'); over obs' valid actions with
+        boot_mask [B, A]."""
         with torch.no_grad():
             boot = target_net.quantiles(boot_obs)
             chooser = q_net.quantiles(boot_obs) if self.double_q else boot
-            best = chooser.mean(dim=-1).argmax(dim=-1)
+            best = masked_scores(chooser.mean(dim=-1), boot_mask).argmax(dim=-1)
             return boot[torch.arange(boot.shape[0], device=boot.device), best]
 
-    def loss(self, q_net, target_net, obs, actions, rewards, done, boot_obs, weights=None):
+    def loss(self, q_net, target_net, obs, actions, rewards, done, boot_obs, weights=None,
+             boot_mask=None):
         """(quantile Huber loss, Q-bar [B], R-bar [B]) of B sampled windows, the arguments of
         DQN.loss.  theta_i = quantiles(obs)[a, i] at tau_i = (2i + 1) / (2N), T_j the n-step
         recursion on each bootstrap quantile, u_ij = T_j - theta_i, and the row loss
@@ -97,7 +117,7 @@ class QuantileDQN(DQN):
         over rows of w_g times it (w = 1 without weights).  Q-bar = mean_i theta_i and
         R-bar = mean_j T_j feed the metrics and the priorities."""
         with torch.no_grad():
-            boot = self.bootstrap_quantiles(q_net, target_net, boot_obs)
+            boot = self.bootstrap_quantiles(q_net, target_net, boot_obs, boot_mask)
             targets = self.sampled_returns(rewards[..., None], done[..., None], boot)
         quantiles = q_net.quantiles(obs)
         n = quantiles.shape[-1]
@@ -120,16 +140,18 @@ class ImplicitQuantileDQN(DQN):
     tests/iqn_reference.py.  The levels come in: `taus` [B, N + N'] holds each loss row's N
     online levels tau_i, then its N' target levels tau'_j.  `huber_delta` is kappa."""
 
-    def bootstrap_quantiles(self, q_net, target_net, boot_obs, taus_prime):
+    def bootstrap_quantiles(self, q_net, target_net, boot_obs, taus_prime, boot_mask=None):
         """The target's Z at tau'_j of a* [B, N'] (no gradient), a* the first argmax of the
-        collapsed Q of online(obs') with double_q, else of target(obs')."""
+        collapsed Q of online(obs') with double_q, else of target(obs'); over obs' valid
+        actions with boot_mask [B, A]."""
         with torch.no_grad():
-            best = (q_net if self.double_q else target_net).q_values(boot_obs).argmax(dim=-1)
+            best = masked_scores((q_net if self.double_q else target_net).q_values(boot_obs),
+                                 boot_mask).argmax(dim=-1)
             z = target_net.quantiles_at(boot_obs, taus_prime)           # [B, N', A]
             return z.gather(-1, best[:, None, None].expand(-1, z.shape[1], 1))[..., 0]
 
     def loss(self, q_net, target_net, obs, actions, rewards, done, boot_obs, weights=None,
-             taus=None):
+             taus=None, boot_mask=None):
         """(quantile Huber loss, Q-bar [B], R-bar [B]) of B sampled windows, the arguments of
         DQN.loss and the levels `taus`.  theta_i = Z_tau_i(obs)[a], T_j the n-step recursion on
         the target's Z_tau'_j(obs')[a*], u_ij = T_j - theta_i, and the row loss
@@ -140,7 +162,7 @@ class ImplicitQuantileDQN(DQN):
         assert taus is not None and taus.shape == (obs.shape[0], n + q_net.num_tau_prime_samples)
         tau, tau_prime = taus[:, :n].to(obs.dtype), taus[:, n:].to(obs.dtype)
         with torch.no_grad():
-            boot = self.bootstrap_quantiles(q_net, target_net, boot_obs, tau_prime)
+            boot = self.bootstrap_quantiles(q_net, target_net, boot_obs, tau_prime, boot_mask)
             targets = self.sampled_returns(rewards[..., None], done[..., None], boot)
         z = q_net.quantiles_at(obs, tau)                                 # [B, N, A]
         a = actions.long().reshape(-1)
@@ -165,15 +187,18 @@ class CategoricalDQN(DQN):
     IQN, so the store is shared by every Q network; Rainbow uses the row's cross-entropy
     instead -- a deliberate divergence."""
 
-    def bootstrap_distribution(self, q_net, target_net, boot_obs):
+    def bootstrap_distribution(self, q_net, target_net, boot_obs, boot_mask=None):
         """p' = softmax(target.logits(obs')[a*]) [B, N] (no gradient), a* the first argmax of
-        the expectation of online(obs') with double_q, else of target(obs')."""
+        the expectation of online(obs') with double_q, else of target(obs'); over obs' valid
+        actions with boot_mask [B, A] (wdb_c51_update_masked)."""
         with torch.no_grad():
-            best = (q_net if self.double_q else target_net).q_values(boot_obs).argmax(dim=-1)
+            best = masked_scores((q_net if self.double_q else target_net).q_values(boot_obs),
+                                 boot_mask).argmax(dim=-1)
             p = target_net.probabilities(boot_obs)
             return p[torch.arange(p.shape[0], device=p.device), best]
 
-    def loss(self, q_net, target_net, obs, actions, rewards, done, boot_obs, weights=None):
+    def loss(self, q_net, target_net, obs, actions, rewards, done, boot_obs, weights=None,
+             boot_mask=None):
         """(cross-entropy loss, Q-bar [B], R-bar [B]) of B sampled windows, the arguments of
         DQN.loss.  Tz_j is the n-step recursion on each atom z_j, clamped to [z_0, z_{N-1}];
         the projection m_i = sum_j clip(1 - |Tz_j - z_i| / dz, 0, 1) p'_j (Dopamine's dense
@@ -182,7 +207,7 @@ class CategoricalDQN(DQN):
         Q-bar = sum_i z_i p_i and R-bar = sum_i z_i m_i feed the metrics and the priorities."""
         z = q_net.support.to(obs.dtype)
         with torch.no_grad():
-            p_boot = self.bootstrap_distribution(q_net, target_net, boot_obs)
+            p_boot = self.bootstrap_distribution(q_net, target_net, boot_obs, boot_mask)
             tz = self.sampled_returns(rewards[..., None], done[..., None],
                                       z.expand(obs.shape[0], -1))
             tz = tz.clamp(z[0], z[-1])

@@ -10,7 +10,11 @@ DQN (FusedC51Update).  A dueling DQN or C51 network runs the same passes on its 
 after it).  A noisy DQN or C51 network, plain or dueling, runs them on its materialized head
 (FusedNoisyUpdate; csrc/wdb_noisy.cu draws the update's noise and writes the effective layers
 before the pass, and maps their gradients onto mu and sigma after it).  The torch autograd
-updates (algorithms/dqn.py) stay for the shapes these do not take."""
+updates (algorithms/dqn.py) stay for the shapes these do not take.  An action-masked DQN or C51
+network (plain, dueling or noisy) runs `wdb_dqn_update_masked` / `wdb_c51_update_masked`
+(csrc/wdb_masked_q.cu; FusedMaskedDQNUpdate, FusedMaskedC51Update), whose bootstrap ranges over
+the valid actions of obs' own mask; masked QR-DQN and IQN networks train through the torch
+losses."""
 import ctypes
 
 import torch
@@ -21,6 +25,11 @@ from warp_drive_b200.training.algorithms.fused_ddpg import (
 from warp_drive_b200.training.models.fully_connected_q import (
     FullyConnectedCategoricalQ, FullyConnectedIQN, FullyConnectedQ, FullyConnectedQuantileQ)
 from warp_drive_b200.utils.spaces import Box
+
+
+def _masked(q_net):
+    """Whether a Q network's observations carry an action mask (FullyConnectedQ.masked)."""
+    return bool(getattr(q_net, "masked", False))
 
 
 def _shape_struct(algo, q_net, n_envs, n_agents, capacity):
@@ -43,6 +52,7 @@ class FusedQUpdate:
     launch)."""
     model = None
     entry = None
+    masked = False                             # the pass takes action-masked networks only
 
     @staticmethod
     def shape_args(q_net):
@@ -50,10 +60,13 @@ class FusedQUpdate:
 
     @classmethod
     def supported(cls, algo, q_net, n_envs, n_agents, capacity, replay_rows):
-        """True if `wdb_<entry>` takes this policy: a `model` over a Box observation with at most
-        3 hidden layers, no dueling head (FusedDuelingUpdate) and no noisy head
-        (FusedNoisyUpdate), in the pass's envelope for replay_rows sampled windows per update."""
-        if type(q_net) is not cls.model or not isinstance(q_net.observation_space, Box):
+        """True if `wdb_<entry>` takes this policy: a `model` over a Box observation (a masked
+        pass: an action-masked network, over its Dict observation) with at most 3 hidden layers,
+        no dueling head (FusedDuelingUpdate) and no noisy head (FusedNoisyUpdate), in the pass's
+        envelope for replay_rows sampled windows per update."""
+        if type(q_net) is not cls.model or _masked(q_net) != cls.masked:
+            return False
+        if not cls.masked and not isinstance(q_net.observation_space, Box):
             return False
         if q_net.dueling or q_net.noisy or len(q_net.fc_dims) > 3:
             return False
@@ -208,6 +221,44 @@ class FusedC51Update(FusedQUpdate):
         return self.shape_args(self.models[0]) + (_lib.ptr(self.support), self.delta_z)
 
 
+class _MaskedQPass:
+    """The action-masked form of a Q pass: `launch` also takes `action_mask`, the ring's mask
+    array float32 [C, E, Np, A] (action_mask_batch_{p}), and `wdb_<entry>` takes it after the
+    windows and the weights.  The bootstrap's a* ranges over the valid actions of obs' own mask
+    row; the struct, workspace, sums and outputs are the unmasked pass's."""
+    masked = True
+
+    def launch(self, obs, actions, rewards, done, windows, outputs=None, weights=None,
+               action_mask=None):
+        assert action_mask is not None and action_mask.dtype == torch.float32
+        assert action_mask.is_contiguous()
+        assert tuple(action_mask.shape) == tuple(actions.shape[:-1]) + (self.u.n_actions,)
+        self.action_mask = action_mask
+        return super().launch(obs, actions, rewards, done, windows, outputs, weights)
+
+    def _run(self, u, windows, weights):
+        _lib.check(getattr(self.lib, f"wdb_{self.entry}")(
+            _lib.stream_ptr(), u, *self.launch_args(), windows, _lib.ptr(weights),
+            _lib.ptr(self.action_mask)), self.entry)
+
+
+class FusedMaskedDQNUpdate(_MaskedQPass, FusedDQNUpdate):
+    """`wdb_dqn_update_masked` (an action-masked FullyConnectedQ): FusedDQNUpdate's shapes, sums
+    and outputs, uniform or weighted, with the masked bootstrap."""
+    entry = "dqn_update_masked"
+
+
+class FusedMaskedC51Update(_MaskedQPass, FusedC51Update):
+    """`wdb_c51_update_masked` (an action-masked FullyConnectedCategoricalQ): FusedC51Update's
+    shapes, sums and outputs, uniform or weighted, with the masked a*."""
+    entry = "c51_update_masked"
+
+
+def _mask_kwargs(action_mask):
+    """The `action_mask` keyword of a plain pass's launch: only for a masked one."""
+    return {} if action_mask is None else {"action_mask": action_mask}
+
+
 def folded_widths(q_net):
     """The hidden widths of a dueling network's folded form: the trunk's, then the stacked
     stream hidden layer 2S when S > 0 (DuelingHead.folded)."""
@@ -299,7 +350,10 @@ class FusedDuelingUpdate:
 
     @staticmethod
     def plain_type(q_net):
-        return FusedC51Update if getattr(q_net, "is_categorical_q", False) else FusedDQNUpdate
+        categorical = getattr(q_net, "is_categorical_q", False)
+        if _masked(q_net):
+            return FusedMaskedC51Update if categorical else FusedMaskedDQNUpdate
+        return FusedC51Update if categorical else FusedDQNUpdate
 
     @classmethod
     def supported(cls, algo, q_net, n_envs, n_agents, capacity, replay_rows):
@@ -311,7 +365,9 @@ class FusedDuelingUpdate:
             return False
         if q_net.noisy:                        # FusedNoisyUpdate
             return False
-        if not isinstance(q_net.observation_space, Box) or len(folded_widths(q_net)) > 3:
+        if not (_masked(q_net) or isinstance(q_net.observation_space, Box)):
+            return False
+        if len(folded_widths(q_net)) > 3:
             return False
         head = ctypes.byref(dueling_shape(q_net.policy_head))
         if not _lib.load().wdb_dueling_fold_supported(head):
@@ -336,11 +392,13 @@ class FusedDuelingUpdate:
                 for i, (w, b) in enumerate([(w.grad, b.grad) for w, b in trunk] + folded.grads):
                     net.gw[i], net.gb[i] = _lib.ptr(w), _lib.ptr(b)
 
-    def launch(self, obs, actions, rewards, done, windows, outputs=None, weights=None):
+    def launch(self, obs, actions, rewards, done, windows, outputs=None, weights=None,
+               action_mask=None):
         """The network's gradient (trunk and both streams) into its `.grad`; the arguments of
-        FusedQUpdate.launch."""
+        FusedQUpdate.launch, and a masked network's `action_mask` for its masked pass."""
         fold(self.online, self.target)
-        self.plain.launch(obs, actions, rewards, done, windows, outputs, weights)
+        self.plain.launch(obs, actions, rewards, done, windows, outputs, weights,
+                          **_mask_kwargs(action_mask))
         _lib.check(_lib.load().wdb_dueling_unfold_grads(
             _lib.stream_ptr(), ctypes.byref(self.online.struct())), "dueling_unfold_grads")
         return self.sums
@@ -463,7 +521,7 @@ class FusedNoisyUpdate:
         (folded, for a dueling head) is in the plain pass's envelope."""
         if type(q_net) not in (FullyConnectedQ, FullyConnectedCategoricalQ) or not q_net.noisy:
             return False
-        if not isinstance(q_net.observation_space, Box):
+        if not (_masked(q_net) or isinstance(q_net.observation_space, Box)):
             return False
         shape = NoisyHead.shape(q_net)
         if shape is None or not _lib.load().wdb_noisy_supported(ctypes.byref(shape)):
@@ -510,13 +568,16 @@ class FusedNoisyUpdate:
                 for i, (w, b) in enumerate([(w.grad, b.grad) for w, b in trunk] + head):
                     net.gw[i], net.gb[i] = _lib.ptr(w), _lib.ptr(b)
 
-    def launch(self, obs, actions, rewards, done, windows, outputs=None, weights=None, update=0):
+    def launch(self, obs, actions, rewards, done, windows, outputs=None, weights=None, update=0,
+               action_mask=None):
         """The network's gradient (trunk, mu and sigma) into its `.grad` under update `update`'s
-        noise; the other arguments are FusedQUpdate.launch's."""
+        noise; the other arguments are FusedQUpdate.launch's, and a masked network's
+        `action_mask` for its masked pass."""
         materialize(self.online, self.target, self.seed, update)
         if self.dueling:
             fold(self.fold_online, self.fold_target)
-        self.plain.launch(obs, actions, rewards, done, windows, outputs, weights)
+        self.plain.launch(obs, actions, rewards, done, windows, outputs, weights,
+                          **_mask_kwargs(action_mask))
         if self.dueling:
             _lib.check(_lib.load().wdb_dueling_unfold_grads(
                 _lib.stream_ptr(), ctypes.byref(self.fold_online.struct())),

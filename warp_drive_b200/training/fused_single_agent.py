@@ -71,7 +71,7 @@ class FusedSingleAgentRollout:
                 return False
             if len(model.output_dims) != 1 or (continuous and model.output_dims[0] != 1):
                 return False
-            if getattr(model, "action_mask", None) is not None:
+            if getattr(model, "action_mask", None) is not None or getattr(model, "masked", False):
                 return False
             # a noisy head draws fresh noise per env and step: the noisy Q kind takes a plain
             # head of one NoisyLinear; noisy C51 and noisy dueling heads act per step

@@ -16,6 +16,13 @@ head -- the plain head's output layer, or every stream layer of a DuelingHead --
 with factorized Gaussian noise (`noisy_sigma0`, 0.5 by default); the trunk stays plain.  A layer
 uses noise only while its `noise` is set (the update's sample, or per-row acting noise), and is
 the mean network otherwise, so the evaluator plays the mean network.
+
+Action masks: the model key `masked: true` over a Dict observation space with an `action_mask`
+key of width A sets `masked` (without the key such a space is refused, as before).  The
+mask is not a model input (`flattened_obs_size` excludes it) and the Q values stay raw: the
+rollout's epsilon-greedy sampler acts over the valid actions
+(CUDASampler.sample_epsilon_greedy's `action_mask`) and the losses bootstrap over the valid
+actions of obs' (algorithms/dqn.py's `boot_mask`).
 """
 import math
 
@@ -25,7 +32,10 @@ from torch.nn import functional as func
 
 from warp_drive_b200.training.utils.data_loader import (
     action_head_sizes, dict_observation_keys, get_flattened_obs_size)
+from warp_drive_b200.utils.constants import Constants
 from warp_drive_b200.utils.spaces import Discrete
+
+_ACTION_MASK = Constants.ACTION_MASK
 
 
 def dueling_settings(model_config, model_type):
@@ -62,6 +72,28 @@ def noisy_settings(model_config, model_type):
     if isinstance(s, bool) or not isinstance(s, (int, float)) or not math.isfinite(s) or s <= 0:
         raise ValueError(f"{model_type}'s model.noisy_sigma0 is a finite number > 0, got {s!r}")
     return noisy, float(s)
+
+
+def masked_settings(model_config, observation_space, n_actions):
+    """model.masked (bool, False) of a Q model config, validated against the observation space:
+    an `action_mask` key is refused without `masked: true`, `masked: true` is refused without
+    one, and the mask must have one entry per action."""
+    masked = model_config.get("masked", False)
+    if not isinstance(masked, bool):
+        raise ValueError(f"a Q model's model.masked is true or false, got {masked!r}")
+    _, has_mask = dict_observation_keys(observation_space)
+    if has_mask and not masked:
+        raise ValueError("fully_connected_q does not take observations with an action_mask "
+                         "unless model.masked is true")
+    if masked and not has_mask:
+        raise ValueError("model.masked: true needs a Dict observation space with an "
+                         f"{_ACTION_MASK!r} key")
+    if masked:
+        width = get_flattened_obs_size(observation_space[_ACTION_MASK])
+        if width != n_actions:
+            raise ValueError(f"a masked Q model's action_mask must have one entry per action "
+                             f"({n_actions}), got width {width}")
+    return masked
 
 
 class NoisyLinear(nn.Module):
@@ -203,9 +235,9 @@ class FullyConnectedQ(nn.Module):
             raise ValueError("fully_connected_q takes a single Discrete action head, got "
                              f"{type(action_space).__name__}")
         heads, _ = action_head_sizes(action_space)
-        _, masked = dict_observation_keys(self.observation_space)
-        if masked:
-            raise ValueError("fully_connected_q does not take observations with an action_mask")
+        # `masked: true` with an `action_mask` key: the Q values stay raw, the sampler and the
+        # losses apply the mask
+        self.masked = masked_settings(model_config, self.observation_space, int(heads[0]))
         self.flattened_obs_size = get_flattened_obs_size(self.observation_space)
         self.output_dims = [int(heads[0])]
         dims = [self.flattened_obs_size] + self.fc_dims

@@ -525,6 +525,9 @@ class RolloutEngine:
             obs_p.update(self._obs_scratch)
             if self._obs_scratch:
                 self._move_rows(obs, self._obs_scratch)
+        # a Q network's forward leaves its outputs raw: the epsilon-greedy sampler applies the
+        # step's mask rows (sample_actions)
+        self._q_masks = mask_p
         per_policy = {}
         for p in self.policies:
             if self.fused_forward:
@@ -618,17 +621,22 @@ class RolloutEngine:
     def _sample_epsilon_greedy(self, q_values, suffix, sample_params):
         """{policy: Q values [E, Np, A]} -> sampled_actions{suffix} [E, N, 1] int32, as
         _sample_gaussian: one policy covering the array samples into it, several sample their
-        own rows, which one launch scatters into place."""
+        own rows, which one launch scatters into place.  A masked policy samples over the valid
+        actions of the mask rows its last evaluate_policies gathered (the batch slot, or the
+        scratch rows of an evaluation step)."""
         actions = self._tensor(f"{_ACTIONS}{suffix}")
+        masks = getattr(self, "_q_masks", {})
         if len(q_values) == 1:
-            (_, q), = q_values.items()
-            self.sampler.sample_epsilon_greedy(q, actions, **sample_params)
+            (p, q), = q_values.items()
+            self.sampler.sample_epsilon_greedy(q, actions, action_mask=masks.get(p),
+                                               **sample_params)
             return
         if not hasattr(self, "_q_rows"):
             self._q_rows = {p: torch.empty(q.shape[:-1] + (1,), dtype=torch.int32,
                                            device=q.device) for p, q in q_values.items()}
         for p, q in q_values.items():
-            self.sampler.sample_epsilon_greedy(q, self._q_rows[p], **sample_params)
+            self.sampler.sample_epsilon_greedy(q, self._q_rows[p], action_mask=masks.get(p),
+                                               **sample_params)
         self._move_rows(actions, self._q_rows, scatter=True)
 
     def sample_actions(self, probs, t, **sample_params):

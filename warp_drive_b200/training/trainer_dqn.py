@@ -65,6 +65,15 @@ buffers (wdb_noisy_draw) and differentiates through NoisyLinear.materialized(). 
 fresh noise per env row and step on the rollout engine's per-step path; the evaluator plays the
 mean network.  Logging iterations add `Noisy sigma`, the mean |sigma_W| over the head's noisy
 layers.
+
+Action masks: a Q model with `masked: true` over a Dict observation with an `action_mask` key
+acts epsilon-greedily over the valid actions of each step's mask
+(CUDASampler.sample_epsilon_greedy with `action_mask`), and the evaluator plays the masked greedy action.  The ring stores each
+step's mask in action_mask_batch_{p}, and every update bootstraps over the valid actions of
+obs' own mask, the row at the window's slot(n_step): the native DQN and C51 passes, plain,
+dueling or noisy, through wdb_dqn_update_masked / wdb_c51_update_masked (FusedMaskedDQNUpdate,
+FusedMaskedC51Update), and QR-DQN, IQN and every shape outside the passes through the torch
+losses' `boot_mask`.  A row with no valid action falls back to the unmasked rule.
 """
 import os
 
@@ -74,7 +83,7 @@ from warp_drive_b200.training.algorithms.dqn import (
     DQN, CategoricalDQN, ImplicitQuantileDQN, QuantileDQN)
 from warp_drive_b200.training.algorithms.fused_dqn import (
     NOISY_UPDATE, FusedC51Update, FusedDQNUpdate, FusedDuelingUpdate, FusedIQNUpdate,
-    FusedNoisyUpdate, FusedQRDQNUpdate, draw_noise)
+    FusedMaskedC51Update, FusedMaskedDQNUpdate, FusedNoisyUpdate, FusedQRDQNUpdate, draw_noise)
 from warp_drive_b200.training.trainer_ddpg import (
     RingRolloutEngine, TrainerDDPG, hard_update, soft_update)
 from warp_drive_b200.training.utils.param_scheduler import ParamScheduler
@@ -85,6 +94,7 @@ _ACTIONS = Constants.ACTIONS
 _REWARDS = Constants.REWARDS
 _DONE_FLAGS = Constants.DONE_FLAGS
 _PROCESSED_OBSERVATIONS = Constants.PROCESSED_OBSERVATIONS
+_ACTION_MASK = Constants.ACTION_MASK
 
 
 def epsilon_schedule(config):
@@ -234,9 +244,11 @@ class TrainerDQN(TrainerDDPG):
             if self._tau_generator is None:
                 self._tau_generator = torch.Generator(device=dev)
                 self._tau_generator.manual_seed(self.seed)
+        masked = q_net.masked                  # masked QR-DQN / IQN: the torch losses
         fused = (FusedNoisyUpdate if q_net.noisy else FusedDuelingUpdate if q_net.dueling
-                 else FusedC51Update if categorical else FusedIQNUpdate if implicit
-                 else FusedQRDQNUpdate if quantile else FusedDQNUpdate)
+                 else (FusedMaskedC51Update if masked else FusedC51Update) if categorical
+                 else FusedIQNUpdate if implicit else FusedQRDQNUpdate if quantile
+                 else FusedMaskedDQNUpdate if masked else FusedDQNUpdate)
         if fused.supported(algo, q_net, self.num_envs, n_agents, self.ring_capacity, rows):
             extra = (self.seed,) if q_net.noisy else ()
             self.fused_updates[policy] = fused(
@@ -336,6 +348,7 @@ class TrainerDQN(TrainerDDPG):
         try:
             loss, q, returns = algo.loss(*nets, *self._gather_windows(policy),
                                          weights=None if store is None else store.weights,
+                                         boot_mask=self._gather_boot_mask(policy),
                                          **self._levels(policy))
         finally:
             for L in noisy:
@@ -367,12 +380,26 @@ class TrainerDQN(TrainerDDPG):
                             eng._tensor(f"{_DONE_FLAGS}_batch"), self.replay_windows[policy],
                             outputs, weights, **self._levels(policy),
                             **({"update": self.update_count[policy]}
-                               if isinstance(fused, FusedNoisyUpdate) else {}))
+                               if isinstance(fused, FusedNoisyUpdate) else {}),
+                            **({"action_mask": eng._tensor(f"{_ACTION_MASK}_batch_{policy}")}
+                               if self.q_models[policy].masked else {}))
         if not logging_flag:
             return {}
         s = sums.tolist()
         return self.trainers[policy].loss_metrics(s[0] / fused.rows, s[1] / fused.rows,
                                                   outputs[1])
+
+    def _gather_boot_mask(self, policy):
+        """For an action-masked policy, obs' own mask [B, A] of the sampled windows: the ring's
+        action_mask_batch_{p} row at each window's slot(n_step), the row the masked native
+        passes read; None otherwise."""
+        if not self.q_models[policy].masked:
+            return None
+        C = self.ring_capacity
+        windows = self.replay_windows[policy].long()
+        slot = (windows[:, 0] + self.n_step) % C
+        mask = self.engine._tensor(f"{_ACTION_MASK}_batch_{policy}")
+        return mask.reshape(C, -1, mask.shape[-1])[slot, windows[:, 1]]
 
     def _levels(self, policy):
         """IQN's levels of this update, as the `taus` argument of its loss and its native pass
