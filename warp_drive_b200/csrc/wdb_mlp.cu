@@ -26,6 +26,8 @@
 //   * final epilogue = bias + two softmaxes + value: the logits go through the staging
 //     buffer, two threads per row (head 0 | head 1 + value) compute the softmaxes, and the
 //     warpgroup's 64 rows of each output are copied to global memory with coalesced stores.
+//     The sampling forward (mlp_forward_sampled_kernel) gives this epilogue, and the
+//     sampling of both heads, to a third warpgroup, so its two MMA warpgroups only run MMAs.
 //
 // Numerics: bf16 operands, fp32 accumulation (the reference is fp32; SURVEY.md section 8
 // row a3 allows TF32/BF16 for the forward that feeds the sampler).  Pinned to a float64
@@ -423,25 +425,136 @@ using AnyShape = MlpShape<0, 0, 0>;
 // at the top of the tile.
 using FastShape = MlpShape<80, 256, 48>;
 
-// SAMPLE (FastShape only, wdb_mlp_policy_forward_sampled): the epilogue also draws both
-// heads' actions of every row, as the fused TagContinuous step would from the stored
-// probabilities.  Row r = env * Np + slot of the policy is agent gi = env * N + agent[slot].
-struct MlpSampling {
-  int *actions;               // [rows, 2]
-  void *rng;                  // RNG state of E * N streams (NULL with uniforms)
-  const float *uniforms;      // [E * N * 2] or NULL
-  const int *agent;           // [Np]
-  int N, Np;
-};
+// ---- the FastShape schedule of one warpgroup's tile, in two parts (the caller marks the
+// phase clock between them).  Layer 1 (A = a1, in registers) -> h: packed bf16 A fragments
+// of layer 2.
+__device__ __forceinline__ void fast_layer1(const uint32_t (&a1)[FastShape::K1 / 4],
+                                            uint32_t s_w1, uint32_t sbo_a, const float *s_b1,
+                                            uint32_t (&h)[kMaxK / 4]) {
+  slice_pipeline(
+      FastShape::H / kSliceN,
+      [&](int c, float(&d)[kSliceN / 2]) {
+#pragma unroll
+        for (int kk = 0; kk < FastShape::K1 / 16; kk++)
+          wgmma_n64(d, &a1[4 * kk], s_w1 + kSliceN / 8 * c * sbo_a + kk * 256, sbo_a, kk);
+      },
+      [&](int c, const float(&d)[kSliceN / 2]) {
+        bias_relu_slice(d, s_b1, c, &h[kSliceN / 4 * c]);
+      });
+}
 
-template <bool TILES, class Shape, bool MASK = false, bool SAMPLE = false>
+// Layer 2 (A = h) streamed into layer 3 ([head0 | head1 | value | pad], one m64n48k16 per
+// k-step, accumulated in o48): as soon as a 64-column slice of layer 2 is packed, the four
+// layer-3 k-steps it feeds are issued, so layer 2's output is never held whole.  Every
+// layer-3 output still accumulates its k-steps 0, 1, ..., H / 16 - 1 in order, the first
+// with scale-d = 0.  The n48 accumulator fragment holds columns 8 j + 2 t (+ 1) at [4 j ..].
+// When have_next, the observations of the warpgroup's next tile (first row next_row0) load
+// meanwhile, half after slice 0 and half after slice 1, each packed into a1 (which layer 1
+// no longer reads) one slice after its loads were issued.  Returns with layer 3's MMAs
+// still in flight (the caller's wgmma_wait<0> completes o48).
+template <bool TILES>
+__device__ __forceinline__ void fast_layers23(const uint32_t (&h)[kMaxK / 4], uint32_t s_w2,
+                                              uint32_t s_w3, uint32_t sbo_h, const float *s_b2,
+                                              float (&o48)[48 / 2],
+                                              ObsFrag<TILES, FastShape::K1> &next,
+                                              uint32_t (&a1)[FastShape::K1 / 4], bool have_next,
+                                              const void *input, long long rows, int F,
+                                              long long next_row0) {
+  slice_pipeline(
+      FastShape::H / kSliceN,
+      [&](int c, float(&d)[kSliceN / 2]) {
+#pragma unroll
+        for (int kk = 0; kk < FastShape::H / 16; kk++)
+          wgmma_n64(d, &h[4 * kk], s_w2 + kSliceN / 8 * c * sbo_h + kk * 256, sbo_h, kk);
+      },
+      [&](int c, const float(&d)[kSliceN / 2]) {
+        uint32_t a[kSliceN / 4];
+        bias_relu_slice(d, s_b2, c, a);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kSliceN / 16; k++)
+          wgmma_n48(o48, &a[4 * k], s_w3 + (kSliceN / 16 * c + k) * 256, sbo_h,
+                    kSliceN / 16 * c + k);
+        wgmma_commit();
+        if (have_next && (c == 1 || c == 2)) obs_frag_pack(next, c - 1, a1);
+        if (have_next && (c == 0 || c == 1)) obs_frag_load(next, c, input, rows, F, next_row0);
+      });
+}
+
+// ---- output epilogue of a warpgroup's 64 rows.  The logits are staged [64 rows x N3] with
+// column col of row r at col ^ (r & 14): the softmax reads one column of 32 consecutive rows
+// per warp, which with N3 = 48 would otherwise fall into two shared-memory banks (16-way
+// conflicts; 2-way with it).  The swizzle stays inside the column's 16-column group (N3 is a
+// multiple of 16) and keeps the pairs (col, col + 1) of even col together, so they are still
+// float2 stores.
+__device__ __forceinline__ int logit_at(int r, int col, int N3) {
+  return r * N3 + (col ^ (r & 14));
+}
+
+// layer 3's accumulators + bias -> staging: o[c][4 j + 0/1] is row lr = 16 wr + g,
+// o[c][4 j + 2/3] row lr + 8, columns 16 c + 8 j + 2 t (+1)
+__device__ __forceinline__ void stage_logits(const float (&o)[kMaxN3 / 16][8], const float *s_b3,
+                                             int N3, int lr, int t, float *s_o) {
+#pragma unroll
+  for (int c = 0; c < kMaxN3 / 16; c++) {
+    if (c < N3 / 16) {
+#pragma unroll
+      for (int j = 0; j < 2; j++) {
+        const int col = 16 * c + 8 * j + 2 * t;
+        const float2 b = *reinterpret_cast<const float2 *>(s_b3 + col);
+        *reinterpret_cast<float2 *>(s_o + logit_at(lr, col, N3)) =
+            make_float2(o[c][4 * j] + b.x, o[c][4 * j + 1] + b.y);
+        *reinterpret_cast<float2 *>(s_o + logit_at(lr + 8, col, N3)) =
+            make_float2(o[c][4 * j + 2] + b.x, o[c][4 * j + 3] + b.y);
+      }
+    }
+  }
+}
+
+// Softmax of the cnt staged logits of `row` from column cbase: lg[i] = 2^(l_i log2(e) - max)
+// (0 for i >= cnt), returns 1 / sum; `value` = the logit just past the head (the value
+// column, for head 1).  Logits pre-scaled by log2(e), branch-free over 32 statically indexed
+// registers, 4-way max and sum.
+__device__ __forceinline__ float softmax_row(const float *s_o, int N3, int row, int cbase,
+                                             int cnt, float (&lg)[32], float &value) {
+  constexpr float kLog2e = 1.4426950408889634f;
+  float mx[4] = {-CUDART_INF_F, -CUDART_INF_F, -CUDART_INF_F, -CUDART_INF_F};
+  value = 0.0f;
+#pragma unroll
+  for (int i = 0; i < 32; i++) {
+    const float x = s_o[logit_at(row, min(cbase + i, N3 - 1), N3)];
+    lg[i] = i < cnt ? x * kLog2e : -CUDART_INF_F;
+    mx[i & 3] = fmaxf(mx[i & 3], lg[i]);
+    value = (i == cnt) ? x : value;
+  }
+  const float m = fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3]));
+  float zz[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+#pragma unroll
+  for (int i = 0; i < 32; i++) {
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(lg[i]) : "f"(lg[i] - m));   // 2^-inf = 0
+    zz[i & 3] += lg[i];
+  }
+  return 1.0f / ((zz[0] + zz[1]) + (zz[2] + zz[3]));
+}
+
+// staged [probs0 64 x A0 | probs1 64 x A1 | values 64] of the 64 rows from rb -> global
+__device__ __forceinline__ void copy_outputs(const float *s_o, long long rb, long long rows,
+                                             int A0, int A1, float *__restrict__ probs0,
+                                             float *__restrict__ probs1,
+                                             float *__restrict__ values, int lt) {
+  const float *s_p0 = s_o, *s_p1 = s_o + kWgRows * A0, *s_v = s_p1 + kWgRows * A1;
+  const int valid = (int)min((long long)kWgRows, rows - rb);
+  copy_out(probs0 + rb * A0, s_p0, valid * A0, lt);
+  copy_out(probs1 + rb * A1, s_p1, valid * A1, lt);
+  if (values && lt < valid) values[rb + lt] = s_v[lt];
+}
+
+template <bool TILES, class Shape, bool MASK = false>
 __device__ __forceinline__ void
 mlp_forward_body(const unsigned char *__restrict__ blob, const void *__restrict__ input,
                  long long rows, float *__restrict__ probs0, float *__restrict__ probs1,
                  float *__restrict__ values, const unsigned bid, const unsigned gdim,
-                 const int flags, const float *__restrict__ mask = nullptr,
-                 const MlpSampling &smp = MlpSampling{}) {
-  static_assert(!SAMPLE || (Shape::H != 0 && !MASK), "sampling is a FastShape epilogue");
+                 const int flags, const float *__restrict__ mask = nullptr) {
   extern __shared__ __align__(128) unsigned char smem[];
   const MlpHeader hd = *reinterpret_cast<const MlpHeader *>(blob);
   const int F = hd.F, A0 = hd.A0, A1 = hd.A1;
@@ -533,53 +646,17 @@ mlp_forward_body(const unsigned char *__restrict__ blob, const void *__restrict_
 
     float o[kMaxN3 / 16][8];   // layer-3 logits
     if constexpr (kOverlap) {
-      // ---- layer 1 (A = a1, in registers) -> h: packed bf16 A fragments of layer 2
+      static_assert(Shape::K1 == FastShape::K1 && Shape::H == FastShape::H &&
+                    Shape::N3 == FastShape::N3, "the overlapped schedule is FastShape's");
       uint32_t h[kMaxK / 4];
-      slice_pipeline(
-          H / kSliceN,
-          [&](int c, float(&d)[kSliceN / 2]) {
-#pragma unroll
-            for (int kk = 0; kk < K1 / 16; kk++)
-              wgmma_n64(d, &a1[4 * kk], s_w1 + kSliceN / 8 * c * sbo_a + kk * 256, sbo_a, kk);
-          },
-          [&](int c, const float(&d)[kSliceN / 2]) {
-            bias_relu_slice(d, s_b1, c, &h[kSliceN / 4 * c]);
-          });
+      fast_layer1(a1, s_w1, sbo_a, s_b1, h);
       MLP_MARK(mark0 + 1);
-
-      // ---- layer 2 (A = h) streamed into layer 3 ([head0 | head1 | value | pad], one
-      // m64n48k16 per k-step, accumulated in o): as soon as a 64-column slice of layer 2 is
-      // packed, the four layer-3 k-steps it feeds are issued, so layer 2's output is never held
-      // whole.  Every layer-3 output still accumulates its k-steps 0, 1, ..., H / 16 - 1 in
-      // order, the first with scale-d = 0.  The n48 accumulator fragment holds columns
-      // 8 j + 2 t (+ 1) at [4 j ..], so it is o[n][4 j' ..] (columns 16 n + 8 j' + 2 t) laid
-      // out flat.  The next tile's observations load meanwhile, half after slice 0 and half
-      // after slice 1, each packed into a1 (which layer 1 no longer reads) one slice after its
-      // loads were issued.
-      static_assert(Shape::N3 == 48, "layer 3 of the overlapped schedule is one m64n48k16");
+      // layer 3's n48 fragment (columns 8 j + 2 t (+ 1) at [4 j ..]) is o[n][4 j' ..]
+      // (columns 16 n + 8 j' + 2 t) laid out flat
       float(&o48)[48 / 2] = *reinterpret_cast<float(*)[48 / 2]>(&o[0][0]);
-      const bool have_next = row0 + (long long)gdim * kTileM < rows;
-      slice_pipeline(
-          H / kSliceN,
-          [&](int c, float(&d)[kSliceN / 2]) {
-#pragma unroll
-            for (int kk = 0; kk < kMaxK / 16; kk++)
-              if (kk < H / 16)
-                wgmma_n64(d, &h[4 * kk], s_w2 + kSliceN / 8 * c * sbo_h + kk * 256, sbo_h, kk);
-          },
-          [&](int c, const float(&d)[kSliceN / 2]) {
-            uint32_t a[kSliceN / 4];
-            bias_relu_slice(d, s_b2, c, a);
-            wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < kSliceN / 16; k++)
-              wgmma_n48(o48, &a[4 * k], s_w3 + (kSliceN / 16 * c + k) * 256, sbo_h,
-                        kSliceN / 16 * c + k);
-            wgmma_commit();
-            if (have_next && (c == 1 || c == 2)) obs_frag_pack(next, c - 1, a1);
-            if (have_next && (c == 0 || c == 1))
-              obs_frag_load(next, c, input, rows, F, row0 + (long long)gdim * kTileM);
-          });
+      fast_layers23<TILES>(h, s_w2, s_w3, sbo_h, s_b2, o48, next, a1,
+                           row0 + (long long)gdim * kTileM < rows, input, rows, F,
+                           row0 + (long long)gdim * kTileM);
       wgmma_wait<0>();
     } else {
       // ---- layer 1 A operand -> this warpgroup's staging buffer (canonical K-major layout:
@@ -633,53 +710,11 @@ mlp_forward_body(const unsigned char *__restrict__ blob, const void *__restrict_
     }
     MLP_MARK(mark0 + 2);
 
-    // SAMPLE: thread lt draws head lt / 64 of row lt % 64, the head its softmax below
-    // computes.  Its uniform's inputs are requested here, so that the loads overlap the
-    // epilogue; both threads of a row read the RNG offset before the wg_sync after the softmax,
-    // the head-0 thread advances it after that barrier.
-    const long long s_row = tile * kTileM + wg * kWgRows + (lt & 63);
-    const bool s_valid = SAMPLE && s_row < rows;
-    long long s_gi = 0;
-    unsigned long long s_seed = 0, s_off = 0;
-    float s_u = 0.0f;
-    if constexpr (SAMPLE) {
-      if (s_valid) {
-        const long long env = s_row / smp.Np;
-        s_gi = env * smp.N + __ldg(smp.agent + (int)(s_row - env * smp.Np));
-        if (smp.uniforms) {
-          s_u = __ldg(smp.uniforms + 2 * s_gi + (lt >> 6));
-        } else {
-          s_seed = reinterpret_cast<const RngHeader *>(smp.rng)->seed;
-          s_off = rng_offsets(smp.rng)[s_gi];
-        }
-      }
-    }
-
-    // ---- output epilogue.  Logits (+ bias) -> staging [64 rows x N3]: o[c][4 j + 0/1] is
-    // row 16 wr + g, o[c][4 j + 2/3] row + 8, columns 16 c + 8 j + 2 t (+1).  (The previous
-    // tile's output copy and, for other shapes, the layer-1 MMAs that read the staging buffer
-    // have completed in every warp.)  Column col of row r is stored at col ^ (r & 14):
-    // the softmax below reads one column of 32 consecutive rows per warp, which with N3 = 48
-    // would otherwise fall into two shared-memory banks (16-way conflicts; 2-way with it).
-    // The swizzle stays inside the column's 16-column group (N3 is a multiple of 16) and
-    // keeps the pairs (col, col + 1) of even col together, so they are still float2 stores.
+    // ---- output epilogue: logits (+ bias) -> staging, softmax, probabilities -> staging ->
+    // global.  (The previous tile's output copy and, for other shapes, the layer-1 MMAs that
+    // read the staging buffer have completed in every warp.)
     wg_sync(wg);
-    auto logit_at = [&](int r, int col) { return r * N3 + (col ^ (r & 14)); };
-    const int lr = wr * 16 + g;
-#pragma unroll
-    for (int c = 0; c < kMaxN3 / 16; c++) {
-      if (c < N3 / 16) {
-#pragma unroll
-        for (int j = 0; j < 2; j++) {
-          const int col = 16 * c + 8 * j + 2 * t;
-          const float2 b = *reinterpret_cast<const float2 *>(s_b3 + col);
-          *reinterpret_cast<float2 *>(s_o + logit_at(lr, col)) =
-              make_float2(o[c][4 * j] + b.x, o[c][4 * j + 1] + b.y);
-          *reinterpret_cast<float2 *>(s_o + logit_at(lr + 8, col)) =
-              make_float2(o[c][4 * j + 2] + b.x, o[c][4 * j + 3] + b.y);
-        }
-      }
-    }
+    stage_logits(o, s_b3, N3, wr * 16 + g, t, s_o);
     wg_sync(wg);
     if constexpr (MASK) {
       // apply_logit_mask in fp32 before the max: logit + (1 - m) * -1e20.  The warpgroup's
@@ -690,65 +725,28 @@ mlp_forward_body(const unsigned char *__restrict__ blob, const void *__restrict_
       const float *src = mask + mb * am;
       for (int i = lt; i < n; i += 128) {
         const int r = i / am, col = i - r * am;
-        float &x = s_o[logit_at(r, col)];
+        float &x = s_o[logit_at(r, col, N3)];
         x = __fadd_rn(x, __fmul_rn(1.0f - __ldg(src + i), -1.0e20f));
       }
       wg_sync(wg);
     }
-    // thread lt: row lt % 64; lt < 64 head 0, else head 1 + the value.  Logits pre-scaled by
-    // log2(e): softmax = 2^(l - max) / sum, branch-free over 32 statically indexed registers.
+    // thread lt: row lt % 64; lt < 64 head 0, else head 1 + the value
     const int row = lt & 63, part = lt >> 6;
     const int cbase = part ? A0 : 0, cnt = part ? A1 : A0;
-    constexpr float kLog2e = 1.4426950408889634f;
-    float lg[32];
-    float mx[4] = {-CUDART_INF_F, -CUDART_INF_F, -CUDART_INF_F, -CUDART_INF_F};
-    float value = 0.0f;
-#pragma unroll
-    for (int i = 0; i < 32; i++) {
-      const float x = s_o[logit_at(row, min(cbase + i, N3 - 1))];
-      lg[i] = i < cnt ? x * kLog2e : -CUDART_INF_F;
-      mx[i & 3] = fmaxf(mx[i & 3], lg[i]);
-      value = (i == cnt) ? x : value;
-    }
-    const float m = fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3]));
-    float zz[4] = {0.0f, 0.0f, 0.0f, 0.0f};
-#pragma unroll
-    for (int i = 0; i < 32; i++) {
-      asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(lg[i]) : "f"(lg[i] - m));   // 2^-inf = 0
-      zz[i & 3] += lg[i];
-    }
-    const float inv = 1.0f / ((zz[0] + zz[1]) + (zz[2] + zz[3]));
+    float lg[32], value;
+    const float inv = softmax_row(s_o, N3, row, cbase, cnt, lg, value);
     MLP_MARK(mark0 + 3);
     wg_sync(wg);
-    if constexpr (SAMPLE) {
-      // the probabilities exactly as they are stored below, sampled in registers
-#pragma unroll
-      for (int i = 0; i < 32; i++) lg[i] = lg[i] * inv;
-      if (s_valid) {
-        if (!smp.uniforms) {
-          RngHeader h;
-          h.seed = s_seed; h.n_streams = 0;
-          const uint4 d = rng_draw4(h, (unsigned long long)s_gi, s_off);
-          s_u = u32_to_uniform(part ? d.y : d.x);
-          if (!part) rng_offsets(smp.rng)[s_gi] = s_off + 1;
-        }
-        smp.actions[2 * s_row + part] = sample_cdf_regs(lg, cnt, s_u);
-      }
-    }
     // staging = [probs0 64 x A0 | probs1 64 x A1 | values 64]: the warpgroup's rows of each
     // output are contiguous in global memory
     float *s_p0 = s_o, *s_p1 = s_o + kWgRows * A0, *s_v = s_p1 + kWgRows * A1;
     float *dst = (part ? s_p1 : s_p0) + row * cnt;
 #pragma unroll
     for (int i = 0; i < 32; i++)
-      if (i < cnt) dst[i] = SAMPLE ? lg[i] : lg[i] * inv;
+      if (i < cnt) dst[i] = lg[i] * inv;
     if (part) s_v[row] = value;
     wg_sync(wg);
-    const long long rb = tile * kTileM + wg * kWgRows;   // first row of the warpgroup
-    const int valid = (int)min((long long)kWgRows, rows - rb);
-    copy_out(probs0 + rb * A0, s_p0, valid * A0, lt);
-    copy_out(probs1 + rb * A1, s_p1, valid * A1, lt);
-    if (values && lt < valid) values[rb + lt] = s_v[lt];
+    copy_outputs(s_o, tile * kTileM + wg * kWgRows, rows, A0, A1, probs0, probs1, values, lt);
     MLP_MARK(mark0 + 4);
   }
 #ifdef WDB_PHASE_CLOCKS
@@ -767,13 +765,238 @@ mlp_forward_kernel(const unsigned char *__restrict__ blob, const void *__restric
   mlp_forward_body<TILES, Shape>(blob, input, rows, probs0, probs1, values, blockIdx.x, gridDim.x, flags);
 }
 
+// ---- The sampling forward (FastShape only, wdb_mlp_policy_forward_sampled): besides the
+// probabilities and values it draws both heads' actions of every row, as the fused
+// TagContinuous step would from the stored probabilities.  Row r = env * Np + slot of the
+// policy is agent gi = env * N + agent[slot].
+struct MlpSampling {
+  int *actions;               // [rows, 2]
+  void *rng;                  // RNG state of E * N streams (NULL with uniforms)
+  const float *uniforms;      // [E * N * 2] or NULL
+  const int *agent;           // [Np]
+  int N, Np;
+};
+
+// Three warpgroups with fixed roles.  Warpgroups 0 and 1 each own 64 rows of every 128-row
+// tile: they run the FastShape schedule of mlp_forward_body on them, then the softmax, and
+// stage the probabilities and values in their staging buffer.  Warpgroup 2 draws both heads'
+// actions from the staged probabilities and copies the outputs to global memory, for both
+// buffers in tile order, while the MMA warpgroups go on to their next tile.  Each staging
+// buffer is single-buffered between a full / empty mbarrier pair: the MMA warpgroup waits on
+// `empty` only when it is about to stage its next tile, a whole tile of MMAs later.  (The
+// softmax stays with the MMA warpgroups: measured with WDB_PHASE_CLOCKS, one warpgroup doing
+// the softmax too for both halves of a tile took longer than the tile's MMAs.)
+// Registers: the CTA starts at 168 per thread (65536 / 384, in steps of 8) and setmaxnreg
+// moves them between the roles.  A warpgroup can only grow by what the CTA's other warpgroups
+// released, so 2 x kMmaRegs + kEpiRegs must not exceed 3 x 168 (more and the MMA warpgroups
+// would wait for registers forever).
+constexpr int kSampledThreads = kThreads + 128;
+constexpr int kSampledLaunchRegs = (65536 / kSampledThreads) & ~7;
+// (ptxas 12.9: neither role spills)
+constexpr int kMmaRegs = 224, kEpiRegs = 56;
+static_assert(kWarpgroups * kMmaRegs + kEpiRegs <= (kWarpgroups + 1) * kSampledLaunchRegs,
+              "setmaxnreg can only hand out the registers the CTA was launched with");
+// named barrier of the epilogue warpgroup (1 and 2 are the MMA warpgroups' wg_sync)
+__device__ __forceinline__ void epi_sync() { asm volatile("bar.sync 3, 128;" ::: "memory"); }
+__device__ __forceinline__ void mbar_arrive(uint32_t mbar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(mbar) : "memory");
+}
+// shared memory: weights | a staging buffer per MMA warpgroup (its logits, then the epilogue's
+// outputs) | mbarriers: weights landed, full[2], empty[2]
+constexpr int kSampledStageBytes = kWgRows * FastShape::N3 * 4;
+constexpr int kSampledBarriers = 1 + 2 * kWarpgroups;
+
+// Profiling aid (-DWDB_PHASE_CLOCKS): like mlp_forward_body's, but per tile k < 18 of the CTA
+// [3 + 5 k + p]: p = 0 tile start (warpgroup 0), 1 warpgroup 0's layer 1 done, 2 warpgroup 0's
+// MMAs done, 3 warpgroup 1's MMAs done, 4 the epilogue warpgroup has stored both halves.
 template <bool TILES>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(kSampledThreads, 1)
 mlp_forward_sampled_kernel(const unsigned char *__restrict__ blob, const void *__restrict__ input,
                            long long rows, float *__restrict__ probs0, float *__restrict__ probs1,
                            float *__restrict__ values, const __grid_constant__ MlpSampling smp) {
-  mlp_forward_body<TILES, FastShape, false, true>(blob, input, rows, probs0, probs1, values,
-                                                  blockIdx.x, gridDim.x, 0, nullptr, smp);
+  using Shape = FastShape;
+  extern __shared__ __align__(128) unsigned char smem[];
+  const MlpHeader hd = *reinterpret_cast<const MlpHeader *>(blob);
+  const int F = hd.F, A0 = hd.A0, A1 = hd.A1;
+  constexpr int N3 = Shape::N3;
+  constexpr MlpLayout lay = mlp_layout(Shape::K1, Shape::H, Shape::N3);
+  constexpr int w_bytes = lay.total_bytes - lay.off_w1;  // W1 | W2 | W3 | biases, contiguous
+  unsigned char *s_w = smem;
+  const uint32_t s_w1 = smem_addr(s_w);
+  const uint32_t s_w2 = s_w1 + (lay.off_w2 - lay.off_w1);
+  const uint32_t s_w3 = s_w1 + (lay.off_w3 - lay.off_w1);
+  const float *s_b1 = reinterpret_cast<const float *>(s_w + (lay.off_b - lay.off_w1));
+  const float *s_b2 = s_b1 + Shape::H;
+  const float *s_b3 = s_b2 + Shape::H;
+  constexpr int stage0 = (w_bytes + 127) & ~127;
+  const uint32_t bar_w = smem_addr(s_w + stage0 + kWarpgroups * kSampledStageBytes);
+  auto bar_full = [&](int w) { return bar_w + 8 * (1 + w); };
+  auto bar_empty = [&](int w) { return bar_w + 8 * (1 + kWarpgroups + w); };
+  auto stage = [&](int w) { return reinterpret_cast<float *>(s_w + stage0 + w * kSampledStageBytes); };
+  const int tid = threadIdx.x, lt = tid & 127, wg = tid >> 7;
+  const unsigned bid = blockIdx.x, gdim = gridDim.x;
+  const long long n_tiles = (rows + kTileM - 1) / kTileM;
+#ifdef WDB_PHASE_CLOCKS
+  __shared__ int s_rec;
+  if (tid == 0) {
+    s_rec = bid == 0 && atomicCAS(&g_mlp_clocks_busy, 0, 1) == 0;
+    if (s_rec) {
+      for (int i = 0; i < kMlpClockSlots; i++) g_mlp_clocks[i] = 0;
+      g_mlp_clocks[0] = rows;
+    }
+  }
+  __syncthreads();
+  const bool rec_clocks = s_rec && lt == 0;
+  int clock_tile = 0;
+#endif
+  if (tid == 0) MLP_MARK(1);
+  if (tid == 0) {
+    mbar_init(bar_w, 1);
+    for (int w = 0; w < kWarpgroups; w++) {
+      mbar_init(bar_full(w), 128);
+      mbar_init(bar_empty(w), 128);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  // (the PDL order of mlp_forward_body with flags = 0: the weights are read after the wait)
+  griddep_wait();
+  if (tid == 0) {                                         // weights: TMA bulk copies
+    mbar_expect_tx(bar_w, (uint32_t)w_bytes);
+    uint32_t off = 0;
+    while (off < (uint32_t)w_bytes) {
+      const uint32_t n = min((uint32_t)w_bytes - off, 65536u);
+      tma_load(s_w1 + off, blob + lay.off_w1 + off, n, bar_w);
+      off += n;
+    }
+  }
+  griddep_launch_dependents();
+
+  if (wg < kWarpgroups) {
+    // ---- MMA warpgroup wg: rows [tile * 128 + 64 wg, + 64) of each of the CTA's tiles
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kMmaRegs));
+    ObsFrag<TILES, Shape::K1> next;
+    uint32_t a1[Shape::K1 / 4];
+    const bool have_first = bid < n_tiles && bid * kTileM + wg * kWgRows < rows;
+    if (have_first) obs_frag_load(next, 0, input, rows, F, bid * kTileM + wg * kWgRows);
+    mbar_wait(bar_w, 0);
+    if (tid == 0) MLP_MARK(2);
+    if (have_first) {
+      obs_frag_pack(next, 0, a1);
+      obs_frag_load(next, 1, input, rows, F, bid * kTileM + wg * kWgRows);
+      obs_frag_pack(next, 1, a1);
+    }
+    constexpr uint32_t sbo_a = (uint32_t)(Shape::K1 / 8) * 128u;
+    constexpr uint32_t sbo_h = (uint32_t)(Shape::H / 8) * 128u;
+    const int lane = tid & 31, lr = ((tid >> 5) & 3) * 16 + (lane >> 2), t = lane & 3;
+    uint32_t phase = 1;          // an empty buffer: the wait on the phase before the first passes
+    for (long long tile = bid; tile < n_tiles; tile += gdim) {
+      const long long row0 = tile * kTileM + wg * kWgRows;
+      if (row0 >= rows) break;   // (warpgroup-uniform; so are all later tiles)
+#ifdef WDB_PHASE_CLOCKS
+      const int mark0 = 3 + 5 * (clock_tile < 18 ? clock_tile : kMlpClockSlots);
+      clock_tile++;
+#endif
+      if (wg == 0) MLP_MARK(mark0);
+      uint32_t h[kMaxK / 4];
+      fast_layer1(a1, s_w1, sbo_a, s_b1, h);
+      if (wg == 0) MLP_MARK(mark0 + 1);
+      float o[kMaxN3 / 16][8];
+      float(&o48)[48 / 2] = *reinterpret_cast<float(*)[48 / 2]>(&o[0][0]);
+      fast_layers23<TILES>(h, s_w2, s_w3, sbo_h, s_b2, o48, next, a1,
+                           row0 + (long long)gdim * kTileM < rows, input, rows, F,
+                           row0 + (long long)gdim * kTileM);
+      wgmma_wait<0>();
+      MLP_MARK(mark0 + 2 + wg);
+      mbar_wait(bar_empty(wg), phase);      // the epilogue has copied out the previous tile
+      phase ^= 1;
+      float *s_o = stage(wg);
+      stage_logits(o, s_b3, N3, lr, t, s_o);
+      wg_sync(wg);
+      // thread lt: row lt % 64; lt < 64 head 0, else head 1 + the value (mlp_forward_body's
+      // softmax).  (Derived from an opaque copy of lt: otherwise they, and the 32
+      // staged-logit addresses, are hoisted out of the tile loop and held across its MMAs.)
+      int l = lt;
+      asm volatile("" : "+r"(l));
+      const int row = l & 63, part = l >> 6;
+      const int cbase = part ? A0 : 0, cnt = part ? A1 : A0;
+      float lg[32], value;
+      const float inv = softmax_row(s_o, N3, row, cbase, cnt, lg, value);
+      wg_sync(wg);                          // every logit has been read
+      float *dst = s_o + (part ? kWgRows * A0 : 0) + row * cnt;
+#pragma unroll
+      for (int i = 0; i < 32; i++)
+        if (i < cnt) dst[i] = lg[i] * inv;
+      if (part) s_o[kWgRows * (A0 + A1) + row] = value;
+      mbar_arrive(bar_full(wg));
+    }
+  } else {
+    // ---- epilogue warpgroup: thread lt samples head lt / 64 of row lt % 64 of each staged
+    // half-tile, in tile order, and the warpgroup copies the half-tile's outputs out
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kEpiRegs));
+    const int row = lt & 63, part = lt >> 6;
+    const int cnt = part ? A1 : A0;
+    uint32_t phase = 0;
+    for (long long tile = bid; tile < n_tiles; tile += gdim) {
+#ifdef WDB_PHASE_CLOCKS
+      const int mark0 = 3 + 5 * (clock_tile < 18 ? clock_tile : kMlpClockSlots);
+      clock_tile++;
+#endif
+#pragma unroll 1
+      for (int w = 0; w < kWarpgroups; w++) {
+        const long long rb = tile * kTileM + w * kWgRows;   // first row of the half-tile
+        if (rb >= rows) break;
+        // this thread's uniform's inputs, requested before the wait so that the loads overlap
+        // it; both threads of a row read the RNG offset before the epi_sync below, the head-0
+        // thread advances it after that barrier
+        const long long s_row = rb + row;
+        const bool s_valid = s_row < rows;
+        long long s_gi = 0;
+        unsigned long long s_seed = 0, s_off = 0;
+        float s_u = 0.0f;
+        if (s_valid) {
+          const long long env = s_row / smp.Np;
+          s_gi = env * smp.N + __ldg(smp.agent + (int)(s_row - env * smp.Np));
+          if (smp.uniforms) {
+            s_u = __ldg(smp.uniforms + 2 * s_gi + part);
+          } else {
+            s_seed = reinterpret_cast<const RngHeader *>(smp.rng)->seed;
+            s_off = rng_offsets(smp.rng)[s_gi];
+          }
+        }
+        const float *s_o = stage(w);
+        mbar_wait(bar_full(w), phase);
+        epi_sync();
+        if (s_valid) {
+          if (!smp.uniforms) {
+            RngHeader h;
+            h.seed = s_seed; h.n_streams = 0;
+            const uint4 d = rng_draw4(h, (unsigned long long)s_gi, s_off);
+            s_u = u32_to_uniform(part ? d.y : d.x);
+            if (!part) rng_offsets(smp.rng)[s_gi] = s_off + 1;
+          }
+          // the probabilities exactly as they were stored, sampled in registers
+          const float *src = s_o + (part ? kWgRows * A0 : 0) + row * cnt;
+          float p[32];
+#pragma unroll
+          for (int i = 0; i < 32; i++) p[i] = i < cnt ? src[i] : 0.0f;
+          smp.actions[2 * s_row + part] = sample_cdf_regs(p, cnt, s_u);
+        }
+        copy_outputs(s_o, rb, rows, A0, A1, probs0, probs1, values, lt);
+        mbar_arrive(bar_empty(w));                           // the buffer may be restaged
+      }
+      phase ^= 1;
+      MLP_MARK(mark0 + 4);
+    }
+  }
+#ifdef WDB_PHASE_CLOCKS
+  __syncthreads();
+  if (tid == 0 && s_rec) {
+    __threadfence();
+    atomicExch(&g_mlp_clocks_busy, 0);
+  }
+#endif
 }
 
 template <class Shape>
@@ -979,7 +1202,9 @@ int launch_forward_sampled(void *stream, const void *blob, int F, int H, int A0,
   if (reinterpret_cast<uintptr_t>(s->actions) & 7) return (int)cudaErrorMisalignedAddress;
   if (s->n_policy_agents < 1 || s->n_agents < s->n_policy_agents || rows % s->n_policy_agents)
     return (int)cudaErrorInvalidValue;
-  const size_t smem = mlp_smem_bytes(make_header(F, H, A0, A1));
+  constexpr MlpLayout lay = mlp_layout(FastShape::K1, FastShape::H, FastShape::N3);
+  const size_t smem = (size_t)((lay.total_bytes - lay.off_w1 + 127) & ~127) +
+                      kWarpgroups * kSampledStageBytes + 8 * kSampledBarriers;
   static size_t configured = 0;
   if (smem > configured) {
     const cudaError_t e = cudaFuncSetAttribute(mlp_forward_sampled_kernel<TILES>,
@@ -993,7 +1218,7 @@ int launch_forward_sampled(void *stream, const void *blob, int F, int H, int A0,
   const long long n_tiles = (rows + kTileM - 1) / kTileM;
   const int sm_budget = (g_mlp_max_ctas > 0 && g_mlp_max_ctas < kNumSMs) ? g_mlp_max_ctas : kNumSMs;
   const int grid = (int)min((long long)sm_budget, n_tiles);
-  mlp_forward_sampled_kernel<TILES><<<grid, kThreads, smem, as_stream(stream)>>>(
+  mlp_forward_sampled_kernel<TILES><<<grid, kSampledThreads, smem, as_stream(stream)>>>(
       reinterpret_cast<const unsigned char *>(blob), input, rows, probs0, probs1, values, smp);
   return finish_launch();
 }
