@@ -408,9 +408,11 @@ typedef struct wdb_sa_rollout {
    * action_bias (use_argmax: u = mu).  No OU state. */
   const float *log_std;              /* required with gaussian_head: [1] the log-std (1), or
                                       * [2] the log-std's clamp bounds min <= max (2) */
-  int gaussian_head;                 /* 0: tanh + OU, 1: Gaussian, 2: squashed Gaussian;
-                                      * discrete kinds: 3 = Q head, 4 = categorical Q head,
-                                      * 5 = noisy Q head, else softmax */
+  int gaussian_head;                 /* 0: tanh + OU, 1: Gaussian, 2: squashed Gaussian,
+                                      * 3: Gaussian on normalized observations; discrete
+                                      * kinds: 3 = Q head, 4 = categorical Q head, 5 = noisy
+                                      * Q head, 6 = softmax on normalized observations, else
+                                      * softmax */
   /* Discrete kinds, Q head (gaussian_head = 3; DQN's FullyConnectedQ): the head's raw outputs
    * are Q values, written to probs_batch when given, and the action is sampled as
    * wdb_sample_epsilon_greedy (stream = env, one draw per step) with epsilon = log_std[0], a
@@ -429,7 +431,12 @@ typedef struct wdb_sa_rollout {
    * = the given step + t at timestep t.  Output j = fmaf(f(eps_out)_j, s_j, m_j): m_j the Q head's
    * output (bias, then fmaf over the inputs in order), s_j = sigma_b_j then fmaf(sigma_W[j][i],
    * f(eps_in)_i * h_i, .) over i in order; use_argmax: m_j alone (the mean network) and epsilon
-   * 0.  Then sampled as the Q head is. */
+   * 0.  Then sampled as the Q head is.
+   * Normalized observations (gaussian_head = 6 on a discrete kind: the softmax head; 3 on a
+   * continuous kind: the Gaussian head): each observation element x enters the first layer as
+   * clamp((x - shift_i) * scale_i, -clip, clip) (a rounded subtract, then a rounded multiply,
+   * then the clamp: wdb_obs_normalize's arithmetic); obs_batch keeps the raw x.  log_std =
+   * [shift F | scale F | clip] on the device, after the log-std for the Gaussian head. */
 } wdb_sa_rollout;
 
 int wdb_single_agent_rollout_supported(int n_hidden, const int *dims);
@@ -1328,6 +1335,34 @@ int wdb_per_sample_windows(void *stream, const wdb_per_store *store,
 int wdb_per_set_priorities(void *stream, const wdb_per_store *store, const int *windows,
                            int n_windows, const float *q_values, const float *returns,
                            int oldest, int filled);
+
+/* Running observation statistics (per feature of a row-major [rows, F] float32 batch) and the
+ * normalization they drive.  A moments record is rows of float64 [n, mean_0 .. mean_{F-1},
+ * M2_0 .. M2_{F-1}] (M2 = the sum of squared deviations).  The running state is count
+ * (device scalar), mean [F] and M2 [F] in float64, and the float32 shift [F] = mean and scale
+ * [F] = 1 / sqrt(M2 / count + 1e-8) that the forwards read (count 0: shift 0, scale 1).
+ * Merges are Chan et al.'s in a fixed order, with no float atomics: bit-reproducible.
+ * 1 <= F <= 65536.  cudaErrorInvalidValue without launching on a bad shape or NULL pointer. */
+/* float64 elements of the scratch the update and batch passes take for `rows` x F (-1: bad
+ * shape). */
+long long wdb_obs_moments_scratch_doubles(long long rows, int F);
+/* Merges the batch x [rows, F] into the running state and rewrites shift and scale.  Two
+ * launches (per-CTA Welford records over fixed row ranges into scratch, then one CTA merging
+ * them in order), no host wait. */
+int wdb_obs_moments_update(void *stream, const float *x, long long rows, int F, double *scratch,
+                           double *count, double *mean, double *m2, float *shift, float *scale);
+/* The batch's own moments as one record [2F + 1] (two launches): what each GPU contributes
+ * before the records are gathered. */
+int wdb_obs_moments_batch(void *stream, const float *x, long long rows, int F, double *scratch,
+                          double *record);
+/* Merges n_records (<= 512) records [n_records][2F + 1] in order into the running state and
+ * rewrites shift and scale.  One launch. */
+int wdb_obs_moments_merge(void *stream, const double *records, int n_records, int F,
+                          double *count, double *mean, double *m2, float *shift, float *scale);
+/* y [rows, F] = clamp((x - shift) * scale, -clip, clip) per feature (clip finite, > 0): a
+ * rounded subtract, a rounded multiply, then the clamp.  One launch. */
+int wdb_obs_normalize(void *stream, const float *x, float *y, long long rows, int F,
+                      const float *shift, const float *scale, float clip);
 
 #ifdef __cplusplus
 }

@@ -70,6 +70,8 @@ WDB_API int wdb_single_agent_rollout_noisy_supported(int n_hidden, const int *di
 int sa_launch_categorical(void *stream, const wdb_sa_rollout *r, size_t smem);
 // sa_rollout_kernel<kSaNoisyQ>'s launch (wdb_sa_rollout_noisy.cu)
 int sa_launch_noisy(void *stream, const wdb_sa_rollout *r, size_t smem);
+// sa_rollout_kernel<kSaSoftmaxNorm / kSaGaussianNorm>'s launch (wdb_sa_rollout_obs_norm.cu)
+int sa_launch_obs_norm(void *stream, const wdb_sa_rollout *r, size_t smem);
 
 WDB_API int wdb_single_agent_rollout(void *stream, const wdb_sa_rollout *r) {
   if (!r) return (int)cudaErrorInvalidValue;
@@ -78,7 +80,9 @@ WDB_API int wdb_single_agent_rollout(void *stream, const wdb_sa_rollout *r) {
   if (rc != cudaSuccess) return rc;
   const bool continuous = r->env_kind >= WDB_SA_CONTINUOUS_MOUNTAIN_CAR;
   const bool squashed = continuous && r->gaussian_head == 2;
-  const bool gaussian = continuous && r->gaussian_head == 1;
+  // the softmax (6) and Gaussian (3) heads on normalized observations
+  const bool normalized = continuous ? r->gaussian_head == 3 : r->gaussian_head == 6;
+  const bool gaussian = continuous && (r->gaussian_head == 1 || normalized);
   const bool eps_greedy = !continuous && r->gaussian_head == 3;
   const bool categorical = !continuous && r->gaussian_head == 4;
   const bool noisy = !continuous && r->gaussian_head == 5;
@@ -91,8 +95,9 @@ WDB_API int wdb_single_agent_rollout(void *stream, const wdb_sa_rollout *r) {
     return (int)cudaErrorInvalidValue;
   for (int l = 0; l <= r->n_hidden; l++)
     if (!r->w[l] || !r->b[l]) return (int)cudaErrorInvalidValue;
-  if (continuous && (r->gaussian_head < 0 || r->gaussian_head > 2))
+  if (continuous && (r->gaussian_head < 0 || r->gaussian_head > 3))
     return (int)cudaErrorInvalidValue;
+  if (normalized && !r->log_std) return (int)cudaErrorInvalidValue;
   if (squashed || gaussian) {
     // log_std, and a normal source unless the deterministic action draws nothing
     if (!r->log_std || (!r->use_argmax && !r->normals && !r->rng_state))
@@ -121,6 +126,7 @@ WDB_API int wdb_single_agent_rollout(void *stream, const wdb_sa_rollout *r) {
   for (int l = 0; l <= r->n_hidden; l++)
     total += (long long)r->dims[l] * r->dims[l + 1] + r->dims[l + 1];
   const size_t smem = ((size_t)total + (size_t)kSaEnvsPerCta * 2 * kSaPitch) * sizeof(float);
+  if (normalized) return sa_launch_obs_norm(stream, r, smem);
   if (squashed) return sa_launch<kSaSquashed>(stream, r, smem);
   if (gaussian) return sa_launch<kSaGaussian>(stream, r, smem);
   if (eps_greedy) return sa_launch<kSaEpsGreedy>(stream, r, smem);

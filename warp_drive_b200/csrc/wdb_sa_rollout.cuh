@@ -1,14 +1,16 @@
 // wdb_sa_rollout.cuh -- the one-launch single-agent rollout kernel (see wdb_sa_rollout.cu for
 // what it does and why) and its launcher, one template over the action head.  wdb_sa_rollout.cu
 // instantiates the softmax, tanh / OU, Gaussian, squashed Gaussian and Q heads;
-// wdb_sa_rollout_categorical.cu the categorical Q head, in a translation unit of its own so
-// that the other kinds keep their file and machine code.  Each translation unit gets its own
+// wdb_sa_rollout_categorical.cu the categorical Q head, wdb_sa_rollout_noisy.cu the noisy Q head
+// and wdb_sa_rollout_obs_norm.cu the softmax and Gaussian heads on normalized observations, each
+// in a translation unit of its own so that the other kinds keep their file and machine code.  Each translation unit gets its own
 // copy (anonymous namespace).
 #pragma once
 
 #include <type_traits>
 
 #include "wdb_noisy.cuh"
+#include "wdb_obs_norm.cuh"
 #include "wdb_sa_physics.cuh"
 
 using namespace wdb;
@@ -85,6 +87,11 @@ static __device__ __noinline__ float sa_expectation(const float *y, const float 
 // j is fmaf(f(eps_out)_j, sigma_b_j + sum_i sigma_W[j][i] (f(eps_in)_i h_i), mu-part_j), the
 // mu-part computed exactly as the Q kind's head, fresh noise (noisy_f) per env row and step;
 // use_argmax: the mu-part alone.  Then epsilon_greedy_step.
+// kSaSoftmaxNorm, kSaGaussianNorm: the softmax and Gaussian kinds with the observation
+// normalized (obs_normalize) as it enters activation row 0; the batch slot keeps the raw x.
+// [shift F | scale F | clip] sit in the device buffer behind log_std (after the Gaussian
+// head's log-std).  (Each test of the kind is an `if constexpr` or a constant that the earlier
+// kinds evaluate as before: their machine code is unchanged.)
 // noisy_f as a call: the noisy kind's Philox, logf and cosf stay out of the rollout loop's
 // registers (inlined, they push the kernel past its register budget into spills)
 __device__ __noinline__ float sa_noise(unsigned long long seed, unsigned long long step,
@@ -93,12 +100,13 @@ __device__ __noinline__ float sa_noise(unsigned long long seed, unsigned long lo
 }
 
 enum { kSaSoftmax = 0, kSaTanhOu = 1, kSaGaussian = 2, kSaSquashed = 3, kSaEpsGreedy = 4,
-       kSaCategoricalQ = 5, kSaNoisyQ = 6 };
+       kSaCategoricalQ = 5, kSaNoisyQ = 6, kSaSoftmaxNorm = 7, kSaGaussianNorm = 8 };
 template <int kKind>
 __global__ void __launch_bounds__(kSaThreads, 9)
 sa_rollout_kernel(const __grid_constant__ wdb_sa_rollout R) {
   constexpr bool kContinuous = kKind != kSaSoftmax && kKind != kSaEpsGreedy &&
-                               kKind != kSaCategoricalQ && kKind != kSaNoisyQ;
+                               kKind != kSaCategoricalQ && kKind != kSaNoisyQ &&
+                               kKind != kSaSoftmaxNorm;
   extern __shared__ float s_w[];               // per layer: [Wt (in x out) | b (out)]
   __shared__ int s_dims[8];                    // layer widths (dynamic indexing of the kernel
   if (threadIdx.x < 5) s_dims[threadIdx.x] = R.dims[threadIdx.x];   // parameter goes through
@@ -181,6 +189,12 @@ sa_rollout_kernel(const __grid_constant__ wdb_sa_rollout R) {
         const float x = obs[i];
         buf0[i] = x;
         if (ob && live) ob[i] = x;
+      }
+      // the normalizing kinds: each lane normalizes the elements it just wrote
+      if constexpr (kKind == kSaSoftmaxNorm || kKind == kSaGaussianNorm) {
+        const float *nrm = R.log_std + (kKind == kSaGaussianNorm ? 1 : 0);
+        for (int i = sub; i < F; i += kSaGroup)
+          buf0[i] = obs_normalize(buf0[i], nrm[i], nrm[F + i], nrm[2 * F]);
       }
     }
     __syncwarp();
@@ -296,7 +310,7 @@ sa_rollout_kernel(const __grid_constant__ wdb_sa_rollout R) {
             rng_off, R.use_argmax);
         action = *dst;
         if (R.actions_batch) static_cast<float *>(R.actions_batch)[(size_t)t * E + env] = action;
-      } else if constexpr (kKind == kSaGaussian) {
+      } else if constexpr (kKind == kSaGaussian || kKind == kSaGaussianNorm) {
         // Gaussian head: the raw linear output is the mean; the stand-alone sampler's own step
         // writes the action straight into sampled_actions
         if (R.probs_batch) R.probs_batch[(size_t)t * E + env] = cur[0];

@@ -520,6 +520,11 @@ _SIGNATURES = {
     "wdb_single_agent_rollout_categorical_supported": (_i, [_i, ctypes.POINTER(_i), _i]),
     "wdb_single_agent_rollout_noisy_supported": (_i, [_i, ctypes.POINTER(_i)]),
     "wdb_single_agent_rollout": (_i, [_vp, ctypes.POINTER(SaRollout)]),
+    "wdb_obs_moments_scratch_doubles": (_ll, [_ll, _i]),
+    "wdb_obs_moments_update": (_i, [_vp, _vp, _ll, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "wdb_obs_moments_batch": (_i, [_vp, _vp, _ll, _i, _vp, _vp]),
+    "wdb_obs_moments_merge": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "wdb_obs_normalize": (_i, [_vp, _vp, _vp, _ll, _i, _vp, _vp, _f]),
     "wdb_mountain_car_step": (
         _i, [_vp, _i, _vp, _vp, _vp, _vp, _vp] + [_f] * 7 + [_vp, _i]),
     "wdb_continuous_mountain_car_step": (

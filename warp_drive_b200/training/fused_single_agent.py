@@ -73,6 +73,10 @@ class FusedSingleAgentRollout:
                 return False
             if getattr(model, "action_mask", None) is not None or getattr(model, "masked", False):
                 return False
+            # normalized observations: the softmax and Gaussian heads have kinds that normalize
+            if getattr(model, "normalize_observations", False) and continuous and not getattr(
+                    model, "is_gaussian", False):
+                return False
             # a noisy head draws fresh noise per env and step: the noisy Q kind takes a plain
             # head of one NoisyLinear; noisy C51 and noisy dueling heads act per step
             noisy = getattr(model, "noisy", False)
@@ -194,6 +198,15 @@ class FusedSingleAgentRollout:
         elif self.gaussian:
             r.gaussian_head = 1
             self._log_std = _unwrap(model).log_std
+        # normalized observations: the softmax (6) or Gaussian (3) kind that normalizes, reading
+        # [log_std (Gaussian) | shift F | scale F | clip] from a device buffer refreshed from the
+        # model's statistics at every launch
+        self.normalizing = bool(getattr(_unwrap(model), "normalize_observations", False))
+        if self.normalizing:
+            r.gaussian_head = 3 if self.gaussian else 6
+            self._norm_args = torch.empty(int(self.gaussian) + 2 * self.F + 1,
+                                          dtype=torch.float32, device=dm.device)
+            self._norm_args[-1] = float(_unwrap(model).observation_clip)
         elif self.continuous:
             actor = _unwrap(model)
             r.action_scale = float(actor.action_scale)
@@ -266,6 +279,11 @@ class FusedSingleAgentRollout:
             r.w[i], r.b[i] = _p(w.data), _p(b.data)
         if self.gaussian:
             r.log_std = _p(self._log_std.data)
+        if self.normalizing:
+            m = _unwrap(self.model)
+            parts = ([m.log_std.detach()] if self.gaussian else []) + [m.obs_shift, m.obs_scale]
+            torch.cat(parts, out=self._norm_args[:-1])
+            r.log_std = _p(self._norm_args)
         r.n_steps = int(n_steps)
         r.use_argmax = int(bool(use_argmax))
         r.uniforms = _p(uniforms)

@@ -12,6 +12,7 @@ import torch
 from torch import nn
 from torch.nn import functional as func
 
+from warp_drive_b200.training import obs_norm
 from warp_drive_b200.training.utils.data_loader import (
     action_head_sizes, get_flattened_obs_size)
 from warp_drive_b200.utils.constants import Constants
@@ -32,6 +33,7 @@ def apply_logit_mask(logits, mask=None):
 
 class FullyConnected(nn.Module):
     name = "torch_fully_connected"
+    normalize_observations = False
 
     def __init__(self, env, model_config, policy, policy_tag_to_agent_id_map,
                  create_separate_placeholders_for_each_policy=False,
@@ -69,6 +71,17 @@ class FullyConnected(nn.Module):
         self.use_fused_train_forward = bool(model_config.get("fused_train_forward", True))
         name = f"{_PROCESSED_OBSERVATIONS}_batch_{policy}"
         self.batch_size = env.cuda_data_manager.get_shape(name=name)[0]
+        # running observation statistics (training/obs_norm.py): buffers only when the key is
+        # on, so the state_dict of a model without it is unchanged
+        self.normalize_observations, self.observation_clip = obs_norm.obs_norm_settings(
+            model_config, model_config.get("type", "fully_connected"))
+        if self.normalize_observations:
+            obs_norm.register_buffers(self, self.flattened_obs_size)
+
+    def normalized_input(self, obs):
+        """The observations the first layer reads: normalized by the running statistics when
+        the model normalizes, else as given."""
+        return obs_norm.normalize(self, obs) if self.normalize_observations else obs
 
     # ---- observation plumbing (model_base.py:93-200)
     def reshape_and_flatten_obs(self, obs):
@@ -135,7 +148,7 @@ class FullyConnected(nn.Module):
 
             if fused_mlp_train.supported(self, obs, mask):
                 return fused_mlp_train.fused_train_forward(self, obs, mask)
-        x = obs
+        x = self.normalized_input(obs)
         for i in range(len(self.fc)):
             x = self.fc[str(i)](x)
         if self.is_deterministic:
@@ -180,7 +193,7 @@ class FullyConnectedGaussian(FullyConnected):
         self.use_fused_train_forward = False
 
     def forward(self, obs=None, action=None, action_mask=None):
-        x = obs
+        x = self.normalized_input(obs)
         for i in range(len(self.fc)):
             x = self.fc[str(i)](x)
         return [self.policy_head(x)], self.vf_head(x)[..., 0]

@@ -19,6 +19,9 @@ class FusedPolicyForward:
         try:
             if getattr(model, "is_deterministic", True) or len(model.fc) != 2:
                 return False
+            # (this forward reads raw observations)
+            if getattr(model, "normalize_observations", False):
+                return False
             dims = list(model.fc_dims)
             if dims[0] != dims[1] or len(model.output_dims) not in (1, 2):
                 return False

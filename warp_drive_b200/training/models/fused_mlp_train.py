@@ -153,6 +153,8 @@ def fused_train_forward(model, obs, mask=None):
     """FullyConnected.forward(obs, action_mask=mask) -> ([probs per head], values) through the
     fused node."""
     lead = obs.shape[:-1]
+    if getattr(model, "normalize_observations", False):
+        obs = model.normalized_input(obs)
     x = obs.reshape(-1, obs.shape[-1])
     if not x.is_contiguous():
         x = x.contiguous()

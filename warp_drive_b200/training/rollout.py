@@ -225,6 +225,9 @@ class RolloutEngine:
             return False
         if any(getattr(m, "action_mask", None) is not None for m in self.models.values()):
             return False
+        # its forwards read raw observations
+        if any(getattr(m, "normalize_observations", False) for m in self.models.values()):
+            return False
         # the library's launch plan decides the rest (shapes no kernel takes, e.g. envs too
         # large for the shared-memory observation tile, run the generic multi-launch path)
         from warp_drive_b200.training.fused_tag_continuous import FusedTagContinuousStep

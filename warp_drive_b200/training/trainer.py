@@ -26,6 +26,7 @@ import yaml
 from torch import nn
 
 from warp_drive_b200.managers.function_manager import CUDALogController, CUDASampler
+from warp_drive_b200.training import obs_norm
 from warp_drive_b200.training.algorithms.policygradient import A2C, PPO
 from warp_drive_b200.training.models.fully_connected import ModelFactory
 from warp_drive_b200.training.rollout import RolloutEngine
@@ -526,12 +527,24 @@ class Trainer:
                         float(self.engine.episodic_step_sum) / (n_done + _EPSILON)})
                 metrics_dict[policy] = metrics
         self.engine.refresh_forward_weights()
+        self._update_observation_statistics()
         if logging_flag:
             for policy in self.policies:
                 self.engine.episodic_reward_sum[policy].zero_()
             self.engine.episodic_step_sum.zero_()
             self.engine.num_completed_episodes.zero_()
         return metrics_dict
+
+    def _update_observation_statistics(self):
+        """Merge this iteration's raw observation batch into the running statistics of every
+        trained policy that normalizes its observations (training/obs_norm.py): after the last
+        optimizer step, so the next rollout and update see the new statistics."""
+        dm = self.cuda_envs.cuda_data_manager
+        for policy in self.policies_to_train:
+            model = self.models[policy]
+            if getattr(model, "normalize_observations", False):
+                obs = dm.data_on_device_via_torch(f"{_PROCESSED_OBSERVATIONS}_batch_{policy}")
+                obs_norm.update_moments(model, obs, self.num_devices)
 
     # ------------------------------------------------------------------ logging / ckpt
     def _log_metrics(self, metrics):
