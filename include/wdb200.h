@@ -1364,6 +1364,17 @@ int wdb_obs_moments_merge(void *stream, const double *records, int n_records, in
 int wdb_obs_normalize(void *stream, const float *x, float *y, long long rows, int F,
                       const float *shift, const float *scale, float clip);
 
+/* The running discounted return of reward scaling (SB3 VecNormalize's return filter), forward
+ * in time for every (env, agent) row i of rewards [T, E, Np] f32 and done [T, E] i32:
+ *   ret = __fadd_rn(__fmul_rn(gamma, carry[i]), r[t][i]);  returns[t][i] = ret;
+ *   carry[i] = done[t][env] > 0 ? 0 : ret.
+ * carry [E, Np] f32 is read and left holding the return after step T - 1.  No FMA is
+ * contracted, so a float32 restatement gives the same bits.  One launch, one thread per row.
+ * cudaErrorInvalidValue without launching on a NULL pointer or T, n_envs or n_agents < 1. */
+int wdb_discounted_return_scan(void *stream, const float *rewards, const int *done, int T,
+                               int n_envs, int n_agents, float gamma, float *carry,
+                               float *returns);
+
 #ifdef __cplusplus
 }
 #endif

@@ -525,6 +525,7 @@ _SIGNATURES = {
     "wdb_obs_moments_batch": (_i, [_vp, _vp, _ll, _i, _vp, _vp]),
     "wdb_obs_moments_merge": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "wdb_obs_normalize": (_i, [_vp, _vp, _vp, _ll, _i, _vp, _vp, _f]),
+    "wdb_discounted_return_scan": (_i, [_vp, _vp, _vp, _i, _i, _i, _f, _vp, _vp]),
     "wdb_mountain_car_step": (
         _i, [_vp, _i, _vp, _vp, _vp, _vp, _vp] + [_f] * 7 + [_vp, _i]),
     "wdb_continuous_mountain_car_step": (

@@ -16,7 +16,6 @@ import torch
 from warp_drive_b200 import lib as _lib
 
 DEFAULT_CLIP = 10.0
-_BUFFERS = ("obs_count", "obs_mean", "obs_m2", "obs_shift", "obs_scale")
 
 
 def obs_norm_settings(model_config, model_type):
@@ -69,7 +68,7 @@ def _rows(x, n_features, what):
         raise ValueError(f"{what}: a float32 CUDA batch [..., {n_features}] is normalized, got "
                          f"{x.dtype} {tuple(x.shape)} on {x.device}")
     if not x.is_contiguous():
-        raise ValueError(f"{what}: the observation batch must be [rows, F] contiguous")
+        raise ValueError(f"{what}: the batch must be [rows, F] contiguous")
     return x.numel() // n_features
 
 
@@ -88,39 +87,41 @@ def normalize(model, obs):
     return out
 
 
-def _state(model):
-    return [_lib.ptr(getattr(model, n)) for n in _BUFFERS]
+def _state(model, prefix):
+    return [_lib.ptr(getattr(model, f"{prefix}_{n}"))
+            for n in ("count", "mean", "m2", "shift", "scale")]
 
 
-def _scratch(model, rows, F):
+def _scratch(model, rows, F, prefix):
     n = int(_lib.load().wdb_obs_moments_scratch_doubles(rows, F))
-    buf = getattr(model, "_obs_moments_scratch", None)
-    if buf is None or buf.numel() < n or buf.device != model.obs_mean.device:
-        buf = torch.empty(n, dtype=torch.float64, device=model.obs_mean.device)
-        model._obs_moments_scratch = buf
+    name, dev = f"_{prefix}_moments_scratch", getattr(model, f"{prefix}_mean").device
+    buf = getattr(model, name, None)
+    if buf is None or buf.numel() < n or buf.device != dev:
+        buf = torch.empty(n, dtype=torch.float64, device=dev)
+        setattr(model, name, buf)
     return buf
 
 
-def update_moments(model, obs_batch, num_devices=1):
-    """Merge the raw observation batch (every row of the policy's [T, E, Np, F] batch) into the
-    model's running statistics and rewrite shift and scale, in place, without a host wait.
-    Several GPUs: each rank's batch moments are all-gathered and merged in rank order, so every
-    rank holds the same bits (one all-gather of 2F + 1 float64 per policy)."""
-    F = int(model.obs_shift.numel())
-    rows = _rows(obs_batch, F, "normalize_observations")
+def update_moments(model, batch, num_devices=1, prefix="obs"):
+    """Merge the raw batch [..., F] (for observations every row of the policy's [T, E, Np, F]
+    batch) into the model's running statistics `{prefix}_count`, `_mean`, `_m2` and rewrite
+    `{prefix}_shift` and `_scale`, in place, without a host wait.  Several GPUs: each rank's
+    batch moments are all-gathered and merged in rank order, so every rank holds the same bits
+    (one all-gather of 2F + 1 float64 per policy)."""
+    F = int(getattr(model, f"{prefix}_shift").numel())
+    rows = _rows(batch, F, f"the {prefix}_* statistics")
     L, s = _lib.load(), _lib.stream_ptr()
-    scratch = _scratch(model, rows, F)
+    scratch = _scratch(model, rows, F, prefix)
     if num_devices <= 1:
-        _lib.check(L.wdb_obs_moments_update(s, _lib.ptr(obs_batch), rows, F, _lib.ptr(scratch),
-                                            *_state(model)), "obs_moments_update")
+        _lib.check(L.wdb_obs_moments_update(s, _lib.ptr(batch), rows, F, _lib.ptr(scratch),
+                                            *_state(model, prefix)), "obs_moments_update")
         return
     import torch.distributed as dist
 
-    record = torch.empty(2 * F + 1, dtype=torch.float64, device=obs_batch.device)
-    _lib.check(L.wdb_obs_moments_batch(s, _lib.ptr(obs_batch), rows, F, _lib.ptr(scratch),
+    record = torch.empty(2 * F + 1, dtype=torch.float64, device=batch.device)
+    _lib.check(L.wdb_obs_moments_batch(s, _lib.ptr(batch), rows, F, _lib.ptr(scratch),
                                        _lib.ptr(record)), "obs_moments_batch")
-    gathered = torch.empty((num_devices, 2 * F + 1), dtype=torch.float64,
-                           device=obs_batch.device)
+    gathered = torch.empty((num_devices, 2 * F + 1), dtype=torch.float64, device=batch.device)
     dist.all_gather_into_tensor(gathered, record)
     _lib.check(L.wdb_obs_moments_merge(_lib.stream_ptr(), _lib.ptr(gathered), num_devices, F,
-                                       *_state(model)), "obs_moments_merge")
+                                       *_state(model, prefix)), "obs_moments_merge")

@@ -26,7 +26,7 @@ import yaml
 from torch import nn
 
 from warp_drive_b200.managers.function_manager import CUDALogController, CUDASampler
-from warp_drive_b200.training import obs_norm
+from warp_drive_b200.training import obs_norm, reward_scale
 from warp_drive_b200.training.algorithms.policygradient import A2C, PPO
 from warp_drive_b200.training.models.fully_connected import ModelFactory
 from warp_drive_b200.training.rollout import RolloutEngine
@@ -134,6 +134,8 @@ class Trainer:
         self.policies = list(config["policy"].keys())
         assert set(self.policies) == set(self.policy_tag_to_agent_id_map.keys())
         self.policies_to_train = [p for p in self.policies if config["policy"][p]["to_train"]]
+        reward_scaling = {p: reward_scale.reward_scale_settings(config["policy"][p], p)
+                          for p in self.policies}
 
         t = config["trainer"]
         self.num_episodes = t["num_episodes"]
@@ -175,6 +177,8 @@ class Trainer:
         for policy in self.policies:
             self.current_timestep[policy] = 0
             self._initialize_policy_model(policy)
+            if reward_scaling[policy][0]:
+                reward_scale.register_buffers(self.models[policy])
         self.load_model_checkpoint()
         for policy in self.policies:
             for model in self._all_networks(policy):
@@ -193,6 +197,16 @@ class Trainer:
         for policy in self.policies_to_train:
             self._initialize_policy_algorithm(policy)
         self._minibatch_steps = self._minibatch_schedule()
+        # running reward scaling (training/reward_scale.py) of the trained policies with the key
+        self._reward_scalers = {}
+        for policy in self.policies_to_train:
+            on, clip = reward_scaling[policy]
+            if on:
+                r = self.cuda_envs.cuda_data_manager.data_on_device_via_torch(
+                    f"{_REWARDS}_batch_{policy}")
+                self._reward_scalers[policy] = reward_scale.RewardScaler(
+                    self.models[policy], tuple(r.shape), config["policy"][policy]["gamma"],
+                    clip, r.device)
         if self.num_devices > 1:
             self._broadcast_parameters()
         self.engine = self._make_engine(use_cuda_graph)
@@ -338,7 +352,7 @@ class Trainer:
 
     # ------------------------------------------------------------------ training loop
     def train(self):
-        self.cuda_envs.reset_all_envs()
+        self._reset_all_envs()
         self.engine.resync_observations()
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
         n_agents = self.cuda_envs.n_agents
@@ -374,10 +388,11 @@ class Trainer:
         logging_flag = self._is_logging_iteration(iteration)
         dm = self.cuda_envs.cuda_data_manager
         done_flags_batch = dm.data_on_device_via_torch(f"{_DONE_FLAGS}_batch")
+        training_rewards = self._training_rewards(done_flags_batch)
         loss_metrics = {}
         for policy in self.policies_to_train:
             actions = dm.data_on_device_via_torch(f"{_ACTIONS}_batch_{policy}")
-            rewards = dm.data_on_device_via_torch(f"{_REWARDS}_batch_{policy}")
+            rewards = training_rewards[policy]
             obs = dm.data_on_device_via_torch(f"{_PROCESSED_OBSERVATIONS}_batch_{policy}")
             # every timestep of the batch is trained under its own action mask (the reference
             # applies the mask of the rollout's last step to all of them)
@@ -410,6 +425,7 @@ class Trainer:
         logging_flag = self._is_logging_iteration(iteration)
         dm = self.cuda_envs.cuda_data_manager
         done_flags_batch = dm.data_on_device_via_torch(f"{_DONE_FLAGS}_batch")
+        training_rewards = self._training_rewards(done_flags_batch)
         batches = {}
         for policy in self.policies_to_train:
             mask_name = f"{_ACTION_MASK}_batch_{policy}"
@@ -420,8 +436,7 @@ class Trainer:
                 self.models[policy],
                 dm.data_on_device_via_torch(f"{_PROCESSED_OBSERVATIONS}_batch_{policy}"),
                 dm.data_on_device_via_torch(f"{_ACTIONS}_batch_{policy}"),
-                dm.data_on_device_via_torch(f"{_REWARDS}_batch_{policy}"), done_flags_batch,
-                mask)
+                training_rewards[policy], done_flags_batch, mask)
         if self._perm_generator is None:
             self._perm_generator = torch.Generator(device=done_flags_batch.device)
             self._perm_generator.manual_seed(self.seed)
@@ -453,6 +468,19 @@ class Trainer:
                 loss_metrics[policy] = self.trainers[policy].minibatch_metrics(
                     batches[policy], sums[policy] / n_steps, self.current_timestep[policy])
         return self._finish_update(loss_metrics, step_info, logging_flag)
+
+    def _training_rewards(self, done_flags_batch):
+        """{trained policy: the rewards batch its update reads}: the data manager's own
+        `rewards_batch_{p}`, or for a policy with scale_rewards its scaled copy, made here from
+        the raw batch after the rollout and before any update work (training/reward_scale.py)."""
+        dm = self.cuda_envs.cuda_data_manager
+        out = {}
+        for policy in self.policies_to_train:
+            rewards = dm.data_on_device_via_torch(f"{_REWARDS}_batch_{policy}")
+            scaler = self._reward_scalers.get(policy)
+            out[policy] = (rewards if scaler is None
+                           else scaler.scale(rewards, done_flags_batch, self.num_devices))
+        return out
 
     def minibatch_permutation(self, n_rows):
         """The next epoch's order of a policy's n_rows batch rows (int32, on the device), drawn
@@ -518,6 +546,8 @@ class Trainer:
                 n_done = int(self.engine.num_completed_episodes)
                 metrics = loss_metrics.get(policy, {})
                 metrics["Current timestep"] = self.current_timestep[policy]
+                if policy in self._reward_scalers:
+                    metrics["Reward scale"] = float(self.models[policy].return_scale)
                 metrics.update({k: float(v) for k, v in norms.items()})
                 metrics.update(lrs)
                 metrics.update({
@@ -545,6 +575,12 @@ class Trainer:
             if getattr(model, "normalize_observations", False):
                 obs = dm.data_on_device_via_torch(f"{_PROCESSED_OBSERVATIONS}_batch_{policy}")
                 obs_norm.update_moments(model, obs, self.num_devices)
+
+    def _reset_all_envs(self):
+        """Restart every env; the running returns of reward scaling restart with them."""
+        self.cuda_envs.reset_all_envs()
+        for scaler in self._reward_scalers.values():
+            scaler.reset()
 
     # ------------------------------------------------------------------ logging / ckpt
     def _log_metrics(self, metrics):
@@ -629,7 +665,7 @@ class Trainer:
                       for p, ids in self.policy_tag_to_agent_id_map.items()}
         step_sum = {p: torch.zeros(self.num_envs, dtype=torch.int32, device=dev)
                     for p in self.policies}
-        self.cuda_envs.reset_all_envs()
+        self._reset_all_envs()
         done = dm.data_on_device_via_torch("_done_")
         with torch.no_grad():
             for _ in range(self.cuda_envs.episode_length):
@@ -644,7 +680,7 @@ class Trainer:
                 # done envs restart but keep their flag: one episode per env is counted
                 self.cuda_envs.reset_only_done_envs(undo_done_after_reset=False)
         eng.fused = fused
-        self.cuda_envs.reset_all_envs()
+        self._reset_all_envs()
         eng.resync_observations()
         return reward_sum, step_sum
 
@@ -667,7 +703,7 @@ class Trainer:
         assert 0 <= env_id < self.num_envs
         assert isinstance(list_of_states, list) and list_of_states
         dm = self.cuda_envs.cuda_data_manager
-        self.cuda_envs.reset_all_envs()
+        self._reset_all_envs()
         self.engine.resync_observations()
         T = self.cuda_envs.episode_length
         logger = CUDALogController(self.cuda_envs.cuda_function_manager)
@@ -730,7 +766,7 @@ class Trainer:
         finally:
             self.engine.fused = fused
             self.engine.sa = sa
-            self.cuda_envs.reset_all_envs()
+            self._reset_all_envs()
             self.engine.resync_observations()
         return out
 
@@ -741,7 +777,7 @@ class Trainer:
         assert 0 <= env_id < self.num_envs
         assert isinstance(list_of_states, list) and list_of_states
         dm = self.cuda_envs.cuda_data_manager
-        self.cuda_envs.reset_all_envs()
+        self._reset_all_envs()
         self.engine.resync_observations()
         T = self.cuda_envs.episode_length
         out = {}
@@ -774,7 +810,7 @@ class Trainer:
                     break
         finally:
             self.engine.fused = fused
-            self.cuda_envs.reset_all_envs()
+            self._reset_all_envs()
             self.engine.resync_observations()
         return out
 

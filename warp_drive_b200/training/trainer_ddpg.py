@@ -193,8 +193,10 @@ class TrainerDDPG(Trainer):
             "arrays: separate per-policy placeholders are not supported")
         if config is not None:
             from warp_drive_b200.training.obs_norm import refuse_obs_norm
+            from warp_drive_b200.training.reward_scale import refuse_reward_scale
 
             refuse_obs_norm(config, type(self).__name__)
+            refuse_reward_scale(config, type(self).__name__)
         super().__init__(env_wrapper, config, policy_tag_to_agent_id_map,
                          create_separate_placeholders_for_each_policy,
                          obs_dim_corresponding_to_num_agents, num_devices, device_id,
