@@ -1375,6 +1375,62 @@ int wdb_discounted_return_scan(void *stream, const float *rewards, const int *do
                                int n_envs, int n_agents, float gamma, float *carry,
                                float *returns);
 
+/* One discrete-action SAC update of one policy (Christodoulou 2019) over B sampled windows, read
+ * as wdb_dqn_update_sampled reads them, as two passes of two launches each (a tile kernel and
+ * the fixed-order reduction: bit-reproducible).  The actor and the four Q networks map F -> A
+ * (hidden Linear + ReLU layers, a raw Linear head): the actor's head is the logits z of a
+ * categorical policy, log pi = z - max z - log sum_a exp(z_a - max z) (a log-softmax), and each Q
+ * network's head is A action values.  alpha = exp(*log_alpha), read on the device.  Every sum
+ * over actions runs a = 0 .. A - 1 in order.
+ * Critic pass (wdb_sac_discrete_critic_update_sampled), per loss row g with the int32 action a
+ * at slot(0), obs at slot(0) and obs' at slot(n_step):
+ *   V' = sum_a pi'_a (min(target_critic(obs'), target_critic2(obs'))_a - alpha log pi'_a),
+ *        pi' = the actor's policy at obs' (no target actor),
+ *   R  = DQN's n-step recursion on V' (float32, every non-zero done flag terminal),
+ *   gradients of mse(critic(obs)[a], R) + mse(critic2(obs)[a], R) into critic / critic2.
+ * Actor pass (wdb_sac_discrete_actor_update_sampled), with h_a = alpha log pi_a - min(critic(obs),
+ *   critic2(obs))_a: the gradient of (1/B) sum_g sum_a pi_a h_a, d/dz_j = pi_j (h_j - sum_a pi_a
+ *   h_a) / B, into actor.gw / gb (no critic gradient).
+ * The critic pass reads actor, critic, critic2 and both target critics; the actor pass reads
+ * actor, critic and critic2. */
+typedef struct wdb_sac_discrete_update_args {
+  int n_envs, n_agents, obs_dim, n_actions;   /* E, Np, F, A */
+  int capacity, n_step;              /* ring slots C, n-step horizon (n_step + 1 <= C) */
+  float gamma;
+  const float *obs;                  /* [C, E, Np, F] */
+  const int *actions;                /* [C, E, Np, 1] */
+  const float *rewards;              /* [C, E, Np] */
+  const int *done;                   /* [C, E] */
+  const float *log_alpha;            /* device [1] */
+  wdb_ddpg_net actor, critic, critic2;          /* gradients: actor (actor pass), critics */
+  wdb_ddpg_net target_critic, target_critic2;   /* the critic's shape */
+  float *q1_values, *q2_values, *returns;       /* critic pass out [B]: Q1(obs)[a], Q2(obs)[a],
+                                                   R; or NULL */
+  float *entropies;                  /* actor pass out [B]: -sum_a pi_a log pi_a, or NULL */
+  double *sums;                      /* out [4]: sum (Q1 - R)^2, sum (Q2 - R)^2 (critic pass),
+                                        sum_g sum_a pi_a min(Q1, Q2)_a, sum_g sum_a pi_a log pi_a
+                                        (actor pass) */
+  void *workspace;                   /* the pass's _workspace_bytes() bytes */
+} wdb_sac_discrete_update_args;
+/* 1 if a pass takes the shapes: 0..3 hidden layers of width 1..64 per network, the four Q
+ * networks shaped alike, 2 <= A <= 64, F <= 63, E, Np >= 1, 1 <= n_step, n_step + 1 <= capacity,
+ * n_windows >= 1, and the pass's networks, gradient blocks and row tiles in one CTA's shared
+ * memory (the critic pass holds the actor, four Q networks and two gradient blocks).  No CUDA
+ * call. */
+int wdb_sac_discrete_critic_update_sampled_supported(const wdb_sac_discrete_update_args *update,
+                                                     int n_windows);
+long long wdb_sac_discrete_critic_update_sampled_workspace_bytes(
+    const wdb_sac_discrete_update_args *update, int n_windows);   /* -1: unsupported */
+int wdb_sac_discrete_actor_update_sampled_supported(const wdb_sac_discrete_update_args *update,
+                                                    int n_windows);
+long long wdb_sac_discrete_actor_update_sampled_workspace_bytes(
+    const wdb_sac_discrete_update_args *update, int n_windows);   /* -1: unsupported */
+/* cudaErrorInvalidValue without launching if unsupported or a required pointer is NULL. */
+int wdb_sac_discrete_critic_update_sampled(void *stream, const wdb_sac_discrete_update_args *update,
+                                           const wdb_replay_windows *windows);
+int wdb_sac_discrete_actor_update_sampled(void *stream, const wdb_sac_discrete_update_args *update,
+                                          const wdb_replay_windows *windows);
+
 #ifdef __cplusplus
 }
 #endif

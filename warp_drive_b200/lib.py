@@ -289,6 +289,20 @@ class SacUpdate(ctypes.Structure):
     ]
 
 
+class SacDiscreteUpdate(ctypes.Structure):
+    """struct wdb_sac_discrete_update_args (include/wdb200.h)."""
+
+    _fields_ = [
+        ("n_envs", _i), ("n_agents", _i), ("obs_dim", _i), ("n_actions", _i),
+        ("capacity", _i), ("n_step", _i), ("gamma", _f),
+        ("obs", _fp), ("actions", _fp), ("rewards", _fp), ("done", _fp), ("log_alpha", _fp),
+        ("actor", DdpgNet), ("critic", DdpgNet), ("critic2", DdpgNet),
+        ("target_critic", DdpgNet), ("target_critic2", DdpgNet),
+        ("q1_values", _fp), ("q2_values", _fp), ("returns", _fp), ("entropies", _fp),
+        ("sums", _fp), ("workspace", _fp),
+    ]
+
+
 class ReplayWindows(ctypes.Structure):
     """struct wdb_replay_windows (include/wdb200.h)."""
 
@@ -498,6 +512,18 @@ _SIGNATURES = {
     "wdb_c51_update_masked": (
         _i, [_vp, ctypes.POINTER(DqnUpdate), _i, _vp, _f, ctypes.POINTER(ReplayWindows), _vp,
              _vp]),
+    "wdb_sac_discrete_critic_update_sampled_supported": (
+        _i, [ctypes.POINTER(SacDiscreteUpdate), _i]),
+    "wdb_sac_discrete_critic_update_sampled_workspace_bytes": (
+        _ll, [ctypes.POINTER(SacDiscreteUpdate), _i]),
+    "wdb_sac_discrete_critic_update_sampled": (
+        _i, [_vp, ctypes.POINTER(SacDiscreteUpdate), ctypes.POINTER(ReplayWindows)]),
+    "wdb_sac_discrete_actor_update_sampled_supported": (
+        _i, [ctypes.POINTER(SacDiscreteUpdate), _i]),
+    "wdb_sac_discrete_actor_update_sampled_workspace_bytes": (
+        _ll, [ctypes.POINTER(SacDiscreteUpdate), _i]),
+    "wdb_sac_discrete_actor_update_sampled": (
+        _i, [_vp, ctypes.POINTER(SacDiscreteUpdate), ctypes.POINTER(ReplayWindows)]),
     "wdb_dueling_fold_supported": (_i, [ctypes.POINTER(DuelingHead)]),
     "wdb_dueling_unfold_grads_supported": (_i, [ctypes.POINTER(DuelingHead)]),
     "wdb_dueling_fold": (
