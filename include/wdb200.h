@@ -1431,6 +1431,65 @@ int wdb_sac_discrete_critic_update_sampled(void *stream, const wdb_sac_discrete_
 int wdb_sac_discrete_actor_update_sampled(void *stream, const wdb_sac_discrete_update_args *update,
                                           const wdb_replay_windows *windows);
 
+/* One TQC update of one policy (Kuznetsov et al. 2020, "Controlling Overestimation Bias with
+ * Truncated Mixture of Continuous Distributional Quantile Critics") over B sampled windows, read
+ * as wdb_sac_*_update_sampled read them, as two passes of two launches each (a tile kernel and
+ * the fixed-order reduction: bit-reproducible).  The actor is SAC's squashed Gaussian
+ * (wdb_sac_update_args: head 2A, the same sample and log pi); the two critics and their targets
+ * map obs ++ action to N quantiles theta_m,i (hidden Linear + ReLU layers, a raw Linear(H, N)
+ * head).  tau_i = (2i + 1) / (2N) in float32, K = 2 (N - n_drop), alpha = exp(*log_alpha) read
+ * on the device, H(u) = u^2 / 2 for |u| <= 1 else |u| - 1/2.
+ * Critic pass (wdb_tqc_critic_update_sampled), eps' = critic_noise[g] at obs' = obs at slot(n_step):
+ *   a', log pi' = the actor's sample at obs' (no target actor),
+ *   y_0 <= .. <= y_{K-1} = the K smallest of the 2N pooled atoms target_critic(obs', a') ++
+ *       target_critic2(obs', a') (pooled index m N + j; ties to the lower index: a stable sort),
+ *   T_k = the n-step return of the sampled passes bootstrapped with y_k - alpha log pi',
+ *   loss = sum_g sum_m,i,k |tau_i - 1{u < 0}| H(u) / (B 2 N K),  u = T_k - theta_m,i(obs, a),
+ *   its gradient d theta_m,i = -sum_k |tau_i - 1{u < 0}| clamp(u, -1, 1) / (B 2 N K) (each sum
+ *   over k ascending) back through critic / critic2 into their gw / gb (the targets detached).
+ * Actor pass (wdb_tqc_actor_update_sampled), eps = actor_noise[g] at obs: the gradient of
+ *   (1/B) sum_g (alpha log pi - Qbar_g), Qbar_g = the mean of the 2N quantiles of both critics at
+ *   (obs, a), into actor.gw / gb (the critics' weights only carry it to their action inputs).
+ * The critic pass reads actor, critic, critic2 and both target critics; the actor pass reads
+ * actor, critic and critic2. */
+typedef struct wdb_tqc_update_args {
+  int n_envs, n_agents, obs_dim, action_dim;   /* E, Np, F, A (the actor's head is 2A wide) */
+  int capacity, n_step;              /* ring slots C, n-step horizon (n_step + 1 <= C) */
+  int n_quantiles, n_drop;           /* N per critic, the top quantiles dropped per critic */
+  float gamma, action_scale, action_bias;
+  float log_std_min, log_std_max;
+  const float *log_alpha;            /* device [1] */
+  const float *obs;                  /* [C, E, Np, F] */
+  const float *actions;              /* [C, E, Np, A] */
+  const float *rewards;              /* [C, E, Np] */
+  const int *done;                   /* [C, E] */
+  const float *critic_noise;         /* [B, A] standard normal (eps') */
+  const float *actor_noise;          /* [B, A] (eps) */
+  wdb_ddpg_net actor, critic, critic2;          /* gradients: actor (actor pass), critics */
+  wdb_ddpg_net target_critic, target_critic2;   /* the critic's shape, head N */
+  float *q_means, *target_means;     /* critic pass out [B]: mean_m,i theta, mean_k T_k; or NULL */
+  float *log_probs;                  /* actor pass out [B]: log pi(a | obs), or NULL */
+  double *sums;                      /* out [4]: sum_g loss_g, sum_g mean theta (critic pass),
+                                        sum_g Qbar_g, sum_g log pi (actor pass) */
+  void *workspace;                   /* the pass's _workspace_bytes() bytes */
+} wdb_tqc_update_args;
+/* 1 if a pass takes the shapes: 0..3 hidden layers of width 1..64 per network, the four critics
+ * shaped alike, 2 <= N and 2N <= 64, 0 <= n_drop < N, A <= 32, F + A <= 64, E, Np >= 1,
+ * 1 <= n_step, n_step + 1 <= capacity, n_windows >= 1, log_std_min <= log_std_max, and the pass's
+ * networks, gradient blocks and row tiles in one CTA's shared memory (the critic pass holds the
+ * actor, four critics, two gradient blocks and 8 + 2 (hidden layers) row tiles).  No CUDA call. */
+int wdb_tqc_critic_update_sampled_supported(const wdb_tqc_update_args *update, int n_windows);
+long long wdb_tqc_critic_update_sampled_workspace_bytes(const wdb_tqc_update_args *update,
+                                                        int n_windows);   /* -1: unsupported */
+int wdb_tqc_actor_update_sampled_supported(const wdb_tqc_update_args *update, int n_windows);
+long long wdb_tqc_actor_update_sampled_workspace_bytes(const wdb_tqc_update_args *update,
+                                                       int n_windows);    /* -1: unsupported */
+/* cudaErrorInvalidValue without launching if unsupported or a required pointer is NULL. */
+int wdb_tqc_critic_update_sampled(void *stream, const wdb_tqc_update_args *update,
+                                  const wdb_replay_windows *windows);
+int wdb_tqc_actor_update_sampled(void *stream, const wdb_tqc_update_args *update,
+                                 const wdb_replay_windows *windows);
+
 #ifdef __cplusplus
 }
 #endif

@@ -303,6 +303,23 @@ class SacDiscreteUpdate(ctypes.Structure):
     ]
 
 
+class TqcUpdate(ctypes.Structure):
+    """struct wdb_tqc_update_args (include/wdb200.h)."""
+
+    _fields_ = [
+        ("n_envs", _i), ("n_agents", _i), ("obs_dim", _i), ("action_dim", _i),
+        ("capacity", _i), ("n_step", _i), ("n_quantiles", _i), ("n_drop", _i),
+        ("gamma", _f), ("action_scale", _f), ("action_bias", _f),
+        ("log_std_min", _f), ("log_std_max", _f), ("log_alpha", _fp),
+        ("obs", _fp), ("actions", _fp), ("rewards", _fp), ("done", _fp),
+        ("critic_noise", _fp), ("actor_noise", _fp),
+        ("actor", DdpgNet), ("critic", DdpgNet), ("critic2", DdpgNet),
+        ("target_critic", DdpgNet), ("target_critic2", DdpgNet),
+        ("q_means", _fp), ("target_means", _fp), ("log_probs", _fp),
+        ("sums", _fp), ("workspace", _fp),
+    ]
+
+
 class ReplayWindows(ctypes.Structure):
     """struct wdb_replay_windows (include/wdb200.h)."""
 
@@ -524,6 +541,14 @@ _SIGNATURES = {
         _ll, [ctypes.POINTER(SacDiscreteUpdate), _i]),
     "wdb_sac_discrete_actor_update_sampled": (
         _i, [_vp, ctypes.POINTER(SacDiscreteUpdate), ctypes.POINTER(ReplayWindows)]),
+    "wdb_tqc_critic_update_sampled_supported": (_i, [ctypes.POINTER(TqcUpdate), _i]),
+    "wdb_tqc_critic_update_sampled_workspace_bytes": (_ll, [ctypes.POINTER(TqcUpdate), _i]),
+    "wdb_tqc_critic_update_sampled": (
+        _i, [_vp, ctypes.POINTER(TqcUpdate), ctypes.POINTER(ReplayWindows)]),
+    "wdb_tqc_actor_update_sampled_supported": (_i, [ctypes.POINTER(TqcUpdate), _i]),
+    "wdb_tqc_actor_update_sampled_workspace_bytes": (_ll, [ctypes.POINTER(TqcUpdate), _i]),
+    "wdb_tqc_actor_update_sampled": (
+        _i, [_vp, ctypes.POINTER(TqcUpdate), ctypes.POINTER(ReplayWindows)]),
     "wdb_dueling_fold_supported": (_i, [ctypes.POINTER(DuelingHead)]),
     "wdb_dueling_unfold_grads_supported": (_i, [ctypes.POINTER(DuelingHead)]),
     "wdb_dueling_fold": (

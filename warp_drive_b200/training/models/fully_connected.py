@@ -235,15 +235,18 @@ class ModelFactory:
             cls._registry[model_name] = FullyConnectedCategoricalQ
         if model_name not in cls._registry and model_name in (
                 "fully_connected_actor", "fully_connected_action_value_critic",
-                "fully_connected_sac_actor"):
-            # the DDPG pair (reference factory.py:10-16) and SAC's actor, imported on first use
+                "fully_connected_sac_actor", "fully_connected_quantile_critic"):
+            # the DDPG pair (reference factory.py:10-16), SAC's actor and TQC's critic,
+            # imported on first use
             from warp_drive_b200.training.models.fully_connected_actor_critic import (
-                FullyConnectedActionValueCritic, FullyConnectedActor, FullyConnectedSACActor)
+                FullyConnectedActionValueCritic, FullyConnectedActor,
+                FullyConnectedQuantileCritic, FullyConnectedSACActor)
 
             cls._registry["fully_connected_actor"] = FullyConnectedActor
             cls._registry["fully_connected_action_value_critic"] = (
                 FullyConnectedActionValueCritic)
             cls._registry["fully_connected_sac_actor"] = FullyConnectedSACActor
+            cls._registry["fully_connected_quantile_critic"] = FullyConnectedQuantileCritic
         if model_name not in cls._registry:
             raise ValueError(f"unknown model type '{model_name}'")
         return cls._registry[model_name]

@@ -131,6 +131,50 @@ class FullyConnectedActionValueCritic(FullyConnected):
         return self.vf_head(x)[..., 0]
 
 
+class FullyConnectedQuantileCritic(FullyConnectedActionValueCritic):
+    """TQC's distributional critic: the FullyConnectedActionValueCritic trunk on obs ++ action
+    and a raw `vf_head = Linear(H, N)`, N = model config key `num_quantiles` (default 25, an
+    integer in [2, 64]).  `forward(obs, action)` is the N quantiles [..., N] at the midpoint
+    fractions (2i + 1) / (2N)."""
+
+    name = "torch_fully_connected_quantile_critic"
+
+    def __init__(self, env, model_config, *args, **kwargs):
+        n = model_config.get("num_quantiles", 25)
+        if isinstance(n, bool) or not isinstance(n, int) or not 2 <= n <= 64:
+            raise ValueError(f"num_quantiles must be an integer in [2, 64], got {n!r}")
+        super().__init__(env, model_config, *args, **kwargs)
+        self.num_quantiles = n
+        self.vf_head = nn.Linear(self.fc_dims[-1], n)
+
+    def forward(self, obs=None, action=None):
+        assert action is not None
+        parts = [obs] + (list(action) if isinstance(action, (list, tuple)) else [action])
+        x = torch.cat(parts, dim=-1)
+        for i in range(len(self.fc)):
+            x = self.fc[str(i)](x)
+        return self.vf_head(x)
+
+
+class QuantileCritics(nn.Module):
+    """TQC's M quantile critics as one module: what the critic optimizer steps (and clips by
+    their joint norm) and the `{policy}_critic_{t}` checkpoint holds.  `forward(obs, action)` is
+    [..., M, N]."""
+
+    def __init__(self, critics):
+        super().__init__()
+        self.critics = nn.ModuleList(critics)
+
+    def __len__(self):
+        return len(self.critics)
+
+    def __getitem__(self, m):
+        return self.critics[m]
+
+    def forward(self, obs=None, action=None):
+        return torch.stack([c(obs=obs, action=action) for c in self.critics], dim=-2)
+
+
 class ActorAsPolicy(nn.Module):
     """Adapter for the rollout engine, whose forward contract is `(probs, values)`.  A
     squashed-Gaussian actor hands the engine its raw head output [mu ++ log-std], which
