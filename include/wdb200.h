@@ -1186,6 +1186,68 @@ int wdb_c51_update_masked(void *stream, const wdb_dqn_update_args *update, int n
                           const float *support, float delta_z, const wdb_replay_windows *windows,
                           const float *weights, const float *action_mask);
 
+/* Action branching (Tavakoli, Pardo & Kormushev 2018): one Q head per action dimension of a
+ * MultiDiscrete space on a shared trunk.  Heads d = 0 .. D-1 have sizes A_d and offsets
+ * o_d = A_0 + ... + A_{d-1}; the network's raw head has A = sum_d A_d outputs and Q_d(s, .) is
+ * columns o_d .. o_d + A_d - 1.  Actions are laid out [rows, D]: one int32 per head. */
+typedef struct wdb_q_branches {
+  int n_heads;                       /* D, 1 .. 16 */
+  int sizes[16];                     /* A_d >= 1 for d < D; the rest are not read */
+} wdb_q_branches;
+
+/* Epsilon-greedy per head: row r's head d applies wdb_sample_epsilon_greedy's rule to Q_d with
+ * ONE Philox block on stream r at offset o_r + d (o_r the row's offset), or with the words
+ * (x, y) = words[r][d] ([n_rows][D][2], test hook; no RNG state read or advanced); the row's
+ * offset then advances by D.  Each head explores on its own with probability epsilon.
+ * q_values [n_rows, A], actions [n_rows, D].  At D = 1 the actions and offsets are
+ * wdb_sample_epsilon_greedy's bit for bit.  One launch.  cudaErrorInvalidValue unless
+ * 0 <= epsilon <= 1 and the branches are valid (1 <= D <= 16, every A_d >= 1). */
+int wdb_sample_epsilon_greedy_branching(void *stream, void *rng_state, const float *q_values,
+                                        const wdb_q_branches *branches, int *actions,
+                                        long long n_rows, float epsilon,
+                                        const unsigned int *words);
+
+/* One branching double-DQN update over B sampled windows, read as wdb_dqn_update_sampled reads
+ * them, with update->n_actions = A and actions [C, E, Np, D].  Per window g with the D actions
+ * a_d at slot(0), every float32 operation in ascending d:
+ *   a*_d   = the first argmax of online_d(obs') (double_q),
+ *   boot_d = target_d(obs')[a*_d]  (double_q) or max target_d(obs'),
+ *   boot   = (sum_d boot_d) / D (the mean target of BDQ),
+ *   R      = DQN's n-step recursion from boot (every non-zero done flag terminal),
+ *   loss   = (1/B) sum_g w_g (1/D) sum_d huber(Q_d(obs, a_d) - R, delta),
+ * and its gradient w_g clamp(Q_d - R, -delta, delta) * (float)(1 / (B D)) in column o_d + a_d,
+ * back through the online network into q.gw / gb (w_g = weights[g], or 1 without weights).  An
+ * action outside [0, A_d) contributes nothing.  sums[0] = sum_g w_g (1/D) sum_d huber,
+ * sums[1] = sum_g Q-bar_g; the optional outputs [B] are q_values = Q-bar_g = (sum_d
+ * Q_d(obs, a_d)) / D and returns = R.  Every divide by D is exact at D = 1, so one head gives
+ * wdb_dqn_update_sampled's / _prioritized's bits.  Per-CTA partials summed in a fixed order by
+ * a second launch: bit-reproducible.  Two launches.
+ * Supported: the shapes of wdb_dqn_update_sampled_supported with 1 <= D <= 16, every A_d >= 1
+ * and sum_d A_d = A <= 64.  No CUDA call. */
+int wdb_branching_dqn_update_sampled_supported(const wdb_dqn_update_args *update,
+                                               const wdb_q_branches *branches, int n_windows);
+long long wdb_branching_dqn_update_sampled_workspace_bytes(const wdb_dqn_update_args *update,
+                                                           const wdb_q_branches *branches,
+                                                           int n_windows);
+/* cudaErrorInvalidValue without launching if unsupported or a required pointer is NULL. */
+int wdb_branching_dqn_update_sampled(void *stream, const wdb_dqn_update_args *update,
+                                     const wdb_q_branches *branches,
+                                     const wdb_replay_windows *windows);
+/* The importance-weighted form (weights [B], wdb_per_sample_windows): the same shapes,
+ * workspace, sums and launches.  Unit weights reproduce the uniform pass bit for bit. */
+int wdb_branching_dqn_update_prioritized_supported(const wdb_dqn_update_args *update,
+                                                   const wdb_q_branches *branches,
+                                                   int n_windows);
+long long wdb_branching_dqn_update_prioritized_workspace_bytes(const wdb_dqn_update_args *update,
+                                                               const wdb_q_branches *branches,
+                                                               int n_windows);
+/* cudaErrorInvalidValue without launching if unsupported or a required pointer (weights
+ * included) is NULL. */
+int wdb_branching_dqn_update_prioritized(void *stream, const wdb_dqn_update_args *update,
+                                         const wdb_q_branches *branches,
+                                         const wdb_replay_windows *windows,
+                                         const float *weights);
+
 /* Dueling head (Wang et al. 2016, the mean combine) of a DQN or C51 network, and its fold into
  * the plain MLP head the passes above run.  The head reads the trunk output h (width H) through
  * two streams, each with one hidden Linear(H, S) + ReLU when S > 0 and none when S = 0 (the

@@ -1,7 +1,8 @@
 // wdb_dqn_pass.cuh -- DQN's replay-update tile body and its plan (QR-DQN's at N = 1), shared by
-// wdb_ddpg_update.cu (dqn_pass_kernel, dqn_weighted_kernel, and QR-DQN's plan) and
-// wdb_masked_q.cu (the action-masked kernels).  kMasked = false is the code the pinned kernels
-// were compiled from; the masked bootstrap sits under `if constexpr`.
+// wdb_ddpg_update.cu (dqn_pass_kernel, dqn_weighted_kernel, and QR-DQN's plan),
+// wdb_masked_q.cu (the action-masked kernels) and wdb_branching_q.cu (the action-branching
+// kernels).  kMasked = kBranching = false is the code the pinned kernels were compiled from; the
+// masked bootstrap and the branching bootstrap and gradient sit under `if constexpr`.
 #pragma once
 
 #include "wdb_common.cuh"
@@ -43,11 +44,17 @@ long long dqn_workspace_bytes(const Plan &P) { return 16ll * P.grid + 4ll * P.gr
 // thread; a row with no valid action takes every action.  The first maximum among the valid
 // actions is the first maximum overall when every action is valid, so an all-ones mask gives
 // the unmasked pass's bits.
-template <bool kWeighted, bool kMasked = false>
+// kBranching (wdb_branching_dqn_update_sampled / _prioritized): the head holds D branches
+// (*branches), the row's D actions sit at actions[(slot(0) * EN + n) * D + d], the bootstrap is
+// the mean over the branches of each branch's DQN bootstrap, and each valid branch action gets
+// the Huber gradient against the shared return, scaled by 1 / (B D); the loss row and Q-bar are
+// the means over the branches.  Every divide by D is exact at D = 1: DQN's bits.
+template <bool kWeighted, bool kMasked = false, bool kBranching = false>
 __device__ __forceinline__ void dqn_tile_pass(const wdb_dqn_update_args &U, const Plan &Pg,
                                               float *partials, double *psums,
                                               const int2 *windows, const float *weights,
-                                              const float *action_mask = nullptr) {
+                                              const float *action_mask = nullptr,
+                                              const wdb_q_branches *branches = nullptr) {
   extern __shared__ __align__(16) float smem[];
   __shared__ Plan P;
   __shared__ double s_h[kRows], s_q[kRows];
@@ -106,10 +113,24 @@ __device__ __forceinline__ void dqn_tile_pass(const wdb_dqn_update_args &U, cons
       for (int c = 0; c < A; c++) dq[c] = 0.0f;
       if (g < M) {
         const Row w = rows.at(g);
-        const int a = U.actions[(long long)rows.slot(w, 0) * EN + w.n];
+        const int a = kBranching ? 0 : U.actions[(long long)rows.slot(w, 0) * EN + w.n];
         const float *qt = QT + r * kPitch;
         float boot;
-        if constexpr (kMasked) {
+        if constexpr (kBranching) {
+          // per branch: the target's value of the online first argmax, or the target's max
+          // (its value at the target's own first argmax); then their mean
+          const float *qc = U.double_q ? QD + r * kPitch : qt;
+          const int D = branches->n_heads;
+          float sum = 0.0f;
+          for (int d = 0, o = 0; d < D; o += branches->sizes[d], d++) {
+            float best = qc[o];
+            int k = o;
+            for (int c = o + 1; c < o + branches->sizes[d]; c++)
+              if (best < qc[c]) { best = qc[c]; k = c; }
+            sum = d == 0 ? qt[k] : __fadd_rn(sum, qt[k]);
+          }
+          boot = __fdiv_rn(sum, (float)D);
+        } else if constexpr (kMasked) {
           // a* over the valid actions of obs' own mask (slot n_step); none valid: every action
           const float *mk = action_mask + ((long long)rows.slot(w, ns) * EN + w.n) * A;
           bool any = false;
@@ -140,8 +161,43 @@ __device__ __forceinline__ void dqn_tile_pass(const wdb_dqn_update_args &U, cons
           ret = __fadd_rn(__fmul_rn(__fmul_rn(om, gamma), ret),
                           U.rewards[(long long)pk * EN + w.n]);
         }
-        // (an action outside [0, A) -- never written by the samplers -- contributes nothing)
-        if (a >= 0 && a < A) {
+        if constexpr (kBranching) {
+          // (a branch action outside [0, A_d) -- never written by the samplers -- contributes
+          // nothing)
+          const int D = branches->n_heads;
+          const float nd = (float)(1.0 / ((double)M * (double)D));
+          const int *acts = U.actions + ((long long)rows.slot(w, 0) * EN + w.n) * D;
+          double h_row = 0.0;
+          float q_sum = 0.0f;
+          bool any = false;
+          for (int d = 0, o = 0; d < D; o += branches->sizes[d], d++) {
+            const int ab = acts[d];
+            if (ab < 0 || ab >= branches->sizes[d]) continue;
+            const float q = QS[r * kPitch + o + ab];
+            const float diff = __fsub_rn(q, ret);
+            const double ad = fabs((double)diff);
+            if constexpr (kWeighted) {
+              const float w = weights[g];
+              const double wd = (double)w;
+              dq[o + ab] = __fmul_rn(__fmul_rn(fminf(fmaxf(diff, -delta), delta), w), nd);
+              h_row += ad < (double)delta ? (0.5 * wd) * ad * ad
+                                          : (wd * (double)delta) * (ad - 0.5 * (double)delta);
+            } else {
+              dq[o + ab] = __fmul_rn(fminf(fmaxf(diff, -delta), delta), nd);
+              h_row += ad < (double)delta ? 0.5 * ad * ad
+                                          : (double)delta * (ad - 0.5 * (double)delta);
+            }
+            q_sum = any ? __fadd_rn(q_sum, q) : q;
+            any = true;
+          }
+          if (any) {
+            const float q_bar = __fdiv_rn(q_sum, (float)D);
+            h_acc += h_row / (double)D;
+            q_acc += (double)q_bar;
+            if (U.q_values) U.q_values[g] = q_bar;
+          }
+        } else if (a >= 0 && a < A) {
+          // (an action outside [0, A) -- never written by the samplers -- contributes nothing)
           const float q = QS[r * kPitch + a];
           const float diff = __fsub_rn(q, ret);
           const double ad = fabs((double)diff);

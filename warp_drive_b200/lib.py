@@ -347,6 +347,15 @@ class IqnArgs(ctypes.Structure):
     ]
 
 
+Q_MAX_BRANCHES = 16                          # wdb_q_branches.sizes
+
+
+class QBranches(ctypes.Structure):
+    """struct wdb_q_branches (include/wdb200.h)."""
+
+    _fields_ = [("n_heads", _i), ("sizes", _i * Q_MAX_BRANCHES)]
+
+
 class DuelingHead(ctypes.Structure):
     """struct wdb_dueling_head (include/wdb200.h)."""
 
@@ -529,6 +538,22 @@ _SIGNATURES = {
     "wdb_c51_update_masked": (
         _i, [_vp, ctypes.POINTER(DqnUpdate), _i, _vp, _f, ctypes.POINTER(ReplayWindows), _vp,
              _vp]),
+    "wdb_sample_epsilon_greedy_branching": (
+        _i, [_vp, _vp, _vp, ctypes.POINTER(QBranches), _vp, _ll, _f, _vp]),
+    "wdb_branching_dqn_update_sampled_supported": (
+        _i, [ctypes.POINTER(DqnUpdate), ctypes.POINTER(QBranches), _i]),
+    "wdb_branching_dqn_update_sampled_workspace_bytes": (
+        _ll, [ctypes.POINTER(DqnUpdate), ctypes.POINTER(QBranches), _i]),
+    "wdb_branching_dqn_update_sampled": (
+        _i, [_vp, ctypes.POINTER(DqnUpdate), ctypes.POINTER(QBranches),
+             ctypes.POINTER(ReplayWindows)]),
+    "wdb_branching_dqn_update_prioritized_supported": (
+        _i, [ctypes.POINTER(DqnUpdate), ctypes.POINTER(QBranches), _i]),
+    "wdb_branching_dqn_update_prioritized_workspace_bytes": (
+        _ll, [ctypes.POINTER(DqnUpdate), ctypes.POINTER(QBranches), _i]),
+    "wdb_branching_dqn_update_prioritized": (
+        _i, [_vp, ctypes.POINTER(DqnUpdate), ctypes.POINTER(QBranches),
+             ctypes.POINTER(ReplayWindows), _vp]),
     "wdb_sac_discrete_critic_update_sampled_supported": (
         _i, [ctypes.POINTER(SacDiscreteUpdate), _i]),
     "wdb_sac_discrete_critic_update_sampled_workspace_bytes": (

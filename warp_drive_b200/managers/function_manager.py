@@ -549,7 +549,8 @@ class CUDASampler:
             "sample_squashed_gaussian")
 
     def sample_epsilon_greedy(self, q_values: torch.Tensor, actions: torch.Tensor,
-                              epsilon: float = 0.0, words=None, action_mask=None):
+                              epsilon: float = 0.0, words=None, action_mask=None,
+                              branch_sizes=None):
         """Epsilon-greedy over Q values (DQN): q_values [n_envs, n_agents, A] float32 ->
         actions [n_envs, n_agents, 1] int32.  Row r of the [n_envs * n_agents] rows draws one
         Philox block on RNG stream r (its offset advances by 1) and explores iff the uniform of
@@ -559,11 +560,20 @@ class CUDASampler:
         `action_mask` (float32 [n_envs, n_agents, A], non-zero = valid): the same draw over the
         row's valid actions only, the k-th valid one when exploring and the first maximum among
         them otherwise; a row with none valid takes the unmasked action
-        (wdb_sample_epsilon_greedy_masked)."""
+        (wdb_sample_epsilon_greedy_masked).  `branch_sizes` [A_0, ..., A_{D-1}] (action
+        branching, sum A_d = A): head d of each row is epsilon-greedy over its Q columns
+        o_d .. o_d + A_d - 1 on its own, with the Philox block at the row's offset + d; the
+        offset then advances by D, and actions are [n_envs, n_agents, D]
+        (wdb_sample_epsilon_greedy_branching; `words` [n_envs, n_agents, D, 2])."""
         assert self._random_initialized, (
             "sample_epsilon_greedy() requires the random seed initialized first, call "
             "init_random()")
         assert q_values.shape[0] == self._num_envs and q_values.dim() == 3
+        if branch_sizes is not None:
+            assert action_mask is None, "branching Q values take no action mask"
+            self._sample_epsilon_greedy_branching(q_values, actions, epsilon, words,
+                                                  branch_sizes)
+            return
         assert tuple(actions.shape) == tuple(q_values.shape[:-1]) + (1,)
         assert actions.dtype == torch.int32 and actions.is_contiguous()
         assert q_values.shape[0] * q_values.shape[1] <= self._num_envs * self._num_agents
@@ -585,6 +595,31 @@ class CUDASampler:
             _stream(), _P(self.rng_state), _P(q_values), _P(actions),
             int(q_values.shape[0] * q_values.shape[1]), int(q_values.shape[-1]),
             float(epsilon), _P(words)), "sample_epsilon_greedy")
+
+    def _sample_epsilon_greedy_branching(self, q_values, actions, epsilon, words, branch_sizes):
+        sizes = [int(a) for a in branch_sizes]
+        D = len(sizes)
+        if not 1 <= D <= _libmod.Q_MAX_BRANCHES or min(sizes) < 1:
+            raise ValueError(f"branch_sizes holds 1 to {_libmod.Q_MAX_BRANCHES} head sizes >= 1, "
+                             f"got {sizes}")
+        assert q_values.shape[-1] == sum(sizes)
+        assert tuple(actions.shape) == tuple(q_values.shape[:-1]) + (D,)
+        assert actions.dtype == torch.int32 and actions.is_contiguous()
+        assert q_values.shape[0] * q_values.shape[1] <= self._num_envs * self._num_agents
+        if not 0.0 <= float(epsilon) <= 1.0:
+            raise ValueError(f"epsilon must be in [0, 1], got {epsilon}")
+        if words is not None:
+            assert tuple(words.shape) == tuple(q_values.shape[:-1]) + (D, 2)
+            assert words.dtype == torch.int32 and words.is_contiguous()
+        q_values = q_values.detach().float().contiguous()
+        b = _libmod.QBranches()
+        b.n_heads = D
+        for d, a in enumerate(sizes):
+            b.sizes[d] = a
+        _libmod.check(_libmod.load().wdb_sample_epsilon_greedy_branching(
+            _stream(), _P(self.rng_state), _P(q_values), ctypes.byref(b), _P(actions),
+            int(q_values.shape[0] * q_values.shape[1]), float(epsilon), _P(words)),
+            "sample_epsilon_greedy_branching")
 
     @staticmethod
     def assign(data_manager: CUDADataManager, actions: np.ndarray, action_name: str):

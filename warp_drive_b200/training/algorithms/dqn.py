@@ -6,7 +6,8 @@ shapes the native pass does not take, and tests/dqn_update_reference.py restates
 NumPy.  QuantileDQN is quantile-regression DQN on the same windows (wdb_qr_dqn_update_sampled,
 tests/qr_dqn_reference.py), ImplicitQuantileDQN implicit quantile networks
 (wdb_iqn_update_sampled, tests/iqn_reference.py), CategoricalDQN categorical DQN
-(wdb_c51_update_sampled, tests/c51_reference.py).
+(wdb_c51_update_sampled, tests/c51_reference.py), BranchingDQN action branching over the heads of
+a MultiDiscrete space (wdb_branching_dqn_update_sampled, tests/branching_q_reference.py).
 
 Action masks: every loss takes `boot_mask` [B, A], obs' own action mask; the bootstrap's argmax /
 max then ranges over its valid actions (masked_scores), the rule of wdb_dqn_update_masked and
@@ -90,6 +91,44 @@ class DQN:
         of the returns [B]."""
         return {"Q loss": float(loss), "Mean Q value": float(mean_q),
                 "Mean return": float(returns.double().mean())}
+
+
+class BranchingDQN(DQN):
+    """Branching DQN (Tavakoli, Pardo & Kormushev 2018) on DQN's windows and n-step recursion,
+    for a FullyConnectedBranchingQ: the torch statement of wdb_branching_dqn_update_sampled
+    (include/wdb200.h), restated in float64 NumPy by tests/branching_q_reference.py.  Heads
+    d = 0 .. D-1 are column blocks of the one Q head; each head bootstraps as DQN does and the
+    return is built on their mean (BDQ's mean target), shared by every head's loss."""
+
+    def bootstrap(self, q_net, target_net, boot_obs, boot_mask=None):
+        """(1/D) sum_d boot_d [B] (no gradient), boot_d = target_d(obs')[argmax online_d(obs')]
+        with double_q (the first maximum), else max target_d(obs'); summed in ascending d."""
+        assert boot_mask is None, "branching DQN takes no action mask"
+        with torch.no_grad():
+            targets = q_net.branches(target_net.q_values(boot_obs))
+            online = q_net.branches(q_net.q_values(boot_obs)) if self.double_q else targets
+            total = None
+            for qt, qc in zip(targets, online):
+                b = qt.gather(-1, qc.argmax(dim=-1, keepdim=True))[..., 0]
+                total = b if total is None else total + b
+            return total / len(targets)
+
+    def loss(self, q_net, target_net, obs, actions, rewards, done, boot_obs, weights=None,
+             boot_mask=None):
+        """(loss, Q-bar [B], R [B]) of B sampled windows, the arguments of DQN.loss with actions
+        [B, D]: (1/B) sum_g w_g (1/D) sum_d huber(Q_d(obs, a_d) - R_g, delta), w = 1 without
+        weights, and Q-bar = (1/D) sum_d Q_d(obs, a_d), which feeds the metrics and the
+        priorities."""
+        with torch.no_grad():
+            returns = self.sampled_returns(rewards, done, self.bootstrap(
+                q_net, target_net, boot_obs, boot_mask))
+        heads = q_net.branches(q_net.q_values(obs))
+        a = actions.long().reshape(obs.shape[0], len(heads))
+        q = torch.stack([h.gather(-1, a[:, d:d + 1])[..., 0] for d, h in enumerate(heads)], -1)
+        rows = func.huber_loss(q, returns[:, None].expand_as(q), reduction="none",
+                               delta=self.huber_delta).mean(dim=-1)
+        loss = rows.mean() if weights is None else (weights * rows).mean()
+        return loss, q.mean(dim=-1), returns
 
 
 class QuantileDQN(DQN):

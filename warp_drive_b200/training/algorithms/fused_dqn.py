@@ -14,7 +14,8 @@ updates (algorithms/dqn.py) stay for the shapes these do not take.  An action-ma
 network (plain, dueling or noisy) runs `wdb_dqn_update_masked` / `wdb_c51_update_masked`
 (csrc/wdb_masked_q.cu; FusedMaskedDQNUpdate, FusedMaskedC51Update), whose bootstrap ranges over
 the valid actions of obs' own mask; masked QR-DQN and IQN networks train through the torch
-losses."""
+losses.  A branching network (one Q head per action dimension of a MultiDiscrete space) runs
+`wdb_branching_dqn_update_sampled` (csrc/wdb_branching_q.cu; FusedBranchingDQNUpdate)."""
 import ctypes
 
 import torch
@@ -23,7 +24,8 @@ from warp_drive_b200 import lib as _lib
 from warp_drive_b200.training.algorithms.fused_ddpg import (
     _set_pointers, _set_shape, replay_windows)
 from warp_drive_b200.training.models.fully_connected_q import (
-    FullyConnectedCategoricalQ, FullyConnectedIQN, FullyConnectedQ, FullyConnectedQuantileQ)
+    FullyConnectedBranchingQ, FullyConnectedCategoricalQ, FullyConnectedIQN, FullyConnectedQ,
+    FullyConnectedQuantileQ)
 from warp_drive_b200.utils.spaces import Box
 
 
@@ -36,6 +38,8 @@ def _shape_struct(algo, q_net, n_envs, n_agents, capacity):
     u = _lib.DqnUpdate()
     u.n_envs, u.n_agents = int(n_envs), int(n_agents)
     u.obs_dim, u.n_actions = int(q_net.flattened_obs_size), int(q_net.output_dims[0])
+    if getattr(q_net, "is_branching_q", False):   # the heads side by side: A = sum_d A_d
+        u.n_actions = int(sum(q_net.branch_sizes))
     u.capacity, u.n_step = int(capacity), int(algo.n_step)
     u.gamma, u.huber_delta = float(algo.discount_factor_gamma), float(algo.huber_delta)
     u.double_q = int(algo.double_q)
@@ -143,6 +147,51 @@ class FusedDQNUpdate(FusedQUpdate):
         else:
             _lib.check(self.lib.wdb_dqn_update_prioritized(
                 _lib.stream_ptr(), u, windows, _lib.ptr(weights)), "dqn_update_prioritized")
+
+
+def q_branches(q_net):
+    """struct wdb_q_branches of a FullyConnectedBranchingQ, or None when it has more heads than
+    the struct holds (such a network trains through the torch loss)."""
+    sizes = q_net.branch_sizes
+    if len(sizes) > _lib.Q_MAX_BRANCHES:
+        return None
+    b = _lib.QBranches()
+    b.n_heads = len(sizes)
+    for d, a in enumerate(sizes):
+        b.sizes[d] = int(a)
+    return b
+
+
+class FusedBranchingDQNUpdate(FusedQUpdate):
+    """`wdb_branching_dqn_update_sampled` (FullyConnectedBranchingQ): DQN's shapes with the head
+    A = sum_d A_d <= 64 and 1 <= D <= 16 heads, the heads' sizes beside the struct; actions
+    [C, E, Np, D].  The sums are sum_g w_g (1/D) sum_d huber(Q_d - R) and sum Q-bar, the outputs
+    Q-bar and R.  With weights the launch is `wdb_branching_dqn_update_prioritized`, which takes
+    the same shapes and workspace."""
+    model = FullyConnectedBranchingQ
+    entry = "branching_dqn_update_sampled"
+
+    @staticmethod
+    def shape_args(q_net):
+        return (ctypes.byref(q_branches(q_net)),)
+
+    @classmethod
+    def fits(cls, u, q_net, replay_rows):
+        return q_branches(q_net) is not None and super().fits(u, q_net, replay_rows)
+
+    def __init__(self, algo, q_net, *args, **kwargs):
+        super().__init__(algo, q_net, *args, **kwargs)
+        self.branches = q_branches(q_net)
+
+    def _run(self, u, windows, weights):
+        if weights is None:
+            _lib.check(self.lib.wdb_branching_dqn_update_sampled(
+                _lib.stream_ptr(), u, ctypes.byref(self.branches), windows),
+                "branching_dqn_update_sampled")
+        else:
+            _lib.check(self.lib.wdb_branching_dqn_update_prioritized(
+                _lib.stream_ptr(), u, ctypes.byref(self.branches), windows, _lib.ptr(weights)),
+                "branching_dqn_update_prioritized")
 
 
 class FusedQRDQNUpdate(FusedQUpdate):
@@ -593,3 +642,4 @@ fused_iqn_supported = FusedIQNUpdate.supported
 fused_c51_supported = FusedC51Update.supported
 fused_dueling_supported = FusedDuelingUpdate.supported
 fused_noisy_supported = FusedNoisyUpdate.supported
+fused_branching_dqn_supported = FusedBranchingDQNUpdate.supported

@@ -233,6 +233,12 @@ class ModelFactory:
                 FullyConnectedCategoricalQ)
 
             cls._registry[model_name] = FullyConnectedCategoricalQ
+        if model_name == "fully_connected_branching_q" and model_name not in cls._registry:
+            # branching DQN's Q network (one head per action dimension), imported on first use
+            from warp_drive_b200.training.models.fully_connected_q import (
+                FullyConnectedBranchingQ)
+
+            cls._registry[model_name] = FullyConnectedBranchingQ
         if model_name not in cls._registry and model_name in (
                 "fully_connected_actor", "fully_connected_action_value_critic",
                 "fully_connected_sac_actor", "fully_connected_quantile_critic"):

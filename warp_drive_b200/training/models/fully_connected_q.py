@@ -17,6 +17,10 @@ with factorized Gaussian noise (`noisy_sigma0`, 0.5 by default); the trunk stays
 uses noise only while its `noise` is set (the update's sample, or per-row acting noise), and is
 the mean network otherwise, so the evaluator plays the mean network.
 
+Action branching (Tavakoli, Pardo & Kormushev 2018): FullyConnectedBranchingQ
+(`fully_connected_branching_q`) takes a MultiDiscrete space (or one Discrete head) and puts one Q
+head per action dimension on the shared trunk, as column blocks of one raw Linear.
+
 Action masks: the model key `masked: true` over a Dict observation space with an `action_mask`
 key of width A sets `masked` (without the key such a space is refused, as before).  The
 mask is not a model input (`flattened_obs_size` excludes it) and the Q values stay raw: the
@@ -33,7 +37,7 @@ from torch.nn import functional as func
 from warp_drive_b200.training.utils.data_loader import (
     action_head_sizes, dict_observation_keys, get_flattened_obs_size)
 from warp_drive_b200.utils.constants import Constants
-from warp_drive_b200.utils.spaces import Discrete
+from warp_drive_b200.utils.spaces import Discrete, MultiDiscrete
 
 _ACTION_MASK = Constants.ACTION_MASK
 
@@ -493,3 +497,79 @@ class FullyConnectedCategoricalQ(FullyConnectedQ):
         """The expectation sum_j z_j p_j of every action: [..., A]."""
         p = self.probabilities(obs)
         return (p * self.support.to(p.dtype)).sum(dim=-1)
+
+
+# the model keys of the other Q networks, which branching does not combine with
+_BRANCHING_REFUSED = ("dueling", "stream_fc_dims", "noisy", "noisy_sigma0", "masked",
+                      "num_quantiles", "num_cosines", "num_tau_samples", "num_tau_prime_samples",
+                      "num_quantile_samples", "num_atoms", "v_min", "v_max")
+
+
+class FullyConnectedBranchingQ(nn.Module):
+    """The Q network of branching DQN (algorithms/dqn.py BranchingDQN; Tavakoli, Pardo &
+    Kormushev 2018, "Action Branching Architectures for Deep Reinforcement Learning") for a
+    MultiDiscrete action space, or one Discrete head (D = 1).
+
+    FullyConnectedQ's trunk (`fc.{i}.0`) and ONE raw `policy_head = Linear(H, A)`,
+    A = sum_d A_d over the heads' sizes `branch_sizes`: head d's Q values are columns
+    o_d .. o_d + A_d - 1, o_d = A_0 + ... + A_{d-1}, so the outputs grow with the sum of the head
+    sizes, not their product.  The module names and parameter creation order are
+    FullyConnectedQ's, so at D = 1 the same seed gives the same weights and a checkpoint loads
+    into either type.  `q_values` returns [..., A] and `forward` `([Q], None)`; the rollout
+    samples each head epsilon-greedily on its own (CUDASampler.sample_epsilon_greedy with
+    `branch_sizes`).
+
+    Refused: Box actions, an `action_mask`, and the keys of the other Q networks (dueling, noisy,
+    masked, quantile, IQN and C51 heads)."""
+    name = "torch_fully_connected_branching_q"
+    is_q_network = True
+    is_branching_q = True
+    is_deterministic = False
+    action_mask = None
+    masked = dueling = noisy = False
+
+    def __init__(self, env, model_config, policy, policy_tag_to_agent_id_map,
+                 create_separate_placeholders_for_each_policy=False,
+                 obs_dim_corresponding_to_num_agents="first"):
+        super().__init__()
+        for key in _BRANCHING_REFUSED:
+            if key in model_config and model_config[key] not in (False, None):
+                raise ValueError(f"fully_connected_branching_q does not take model.{key}, got "
+                                 f"{model_config[key]!r}")
+        self.fc_dims = list(model_config["fc_dims"])
+        self.policy = policy
+        sample_agent = policy_tag_to_agent_id_map[policy][0]
+        self.observation_space = env.env.observation_space[sample_agent]
+        action_space = env.env.action_space[sample_agent]
+        if not isinstance(action_space, (Discrete, MultiDiscrete)):
+            raise ValueError("fully_connected_branching_q takes a Discrete or MultiDiscrete "
+                             f"action space, got {type(action_space).__name__}")
+        if dict_observation_keys(self.observation_space)[1]:
+            raise ValueError("fully_connected_branching_q does not take observations with an "
+                             "action_mask")
+        heads, _ = action_head_sizes(action_space)
+        self.branch_sizes = [int(a) for a in heads]
+        self.output_dims = list(self.branch_sizes)
+        self.flattened_obs_size = get_flattened_obs_size(self.observation_space)
+        dims = [self.flattened_obs_size] + self.fc_dims
+        self.fc = nn.ModuleDict({
+            str(i): nn.Sequential(nn.Linear(dims[i], dims[i + 1]), nn.ReLU())
+            for i in range(len(self.fc_dims))})
+        self.policy_head = nn.Linear(dims[-1], sum(self.branch_sizes))
+
+    def noisy_layers(self):
+        return []
+
+    def branches(self, q):
+        """Q [..., A] split into the heads' Q values [[..., A_d] per head]."""
+        return list(torch.split(q, self.branch_sizes, dim=-1))
+
+    def q_values(self, obs):
+        """Every head's Q values, side by side: [..., A]."""
+        x = obs
+        for i in range(len(self.fc)):
+            x = self.fc[str(i)](x)
+        return self.policy_head(x)
+
+    def forward(self, obs=None, action=None, action_mask=None):
+        return [self.q_values(obs)], None

@@ -225,6 +225,9 @@ class RolloutEngine:
             return False
         if any(getattr(m, "action_mask", None) is not None for m in self.models.values()):
             return False
+        # it samples its heads from softmax probabilities: a Q network acts epsilon-greedily
+        if self.q_network:
+            return False
         # its forwards read raw observations
         if any(getattr(m, "normalize_observations", False) for m in self.models.values()):
             return False
@@ -626,21 +629,31 @@ class RolloutEngine:
         _sample_gaussian: one policy covering the array samples into it, several sample their
         own rows, which one launch scatters into place.  A masked policy samples over the valid
         actions of the mask rows its last evaluate_policies gathered (the batch slot, or the
-        scratch rows of an evaluation step)."""
+        scratch rows of an evaluation step).  A branching Q network of D > 1 heads samples
+        each head on its own into [E, Np, D] rows (and the per-head sampled_actions_{k}{suffix}
+        are written as well)."""
         actions = self._tensor(f"{_ACTIONS}{suffix}")
         masks = getattr(self, "_q_masks", {})
+
+        def draw(p, q, out):
+            sizes = getattr(self.models[p], "branch_sizes", None)
+            kw = {"branch_sizes": sizes} if sizes is not None and len(sizes) > 1 else {
+                "action_mask": masks.get(p)}
+            self.sampler.sample_epsilon_greedy(q, out, **kw, **sample_params)
         if len(q_values) == 1:
             (p, q), = q_values.items()
-            self.sampler.sample_epsilon_greedy(q, actions, action_mask=masks.get(p),
-                                               **sample_params)
-            return
-        if not hasattr(self, "_q_rows"):
-            self._q_rows = {p: torch.empty(q.shape[:-1] + (1,), dtype=torch.int32,
-                                           device=q.device) for p, q in q_values.items()}
-        for p, q in q_values.items():
-            self.sampler.sample_epsilon_greedy(q, self._q_rows[p], action_mask=masks.get(p),
-                                               **sample_params)
-        self._move_rows(actions, self._q_rows, scatter=True)
+            draw(p, q, actions)
+        else:
+            if not hasattr(self, "_q_rows"):
+                self._q_rows = {p: torch.empty(q.shape[:-1] + actions.shape[-1:],
+                                               dtype=torch.int32, device=q.device)
+                                for p, q in q_values.items()}
+            for p, q in q_values.items():
+                draw(p, q, self._q_rows[p])
+            self._move_rows(actions, self._q_rows, scatter=True)
+        if actions.shape[-1] > 1:
+            for k in range(actions.shape[-1]):
+                self._tensor(f"{_ACTIONS}_{k}{suffix}").copy_(actions[..., k:k + 1])
 
     def sample_actions(self, probs, t, **sample_params):
         """probs -> sampled_actions (trainer_base.py:466-512); the per-policy batch push of the

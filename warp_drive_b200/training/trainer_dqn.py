@@ -74,15 +74,25 @@ obs' own mask, the row at the window's slot(n_step): the native DQN and C51 pass
 dueling or noisy, through wdb_dqn_update_masked / wdb_c51_update_masked (FusedMaskedDQNUpdate,
 FusedMaskedC51Update), and QR-DQN, IQN and every shape outside the passes through the torch
 losses' `boot_mask`.  A row with no valid action falls back to the unmasked rule.
+
+Action branching: a `fully_connected_branching_q` model over a MultiDiscrete action space
+(Tavakoli, Pardo & Kormushev 2018) has one Q head per action dimension on a shared trunk.  The
+rollout samples each head epsilon-greedily on its own (CUDASampler.sample_epsilon_greedy with
+`branch_sizes`, one launch), the ring keeps the D actions of every step, and BranchingDQN's loss
+regresses every head on the return built from the mean of the heads' bootstraps
+(wdb_branching_dqn_update_sampled / _prioritized, 2 launches, or torch autograd).  `Mean Q value`
+is the mean of Q-bar, the mean over the heads of Q_d(obs, a_d), and with prioritized replay the
+priorities are (|Q-bar - R| + epsilon)^alpha.
 """
 import os
 
 import torch
 
 from warp_drive_b200.training.algorithms.dqn import (
-    DQN, CategoricalDQN, ImplicitQuantileDQN, QuantileDQN)
+    DQN, BranchingDQN, CategoricalDQN, ImplicitQuantileDQN, QuantileDQN)
 from warp_drive_b200.training.algorithms.fused_dqn import (
-    NOISY_UPDATE, FusedC51Update, FusedDQNUpdate, FusedDuelingUpdate, FusedIQNUpdate,
+    NOISY_UPDATE, FusedBranchingDQNUpdate, FusedC51Update, FusedDQNUpdate, FusedDuelingUpdate,
+    FusedIQNUpdate,
     FusedMaskedC51Update, FusedMaskedDQNUpdate, FusedNoisyUpdate, FusedQRDQNUpdate, draw_noise)
 from warp_drive_b200.training.trainer_ddpg import (
     RingRolloutEngine, TrainerDDPG, hard_update, soft_update)
@@ -188,8 +198,8 @@ class TrainerDQN(TrainerDDPG):
         self.q_models[policy] = self._build_model(policy, model_cfg)
         if not getattr(self.q_models[policy], "is_q_network", False):
             raise ValueError("DQN's model is a `fully_connected_q`, a `fully_connected_quantile_q`, "
-                             "a `fully_connected_iqn` or a `fully_connected_categorical_q`, got "
-                             f"'{model_cfg.get('type')}'")
+                             "a `fully_connected_iqn`, a `fully_connected_categorical_q` or a "
+                             f"`fully_connected_branching_q`, got '{model_cfg.get('type')}'")
         self.target_q_models[policy] = self._build_model(policy, model_cfg)
         hard_update(self.target_q_models[policy], self.q_models[policy])
 
@@ -221,9 +231,10 @@ class TrainerDQN(TrainerDDPG):
         self.update_count[policy] = 0
         quantile = getattr(q_net, "is_quantile_q", False)
         implicit = getattr(q_net, "is_implicit_quantile_q", False)
+        branching = getattr(q_net, "is_branching_q", False)
         algo = self.trainers[policy] = (
             CategoricalDQN if categorical else ImplicitQuantileDQN if implicit
-            else QuantileDQN if quantile else DQN)(
+            else QuantileDQN if quantile else BranchingDQN if branching else DQN)(
             discount_factor_gamma=c["gamma"], n_step=self.n_step, double_q=double_q,
             huber_delta=delta)
         n_agents = len(self.policy_tag_to_agent_id_map[policy])
@@ -248,6 +259,7 @@ class TrainerDQN(TrainerDDPG):
         fused = (FusedNoisyUpdate if q_net.noisy else FusedDuelingUpdate if q_net.dueling
                  else (FusedMaskedC51Update if masked else FusedC51Update) if categorical
                  else FusedIQNUpdate if implicit else FusedQRDQNUpdate if quantile
+                 else FusedBranchingDQNUpdate if branching
                  else FusedMaskedDQNUpdate if masked else FusedDQNUpdate)
         if fused.supported(algo, q_net, self.num_envs, n_agents, self.ring_capacity, rows):
             extra = (self.seed,) if q_net.noisy else ()
@@ -364,7 +376,8 @@ class TrainerDQN(TrainerDDPG):
 
     def _fused_q_gradients(self, policy, fused, logging_flag):
         """The same gradient from the native pass (FusedDQNUpdate, FusedQRDQNUpdate,
-        FusedIQNUpdate, FusedC51Update, FusedDuelingUpdate or FusedNoisyUpdate), written straight
+        FusedIQNUpdate, FusedC51Update, FusedDuelingUpdate, FusedNoisyUpdate or
+        FusedBranchingDQNUpdate), written straight
         into the arena's .grad views; the host waits only on logging iterations (metrics)."""
         eng = self.engine
         outputs, weights = None, None
