@@ -286,6 +286,10 @@ typedef struct wdb_tc_rollout {
                                       * probs0 / probs1 and the RNG are not used.  Only the packed
                                       * kernel of up to 320 threads per CTA takes this mode
                                       * (wdb_tag_continuous_rollout_supported reads this field). */
+  int env_begin, env_count;          /* step envs [env_begin, env_begin + env_count) only (0, 0:
+                                      * all); every array is still the whole [E, ...] one,
+                                      * addressed by global env and agent index.  Only the packed
+                                      * kernel takes a proper subrange. */
 } wdb_tc_rollout;
 
 int wdb_tag_continuous_rollout_step(void *stream, const wdb_tc_env *env,
@@ -575,6 +579,10 @@ typedef struct wdb_mlp_sampling {
   const int *agent_of_slot;          /* [Np] */
   int n_agents;                      /* N */
   int n_policy_agents;               /* Np; rows must be a multiple of it */
+  long long row_offset;              /* the launch's rows are rows [row_offset, + rows) of the
+                                      * policy (a multiple of Np): row r samples agent
+                                      * (row_offset + r) / Np * N + agent_of_slot[...]; actions
+                                      * and every other row array start at the launch's row 0 */
 } wdb_mlp_sampling;
 int wdb_mlp_forward_samples(int F, int H, int A0, int A1);
 int wdb_mlp_policy_forward_sampled(void *stream, const void *blob, int F, int H, int A0, int A1,

@@ -767,14 +767,15 @@ mlp_forward_kernel(const unsigned char *__restrict__ blob, const void *__restric
 
 // ---- The sampling forward (FastShape only, wdb_mlp_policy_forward_sampled): besides the
 // probabilities and values it draws both heads' actions of every row, as the fused
-// TagContinuous step would from the stored probabilities.  Row r = env * Np + slot of the
-// policy is agent gi = env * N + agent[slot].
+// TagContinuous step would from the stored probabilities.  Row r of the launch is row
+// row0 + r = env * Np + slot of the policy, agent gi = env * N + agent[slot].
 struct MlpSampling {
   int *actions;               // [rows, 2]
   void *rng;                  // RNG state of E * N streams (NULL with uniforms)
   const float *uniforms;      // [E * N * 2] or NULL
   const int *agent;           // [Np]
   int N, Np;
+  long long row0;             // the launch's first row among the policy's rows
 };
 
 // Three warpgroups with fixed roles.  Warpgroups 0 and 1 each own 64 rows of every 128-row
@@ -956,8 +957,9 @@ mlp_forward_sampled_kernel(const unsigned char *__restrict__ blob, const void *_
         unsigned long long s_seed = 0, s_off = 0;
         float s_u = 0.0f;
         if (s_valid) {
-          const long long env = s_row / smp.Np;
-          s_gi = env * smp.N + __ldg(smp.agent + (int)(s_row - env * smp.Np));
+          const long long prow = smp.row0 + s_row;          // row of the policy
+          const long long env = prow / smp.Np;
+          s_gi = env * smp.N + __ldg(smp.agent + (int)(prow - env * smp.Np));
           if (smp.uniforms) {
             s_u = __ldg(smp.uniforms + 2 * s_gi + part);
           } else {
@@ -1202,6 +1204,7 @@ int launch_forward_sampled(void *stream, const void *blob, int F, int H, int A0,
   if (reinterpret_cast<uintptr_t>(s->actions) & 7) return (int)cudaErrorMisalignedAddress;
   if (s->n_policy_agents < 1 || s->n_agents < s->n_policy_agents || rows % s->n_policy_agents)
     return (int)cudaErrorInvalidValue;
+  if (s->row_offset < 0 || s->row_offset % s->n_policy_agents) return (int)cudaErrorInvalidValue;
   constexpr MlpLayout lay = mlp_layout(FastShape::K1, FastShape::H, FastShape::N3);
   const size_t smem = (size_t)((lay.total_bytes - lay.off_w1 + 127) & ~127) +
                       kWarpgroups * kSampledStageBytes + 8 * kSampledBarriers;
@@ -1214,7 +1217,7 @@ int launch_forward_sampled(void *stream, const void *blob, int F, int H, int A0,
     configured = smem;
   }
   const MlpSampling smp = {s->actions, s->rng_state, s->uniforms, s->agent_of_slot, s->n_agents,
-                           s->n_policy_agents};
+                           s->n_policy_agents, s->row_offset};
   const long long n_tiles = (rows + kTileM - 1) / kTileM;
   const int sm_budget = (g_mlp_max_ctas > 0 && g_mlp_max_ctas < kNumSMs) ? g_mlp_max_ctas : kNumSMs;
   const int grid = (int)min((long long)sm_budget, n_tiles);

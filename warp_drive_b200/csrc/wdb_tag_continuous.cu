@@ -97,10 +97,10 @@ tag_continuous_kernel(const __grid_constant__ TcParams P, const __grid_constant_
   const int a = tid - le * N;
   // CTAs past full_ctas carry ONE env each (see plan_packed: the last, partly filled wave)
   const bool tail_cta = (int)blockIdx.x >= P.full_ctas;
-  const int env0 = tail_cta ? P.full_ctas * epb + ((int)blockIdx.x - P.full_ctas)
-                            : (int)blockIdx.x * epb;
+  const int env0 = P.env_begin + (tail_cta ? P.full_ctas * epb + ((int)blockIdx.x - P.full_ctas)
+                                           : (int)blockIdx.x * epb);
   const int env = env0 + le;
-  const int envs_here = tail_cta ? min(1, P.n_envs - env0) : min(epb, P.n_envs - env0);
+  const int envs_here = tail_cta ? min(1, P.env_end - env0) : min(epb, P.env_end - env0);
   const bool active = le < envs_here;
   const int gi = env * N + a;
   const int li = le * N + a;
@@ -885,8 +885,9 @@ int g_tc_tail_split = 0;   // wdb_set_option("tc_tail_split", 0/1/2), off by def
 int plan_packed(TcParams &P, const FusedParams *Q, TcPlan &plan) {
   const int N = P.N, K = P.K;
   const bool have_gscratch = P.g_nd && P.g_nid;
+  const int n_envs = P.env_end - P.env_begin;   // the envs of this launch
   int epb = N >= g_tc_threads ? 1 : g_tc_threads / N;
-  if (epb > P.n_envs) epb = P.n_envs;
+  if (epb > n_envs) epb = n_envs;
   const int block = round_up(epb * N, 32);
   const int nwarps = block / 32;
   const int F = 7 * K + 1;
@@ -938,7 +939,7 @@ int plan_packed(TcParams &P, const FusedParams *Q, TcPlan &plan) {
   }
   plan.kernel = TcPlan::kPacked;
   plan.block = block;
-  plan.grid = (P.n_envs + epb - 1) / epb;
+  plan.grid = (n_envs + epb - 1) / epb;
   P.full_ctas = plan.grid;
   // Tail split (option, off): the kernel's time is waves x CTA latency.  When the last wave is
   // less than half full (not at config 2 on 132 SMs: 667 CTAs over 2 x 132 slots = 2 waves +
@@ -949,13 +950,13 @@ int plan_packed(TcParams &P, const FusedParams *Q, TcPlan &plan) {
     // test mode: half of the CTAs as one-env CTAs whatever the size
     const int full = plan.grid / 2;
     P.full_ctas = full;
-    plan.grid = full + (P.n_envs - full * epb);
+    plan.grid = full + (n_envs - full * epb);
   } else if (g_tc_tail_split && epb > 1 && smem > 75 * 1024) {
     const int slots = 2 * kNumSMs;                    // two CTAs of this size per SM
     const int rem = plan.grid % slots;
     if (plan.grid > slots && rem > 0 && 2 * rem <= slots) {
       const int full = plan.grid - rem;
-      const int tail_envs = P.n_envs - full * epb;
+      const int tail_envs = n_envs - full * epb;
       P.full_ctas = full;
       plan.grid = full + tail_envs;
     }
@@ -1017,6 +1018,7 @@ int fill_params(TcParams &P, const wdb_tc_env &e) {
   P.tag_reward = e.tag_reward_for_tagger; P.tag_penalty = e.tag_penalty_for_runner;
   P.end_reward = e.end_of_game_reward_for_runner; P.done = e.done;
   P.timestep = e.env_timestep; P.stats = e.stats;
+  P.env_begin = 0; P.env_end = e.n_envs;
   return 0;
 }
 
@@ -1129,7 +1131,15 @@ int plan_rollout(const wdb_tc_env *env, const wdb_tc_rollout *ro, bool shapes_on
   Q.actions_in = acts_in;
   if (!shapes_only && Q.do_reset && Q.n_reset > 0 && !Q.reset_table)
     return (int)cudaErrorInvalidValue;
-  return tc_plan(P, &Q, obs_next, obs_tiles, env->blocks_per_env, plan);
+  // an env subrange: only the packed kernel takes one
+  const int count = ro->env_count ? ro->env_count : env->n_envs - ro->env_begin;
+  if (ro->env_begin < 0 || count < 1 || ro->env_begin + count > env->n_envs)
+    return (int)cudaErrorInvalidValue;
+  P.env_begin = ro->env_begin; P.env_end = ro->env_begin + count;
+  err = tc_plan(P, &Q, obs_next, obs_tiles, env->blocks_per_env, plan);
+  if (err) return err;
+  if (count != env->n_envs && plan.kernel != TcPlan::kPacked) return (int)cudaErrorInvalidValue;
+  return 0;
 }
 
 }  // namespace

@@ -38,6 +38,8 @@ struct TcParams {
   int force_exact;                   // A/B switch: every agent takes the exact (reference-literal) path
   int full_ctas;                     // CTAs [0, full_ctas) carry epb envs each, the rest ONE env each
                                      // (the tail of the last wave as small CTAs); >= grid: all full
+  int env_begin, env_end;            // the launch steps envs [env_begin, env_end) of the n_envs
+                                     // (packed kernel only; every array is indexed by global env)
   float *loc_x, *loc_y, *speed, *direction, *acceleration;
   const int *agent_types;
   float *edge_pen;

@@ -71,6 +71,7 @@ class TcRollout(ctypes.Structure):
         ("episodic_step_sum", _fp), ("num_completed_episodes", _fp),
         ("reset_table", _fp), ("n_reset_arrays", _i), ("obs_at_reset", _fp),
         ("reset_done_envs", _i), ("launch_after_forward", _i), ("actions_in", _i),
+        ("env_begin", _i), ("env_count", _i),
     ]
 
 
@@ -147,7 +148,7 @@ class MlpSampling(ctypes.Structure):
 
     _fields_ = [
         ("actions", _fp), ("rng_state", _fp), ("uniforms", _fp), ("agent_of_slot", _fp),
-        ("n_agents", _i), ("n_policy_agents", _i),
+        ("n_agents", _i), ("n_policy_agents", _i), ("row_offset", ctypes.c_longlong),
     ]
 
 

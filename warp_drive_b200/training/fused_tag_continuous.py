@@ -124,11 +124,12 @@ class FusedTagContinuousStep:
 
     def launch(self, probs, actions_batch=None, rewards_batch=None, obs_next=None,
                done_batch=None, uniforms=None, reset_done_envs=True, obs_next_tiles=None,
-               after_forward=False, actions_in=False):
+               after_forward=False, actions_in=False, envs=None):
         """probs: {policy: [probs_head0 [E,Np,A0], probs_head1 [E,Np,A1]]}; the *_batch /
         obs_next dicts hold this timestep's slots (tensors) per policy, or None.
         actions_in: the forward already sampled the actions into `actions_batch` (required),
-        which the step then reads instead of sampling from `probs` (may be None)."""
+        which the step then reads instead of sampling from `probs` (may be None).
+        envs: (begin, end), step only these envs (every tensor still covers all E)."""
         ro = self.ro
         for pi, p in enumerate(self.policies):
             io = ro.policy[pi]
@@ -142,5 +143,6 @@ class FusedTagContinuousStep:
         ro.reset_done_envs = int(bool(reset_done_envs))
         ro.launch_after_forward = int(bool(after_forward))
         ro.actions_in = int(bool(actions_in))
+        ro.env_begin, ro.env_count = (0, 0) if envs is None else (envs[0], envs[1] - envs[0])
         _lib.check(self.lib.wdb_tag_continuous_rollout_step(
             _lib.stream_ptr(), self._env_ref, self._ro_ref), "tag_continuous_rollout_step")

@@ -62,14 +62,18 @@ class FusedPolicyForward:
             self.F, self.H, self.A0, self.A1), "mlp_pack_weights")
         self._keep = ts
 
-    def sampling(self, actions, agent_of_slot, n_agents, rng_state=None, uniforms=None):
+    def sampling(self, actions, agent_of_slot, n_agents, rng_state=None, uniforms=None,
+                 env_begin=0):
         """The sampling arguments of a forward (see `__call__`): both heads' actions of every
         row go to `actions` [E, Np, 2] int32; row env * Np + slot is agent
-        env * n_agents + agent_of_slot[slot] of the RNG state (or of `uniforms` [E, N, 2])."""
+        env * n_agents + agent_of_slot[slot] of the RNG state (or of `uniforms` [E, N, 2]).
+        env_begin: the forward's rows are those of envs env_begin, env_begin + 1, ... (its
+        obs, probabilities and `actions` start at env env_begin's rows)."""
         s = _lib.MlpSampling()
         s.actions, s.rng_state, s.uniforms = _lib.ptr(actions), _lib.ptr(rng_state), _lib.ptr(uniforms)
         s.agent_of_slot = _lib.ptr(agent_of_slot)
         s.n_agents, s.n_policy_agents = int(n_agents), int(agent_of_slot.numel())
+        s.row_offset = int(env_begin) * s.n_policy_agents
         return s
 
     def _sampled(self, input_, tiles, rows, probs0, probs1, values, sampling):

@@ -160,6 +160,7 @@ class RolloutEngine:
 
         # ---- tensor-core forward (wgmma MLP kernel) for the fused path
         self.fused_forward = {}
+        self._fwd_streams_of = {}     # per env group: the side streams of the smaller policies
         self.obs_tiles = {}
         self.sample_in_forward = False
         # (not for Q networks: that forward ends in a softmax)
@@ -197,9 +198,28 @@ class RolloutEngine:
                     self._agent_of_slot = {
                         p: torch.as_tensor(self.policy_map[p], dtype=torch.int32, device=dev)
                         for p in self.policies}
-                    self._sampling = {
-                        p: self.fused_forward[p].sampling(None, self._agent_of_slot[p], self.N)
-                        for p in self.policies}
+                    self._set_env_groups()
+
+    def _set_env_groups(self, n_groups=None):
+        """The sampling forward's schedule: the envs as one group, or as two halves that each
+        run their own chain (forwards -> env step -> forwards ...) on their own streams, so one
+        half's env step fills the SMs the other half's forwards leave idle (kernel tails,
+        launch gaps).  Env replicas never interact, and every kernel indexes the shared arrays
+        by global env, so both schedules compute the same bits.  Two groups when each half
+        fills at least two env-step CTAs (a CTA carries up to 320 // N envs).  n_groups: force
+        the count (tests and measurements compare the two schedules)."""
+        per_cta = max(1, 320 // self.N)
+        n = 2 if (not self.obs_tiles and self.E >= 4 * per_cta) else 1
+        n = n if n_groups is None else n_groups
+        half = self.E // 2
+        self._groups = [(0, self.E)] if n == 1 else [(0, half), (half, self.E)]
+        self._sampling = [
+            {p: self.fused_forward[p].sampling(None, self._agent_of_slot[p], self.N,
+                                               env_begin=e0) for p in self.policies}
+            for e0, _ in self._groups]
+        self._group_streams = [None] if n == 1 else [torch.cuda.Stream() for _ in self._groups]
+        self._in_rollout = False
+        self._graph = None
 
     def refresh_forward_weights(self):
         """Re-pack the policies' parameters for the tensor-core forward (after every
@@ -269,7 +289,8 @@ class RolloutEngine:
         probs, _ = model(obs_p, **kw)
         return [q.contiguous() for q in probs]
 
-    def _forward_side_by_side(self, obs_in, probs, weights_stable=False, sampling=None):
+    def _forward_side_by_side(self, obs_in, probs, weights_stable=False, sampling=None,
+                              group=0):
         """Every policy's fused forward, concurrently: the persistent MLP kernel uses one CTA
         per SM, so the SMs are split between the policies in proportion to their rows and the
         smaller policies run on side streams (fork/join by events, also under graph capture).
@@ -311,13 +332,14 @@ class RolloutEngine:
                 share = {p: max(1, min(n_sm - 1, -(-n_sm * rows[p] // total))) for p in order[1:]}
                 share[order[0]] = max(1, n_sm - sum(share.values()))
             self._fwd_plan = (order, share)
-            self._fwd_streams = [torch.cuda.Stream() for _ in order[1:]]
         order, share = self._fwd_plan
+        if group not in self._fwd_streams_of:
+            self._fwd_streams_of[group] = [torch.cuda.Stream() for _ in order[1:]]
         cur = torch.cuda.current_stream()
         fork = torch.cuda.Event()
         fork.record(cur)
         joins = []
-        for p, st in zip(order[1:], self._fwd_streams):
+        for p, st in zip(order[1:], self._fwd_streams_of[group]):
             st.wait_event(fork)
             with torch.cuda.stream(st):
                 self._one_forward(p, obs_in, probs, share[p], sampling)
@@ -347,7 +369,7 @@ class RolloutEngine:
             if t >= 0:
                 batches = {p: self._tensor(f"{_PROCESSED_OBSERVATIONS}_batch_{p}")
                            for p in self.policies}
-                if t == 0:
+                if t == 0 and not self.sample_in_forward:
                     for p in self.policies:
                         batches[p][0].copy_(self.cur_obs[p])
                 obs_in = {p: batches[p][t] for p in self.policies}
@@ -365,8 +387,6 @@ class RolloutEngine:
                                          for p in self.policies}
                 obs_next = self._scratch_obs
                 actions_batch = rewards_batch = done_batch = None
-            paired = False
-            sampling = None
             if self.sample_in_forward:
                 # the forwards sample into the batch slot (t < 0: into a scratch buffer), with
                 # the RNG state the step would have sampled with
@@ -377,27 +397,65 @@ class RolloutEngine:
                                            dtype=torch.int32, device=self.dm.device)
                             for p in self.policies}
                     actions_batch = self._scratch_actions
-                sampling = self._sampling
-                for p in self.policies:
-                    s = sampling[p]
-                    s.actions = _lib.ptr(actions_batch[p])
-                    s.rng_state = self.fused.ro.rng_state
-                    s.uniforms = _lib.ptr(uniforms)
-            if self.fused_forward:
-                probs = self._probs
-                # t > 0: the kernel before this forward is the previous env step, not a weight
-                # re-pack -> the weight load may overlap its tail (programmatic launch)
-                paired = self._forward_side_by_side(obs_in, probs, weights_stable=t > 0,
-                                                    sampling=sampling)
+                self._step_groups(t, obs_in, obs_next, actions_batch, rewards_batch, done_batch,
+                                  uniforms)
             else:
-                probs = {p: self._forward(self.models[p], obs_in[p]) for p in self.policies}
-            self.fused.launch(probs, actions_batch=actions_batch, rewards_batch=rewards_batch,
-                              obs_next=obs_next, done_batch=done_batch, uniforms=uniforms,
-                              obs_next_tiles=self.obs_tiles or None, after_forward=paired,
-                              actions_in=sampling is not None)
+                paired = False
+                if self.fused_forward:
+                    probs = self._probs
+                    # t > 0: the kernel before this forward is the previous env step, not a
+                    # weight re-pack -> the weight load may overlap its tail (programmatic launch)
+                    paired = self._forward_side_by_side(obs_in, probs, weights_stable=t > 0)
+                else:
+                    probs = {p: self._forward(self.models[p], obs_in[p]) for p in self.policies}
+                self.fused.launch(probs, actions_batch=actions_batch, rewards_batch=rewards_batch,
+                                  obs_next=obs_next, done_batch=done_batch, uniforms=uniforms,
+                                  obs_next_tiles=self.obs_tiles or None, after_forward=paired)
             if t < 0:
                 for p in self.policies:
                     self.cur_obs[p].copy_(self._scratch_obs[p])
+
+    def _step_groups(self, t, obs_in, obs_next, actions_batch, rewards_batch, done_batch,
+                     uniforms):
+        """One timestep of the sampling forwards and the env step, per env group on the
+        group's stream.  Outside a rollout the groups fork from and join the current stream;
+        inside one (_rollout_eager) they stay apart from the first step to the last."""
+        cur = torch.cuda.current_stream()
+        fork = not self._in_rollout and self._group_streams[0] is not None
+        if fork:
+            ev = torch.cuda.Event()
+            ev.record(cur)
+        for g, ((e0, e1), st) in enumerate(zip(self._groups, self._group_streams)):
+            if fork:
+                st.wait_event(ev)
+            with torch.cuda.stream(st if st is not None else cur):
+                if t == 0:
+                    for p in self.policies:
+                        obs_in[p][e0:e1].copy_(self.cur_obs[p][e0:e1])
+                sampling = self._sampling[g]
+                for p in self.policies:
+                    s = sampling[p]
+                    s.actions = _lib.ptr(actions_batch[p][e0:e1])
+                    s.rng_state = self.fused.ro.rng_state
+                    s.uniforms = _lib.ptr(uniforms)
+                rows = {p: obs_in[p][e0:e1] for p in self.policies}
+                probs = {p: [q[e0:e1] for q in self._probs[p]] for p in self.policies}
+                # t > 0: the kernel before this forward is the previous env step, not a weight
+                # re-pack -> the weight load may overlap its tail (programmatic launch)
+                paired = self._forward_side_by_side(rows, probs, weights_stable=t > 0,
+                                                    sampling=sampling, group=g)
+                self.fused.launch(None, actions_batch=actions_batch, rewards_batch=rewards_batch,
+                                  obs_next=obs_next, done_batch=done_batch, uniforms=uniforms,
+                                  obs_next_tiles=self.obs_tiles or None, after_forward=paired,
+                                  actions_in=True, envs=None if st is None else (e0, e1))
+        if fork:
+            self._join_groups(cur)
+
+    def _join_groups(self, cur):
+        for st in self._group_streams:
+            ev = torch.cuda.Event()
+            ev.record(st)
+            cur.wait_event(ev)
 
     # ------------------------------------------------------------------ one timestep
     def _tensor(self, name):
@@ -804,8 +862,25 @@ class RolloutEngine:
 
     # ------------------------------------------------------------------ T-step rollout
     def _rollout_eager(self, **sample_params):
-        for t in range(self.T):
-            self.step(t, **sample_params)
+        groups = (self.fused is not None and self.sample_in_forward and not sample_params
+                  and self._group_streams[0] is not None)
+        if not groups:
+            for t in range(self.T):
+                self.step(t, **sample_params)
+            return
+        # the env groups run apart for the whole rollout: fork once, join once
+        cur = torch.cuda.current_stream()
+        ev = torch.cuda.Event()
+        ev.record(cur)
+        for st in self._group_streams:
+            st.wait_event(ev)
+        self._in_rollout = True
+        try:
+            for t in range(self.T):
+                self.step(t)
+        finally:
+            self._in_rollout = False
+            self._join_groups(cur)
 
     def _sa_params_ok(self, sample_params):
         """The whole-rollout kernel takes the categorical sampler's argmax switch, or the OU
