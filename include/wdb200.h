@@ -1560,6 +1560,52 @@ int wdb_tqc_critic_update_sampled(void *stream, const wdb_tqc_update_args *updat
 int wdb_tqc_actor_update_sampled(void *stream, const wdb_tqc_update_args *update,
                                  const wdb_replay_windows *windows);
 
+/* ---- recurrent policies (csrc/wdb_recurrent.cu) ----------------------------------------------
+ * FullyConnectedGRU's per-step rollout forward: n_layers (0..2) Linear + ReLU trunk layers, an
+ * nn.GRUCell of width H (gate order r, z, n) and one softmax head per discrete action head,
+ * reading the new state h'.  fp32 throughout; the value head is not evaluated.  Weights are the
+ * torch parameters as they are (Linear [out, in], weight_ih [3H, D], weight_hh [3H, H]). */
+typedef struct wdb_gru_forward {
+  long long n_rows;                  /* R = E * Np */
+  int in_dim;                        /* F */
+  int n_layers;                      /* trunk layers, 0 .. 2 */
+  int dims[2];                       /* their widths (dims[l] for l < n_layers) */
+  int hidden_size;                   /* H */
+  int n_heads;                       /* 1 or 2 */
+  int heads[2];                      /* A_k for k < n_heads */
+  const float *obs;                  /* [R, F] */
+  float *hidden;                     /* [R, H]: h in, h' out (in place) */
+  const float *fc_weight[2], *fc_bias[2];
+  const float *weight_ih, *weight_hh, *bias_ih, *bias_hh;
+  const float *head_weight[2], *head_bias[2];
+  float *probs[2];                   /* out [R, A_k] */
+} wdb_gru_forward;
+/* Dynamic shared memory of wdb_gru_policy_forward at these shapes; 0 if it refuses them:
+ * 1 <= F <= 256, trunk widths and H in 1 .. 128, 1 or 2 heads of 1 .. 64 actions, and the
+ * weights plus a 16-row tile of activations in 227 KB.  No CUDA call. */
+long long wdb_gru_forward_bytes(int in_dim, int n_layers, int d0, int d1, int hidden_size,
+                                int n_heads, int a0, int a1);
+/* One launch: h' into `hidden`, the heads' probabilities into probs[k].  Each output is one
+ * thread's k-ascending fmaf sum plus its bias; sig(x) = 1 / (1 + expf(-x)), tanh = tanhf.
+ * Bit-identical on relaunch.  cudaErrorInvalidValue without launching on refused shapes or a
+ * NULL pointer. */
+int wdb_gru_policy_forward(void *stream, const wdb_gru_forward *args);
+
+#define WDB_RECURRENT_MAX_POLICIES 8
+typedef struct wdb_recurrent_state {
+  float *hidden;                     /* [E, Np, H] */
+  int n_agents;                      /* Np */
+  int hidden_size;                   /* H */
+} wdb_recurrent_state;
+typedef struct wdb_recurrent_reset {
+  const int *done;                   /* [E] the env's _done_ */
+  int n_envs;
+  int n_policies;                    /* 1 .. WDB_RECURRENT_MAX_POLICIES */
+  wdb_recurrent_state policy[WDB_RECURRENT_MAX_POLICIES];
+} wdb_recurrent_reset;
+/* Zeroes hidden[e, :, :] of every listed policy for every env e with done[e] > 0, one launch. */
+int wdb_recurrent_reset_done(void *stream, const wdb_recurrent_reset *table);
+
 #ifdef __cplusplus
 }
 #endif

@@ -402,6 +402,34 @@ class PerStore(ctypes.Structure):
     ]
 
 
+class GruForward(ctypes.Structure):
+    """struct wdb_gru_forward (include/wdb200.h)."""
+
+    _fields_ = [
+        ("n_rows", _ll), ("in_dim", _i), ("n_layers", _i), ("dims", _i * 2),
+        ("hidden_size", _i), ("n_heads", _i), ("heads", _i * 2),
+        ("obs", _fp), ("hidden", _fp), ("fc_weight", _fp * 2), ("fc_bias", _fp * 2),
+        ("weight_ih", _fp), ("weight_hh", _fp), ("bias_ih", _fp), ("bias_hh", _fp),
+        ("head_weight", _fp * 2), ("head_bias", _fp * 2), ("probs", _fp * 2),
+    ]
+
+
+RECURRENT_MAX_POLICIES = 8
+
+
+class RecurrentState(ctypes.Structure):
+    """struct wdb_recurrent_state (include/wdb200.h)."""
+
+    _fields_ = [("hidden", _fp), ("n_agents", _i), ("hidden_size", _i)]
+
+
+class RecurrentReset(ctypes.Structure):
+    """struct wdb_recurrent_reset (include/wdb200.h)."""
+
+    _fields_ = [("done", _vp), ("n_envs", _i), ("n_policies", _i),
+                ("policy", RecurrentState * RECURRENT_MAX_POLICIES)]
+
+
 _SIGNATURES = {
     "wdb_abi_version": (_i, []),
     "wdb_error_string": (ctypes.c_char_p, [_i]),
@@ -609,6 +637,9 @@ _SIGNATURES = {
         _i, [_vp, _i, _vp, _vp, _vp, _vp, _vp] + [_f] * 8 + [_vp, _i]),
     "wdb_pendulum_step": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i]),
     "wdb_acrobot_step": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i]),
+    "wdb_gru_forward_bytes": (_ll, [_i, _i, _i, _i, _i, _i, _i, _i]),
+    "wdb_gru_policy_forward": (_i, [_vp, ctypes.POINTER(GruForward)]),
+    "wdb_recurrent_reset_done": (_i, [_vp, ctypes.POINTER(RecurrentReset)]),
     "wdb_cartpole_step": (
         _i,
         [_vp, _i, _vp, _vp, _vp, _vp, _vp, _f, _f, _f, _f, _f, _f, _f, _f, _f, _vp, _i],

@@ -312,23 +312,36 @@ class _PolicyGradient:
         return loss, metrics
 
     # ---- several epochs over shuffled minibatches
-    def prepare_batch(self, model, obs, actions, rewards, done_flags, action_mask=None):
+    def prepare_batch(self, model, obs, actions, rewards, done_flags, action_mask=None,
+                      hidden_start=None):
         """Once per training batch, at the parameters the rollout used: one forward of the
         training network without gradients (each timestep under its own action mask), the
         values for GAE and old_log_prob of every row by the loss kernel's own formula, then
         advantages / value targets (gae_lambda absent: the discounted returns) and the
         optional per-timestep advantage normalisation over (env, agent).  obs [T, E, Np, F],
         actions [T, E, Np, n_heads] (float [T, E, Np, A] for a Gaussian policy), rewards
-        [T, E, Np], done_flags [T, E]."""
+        [T, E, Np], done_flags [T, E].  A recurrent model (FullyConnectedGRU) runs
+        forward_sequence from hidden_start [E, Np, H], and its minibatches are sets of whole
+        sequences (one (env, agent) pair over the T steps) instead of rows."""
         T, E, Np = rewards.shape
         R = T * E * Np
+        recurrent = bool(getattr(model, "is_recurrent", False))
         if R >= 2 ** 31:
             raise ValueError(f"a training batch of {R} rows (T x E x agents) is too large for "
                              "the minibatch update: it indexes rows with int32")
+        if recurrent and self.num_mini_batches > E * Np:
+            raise ValueError(f"num_mini_batches = {self.num_mini_batches} exceeds the {E * Np} "
+                             "sequences (E x agents) of a training batch: a minibatch of a "
+                             "recurrent policy would be empty")
         if self.num_mini_batches > R:
             raise ValueError(f"num_mini_batches = {self.num_mini_batches} exceeds the {R} rows "
                              "(T x E x agents) of a training batch: a minibatch would be empty")
         log_std = model.log_std if getattr(model, "is_gaussian", False) else None
+        seq = None
+        if recurrent:
+            assert hidden_start is not None and action_mask is None
+            seq = dict(obs=obs.reshape(T, E * Np, -1), h0=hidden_start.reshape(E * Np, -1),
+                       done=done_flags, T=T, Np=Np)
         obs = obs.reshape(R, -1)
         if action_mask is not None:
             action_mask = action_mask.reshape(R, -1).float()
@@ -337,7 +350,12 @@ class _PolicyGradient:
         else:
             flat_actions = actions.reshape(R, -1).to(torch.int32).contiguous()
         with torch.no_grad():
-            probs, values = _training_forward(model, obs, action_mask)
+            if recurrent:
+                probs, values = model.forward_sequence(
+                    seq["obs"].view(T, E, Np, -1), hidden_start, done_flags)
+                probs = [p.reshape(R, -1) for p in probs]
+            else:
+                probs, values = _training_forward(model, obs, action_mask)
             values = values.reshape(T, E, Np)
             if self.use_fused_loss and obs.is_cuda and fused_ppo_loss_supported(probs, log_std):
                 old_log_prob = fused_log_prob(probs, flat_actions, log_std)
@@ -354,7 +372,8 @@ class _PolicyGradient:
                                                 self.discount_factor_gamma, self.gae_lambda)
             norm_adv = self._normalize(advantages) if self.normalize_advantage else advantages
         return PPOBatch(
-            R=R, obs=obs, mask=action_mask, actions=flat_actions, log_std=log_std,
+            R=R, units=E * Np if recurrent else R, rows_per_unit=T if recurrent else 1, seq=seq,
+            obs=obs, mask=action_mask, actions=flat_actions, log_std=log_std,
             advantages=norm_adv.reshape(R).contiguous(),
             value_targets=value_targets.reshape(R).contiguous(),
             old_log_prob=old_log_prob.reshape(R).float().contiguous(),
@@ -362,11 +381,15 @@ class _PolicyGradient:
             returns=value_targets, actions_batch=actions)
 
     def minibatch_loss(self, model, batch, rows, timestep):
-        """The loss of one minibatch (rows: int32 [B] into the batch's R rows) with the
-        training forward under autograd; returns (loss, float64 sums [5] on the device)."""
-        obs = batch.obs.index_select(0, rows)
-        kw = {} if batch.mask is None else {"action_mask": batch.mask.index_select(0, rows)}
-        probs, values = model(obs=obs, **kw)
+        """The loss of one minibatch (rows: int32 [B] into the batch's R rows; for a recurrent
+        model, `units` of the batch's sequences: see sequence_rows) with the training forward
+        under autograd; returns (loss, float64 sums [5] on the device)."""
+        if batch.seq is not None:
+            probs, values, rows = self._sequence_forward(model, batch, rows)
+        else:
+            obs = batch.obs.index_select(0, rows)
+            kw = {} if batch.mask is None else {"action_mask": batch.mask.index_select(0, rows)}
+            probs, values = model(obs=obs, **kw)
         vf_c = self.vf_loss_coeff_schedule.get_param_value(timestep)
         ent_c = self.entropy_coeff_schedule.get_param_value(timestep)
         ppo = self.clip_param is not None
@@ -380,6 +403,28 @@ class _PolicyGradient:
             list(probs), values, batch.actions[idx], batch.advantages[idx],
             batch.value_targets[idx], batch.old_log_prob[idx], ppo, clip, vf_c, ent_c,
             log_std=batch.log_std)
+
+    @staticmethod
+    def sequence_rows(seqs, T, S):
+        """The flat batch rows of sequences `seqs` (int [B_s] of S = E x Np): t * S + s, in
+        (t, chunk) order -- the row order of forward_sequence over [T, B_s].  int32 [T * B_s]."""
+        t = torch.arange(T, dtype=torch.int64, device=seqs.device)[:, None] * S
+        return (t + seqs.to(torch.int64)[None, :]).reshape(-1).to(torch.int32)
+
+    @staticmethod
+    def _sequence_forward(model, batch, seqs):
+        """forward_sequence over the sequences `seqs` of a recurrent batch, from their start
+        states: ([probs per head] [T * B_s, A_k], values [T * B_s], rows int32 [T * B_s])."""
+        sq = batch.seq
+        T, S = sq["obs"].shape[0], sq["obs"].shape[1]
+        idx = seqs.long()
+        obs = sq["obs"].index_select(1, idx)[:, :, None]             # [T, B_s, 1, F]
+        h0 = sq["h0"].index_select(0, idx)[:, None]                  # [B_s, 1, H]
+        done = sq["done"].index_select(1, torch.div(idx, sq["Np"], rounding_mode="floor"))
+        probs, values = model.forward_sequence(obs, h0, done)
+        B = T * idx.numel()
+        return ([p.reshape(B, -1) for p in probs], values.reshape(B),
+                _PolicyGradient.sequence_rows(seqs, T, S))
 
     def minibatch_metrics(self, batch, mean_sums, timestep):
         """The metrics of a logging iteration: the loss terms from `mean_sums` (the per-step

@@ -62,6 +62,8 @@ class FusedSingleAgentRollout:
         if len(policy_map) != 1 or len(models) != 1:
             return False
         model = _unwrap(next(iter(models.values())))
+        if getattr(model, "is_recurrent", False):     # (its forward keeps no state)
+            return False
         continuous = SINGLE_AGENT_ENVS[env.name].continuous
         try:
             # discrete kinds: one softmax head; continuous kinds: one tanh head or one Gaussian

@@ -239,6 +239,11 @@ class ModelFactory:
                 FullyConnectedBranchingQ)
 
             cls._registry[model_name] = FullyConnectedBranchingQ
+        if model_name == "fully_connected_gru" and model_name not in cls._registry:
+            # the recurrent A2C / PPO policy, imported on first use
+            from warp_drive_b200.training.models.fully_connected_gru import FullyConnectedGRU
+
+            cls._registry[model_name] = FullyConnectedGRU
         if model_name not in cls._registry and model_name in (
                 "fully_connected_actor", "fully_connected_action_value_critic",
                 "fully_connected_sac_actor", "fully_connected_quantile_critic"):

@@ -19,6 +19,9 @@ class FusedPolicyForward:
         try:
             if getattr(model, "is_deterministic", True) or len(model.fc) != 2:
                 return False
+            # (a memoryless forward: it would drop a recurrent policy's state)
+            if getattr(model, "is_recurrent", False):
+                return False
             # (this forward reads raw observations)
             if getattr(model, "normalize_observations", False):
                 return False

@@ -134,6 +134,8 @@ def supported(model, obs, mask=None):
     every head's actions per observation row."""
     if getattr(model, "is_deterministic", True) or len(model.fc) != 2:
         return False
+    if getattr(model, "is_recurrent", False):     # (a memoryless node)
+        return False
     if len(model.output_dims) not in (1, 2):
         return False
     if not obs.is_cuda or obs.dtype != torch.float32 or obs.requires_grad:

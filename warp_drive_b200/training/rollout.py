@@ -29,7 +29,7 @@ class RolloutEngine:
                  use_fused_step=True, write_observations=True, stats=None,
                  use_fused_forward=True, use_obs_tiles=False, use_pair_forward=False,
                  create_separate_placeholders_for_each_policy=False,
-                 obs_dim_corresponding_to_num_agents="first"):
+                 obs_dim_corresponding_to_num_agents="first", native_recurrent=True):
         self.env_wrapper = env_wrapper
         # heterogeneous agents: every policy steps through its own observations_{p}[_{key}],
         # sampled_actions[_{k}]_{p} and rewards_{p} arrays, and / or the env writes its
@@ -125,6 +125,33 @@ class RolloutEngine:
         self.num_completed_episodes = torch.zeros((), dtype=torch.int64, device=dev)
         self._graph = None
         self._graph_stream = None
+        # recurrent policies (FullyConnectedGRU): each keeps its agents' state hidden[p]
+        # [E, Np, H] from step to step and rollout to rollout, and hidden_start[p], the state the
+        # batch now in the *_batch* arrays started from (copied at t == 0 of every rollout,
+        # inside the CUDA graph).  After every env step and its bookkeeping, ONE
+        # wdb_recurrent_reset_done launch zeroes the rows of the envs that are done, before the
+        # done-masked reset clears their flags: the step after an episode's end starts from zero
+        # (FullyConnectedGRU.reset_hidden).  Their rollout forward is wdb_gru_policy_forward
+        # where it takes the shape (native_recurrent), the model's torch step otherwise.
+        self.recurrent_of = {p: bool(getattr(models[p], "is_recurrent", False))
+                             for p in self.policies}
+        self.recurrent = any(self.recurrent_of.values())
+        self.hidden, self.hidden_start, self.native_gru = {}, {}, {}
+        for p in self.policies:
+            if self.recurrent_of[p]:
+                shape = (self.E, len(self.policy_map[p]), int(models[p].hidden_size))
+                self.hidden[p] = torch.zeros(shape, device=dev)
+                self.hidden_start[p] = torch.zeros(shape, device=dev)
+                if native_recurrent and forward_dtype is None:
+                    from warp_drive_b200.training.models.fully_connected_gru import (
+                        NativeGruStep)
+
+                    if NativeGruStep.routed(models[p], self.E * len(self.policy_map[p])):
+                        self.native_gru[p] = NativeGruStep(models[p])
+        assert len(self.hidden) <= _lib.RECURRENT_MAX_POLICIES
+        self._recurrent_probs = {
+            p: [torch.empty((self.E, len(self.policy_map[p]), h), device=dev)
+                for h in self.heads_of[p]] for p in self.native_gru}
         # ---- fused single-launch timestep (TagContinuous: 2 discrete heads, Box obs)
         self.fused = None
         if use_fused_step and self._fused_eligible():
@@ -245,6 +272,9 @@ class RolloutEngine:
             return False
         if any(getattr(m, "action_mask", None) is not None for m in self.models.values()):
             return False
+        # its forwards keep no per-agent state
+        if self.recurrent:
+            return False
         # it samples its heads from softmax probabilities: a Q network acts epsilon-greedily
         if self.q_network:
             return False
@@ -257,9 +287,42 @@ class RolloutEngine:
 
         return FusedTagContinuousStep.eligible(self.env_wrapper, self.policy_map)
 
+    def zero_hidden(self):
+        """Restart every recurrent policy's state (all envs restarted)."""
+        for h in self.hidden.values():
+            h.zero_()
+
+    def recurrent_reset_done(self):
+        """Zero the recurrent states of every env whose _done_ is set: ONE launch for every
+        recurrent policy (wdb_recurrent_reset_done)."""
+        k = _lib.RecurrentReset()
+        k.done = _lib.ptr(self._tensor("_done_"))
+        k.n_envs, k.n_policies = self.E, len(self.hidden)
+        for i, (p, h) in enumerate(self.hidden.items()):
+            k.policy[i].hidden = _lib.ptr(h)
+            k.policy[i].n_agents, k.policy[i].hidden_size = h.shape[1], h.shape[2]
+        _lib.check(_lib.load().wdb_recurrent_reset_done(_lib.stream_ptr(), ctypes.byref(k)),
+                   "recurrent_reset_done")
+
+    def _recurrent_forward(self, p, obs_p):
+        """Policy p's probabilities [per head] [E, Np, A_k] from its observation rows, with its
+        state hidden[p] advanced in place."""
+        h = self.hidden[p]
+        R = h.shape[0] * h.shape[1]
+        obs = obs_p.reshape(R, -1)
+        if p in self.native_gru:
+            bufs = self._recurrent_probs[p]
+            self.native_gru[p](obs, h, bufs)
+            return bufs
+        probs, h_new = self.models[p].step(obs, h.view(R, -1))
+        h.copy_(h_new.view_as(h))
+        return [q.view(h.shape[0], h.shape[1], -1) for q in probs]
+
     def resync_observations(self):
         """Re-gather the per-policy observation buffers from `observations` (call after
-        anything outside the engine changed the env state, e.g. reset_all_envs)."""
+        anything outside the engine changed the env state, e.g. reset_all_envs); the recurrent
+        policies' states restart."""
+        self.zero_hidden()
         if self.fused is not None:
             obs = self._tensor(_OBSERVATIONS).view(self.E, self.N, -1)
             for p in self.policies:
@@ -594,7 +657,9 @@ class RolloutEngine:
         self._q_masks = mask_p
         per_policy = {}
         for p in self.policies:
-            if self.fused_forward:
+            if self.recurrent_of[p]:
+                per_policy[p] = self._recurrent_forward(p, obs_p[p])
+            elif self.fused_forward:
                 # wgmma forward straight into the persistent probability buffers
                 bufs = self._probs[p]
                 self.fused_forward[p](obs_p[p], bufs[0], bufs[1] if len(bufs) > 1 else None,
@@ -847,6 +912,9 @@ class RolloutEngine:
             if greedy:
                 sample_params["epsilon"] = 0.0
         with torch.no_grad():
+            if self.recurrent and t == 0:
+                for p, h in self.hidden.items():
+                    self.hidden_start[p].copy_(h)
             noisy = self._set_acting_noise() if self.noisy and not greedy else []
             try:
                 probs = self.evaluate_policies(t)
@@ -856,6 +924,8 @@ class RolloutEngine:
             self.sample_actions(probs, t, **sample_params)
             self.env_wrapper.step_all_envs()
             self.bookkeep(t)
+            if self.recurrent:
+                self.recurrent_reset_done()
             # done-masked reset: a no-op for envs that are not done, so no host-side
             # `if done_flags.any()` (trainer_base.py:421-422) is needed
             self.env_wrapper.reset_only_done_envs()

@@ -270,7 +270,12 @@ class Trainer:
         return cfg
 
     def _build_model(self, policy, model_config):
-        model = ModelFactory.create(model_config["type"])(
+        cls = ModelFactory.create(model_config["type"])
+        algorithm = self.config["policy"][policy].get("algorithm")
+        if getattr(cls, "is_recurrent", False) and algorithm not in ("A2C", "PPO"):
+            raise ValueError(f"policy {policy!r}: a recurrent model ({model_config['type']}) "
+                             f"trains with A2C or PPO, not {algorithm}")
+        model = cls(
             env=self.cuda_envs, model_config=model_config, policy=policy,
             policy_tag_to_agent_id_map=self.policy_tag_to_agent_id_map,
             create_separate_placeholders_for_each_policy=(
@@ -399,7 +404,12 @@ class Trainer:
             mask_name = f"{_ACTION_MASK}_batch_{policy}"
             kw = ({"action_mask": dm.data_on_device_via_torch(mask_name)}
                   if dm.is_data_on_device_via_torch(mask_name) else {})
-            probs, values = self.models[policy](obs=obs, **kw)
+            if getattr(self.models[policy], "is_recurrent", False):
+                # the whole batch as T steps of every sequence, from the state it started from
+                probs, values = self.models[policy].forward_sequence(
+                    obs, self.engine.hidden_start[policy], done_flags_batch)
+            else:
+                probs, values = self.models[policy](obs=obs, **kw)
             self._advance_timestep(policy)
             # a Gaussian policy trains on its float actions under its log_std
             if getattr(self.models[policy], "is_gaussian", False):
@@ -432,11 +442,14 @@ class Trainer:
             mask = (dm.data_on_device_via_torch(mask_name)
                     if dm.is_data_on_device_via_torch(mask_name) else None)
             self._advance_timestep(policy)
+            # a recurrent policy replays its sequences from the state its batch started from
+            kw = ({"hidden_start": self.engine.hidden_start[policy]}
+                  if policy in self.engine.hidden_start else {})
             batches[policy] = self.trainers[policy].prepare_batch(
                 self.models[policy],
                 dm.data_on_device_via_torch(f"{_PROCESSED_OBSERVATIONS}_batch_{policy}"),
                 dm.data_on_device_via_torch(f"{_ACTIONS}_batch_{policy}"),
-                training_rewards[policy], done_flags_batch, mask)
+                training_rewards[policy], done_flags_batch, mask, **kw)
         if self._perm_generator is None:
             self._perm_generator = torch.Generator(device=done_flags_batch.device)
             self._perm_generator.manual_seed(self.seed)
@@ -450,14 +463,14 @@ class Trainer:
                 n_mini = self.trainers[policy].num_mini_batches
                 if step % n_mini == 0:         # a new epoch of this policy
                     chunks[policy] = torch.tensor_split(
-                        self.minibatch_permutation(batches[policy].R), n_mini)
+                        self.minibatch_permutation(batches[policy].units), n_mini)
                 rows = chunks[policy][step % n_mini]
                 loss, s = self.trainers[policy].minibatch_loss(
                     self.models[policy], batches[policy], rows, self.current_timestep[policy])
                 self.optimizers[policy].zero_grad()
                 loss.backward()
                 if logging_flag:
-                    sums[policy] += s / rows.numel()
+                    sums[policy] += s / (rows.numel() * batches[policy].rows_per_unit)
             info = self._optimizer_step(self.policies_to_train, logging_flag)
             step_info = info if step_info is None else self._add_step_info(step_info, info)
         loss_metrics = {}
@@ -577,8 +590,11 @@ class Trainer:
                 obs_norm.update_moments(model, obs, self.num_devices)
 
     def _reset_all_envs(self):
-        """Restart every env; the running returns of reward scaling restart with them."""
+        """Restart every env; the running returns of reward scaling and the recurrent policies'
+        states restart with them."""
         self.cuda_envs.reset_all_envs()
+        if getattr(self, "engine", None) is not None:
+            self.engine.zero_hidden()
         for scaler in self._reward_scalers.values():
             scaler.reset()
 
@@ -677,6 +693,8 @@ class Trainer:
                     r_p, _ = eng.policy_step_arrays(p)
                     reward_sum[p] += r_p * undone[:, None]
                     step_sum[p] += undone.to(torch.int32)
+                if eng.recurrent:
+                    eng.recurrent_reset_done()
                 # done envs restart but keep their flag: one episode per env is counted
                 self.cuda_envs.reset_only_done_envs(undo_done_after_reset=False)
         eng.fused = fused
@@ -735,6 +753,8 @@ class Trainer:
                     probs = self.engine.evaluate_policies(-1)
                     self.engine.sample_actions(probs, -1)
                     self.cuda_envs.step_all_envs()
+                    if self.engine.recurrent:
+                        self.engine.recurrent_reset_done()
                 for name in list_of_states:
                     logger.log_tensor_one_step(rings[name], dm.data_on_device_via_torch(name),
                                                t + 1, env_id)
