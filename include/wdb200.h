@@ -1563,8 +1563,9 @@ int wdb_tqc_actor_update_sampled(void *stream, const wdb_tqc_update_args *update
 /* ---- recurrent policies (csrc/wdb_recurrent.cu) ----------------------------------------------
  * FullyConnectedGRU's per-step rollout forward: n_layers (0..2) Linear + ReLU trunk layers, an
  * nn.GRUCell of width H (gate order r, z, n) and one softmax head per discrete action head,
- * reading the new state h'.  fp32 throughout; the value head is not evaluated.  Weights are the
- * torch parameters as they are (Linear [out, in], weight_ih [3H, D], weight_hh [3H, H]). */
+ * reading the new state h' (head_kind 0), or FullyConnectedGaussianGRU's one raw mean head
+ * (head_kind 1).  fp32 throughout; the value head is not evaluated.  Weights are the torch
+ * parameters as they are (Linear [out, in], weight_ih [3H, D], weight_hh [3H, H]). */
 typedef struct wdb_gru_forward {
   long long n_rows;                  /* R = E * Np */
   int in_dim;                        /* F */
@@ -1579,16 +1580,21 @@ typedef struct wdb_gru_forward {
   const float *weight_ih, *weight_hh, *bias_ih, *bias_hh;
   const float *head_weight[2], *head_bias[2];
   float *probs[2];                   /* out [R, A_k] */
+  int head_kind;                     /* 0: softmax heads (probs[k] = the head's probabilities);
+                                        1: one raw mean head, n_heads == 1: probs[0] = the mean
+                                        [R, A], A = heads[0] (no softmax, no tanh) */
 } wdb_gru_forward;
 /* Dynamic shared memory of wdb_gru_policy_forward at these shapes; 0 if it refuses them:
  * 1 <= F <= 256, trunk widths and H in 1 .. 128, 1 or 2 heads of 1 .. 64 actions, and the
- * weights plus a 16-row tile of activations in 227 KB.  No CUDA call. */
+ * weights plus a 16-row tile of activations in 227 KB.  A mean head of A dimensions is asked
+ * as one head of A actions (n_heads 1, a0 = A); both kinds take the same bytes.  No CUDA call. */
 long long wdb_gru_forward_bytes(int in_dim, int n_layers, int d0, int d1, int hidden_size,
                                 int n_heads, int a0, int a1);
-/* One launch: h' into `hidden`, the heads' probabilities into probs[k].  Each output is one
- * thread's k-ascending fmaf sum plus its bias; sig(x) = 1 / (1 + expf(-x)), tanh = tanhf.
- * Bit-identical on relaunch.  cudaErrorInvalidValue without launching on refused shapes or a
- * NULL pointer. */
+/* One launch: h' into `hidden`, the heads' probabilities (or the mean) into probs[k].  Each
+ * output is one thread's k-ascending fmaf sum plus its bias; sig(x) = 1 / (1 + expf(-x)),
+ * tanh = tanhf.  h' does not depend on head_kind.  Bit-identical on relaunch.
+ * cudaErrorInvalidValue without launching on refused shapes, a NULL pointer, an unknown
+ * head_kind or head_kind 1 with n_heads != 1. */
 int wdb_gru_policy_forward(void *stream, const wdb_gru_forward *args);
 
 #define WDB_RECURRENT_MAX_POLICIES 8

@@ -12,9 +12,15 @@
 //   h' = (1 - z) * n + z * h,   sig(x) = 1 / (1 + expf(-x))
 // with gi = W_ih x + b_ih and gh = W_hh h + b_hh each summed as above, every other operation
 // one IEEE-rounded float op (no contraction).  A head's softmax: m = max_a l_a, s = sum_a
-// expf(l_a - m) ascending, p_a = expf(l_a - m) / s.  tests/recurrent_reference.py bounds every
-// output a priori against a float64 evaluation of the same expression.
+// expf(l_a - m) ascending, p_a = expf(l_a - m) / s.  The mean head kind (FullyConnectedGaussianGRU)
+// writes the logits l of its one head as they are.  The head kind is a template parameter: the
+// trunk and the cell are the same code in both instantiations, so h' is the same bits, and the
+// mean instantiation has no softmax.  tests/recurrent_reference.py (the mean kind:
+// tests/gaussian_recurrent_reference.py) bounds every output a priori against a float64
+// evaluation of the same expression.
 #include <algorithm>
+#include <cstddef>
+#include <cstring>
 
 #include "wdb_common.cuh"
 
@@ -142,8 +148,27 @@ __device__ __forceinline__ float sigmoid(float x) {
   return __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-x)));
 }
 
+// The kernel's parameter: wdb_gru_forward without its trailing head_kind, which picks the
+// instantiation instead.  The parameter block keeps the layout it had before head_kind existed.
+struct GruArgs {
+  long long n_rows;
+  int in_dim, n_layers, dims[2], hidden_size, n_heads, heads[2];
+  const float *obs;
+  float *hidden;
+  const float *fc_weight[2], *fc_bias[2];
+  const float *weight_ih, *weight_hh, *bias_ih, *bias_hh;
+  const float *head_weight[2], *head_bias[2];
+  float *probs[2];
+};
+static_assert(sizeof(GruArgs) == offsetof(wdb_gru_forward, head_kind), "GruArgs layout");
+static_assert(offsetof(GruArgs, obs) == offsetof(wdb_gru_forward, obs), "GruArgs layout");
+static_assert(offsetof(GruArgs, probs) == offsetof(wdb_gru_forward, probs), "GruArgs layout");
+
+enum HeadKind { kSoftmaxHeads = 0, kMeanHead = 1 };
+
+template <int kHeadKind>
 __global__ void __launch_bounds__(kThreads, 1)
-gru_policy_forward_kernel(const __grid_constant__ wdb_gru_forward args,
+gru_policy_forward_kernel(const __grid_constant__ GruArgs args,
                           const __grid_constant__ Layout s) {
   extern __shared__ __align__(16) float sm[];
   // ---- weights, once per CTA
@@ -210,22 +235,28 @@ gru_policy_forward_kernel(const __grid_constant__ wdb_gru_forward args,
       if (r < rows) args.hidden[(r0 + r) * H + c] = hn;
     }
     __syncthreads();
-    // ---- heads: logits, then one thread per (row, head) softmax
+    // ---- heads: logits, then one thread per (row, head) softmax, or the mean copied out
     for (int k = 0, col = 0; k < s.n_heads; col += s.heads[k], k++)
       dense(sm + s.w_head[k], sm + s.b_head[k], sm + s.hn, Hp, s.heads[k], sm + s.logits + col,
             A_all, false);
     __syncthreads();
-    for (int i = threadIdx.x; i < kTileRows * s.n_heads; i += blockDim.x) {
-      const int r = i / s.n_heads, k = i - r * s.n_heads;
-      if (r >= rows) continue;
-      const int A = s.heads[k];
-      const float *l = sm + s.logits + r * A_all + (k == 0 ? 0 : s.heads[0]);
-      float m = l[0];
-      for (int a = 1; a < A; a++) m = fmaxf(m, l[a]);
-      float sum = 0.0f;
-      for (int a = 0; a < A; a++) sum = __fadd_rn(sum, expf(__fsub_rn(l[a], m)));
-      float *p = args.probs[k] + (r0 + r) * A;
-      for (int a = 0; a < A; a++) p[a] = __fdiv_rn(expf(__fsub_rn(l[a], m)), sum);
+    if constexpr (kHeadKind == kSoftmaxHeads) {
+      for (int i = threadIdx.x; i < kTileRows * s.n_heads; i += blockDim.x) {
+        const int r = i / s.n_heads, k = i - r * s.n_heads;
+        if (r >= rows) continue;
+        const int A = s.heads[k];
+        const float *l = sm + s.logits + r * A_all + (k == 0 ? 0 : s.heads[0]);
+        float m = l[0];
+        for (int a = 1; a < A; a++) m = fmaxf(m, l[a]);
+        float sum = 0.0f;
+        for (int a = 0; a < A; a++) sum = __fadd_rn(sum, expf(__fsub_rn(l[a], m)));
+        float *p = args.probs[k] + (r0 + r) * A;
+        for (int a = 0; a < A; a++) p[a] = __fdiv_rn(expf(__fsub_rn(l[a], m)), sum);
+      }
+    } else {
+      // one head (A_all = A): the tile's rows [rows, A] are contiguous in both places
+      for (int i = threadIdx.x; i < rows * A_all; i += blockDim.x)
+        args.probs[0][r0 * A_all + i] = sm[s.logits + i];
     }
     __syncthreads();
   }
@@ -251,11 +282,31 @@ WDB_API long long wdb_gru_forward_bytes(int in_dim, int n_layers, int d0, int d1
   return make_layout(in_dim, n_layers, d0, d1, hidden, n_heads, a0, a1, &L) ? L.floats * 4 : 0;
 }
 
+template <int kHeadKind>
+static int launch_gru_forward(void *stream, const wdb_gru_forward *a, const Layout &L) {
+  const int smem = (int)(L.floats * 4);
+  static int configured = 0;
+  if (smem > 48 * 1024 && smem > configured) {
+    cudaError_t e = cudaFuncSetAttribute(gru_policy_forward_kernel<kHeadKind>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) return (int)e;
+    configured = smem;
+  }
+  GruArgs k;
+  std::memcpy(&k, a, sizeof(k));
+  const long long n_tiles = (a->n_rows + kTileRows - 1) / kTileRows;
+  const int grid = (int)(n_tiles < kNumSMs ? n_tiles : kNumSMs);
+  gru_policy_forward_kernel<kHeadKind><<<grid, kThreads, smem, as_stream(stream)>>>(k, L);
+  return finish_launch();
+}
+
 WDB_API int wdb_gru_policy_forward(void *stream, const wdb_gru_forward *a) {
   Layout L;
   if (!a || a->n_rows < 1 || a->n_layers < 0 || a->n_layers > 2 || a->n_heads < 1 ||
       a->n_heads > 2)
     return (int)cudaErrorInvalidValue;
+  if (a->head_kind != kSoftmaxHeads && a->head_kind != kMeanHead) return (int)cudaErrorInvalidValue;
+  if (a->head_kind == kMeanHead && a->n_heads != 1) return (int)cudaErrorInvalidValue;
   if (!make_layout(a->in_dim, a->n_layers, a->dims[0], a->dims[1], a->hidden_size, a->n_heads,
                    a->heads[0], a->heads[1], &L))
     return (int)cudaErrorInvalidValue;
@@ -265,18 +316,8 @@ WDB_API int wdb_gru_policy_forward(void *stream, const wdb_gru_forward *a) {
     if (!a->fc_weight[l] || !a->fc_bias[l]) return (int)cudaErrorInvalidValue;
   for (int k = 0; k < a->n_heads; k++)
     if (!a->head_weight[k] || !a->head_bias[k] || !a->probs[k]) return (int)cudaErrorInvalidValue;
-  const int smem = (int)(L.floats * 4);
-  static int configured = 0;
-  if (smem > 48 * 1024 && smem > configured) {
-    cudaError_t e = cudaFuncSetAttribute(gru_policy_forward_kernel,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return (int)e;
-    configured = smem;
-  }
-  const long long n_tiles = (a->n_rows + kTileRows - 1) / kTileRows;
-  const int grid = (int)(n_tiles < kNumSMs ? n_tiles : kNumSMs);
-  gru_policy_forward_kernel<<<grid, kThreads, smem, as_stream(stream)>>>(*a, L);
-  return finish_launch();
+  return a->head_kind == kMeanHead ? launch_gru_forward<kMeanHead>(stream, a, L)
+                                   : launch_gru_forward<kSoftmaxHeads>(stream, a, L);
 }
 
 WDB_API int wdb_recurrent_reset_done(void *stream, const wdb_recurrent_reset *t) {

@@ -402,6 +402,9 @@ class PerStore(ctypes.Structure):
     ]
 
 
+GRU_HEAD_SOFTMAX, GRU_HEAD_MEAN = 0, 1     # wdb_gru_forward.head_kind
+
+
 class GruForward(ctypes.Structure):
     """struct wdb_gru_forward (include/wdb200.h)."""
 
@@ -411,6 +414,7 @@ class GruForward(ctypes.Structure):
         ("obs", _fp), ("hidden", _fp), ("fc_weight", _fp * 2), ("fc_bias", _fp * 2),
         ("weight_ih", _fp), ("weight_hh", _fp), ("bias_ih", _fp), ("bias_hh", _fp),
         ("head_weight", _fp * 2), ("head_bias", _fp * 2), ("probs", _fp * 2),
+        ("head_kind", _i),
     ]
 
 

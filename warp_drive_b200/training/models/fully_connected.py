@@ -244,6 +244,12 @@ class ModelFactory:
             from warp_drive_b200.training.models.fully_connected_gru import FullyConnectedGRU
 
             cls._registry[model_name] = FullyConnectedGRU
+        if model_name == "fully_connected_gaussian_gru" and model_name not in cls._registry:
+            # the recurrent Gaussian A2C / PPO policy for Box actions, imported on first use
+            from warp_drive_b200.training.models.fully_connected_gru import (
+                FullyConnectedGaussianGRU)
+
+            cls._registry[model_name] = FullyConnectedGaussianGRU
         if model_name not in cls._registry and model_name in (
                 "fully_connected_actor", "fully_connected_action_value_critic",
                 "fully_connected_sac_actor", "fully_connected_quantile_critic"):

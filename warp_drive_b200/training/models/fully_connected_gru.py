@@ -20,6 +20,12 @@ Discrete or MultiDiscrete actions; Box or Dict observations without an action ma
 a ValueError: Box actions, an action mask, `normalize_observations` (and, in the trainer, any
 algorithm but A2C / PPO).  `forward(obs)` refuses as well: a memoryless call would silently drop
 the recurrence.
+
+FullyConnectedGaussianGRU (`fully_connected_gaussian_gru`) is the same recurrent core for a 1-D
+Box action space of A dimensions, as FullyConnectedGaussian is FullyConnected's: `policy_head` is
+one Linear(H, A) whose raw output is the mean, and `log_std` a state-independent parameter [A]
+(`log_std_init`, default 0).  Its `step` and `forward_sequence` return [mean] where the
+categorical model returns its probabilities.
 """
 import torch
 from torch import nn
@@ -37,6 +43,7 @@ _ACTION_MASK = Constants.ACTION_MASK
 
 class FullyConnectedGRU(FullyConnected):
     name = "torch_fully_connected_gru"
+    model_type = "fully_connected_gru"
     is_recurrent = True
     normalize_observations = False
     # the fused training node and every feed-forward rollout kernel take memoryless models only
@@ -57,15 +64,14 @@ class FullyConnectedGRU(FullyConnected):
         sample_agent = policy_tag_to_agent_id_map[policy][0]
         self.observation_space = env.env.observation_space[sample_agent]
         heads, self.is_deterministic = action_head_sizes(env.env.action_space[sample_agent])
-        if self.is_deterministic:
-            raise ValueError("fully_connected_gru takes Discrete or MultiDiscrete actions, "
-                             "not a Box action space")
+        self._check_action_space(self.is_deterministic)
+        kind = self.model_type
         if isinstance(self.observation_space, Dict) and _ACTION_MASK in self.observation_space:
-            raise ValueError("fully_connected_gru does not take an action mask")
+            raise ValueError(f"{kind} does not take an action mask")
         if model_config.get("normalize_observations", False):
-            raise ValueError("fully_connected_gru does not take normalize_observations")
+            raise ValueError(f"{kind} does not take normalize_observations")
         if not self.fc_dims and "gru_dim" not in model_config:
-            raise ValueError("fully_connected_gru needs fc_dims or gru_dim")
+            raise ValueError(f"{kind} needs fc_dims or gru_dim")
         self.hidden_size = int(model_config.get("gru_dim", self.fc_dims[-1] if self.fc_dims
                                                 else 0))
         if self.hidden_size < 1:
@@ -78,15 +84,29 @@ class FullyConnectedGRU(FullyConnected):
             str(i): nn.Sequential(nn.Linear(dims[i], dims[i + 1]), nn.ReLU())
             for i in range(len(self.fc_dims))})
         self.gru = nn.GRUCell(dims[-1], self.hidden_size)
-        self.policy_head = nn.ModuleList([nn.Linear(self.hidden_size, h) for h in heads])
+        self._build_policy_head(heads)
         self.vf_head = nn.Linear(self.hidden_size, 1)
         self.action_mask = None
         name = f"{_PROCESSED_OBSERVATIONS}_batch_{policy}"
         self.batch_size = env.cuda_data_manager.get_shape(name=name)[0]
 
+    @staticmethod
+    def _check_action_space(is_box):
+        if is_box:
+            raise ValueError("fully_connected_gru takes Discrete or MultiDiscrete actions, "
+                             "not a Box action space (fully_connected_gaussian_gru takes Box "
+                             "actions)")
+
+    def _build_policy_head(self, heads):
+        self.policy_head = nn.ModuleList([nn.Linear(self.hidden_size, h) for h in heads])
+
     def forward(self, obs=None, action=None, action_mask=None):
-        raise RuntimeError("fully_connected_gru is recurrent: call step(obs, h) or "
+        raise RuntimeError(f"{self.model_type} is recurrent: call step(obs, h) or "
                            "forward_sequence(obs, h0, done_flags)")
+
+    def head_layers(self):
+        """The policy head Linears, in output order."""
+        return list(self.policy_head)
 
     # ---- the pieces
     def trunk(self, obs):
@@ -127,15 +147,58 @@ class FullyConnectedGRU(FullyConnected):
         return self.heads(hs), self.vf_head(hs)[..., 0]
 
 
+class FullyConnectedGaussianGRU(FullyConnectedGRU):
+    """The recurrent diagonal Gaussian policy: FullyConnectedGRU's trunk, cell, reset rule and
+    value head; `policy_head` = one Linear(H, A) whose raw output is the mean (no tanh, no
+    scaling) and `log_std` a state-independent parameter [A] (model key `log_std_init`, default
+    0).  `step(obs, h) -> ([mean [R, A]], h')`, `forward_sequence -> ([mean [T, E, Np, A]],
+    values)`.  A 1-D Box action space only; actions are drawn unclipped by
+    CUDASampler.sample_gaussian from the mean and log_std, and the env bounds them."""
+
+    name = "torch_fully_connected_gaussian_gru"
+    model_type = "fully_connected_gaussian_gru"
+    is_gaussian = True
+
+    def __init__(self, env, model_config, policy, policy_tag_to_agent_id_map,
+                 create_separate_placeholders_for_each_policy=False,
+                 obs_dim_corresponding_to_num_agents="first"):
+        super().__init__(env, model_config, policy, policy_tag_to_agent_id_map,
+                         create_separate_placeholders_for_each_policy,
+                         obs_dim_corresponding_to_num_agents)
+        self.log_std = nn.Parameter(torch.full(
+            (self.output_dims[0],), float(model_config.get("log_std_init", 0.0))))
+
+    @staticmethod
+    def _check_action_space(is_box):
+        if not is_box:
+            raise ValueError("fully_connected_gaussian_gru takes a 1-D Box action space, not "
+                             "Discrete or MultiDiscrete actions (fully_connected_gru takes "
+                             "those)")
+
+    def _build_policy_head(self, heads):
+        # (a Box space of A dimensions arrives as A heads of size 1: one mean head of A)
+        self.output_dims = [len(heads)]
+        self.policy_head = nn.Linear(self.hidden_size, len(heads))
+
+    def head_layers(self):
+        return [self.policy_head]
+
+    def heads(self, h):
+        return [self.policy_head(h)]
+
+
 class NativeGruStep:
     """FullyConnectedGRU.step as ONE wdb_gru_policy_forward launch (csrc/wdb_recurrent.cu): the
     trunk, the GRU cell (h' written over h in place) and the heads' softmax, fp32, straight into
-    the sampler's probability buffers.  The value head is not evaluated (the rollout never reads
-    values).  It reads the parameters where they are, so an optimizer step needs no re-pack."""
+    the sampler's probability buffers; for FullyConnectedGaussianGRU the mean head kind, which
+    writes the raw mean [R, A] into the sampler's mean buffer.  The value head is not evaluated
+    (the rollout never reads values).  It reads the parameters where they are, so an optimizer
+    step needs no re-pack."""
 
     @staticmethod
     def shape_args(model):
-        """(F, n_layers, d0, d1, H, n_heads, a0, a1) of wdb_gru_forward_bytes, or None."""
+        """(F, n_layers, d0, d1, H, n_heads, a0, a1) of wdb_gru_forward_bytes, or None.  A
+        Gaussian model's mean head is one head of A."""
         if not getattr(model, "is_recurrent", False) or len(model.fc) > 2:
             return None
         if len(model.output_dims) not in (1, 2):
@@ -156,7 +219,9 @@ class NativeGruStep:
     # torch step's 0.140 ms at gridworld's 0.16 GFLOP step, but 1.89 ms against 1.02 ms at
     # TagContinuous's 15 GFLOP step, where cuBLAS outruns this kernel's CUDA-core sums.  The
     # engine routes a policy here only while its step stays under this many FLOPs (the torch
-    # step costs about its launch overhead, 0.14 ms, up to ~1 GFLOP).
+    # step costs about its launch overhead, 0.14 ms, up to ~1 GFLOP).  The mean head kind
+    # crosses over at the same place: 0.082 ms against 0.163 ms at 0.58 GFLOP (10 000 rows,
+    # F = 3, [64, 64], GRU 64, A = 1), 0.147 ms against 0.134 ms at 1.21 GFLOP.
     MAX_ROUTED_FLOPS = 1e9
 
     @classmethod
@@ -189,6 +254,8 @@ class NativeGruStep:
         a.n_rows = hidden.numel() // H
         a.in_dim, a.n_layers, a.hidden_size, a.n_heads = F, n_layers, H, n_heads
         a.dims[0], a.dims[1], a.heads[0], a.heads[1] = d0, d1, a0, a1
+        a.head_kind = (_lib.GRU_HEAD_MEAN if getattr(m, "is_gaussian", False)
+                       else _lib.GRU_HEAD_SOFTMAX)
         assert obs.numel() == a.n_rows * F and obs.dtype == torch.float32
         a.obs, a.hidden = _lib.ptr(obs), _lib.ptr(hidden)
         for i in range(n_layers):
@@ -197,7 +264,7 @@ class NativeGruStep:
         g = m.gru
         a.weight_ih, a.weight_hh = _lib.ptr(g.weight_ih), _lib.ptr(g.weight_hh)
         a.bias_ih, a.bias_hh = _lib.ptr(g.bias_ih), _lib.ptr(g.bias_hh)
-        for k, head in enumerate(m.policy_head):
+        for k, head in enumerate(m.head_layers()):
             assert probs[k].numel() == a.n_rows * head.out_features
             a.head_weight[k], a.head_bias[k] = _lib.ptr(head.weight), _lib.ptr(head.bias)
             a.probs[k] = _lib.ptr(probs[k])

@@ -132,7 +132,8 @@ class RolloutEngine:
         # wdb_recurrent_reset_done launch zeroes the rows of the envs that are done, before the
         # done-masked reset clears their flags: the step after an episode's end starts from zero
         # (FullyConnectedGRU.reset_hidden).  Their rollout forward is wdb_gru_policy_forward
-        # where it takes the shape (native_recurrent), the model's torch step otherwise.
+        # where it takes the shape (native_recurrent), the model's torch step otherwise; a
+        # recurrent Gaussian policy's forward gives its mean, sampled as any Gaussian policy's.
         self.recurrent_of = {p: bool(getattr(models[p], "is_recurrent", False))
                              for p in self.policies}
         self.recurrent = any(self.recurrent_of.values())
@@ -149,9 +150,10 @@ class RolloutEngine:
                     if NativeGruStep.routed(models[p], self.E * len(self.policy_map[p])):
                         self.native_gru[p] = NativeGruStep(models[p])
         assert len(self.hidden) <= _lib.RECURRENT_MAX_POLICIES
+        # (one [E, Np, A_k] buffer per softmax head, or a Gaussian policy's one mean [E, Np, A])
         self._recurrent_probs = {
             p: [torch.empty((self.E, len(self.policy_map[p]), h), device=dev)
-                for h in self.heads_of[p]] for p in self.native_gru}
+                for h in models[p].output_dims] for p in self.native_gru}
         # ---- fused single-launch timestep (TagContinuous: 2 discrete heads, Box obs)
         self.fused = None
         if use_fused_step and self._fused_eligible():
@@ -305,8 +307,8 @@ class RolloutEngine:
                    "recurrent_reset_done")
 
     def _recurrent_forward(self, p, obs_p):
-        """Policy p's probabilities [per head] [E, Np, A_k] from its observation rows, with its
-        state hidden[p] advanced in place."""
+        """Policy p's probabilities [per head] [E, Np, A_k] (a Gaussian policy: [mean
+        [E, Np, A]]) from its observation rows, with its state hidden[p] advanced in place."""
         h = self.hidden[p]
         R = h.shape[0] * h.shape[1]
         obs = obs_p.reshape(R, -1)
